@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the lwm_b200 hot paths (see BASELINE.json / DESIGN.md §Measurement).
+"""bench.py — headline benchmark of the lwm_b200 hot paths (see DESIGN.md).
 
 Workload (config.workload): ring attention forward+backward of ONE LWM-7B layer
 (H=32, D=128, hidden 4096, B=1, causal) at S=131072 tokens, bf16 in / fp32 accumulate, sequence
-sharded over N GPUs (N=1: the whole 128K sequence on one B200). A "step" is one forward+backward
+sharded over N GPUs (N=1: the whole 128K sequence on one H100). A "step" is one forward+backward
 pass of that layer's attention through the public `ringattention` op. STRONG scaling: total
 work is fixed as N grows.
 
@@ -21,7 +21,10 @@ work is fixed as N grows.
           row-wise oracle (oracle/attn_rows.py): out / dq of one sampled query row per 128-row tile and dk / dv of
           every key row, two heads, fp32 read-out; max relative Frobenius error over ranks (north_star bound 1e-3)
   reference_probe   whether the reference's own JAX implementation (jax + the un-vendored `ringattention` package)
-          is importable on this box — if it ever is, the oracle is pinned against it on a small case right here
+          is importable here — if it ever is, the oracle is pinned against it on a small case right here
+  --dump-outputs DIR   after the timed steps, writes what the last timed step returned to its caller (out and the
+          gradients dq, dk, dv) as DIR/<name>.npy, float32, on a fixed seeded sample of 256 token rows (all heads, all
+          of head_dim): 4 x 4 MB. The inputs are seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -51,7 +54,8 @@ def load_peaks():
         d = json.load(open(p))
         return dict(burst=float(d["bf16_tflops"]), sustained=float(d.get("bf16_tflops_sustained", d["bf16_tflops"])),
                     hbm=float(d["hbm_gbs"]), source="MEASURED_PEAKS.json")
-    return dict(burst=1590.0, sustained=1400.0, hbm=6650.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet: dense bf16 tensor rate and HBM3 bandwidth (a ceiling, not a measured rate)
+    return dict(burst=989.0, sustained=989.0, hbm=3350.0, source="H100 SXM data sheet")
 
 
 class ClockSampler:
@@ -203,7 +207,7 @@ VQ_BYTES_ENC = 815.5e6                                   # minimum activation tr
 
 
 def bench_vqgan(dev, peaks, world, rank, with_cpu=True):
-    """BASELINE 'VQGAN frames/s': encode of a 16-frame 256x256 clip, synthetic weights and pixels, default precision
+    """'VQGAN frames/s': encode of a 16-frame 256x256 clip, synthetic weights and pixels, default precision
     mode, same contract as the attention record: `value` with the clip resident in HBM, `e2e` from pinned host pixels to
     host codes (copies inside the timed region), `roofline` against the HBM roof north_star names (algorithmic bytes =
     SURVEY.md §8d minimum-traffic model with fp32 activations, 815.5 MB / frame) with the tensor-pipe fraction beside
@@ -244,9 +248,6 @@ def bench_vqgan(dev, peaks, world, rank, with_cpu=True):
     fps = 16 / (ms * 1e-3)
     gbs = 16 * VQ_BYTES_ENC / (ms * 1e-3) / 1e9
     traffic = None
-    tp = os.path.join(ROOT, "profiles", "ncu_vqgan_encode16_r02.json")
-    if os.path.exists(tp):
-        traffic = json.load(open(tp)).get("dram_total_bytes_per_clip")
     passes = 2.15        # FLOP-weighted MMA work of the mixed mode (2 on the >= 64x64 levels, 3 below)
     rec = {
         "metric": "vqgan_encode_frames_per_s_256x256x16f", "value": world * fps, "unit": "frames/s", "n_gpus": world,
@@ -254,9 +255,9 @@ def bench_vqgan(dev, peaks, world, rank, with_cpu=True):
         "dtype": "f16 tensor-core operands (activation fp16, weights fp16 hi+lo), fp32 accumulate, fp32 activations in HBM",
         "config": {"workload": "VQGAN encode, 16 frames 256x256x3, LWM VQGANConfig defaults (58.7M encoder params)",
                    "precision": "fp16x2 (mixed: 2-MMA fp16 scheme on the >=64x64 levels, 3-MMA split-bf16 below)",
-                   "l2": "every conv streams 34 MB .. 537 MB of activations per clip: larger than the 126 MB L2 on the "
+                   "l2": "every conv streams 34 MB .. 537 MB of activations per clip: larger than the 50 MB L2 on the "
                          "levels that carry 90 % of the bytes"},
-        "roofline": {"bound": "hbm", "kernel": "whole encode (dominant: conv_umma_kernel)", "achieved": gbs,
+        "roofline": {"bound": "hbm", "kernel": "whole encode (dominant: conv_wgmma_kernel)", "achieved": gbs,
                      "peak": peaks["hbm"], "unit": "GB/s", "frac": gbs / peaks["hbm"], "traffic": traffic,
                      "algorithmic_bytes_per_clip": 16 * VQ_BYTES_ENC,
                      "tensor": {"algorithmic_tflops": 16 * VQ_FLOPS_ENC / (ms * 1e-3) / 1e12,
@@ -293,6 +294,21 @@ def bench_vqgan(dev, peaks, world, rank, with_cpu=True):
     return rec
 
 
+DUMP_ROWS = 256
+
+
+def dump_outputs(dirname, outs, Sl):
+    """out, dq, dk, dv of one step -> DIR/<name>.npy (float32), rows of a fixed seeded sample of this rank's tokens"""
+    import numpy as np
+    import torch
+    os.makedirs(dirname, exist_ok=True)
+    rows = np.sort(np.random.default_rng(0).choice(Sl, size=min(Sl, DUMP_ROWS), replace=False))
+    idx = torch.as_tensor(rows, device=outs[0].device)
+    for name, t in zip(("out", "dq", "dk", "dv"), outs):
+        a = t.detach()[0].index_select(0, idx).float().cpu().numpy()
+        np.save(os.path.join(dirname, name + ".npy"), a)
+
+
 # ------------------------------------------------------------------------------------------------
 def main():
     ap = argparse.ArgumentParser()
@@ -310,6 +326,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-parity", action="store_true", help="(debug) skip the oracle check that precedes the timing")
     ap.add_argument("--no-vqgan", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write a fixed seeded sample of the last timed step's out / dq / dk / dv to DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -324,7 +342,7 @@ def main():
     from lwm_b200 import ringattention as ra
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a B200: lwm_b200 has no CPU fallback (use --impl reference for the CPU arm)")
+        raise SystemExit("bench.py needs an H100: lwm_b200 has no CPU fallback (use --impl reference for the CPU arm)")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     if world > 1:
@@ -401,10 +419,17 @@ def main():
     barrier()
     calls0 = _lib.launch_count()
     t0.record()
-    for _ in range(K):
-        step()
+    last = None
+    for i in range(K):
+        if i == K - 1:
+            last = step()       # what the timed path returned to its caller in its last step
+        else:
+            step()
     t1.record()
     barrier()
+    if args.dump_outputs and rank == 0 and last is not None:
+        dump_outputs(args.dump_outputs, last, Sl)
+    del last
     gpu_launches = _lib.launch_count() - calls0      # C-ABI compute calls of this rank in the timed region
     ms = t0.elapsed_time(t1) / K
     clocks = sampler.stop() if rank == 0 else None
@@ -447,15 +472,12 @@ def main():
         del dq, dk, dv
         fl_bwd = 2.5 * f_fwd(S)
         ach = fl_bwd / (kern_ms["bwd"] * 1e-3) / 1e12
-        traffic = None   # dram__bytes_read+write of one attn_bwd_kernel launch at S=131072 (ncu --set full capture)
-        tp = os.path.join(ROOT, "profiles", "ncu_attn_128k_r02.json")
-        if S == S_TOTAL and os.path.exists(tp):
-            traffic = json.load(open(tp))["attn_bwd_kernel"]["dram_total_bytes"]
+        traffic = None
         roof = {"bound": "tensor", "kernel": "attn_bwd_kernel<%s>" % ("fp16 operands" if prec == "fp16" else "bf16 operands"),
                 "achieved": ach, "peak": peaks["sustained"],
                 "unit": "TFLOP/s", "frac": ach / peaks["sustained"], "traffic": traffic,
-                "traffic_note": "bytes per launch from profiles/ncu_attn_128k_r02.json; algorithmic minimum ~17 GB "
-                                "(q,k,v,dout once + dq/dk/dv fp32 read-modify-write); tensor-bound, HBM < 2 % busy",
+                "traffic_note": "not measured; algorithmic minimum ~17 GB (q,k,v,dout once + dq/dk/dv fp32 "
+                                "read-modify-write)",
                 "peak_source": peaks["source"] + " bf16_tflops_sustained (kernel timed inside a long step); burst=%.1f"
                 % peaks["burst"],
                 "fwd_kernel": {"achieved": f_fwd(S) / (kern_ms["fwd"] * 1e-3) / 1e12,
@@ -563,7 +585,7 @@ def main():
             "warmup": W, "ms_per_step": ms, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
             "dtype": "bf16", "data": "synthetic",
             "config": {"workload": workload_name(S), "sharding": "sequence over %d GPU(s)" % world,
-                       "layout": args.layout, "precision": args.precision or ra._DEFAULT_PRECISION, "l2": "inputs (>=1 GiB per tensor at N=1) larger than the 126 MB L2",
+                       "layout": args.layout, "precision": args.precision or ra._DEFAULT_PRECISION, "l2": "inputs (>=1 GiB per tensor at N=1) larger than the 50 MB L2",
                        "tokens_per_s_definition": "S / (32 layers * t_step), attention only"},
             "tflops_per_gpu": total_flops / (ms * 1e-3) / 1e12 / world,
             "frac_of_bf16_peak_per_gpu": total_flops / (ms * 1e-3) / 1e12 / world / peaks["sustained"],
@@ -592,7 +614,7 @@ def main():
             line["cpu_baseline"] = {
                 "value": 4096 / (LAYERS * dt), "unit": UNIT, "cores": cores, "kind": "port",
                 "gflops": fl / dt / 1e9,
-                "sample": "oracle blockwise fwd+bwd (torch CPU fp32) of one full layer at S=4096 (BASELINE configs[0]; "
+                "sample": "oracle blockwise fwd+bwd (torch CPU fp32) of one full layer at S=4096 ("
                           "32 heads, causal); %.1f s of CPU work; tokens/s = 4096 / (32 layers * t)" % dt}
           except Exception as e:      # noqa: BLE001
             line["cpu_baseline"] = {"error": "%s: %s" % (type(e).__name__, str(e)[:200])}

@@ -1,8 +1,8 @@
-/* lwm_b200 — C ABI of the B200 (sm_100a) hot-path library: liblwm_b200.so
+/* lwm_b200 — C ABI of the H100 (sm_90a) hot-path library: liblwm_b200.so
  *
  * This is the drop-in boundary for the two LWM hot paths (SURVEY.md §8b):
  *   - the blockwise `ringattention(q, k, v, attn_bias, segment_ids, ...)` call bound at
- *     /root/reference lwm/llama.py:539-569 (forward) and its custom_vjp backward;
+ *     the reference's lwm/llama.py:539-569 (forward) and its custom_vjp backward;
  *   - the VQGAN tokenizer ops of lwm/vqgan.py:105-351 (conv / GroupNorm / SiLU / resample /
  *     nearest-codebook lookup).
  * The reference has no native boundary of its own (it is pure Python/JAX); these entry points are
@@ -13,7 +13,7 @@
  *   - plain pointers and sizes only; every pointer is a DEVICE pointer unless named host_*;
  *   - all tensor memory is caller-owned; calls are asynchronous on `stream` (a cudaStream_t);
  *   - return value: 0 on success, LWM_ERR_* otherwise; lwm_last_error() gives the message
- *     (thread-local). There is NO CPU fallback: on a non-sm_100 device every call fails with
+ *     (thread-local). There is NO CPU fallback: on a non-sm_90 device every call fails with
  *     LWM_ERR_DEVICE;
  *   - one host thread per GPU/process (torchrun model); contexts are not thread-safe.
  */
@@ -174,8 +174,7 @@ int lwm_add_f32(float* dst, const float* src, long long n, void* stream);
  * LWM_RING_HANDLE_BYTES-byte handle of lwm_ring_ctx_get_handle with all peers by any means (torch.distributed
  * all_gather here), then lwm_ring_ctx_open_peers(handles of all ranks, rank-major).
  * signal_mode: how the remote flag write is issued — 0 cuStreamWriteValue32 on the peer mapping (default),
- * 1 cuMemsetD32Async, 2 a 4-byte copy-engine transfer (values < 4096); all three were measured on B200 + NVSwitch
- * (profiles/probe_ipc_n2_r02.log).
+ * 1 cuMemsetD32Async, 2 a 4-byte copy-engine transfer (values < 4096); tools/probe_ipc.cu exercises all three.
  * Ownership: the context owns the heap and the mappings; everything else stays caller-owned. Not thread-safe
  * (one host thread per rank). lwm_ring_ctx_heap(ctx, peer) is the address, valid in THIS process, of rank `peer`'s
  * heap payload (the layout inside it is the caller's: lwm_b200/ring_peer.py documents the one the op uses). */
@@ -243,7 +242,7 @@ int lwm_ring_layout(int B, long long Sq, long long Sk, int H, int D, int world, 
  *                  y = silu(groupnorm(x)) when gn_stats != NULL (ResnetBlock, vqgan.py:251-256), else y = x;
  *                  optional nearest 2x upsampling (Upsample, vqgan.py:312-316);
  *                  hi = bf16(y) and, if lo != NULL, lo = bf16(y - hi); planes are [N,H',W',C_pad].
- * lwm_vq_conv2d    flax nn.Conv as an implicit GEMM on tcgen05: ksize 1|3, stride 1 (SAME, pad=ksize/2) or
+ * lwm_vq_conv2d    flax nn.Conv as an implicit GEMM on wgmma: ksize 1|3, stride 1 (SAME, pad=ksize/2) or
  *                  the Downsample conv (stride 2, pad 0 on top/left, implicit zero bottom/right,
  *                  vqgan.py:292-300). Weights pre-packed [taps][Cout_pad][C_pad] bf16 (hi / lo).
  *                  n_pass 1 = bf16 operands; 3 = split-bf16 (hi+lo) operands, fp32-class accuracy.
@@ -268,7 +267,7 @@ int lwm_vq_conv_cin3(const float* x, const float* w_hwio, const float* bias, flo
  * lwm_vq_conv2d_f16  activation = that plane; weights split w = hi + lo (two fp16, pre-multiplied by the power of two
  *                    1/w_scale_inv so that lo stays a normal fp16) and STACKED along Cout: w_stacked
  *                    [taps][Cout_pad/BN][2*BN][C_pad], BN = largest multiple of 16 <= 128 dividing Cout_pad, rows [0,BN) = hi, [BN,2BN) = lo. One
- *                    128 x 2BN UMMA yields A.hi | A.lo side by side; the epilogue adds them, applies w_scale_inv, bias,
+ *                    64 x 2BN wgmma per warpgroup yields A.hi | A.lo side by side; the epilogue adds them, applies w_scale_inv, bias,
  *                    residual, clip. gn_stats_out (optional; zeroed by the caller; [N, groups, 2] float64): the epilogue
  *                    also accumulates (sum, sum of squares) of the OUTPUT per (sample, group) — the statistics of the
  *                    GroupNorm that consumes this tensor (vqgan.py:251,254,161,181), so lwm_vq_gn_stats' extra pass
@@ -290,10 +289,6 @@ int lwm_vq_gather(const int* idx, const float* codebook, float* out, long long N
 int lwm_vq_frame_tokens(const int* codes, const int* frame_idx, int* tokens, int n_clips, int T_in, int T_out,
                         int tokens_per_frame, int eof_token, int eov_token, void* stream);
 int lwm_vq_unframe_tokens(const int* tokens, int* codes, long long n_frames, int tokens_per_frame, void* stream);
-
-/* Debug only: device buffer (>= 64 uint64) that the attention kernels fill with per-role barrier-wait cycle
- * counts of CTA (0,0,0) (tools/prof_waits.py); NULL disables. */
-int lwm_debug_set_prof(void* device_buffer);
 
 #ifdef __cplusplus
 }

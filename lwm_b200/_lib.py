@@ -45,7 +45,6 @@ _SIGNATURES = {
     "lwm_attn_decode_merge": [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_ll, c_void_p],
     "lwm_cast_f32_to_bf16": [c_void_p, c_void_p, c_ll, c_void_p],
     "lwm_add_f32": [c_void_p, c_void_p, c_ll, c_void_p],
-    "lwm_debug_set_prof": [c_void_p],
     "lwm_vq_gn_stats": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "lwm_vq_prep": [c_void_p] * 6 + [c_int] * 7 + [c_float, c_void_p],
     "lwm_vq_conv2d": [c_void_p] * 7 + [c_int] * 13 + [c_void_p],
@@ -70,7 +69,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise LwmError(
-            "liblwm_b200.so not found at %s — run `python __graft_entry__.py` (nvcc, sm_100a) first; "
+            "liblwm_b200.so not found at %s — run `python __graft_entry__.py` (nvcc, sm_90a) first; "
             "lwm_b200 has no CPU/PyTorch fallback" % LIB_PATH)
     lib = ctypes.CDLL(LIB_PATH)
     lib.lwm_last_error.restype = ctypes.c_char_p

@@ -1,30 +1,25 @@
-// Ring-attention backward tile kernel for sm_100a.
+// Ring-attention backward tile kernel for sm_90a.
 //
 // One launch = one ring step of the reference's custom_vjp backward (SURVEY.md Appendix A `bwd`;
 // the op is bound at lwm/llama.py:541): for the held K/V block, recompute P from (q, k, lse) and
 // accumulate dV += P^T dO, dK += dS^T Q / sqrt(D), dQ += dS K / sqrt(D) with
 // dS = P o (dO V^T - rowsum(dO o O)).
 //
-// Mapping to the hardware (K/V-stationary, everything computed TRANSPOSED so that the key index
-// sits on the TMEM lanes and P^T can feed the dV MMA straight from TMEM):
-//   CTA = one 128-key tile of one (batch, head); loop over the 128-row Q tiles that can see it.
-//   Five UMMAs (128x128x128, bf16 in, fp32 acc) per Q tile:
-//     S^T  = K  Q^T     SS  K-major x K-major                          -> TMEM R0
-//     dP^T = V  dO^T    SS  K-major x K-major                          -> TMEM R1
-//     dV  += P^T dO     TS  (P^T bf16 written over S^T in R0) x dO MN-major
-//     dK  += dS^T Q     SS  dS^T from smem (K-major)  x Q MN-major
-//     dQ   = dS  K      SS  the SAME smem tile read MN-major x K MN-major -> TMEM R1 (dP^T is dead)
-//   TMEM: R0 | R1 | dK | dV = 512 columns.
-//   warps 0-3 / 4-7 (compute): key row = TMEM lane; the two warpgroups split the 128 query columns and
-//     produce P^T (exp phase) and dS^T. The exp phase of Q tile i+1 is run right after dS^T(i), i.e.
-//     while the tensor pipe executes dK(i), dQ(i).
-//   warp 8: TMA loads (K,V once; Q + lse + delta double-buffered; dO single-buffered);
-//   warp 9: one lane issues the UMMAs.
-//   warps 12-15 (drain): dQ tile TMEM -> registers -> 128B-swizzled smem -> TMA reduce-add (fp32) into
-//     dq_acc, off the compute warps' critical path; it frees R1 for the next dP^T as soon as its
-//     tcgen05.ld's have landed.
-// The softmax scale is folded into dS before it is rounded to bf16, so dK and dQ need no epilogue
-// scaling. dk_acc / dv_acc are accumulated read-modify-write by the one CTA that owns the tile.
+// Mapping to the hardware (K/V-stationary, everything computed TRANSPOSED so that the key index is
+// the M dimension and P^T / dS^T feed the dV / dK wgmmas straight from registers):
+//   CTA = one 128-key tile of one (batch, head); loop over the 64-row Q tiles that can see it.
+//   warpgroups 0 / 1 own keys [0,64) / [64,128) of the tile; per Q tile each runs (bf16 or fp16 in,
+//   fp32 accumulators in registers):
+//     S^T  = K  Q^T     m64n64   both operands K-major in shared memory
+//     dP^T = V  dO^T    m64n64   both operands K-major in shared memory
+//     dV  += P^T dO     m64n128  A = P^T from registers, dO read MN-major
+//     dK  += dS^T Q     m64n128  A = dS^T from registers, Q read MN-major
+//     dQ   = dS  K      m64n64   A = the shared dS^T tile read MN-major (all 128 keys), B = this
+//                                warpgroup's 64 columns of K read MN-major; added to dq_acc with
+//                                vector fp32 atomics.
+//   warp 8: TMA loads (K, V once; Q + dO + lse + delta double-buffered).
+// The softmax scale is folded into dS before it is rounded, so dK and dQ need no epilogue scaling.
+// dk_acc / dv_acc are accumulated read-modify-write by the one CTA that owns the tile.
 #include "attn_common.cuh"
 #include "tmap.h"
 #include "capi_internal.h"
@@ -39,68 +34,64 @@ struct BwdParams {
   MaskParams mask;
   const float* lse;    // [B,H,Sq] PRE-SCALED: -lse*log2(e) (lwm_attn_bwd_lse), -inf for rows without any unmasked key
   const float* delta;  // [B,H,Sq]
+  float* dq_acc;       // [B,Sq,H,D] fp32
   float* dk_acc;       // [B,Sk,H,D] fp32
   float* dv_acc;       // [B,Sk,H,D] fp32
-  unsigned long long* prof;  // debug wait-time buffer or null
   const float *scale_q, *scale_k, *scale_v, *scale_do;   // fp16 mode: device scalars (x = x16 * scale); else null
   int dkv_init;        // 1: dk_acc/dv_acc rows of this launch are WRITTEN (first visit of the block), 0: accumulated
 };
 
-constexpr int kBwdThreads = 512;
-constexpr int kTB = kTile * kHeadDim * 2;  // 32 KB bf16 tile
-// smem map (bytes): K | V | Q0 | Q1 | dO | dS | dQ staging (2 x 16K, drain warpgroup only)
-constexpr int kOffK = 0, kOffV = kTB, kOffQ = 2 * kTB, kOffDO = 4 * kTB, kOffDS = 5 * kTB, kOffStage = 6 * kTB;
-constexpr int kOffLse = 7 * kTB, kOffDelta = kOffLse + 2 * kTile * 4, kOffBars = kOffDelta + 2 * kTile * 4;
-constexpr int kBwdSmemBytes = kOffBars + 256;  // 231,680 B of the 232,448 B a CTA may own
+constexpr int kBQ = 64;                         // query rows per inner iteration
+constexpr int kBwdThreads = 384;                // 2 consumer warpgroups + 1 producer warpgroup
+constexpr int kBwdConsumerWarps = 8;
+constexpr int kTB = kTile * kHeadDim * 2;       // 32 KB: a 128-row bf16 tile
+constexpr int kQB = kBQ * kHeadDim * 2;         // 16 KB: a 64-row bf16 tile
+// smem map (bytes): K | V | Q0 Q1 | dO0 dO1 | dS^T (128 keys x 64 queries) | lse[2] | delta[2] | barriers
+constexpr int kOffK = 0, kOffV = kTB, kOffQ = 2 * kTB, kOffDO = kOffQ + 2 * kQB, kOffDS = kOffDO + 2 * kQB;
+constexpr int kOffLse = kOffDS + kTile * kBQ * 2, kOffDelta = kOffLse + 2 * kBQ * 4, kOffBars = kOffDelta + 2 * kBQ * 4;
+constexpr int kBwdSmemBytes = kOffBars + 128;
 
 struct BwdBarriers {
   uint64_t kv_full;
-  uint64_t q_full[2], q_empty[2];
-  uint64_t do_full, do_empty;
-  uint64_t s_full, dp_full;
-  uint64_t p_ready, ds_ready;
-  uint64_t dq_full, dq_drained;
-  uint64_t final_bar;
+  uint64_t q_full[2], q_empty[2];   // Q + dO + lse + delta of one Q tile
 };
 
-LWM_DEVICE void load_tile_nb(uint8_t* dst, const CUtensorMap* tm, uint64_t* bar, int h, int row0, int b) {
+LWM_DEVICE void load_tile_nb(uint8_t* dst, const CUtensorMap* tm, uint64_t* bar, int h, int row0, int b, int half_bytes) {
   tma_load_4d(dst, tm, bar, 0, h, row0, b);
-  tma_load_4d(dst + kTB / 2, tm, bar, 64, h, row0, b);
+  tma_load_4d(dst + half_bytes, tm, bar, 64, h, row0, b);
 }
 
 // kF16: fp16 operands (exact scaled copies of the bf16 inputs), P^T and dS^T kept in fp16. dS^T is
 // boosted by 2^8 before rounding (keeps it clear of fp16 subnormals); every scale factor is undone in
-// fp32 where the results leave the tensor pipe (dQ drain, dK/dV epilogue).
+// fp32 where the results leave the tensor cores (dQ atomics, dK/dV epilogue).
 constexpr float kDsBoost = 256.0f;
 // P^T = exp(s - lse) is a NORMALISED probability: at 128K .. 1M keys a typical entry is 1e-5 .. 1e-6, below fp16's
-// smallest normal (6.1e-5), where it would lose its 11 bits (measured: dV error 1.2e-3 at S=131072 against 2e-4 at 2K).
-// The fp16 kernel therefore works on P * 2^14 (<= 16384, never overflows; normal down to 3.7e-9): the host folds the
-// +14 into the pre-scaled lse (lwm_attn_bwd_lse, offset_log2 = LWM_ATTN_F16_P_BOOST_LOG2) and the factor is undone in
-// fp32 in the dV epilogue and in the dS scale.
+// smallest normal (6.1e-5), where it would lose its 11 bits. The fp16 kernel therefore works on P * 2^14 (<= 16384,
+// never overflows; normal down to 3.7e-9): the host folds the +14 into the pre-scaled lse (lwm_attn_bwd_lse,
+// offset_log2 = LWM_ATTN_F16_P_BOOST_LOG2) and the factor is undone in fp32 in the dV epilogue and in the dS scale.
 constexpr float kPBoostInv = 1.0f / 16384.0f;
+
 template <bool kF16>
 __global__ void __launch_bounds__(kBwdThreads, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
-                const __grid_constant__ CUtensorMap tmDQ, const BwdParams p) {
+                const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO, const BwdParams p) {
   // no static shared memory in this kernel: the dynamic window starts 1024-aligned (checked below)
   extern __shared__ __align__(1024) uint8_t smem[];
-  float (*s_lse)[kTile] = reinterpret_cast<float (*)[kTile]>(smem + kOffLse);
-  float (*s_delta)[kTile] = reinterpret_cast<float (*)[kTile]>(smem + kOffDelta);
+  float (*s_lse)[kBQ] = reinterpret_cast<float (*)[kBQ]>(smem + kOffLse);
+  float (*s_delta)[kBQ] = reinterpret_cast<float (*)[kBQ]>(smem + kOffDelta);
   BwdBarriers& bars = *reinterpret_cast<BwdBarriers*>(smem + kOffBars);
-  uint32_t& tmem_base_s = *reinterpret_cast<uint32_t*>(smem + kOffBars + 192);
   if (smem_u32(smem) & 1023u) __trap();
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int n = blockIdx.x;  // kv tile (ascending = heaviest first under causal masking)
   const int h = blockIdx.y, b = blockIdx.z;
-  const int n_q_tiles = p.Sq / kTile;
+  const int n_q_tiles = p.Sq / kBQ;
   // first Q tile with a row that can see key 0 of this tile
   int i_start = 0;
   if (p.mask.causal) {
     const long long diff = (long long)p.mask.k_pos0 + (long long)n * kTile - p.mask.q_pos0;
-    i_start = diff <= 0 ? 0 : int(min(diff / kTile, (long long)n_q_tiles));
+    i_start = diff <= 0 ? 0 : int(min(diff / kBQ, (long long)n_q_tiles));
   }
   const int nq = n_q_tiles - i_start;
   if (nq <= 0) {  // this key tile is invisible to the whole q shard: dk/dv unchanged (zero when this launch initialises them)
@@ -115,402 +106,216 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     return;
   }
 
-  if (warp == 9) {
-    tmem_alloc<512>(&tmem_base_s);
-  } else if (warp == 8 && lane == 0) {
+  if (threadIdx.x == 0) {
     mbar_init(&bars.kv_full, 1);
     for (int s = 0; s < 2; ++s) {
       mbar_init(&bars.q_full[s], 1);
-      mbar_init(&bars.q_empty[s], 1);
+      mbar_init(&bars.q_empty[s], kBwdConsumerWarps);
     }
-    mbar_init(&bars.do_full, 1);
-    mbar_init(&bars.do_empty, 1);
-    mbar_init(&bars.s_full, 1);
-    mbar_init(&bars.dp_full, 1);
-    mbar_init(&bars.p_ready, 256);
-    mbar_init(&bars.ds_ready, 256);
-    mbar_init(&bars.dq_full, 1);
-    mbar_init(&bars.dq_drained, 128);
-    mbar_init(&bars.final_bar, 1);
     fence_mbar_init();
-    tma_prefetch_desc(&tmQ);
-    tma_prefetch_desc(&tmK);
-    tma_prefetch_desc(&tmV);
-    tma_prefetch_desc(&tmDO);
-    tma_prefetch_desc(&tmDQ);
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_base_s;
-  constexpr uint32_t R0 = 0, R1 = 128, RDK = 256, RDV = 384;
 
-  if (warp >= 8 && warp < 12) {
+  if (warp >= 8) {
+    // ------------------------------------------------------------------ TMA producer
     setmaxnreg_dec<40>();
-    if (warp == 8) {
-      // ---------------------------------------------------------------- TMA producer
-      if (lane == 0) {
-        mbar_arrive_expect_tx(&bars.kv_full, 2 * kTB);
-        load_tile_nb(smem + kOffK, &tmK, &bars.kv_full, h, n * kTile, b);
-        load_tile_nb(smem + kOffV, &tmV, &bars.kv_full, h, n * kTile, b);
-        const long long ml_base = ((long long)b * p.H + h) * p.Sq;
-        for (int it = 0; it < nq; ++it) {
-          const int st = it & 1;
-          const int row0 = (i_start + it) * kTile;
-          mbar_wait(&bars.q_empty[st], ((it >> 1) & 1) ^ 1);
-          mbar_arrive_expect_tx(&bars.q_full[st], kTB + 2 * kTile * 4);
-          load_tile_nb(smem + kOffQ + st * kTB, &tmQ, &bars.q_full[st], h, row0, b);
-          bulk_load_1d(s_lse[st], p.lse + ml_base + row0, kTile * 4, &bars.q_full[st]);
-          bulk_load_1d(s_delta[st], p.delta + ml_base + row0, kTile * 4, &bars.q_full[st]);
-          mbar_wait(&bars.do_empty, (it & 1) ^ 1);
-          mbar_arrive_expect_tx(&bars.do_full, kTB);
-          load_tile_nb(smem + kOffDO, &tmDO, &bars.do_full, h, row0, b);
-        }
-      }
-    } else if (warp == 9) {
-      // ---------------------------------------------------------------- UMMA issuer
-      // Whole warp in uniform control flow (descriptors in uniform registers); the elected lane issues.
-      {
-        const bool leader = elect_one();
-        constexpr uint32_t kFmt = kF16 ? kFmtF16 : kFmtBF16;
-        constexpr uint32_t id_kk = make_idesc(kTile, kTile, false, false, kFmt, kFmt);     // S^T, dP^T
-        constexpr uint32_t id_kn = make_idesc(kTile, kHeadDim, false, true, kFmt, kFmt);   // dV (A tmem), dK
-        constexpr uint32_t id_nn = make_idesc(kTile, kHeadDim, true, true, kFmt, kFmt);    // dQ
-        const uint32_t aK = smem_u32(smem + kOffK), aV = smem_u32(smem + kOffV), aDO = smem_u32(smem + kOffDO),
-                       aDS = smem_u32(smem + kOffDS), aQ0 = smem_u32(smem + kOffQ);
-        // base descriptors, built once; per-k-step variants are one add away
-        const uint64_t dK_k = desc_kmajor_sw128(aK), dK_n = desc_mnmajor_sw128(aK, kTB / 2);
-        const uint64_t dV_k = desc_kmajor_sw128(aV);
-        const uint64_t dDO_k = desc_kmajor_sw128(aDO), dDO_n = desc_mnmajor_sw128(aDO, kTB / 2);
-        const uint64_t dDS_k = desc_kmajor_sw128(aDS), dDS_n = desc_mnmajor_sw128(aDS, kTB / 2);
-        const uint64_t dQ_k[2] = {desc_kmajor_sw128(aQ0), desc_kmajor_sw128(aQ0 + kTB)};
-        const uint64_t dQ_n[2] = {desc_mnmajor_sw128(aQ0, kTB / 2), desc_mnmajor_sw128(aQ0 + kTB, kTB / 2)};
-        auto koff = [](int ks) { return uint32_t((ks >> 2) * (kTB / 2) + (ks & 3) * 32); };
-        auto issue_st = [&](int it) {
-          if (leader) {
-#pragma unroll
-            for (int ks = 0; ks < 8; ++ks)
-              umma_ss(tmem + R0, desc_advance(dK_k, koff(ks)), desc_advance(dQ_k[it & 1], koff(ks)), id_kk, ks > 0);
-            umma_commit(&bars.s_full);
-          }
-        };
-        // prof slots 0..5: do_full, dq_drained, p_ready, q_full(next), ds_ready, (unused); 6: total
-        WaitProf wp;
-        wp.init(lane == 0 ? p.prof : nullptr);
-        mbar_wait(&bars.kv_full, 0);
-        mbar_wait(&bars.q_full[0], 0);
-        tc_fence_after();
-        const long long t_start = clock64();
-        issue_st(0);
-        for (int it = 0; it < nq; ++it) {
-          wp.wait(&bars.do_full, it & 1, 0);
-          if (it > 0) wp.wait(&bars.dq_drained, (it - 1) & 1, 1);
-          tc_fence_after();
-          if (leader) {
-#pragma unroll
-            for (int ks = 0; ks < 8; ++ks)  // dP^T = V dO^T
-              umma_ss(tmem + R1, desc_advance(dV_k, koff(ks)), desc_advance(dDO_k, koff(ks)), id_kk, ks > 0);
-            umma_commit(&bars.dp_full);
-          }
-          wp.wait(&bars.p_ready, it & 1, 2);
-          tc_fence_after();
-          if (leader) {
-#pragma unroll
-            for (int ks = 0; ks < 8; ++ks)  // dV += P^T dO ; P^T halves live at R0+[0,32) and R0+[64,96)
-              umma_ts(tmem + RDV, tmem + R0 + (ks >> 2) * 64 + (ks & 3) * 8, desc_advance(dDO_n, ks * 2048), id_kn,
-                      (it > 0) || ks > 0);
-            umma_commit(&bars.do_empty);
-          }
-          if (it + 1 < nq) {
-            wp.wait(&bars.q_full[(it + 1) & 1], ((it + 1) >> 1) & 1, 3);
-            tc_fence_after();
-            issue_st(it + 1);
-          }
-          wp.wait(&bars.ds_ready, it & 1, 4);
-          tc_fence_after();
-          if (leader) {
-#pragma unroll
-            for (int ks = 0; ks < 8; ++ks)  // dQ = dS K  (first: its drain then overlaps the dK UMMAs)
-              umma_ss(tmem + R1, desc_advance(dDS_n, ks * 2048), desc_advance(dK_n, ks * 2048), id_nn, ks > 0);
-            umma_commit(&bars.dq_full);
-#pragma unroll
-            for (int ks = 0; ks < 8; ++ks)  // dK += dS^T Q
-              umma_ss(tmem + RDK, desc_advance(dDS_k, koff(ks)), desc_advance(dQ_n[it & 1], ks * 2048), id_kn,
-                      (it > 0) || ks > 0);
-            umma_commit(&bars.q_empty[it & 1]);
-          }
-        }
-        if (leader) umma_commit(&bars.final_bar);
-        wp.flush(0, 6, clock64() - t_start);
+    if (warp == 8 && lane == 0) {
+      tma_prefetch_desc(&tmQ);
+      tma_prefetch_desc(&tmK);
+      tma_prefetch_desc(&tmV);
+      tma_prefetch_desc(&tmDO);
+      mbar_arrive_expect_tx(&bars.kv_full, 2 * kTB);
+      load_tile_nb(smem + kOffK, &tmK, &bars.kv_full, h, n * kTile, b, kTB / 2);
+      load_tile_nb(smem + kOffV, &tmV, &bars.kv_full, h, n * kTile, b, kTB / 2);
+      const long long ml_base = ((long long)b * p.H + h) * p.Sq;
+      for (int it = 0; it < nq; ++it) {
+        const int st = it & 1;
+        const int row0 = (i_start + it) * kBQ;
+        mbar_wait(&bars.q_empty[st], ((it >> 1) & 1) ^ 1);
+        mbar_arrive_expect_tx(&bars.q_full[st], 2 * kQB + 2 * kBQ * 4);
+        load_tile_nb(smem + kOffQ + st * kQB, &tmQ, &bars.q_full[st], h, row0, b, kQB / 2);
+        load_tile_nb(smem + kOffDO + st * kQB, &tmDO, &bars.q_full[st], h, row0, b, kQB / 2);
+        bulk_load_1d(s_lse[st], p.lse + ml_base + row0, kBQ * 4, &bars.q_full[st]);
+        bulk_load_1d(s_delta[st], p.delta + ml_base + row0, kBQ * 4, &bars.q_full[st]);
       }
     }
-  } else if (warp >= 12) {
-    // ------------------------------------------------------------------ dQ drain warpgroup
-    setmaxnreg_dec<88>();
-    const int r = threadIdx.x & (kTile - 1);   // TMEM lane = query row of the dQ tile
-    const uint32_t tR1 = tmem + (uint32_t((warp & 3) * 32) << 16) + R1;
-    uint8_t* stage = smem + kOffStage;
-    const bool is_issuer = (threadIdx.x & 127) == 0;
-    const float dq_mul = kF16 ? (*p.scale_k) * (1.0f / kDsBoost) : 1.0f;   // dQ = (dS*boost) K16 * scale_k / boost
-    WaitProf wp;
-    wp.init(is_issuer ? p.prof : nullptr);
-    const long long t_start = clock64();
-    for (int it = 0; it < nq; ++it) {
-      const int q_tile_row0 = (i_start + it) * kTile;
-      wp.wait(&bars.dq_full, it & 1, 0);
-      tc_fence_after();
-      auto stage_out = [&](const uint32_t (&a0)[32], const uint32_t (&a1)[32]) {
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumer warpgroups
+  setmaxnreg_inc<232>();
+  const int wg = warp >> 2;      // keys [64 wg, 64 wg + 64) of the tile
+  const int w = warp & 3;
+  const int quad = lane & 3;
+  const int kr0 = wg * 64 + w * 16 + (lane >> 2);   // this thread's key rows in the tile: kr0, kr0 + 8
+  const bool has_bias = p.mask.bias != nullptr, has_seg = p.mask.seg != nullptr;
+  const int* seg_row = has_seg ? p.mask.seg + (long long)b * p.mask.seg_stride : nullptr;
+  int k_pos[2], my_seg[2];
+  float bias_t[2] = {0.f, 0.f};
+  bool key_masked[2] = {false, false};
 #pragma unroll
-        for (int c16 = 0; c16 < 8; ++c16) {
-          uint4 v0 = make_uint4(a0[4 * c16], a0[4 * c16 + 1], a0[4 * c16 + 2], a0[4 * c16 + 3]);
-          uint4 v1 = make_uint4(a1[4 * c16], a1[4 * c16 + 1], a1[4 * c16 + 2], a1[4 * c16 + 3]);
-          if (kF16) {
-            v0.x = __float_as_uint(__uint_as_float(v0.x) * dq_mul); v0.y = __float_as_uint(__uint_as_float(v0.y) * dq_mul);
-            v0.z = __float_as_uint(__uint_as_float(v0.z) * dq_mul); v0.w = __float_as_uint(__uint_as_float(v0.w) * dq_mul);
-            v1.x = __float_as_uint(__uint_as_float(v1.x) * dq_mul); v1.y = __float_as_uint(__uint_as_float(v1.y) * dq_mul);
-            v1.z = __float_as_uint(__uint_as_float(v1.z) * dq_mul); v1.w = __float_as_uint(__uint_as_float(v1.w) * dq_mul);
-          }
-          *reinterpret_cast<uint4*>(stage + swz128_offset(r, c16)) = v0;
-          *reinterpret_cast<uint4*>(stage + kTB / 2 + swz128_offset(r, c16)) = v1;
-        }
-      };
-      auto reduce_out = [&](int half) {
-        fence_proxy_async_smem();
-        named_bar_sync(3, 128);
-        if (is_issuer) {
-          tma_reduce_add_4d(&tmDQ, stage, half * 64, h, q_tile_row0, b);
-          tma_reduce_add_4d(&tmDQ, stage + kTB / 2, half * 64 + 32, h, q_tile_row0, b);
-          tma_commit_group();
-        }
-      };
-      {
-        uint32_t a0[32], a1[32];
-        const long long td0 = wp.on ? clock64() : 0;
-        tmem_ld_x32(tR1, a0);
-        tmem_ld_x32(tR1 + 32, a1);
-        tmem_wait_ld();
-        stage_out(a0, a1);
-        tmem_ld_x32(tR1 + 64, a0);
-        tmem_ld_x32(tR1 + 96, a1);
-        tmem_wait_ld();
-        tc_fence_before();
-        mbar_arrive(&bars.dq_drained);   // every lane of dQ has been read: R1 is free for the next dP^T
-        if (wp.on) wp.acc[1] += clock64() - td0;
-        reduce_out(0);
-        const long long td1 = wp.on ? clock64() : 0;
-        if (is_issuer) tma_wait_group_read<0>();
-        named_bar_sync(3, 128);
-        if (wp.on) wp.acc[2] += clock64() - td1;
-        stage_out(a0, a1);
-        reduce_out(1);
-        // free the staging buffers now (this warpgroup idles until the next dQ anyway), so that the next drain can
-        // start its TMEM loads the moment dq_full fires
-        const long long td2 = wp.on ? clock64() : 0;
-        if (is_issuer) tma_wait_group_read<0>();
-        named_bar_sync(3, 128);
-        if (wp.on) wp.acc[3] += clock64() - td2;
-      }
-    }
-    if (is_issuer) tma_wait_group<0>();
-    if (wp.on) {   // prof slots 16: wait dq_full, 17: ld+stage until drained, 18/19: TMA-read waits, 22: total
-      for (int i = 0; i < 4; ++i) wp.buf[16 + i] = (unsigned long long)wp.acc[i];
-      wp.buf[22] = (unsigned long long)(clock64() - t_start);
-    }
-  } else {
-    // ------------------------------------------------------------------ compute warpgroups
-    setmaxnreg_inc<192>();
-    const int wg = warp >> 2;                  // 0: query columns [0,64) ; 1: [64,128)
-    const int r = threadIdx.x & (kTile - 1);   // TMEM lane = key row (S^T, dP^T, dK, dV)
-    const uint32_t lane_off = uint32_t((warp & 3) * 32) << 16;
-    const uint32_t tR0 = tmem + lane_off + R0 + wg * 64;
-    const uint32_t tR1 = tmem + lane_off + R1 + wg * 64;
-    const long long k_pos = (long long)p.mask.k_pos0 + (long long)n * kTile + r;  // this thread's key
-    const bool has_bias = p.mask.bias != nullptr, has_seg = p.mask.seg != nullptr;
-    const int* seg_row = has_seg ? p.mask.seg + (long long)b * p.mask.seg_stride : nullptr;
-    const int my_seg = has_seg ? seg_row[k_pos] : 0;
-    float bias_t = 0.f;
-    bool key_masked = false;
+  for (int hh = 0; hh < 2; ++hh) {
+    k_pos[hh] = p.mask.k_pos0 + n * kTile + kr0 + 8 * hh;
+    my_seg[hh] = has_seg ? seg_row[k_pos[hh]] : 0;
     if (has_bias) {
-      bias_t = p.mask.bias[(long long)b * p.mask.bias_stride + k_pos] * kLog2e;
-      key_masked = bias_t < kMaskedLogit;
-    }
-    uint8_t* my_ds = smem + kOffDS + wg * (kTB / 2);   // this warpgroup's 64 query columns of the dS^T tile
-    // fp16 mode: logits scale picks up scale_q*scale_k; dP = dO V^T picks up scale_do*scale_v
-    const float scale_log2 = p.scale_log2 * (kF16 ? (*p.scale_q) * (*p.scale_k) : 1.0f);
-    const float dp_mul = kF16 ? (*p.scale_do) * (*p.scale_v) : 1.0f;
-    const float ds_mul = p.scale * (kF16 ? kDsBoost * kPBoostInv : 1.0f);   // pr holds P * 2^14 in fp16 mode
-    float pr[64];
-    // prof slots 8..10: q_full, s_full, dp_full ; 11: total (thread 0 only)
-    WaitProf wp;
-    wp.init(threadIdx.x == 0 ? p.prof : nullptr);
-    const long long t_start = clock64();
-
-    // A) P^T = exp2(S^T * scale_log2 (+bias) - lse2) for Q tile `it`; bf16 P^T overwrites this
-    //    warpgroup's half of S^T in TMEM (32 packed columns).
-    // Two compiled versions (mask / no mask): written as one loop with an inner `if (need_mask)` the compiler
-    // if-converts the mask code into ~10 predicated-off instructions per element that still issue.
-    const int k_pos_i = int(k_pos);
-    auto phase_a_impl = [&](int it, auto mask_tag) {
-      constexpr bool kMask = decltype(mask_tag)::value;
-      const int st = it & 1;
-      const int q_tile_pos = p.mask.q_pos0 + (i_start + it) * kTile;
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        uint32_t s[32];
-        const long long tl0 = wp.on ? clock64() : 0;
-        tmem_ld_x32(tR0 + hh * 32, s);
-        tmem_wait_ld();
-        if (wp.on) wp.acc[3] += clock64() - tl0;
-        const float4* lse4 = reinterpret_cast<const float4*>(&s_lse[st][wg * 64 + hh * 32]);
-#pragma unroll
-        for (int c4 = 0; c4 < 8; ++c4) {
-          const float4 l4 = lse4[c4];
-          const float ls[4] = {l4.x, l4.y, l4.z, l4.w};   // -lse*log2e (or -inf): lwm_attn_bwd_lse
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const int c = c4 * 4 + e;
-            if (!kMask) {
-              pr[hh * 32 + c] = ex2f(fmaf(__uint_as_float(s[c]), scale_log2, ls[e]));
-            } else {
-              float tv = key_masked ? kMaskedLogit : fmaf(__uint_as_float(s[c]), scale_log2, bias_t);
-              const int q_pos = q_tile_pos + wg * 64 + hh * 32 + c;
-              if (has_seg && seg_row[q_pos] != my_seg) tv = kMaskedLogit;
-              if (p.mask.causal && q_pos < k_pos_i) tv = kMaskedLogit;
-              pr[hh * 32 + c] = ex2f(tv + ls[e]);
-            }
-          }
-        }
-      }
-    };
-    auto phase_a = [&](int it) {
-      const int st = it & 1;
-      const long long q_tile_pos = (long long)p.mask.q_pos0 + (long long)(i_start + it) * kTile;
-      const bool need_mask = has_bias || has_seg ||
-                             (p.mask.causal && (q_tile_pos < (long long)p.mask.k_pos0 + (long long)n * kTile + kTile - 1));
-      wp.wait(&bars.q_full[st], (it >> 1) & 1, 0);  // lse / delta of this Q tile are in smem
-      wp.wait(&bars.s_full, it & 1, 1);
-      tc_fence_after();
-      const long long tA0 = wp.on ? clock64() : 0;
-      if (need_mask) phase_a_impl(it, std::true_type{});
-      else phase_a_impl(it, std::false_type{});
-      // all 64 logits of this half have been read: the packed P^T may overwrite columns [0,32)
-      uint32_t pk[32];
-#pragma unroll
-      for (int i = 0; i < 32; ++i) pk[i] = kF16 ? pack_f16x2(pr[2 * i], pr[2 * i + 1]) : pack_bf16x2(pr[2 * i], pr[2 * i + 1]);
-      const long long ts0 = wp.on ? clock64() : 0;
-      tmem_st_x32(tR0, pk);
-      tmem_wait_st();
-      tc_fence_before();
-      mbar_arrive(&bars.p_ready);
-      // fold the softmax scale (and the fp16 boost) into P now: this phase runs in the shadow of the dQ/dK
-      // UMMAs, phase B (dS) is on the critical dP^T -> dS -> dQ -> drain loop
-#pragma unroll
-      for (int i = 0; i < 64; ++i) pr[i] *= ds_mul;
-      if (wp.on) {
-        wp.acc[4] += clock64() - ts0;
-        wp.acc[5] += clock64() - tA0;
-      }
-    };
-
-    // B) dS^T = P^T o (dP^T - delta) * scale  -> smem (bf16, 128B-swizzled K-major tile)
-    auto phase_b = [&](int it) {
-      const int st = it & 1;
-      // delta of this Q tile -> registers BEFORE the dS stores: the compiler cannot hoist shared-memory loads
-      // above the st.shared of the previous 8 elements (possible aliasing), which serialised load->math->store
-      float dl[64];
-      {
-        const float4* dl4 = reinterpret_cast<const float4*>(&s_delta[st][wg * 64]);
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const float4 d4 = dl4[i];
-          dl[4 * i] = d4.x; dl[4 * i + 1] = d4.y; dl[4 * i + 2] = d4.z; dl[4 * i + 3] = d4.w;
-        }
-      }
-      wp.wait(&bars.dp_full, it & 1, 2);
-      tc_fence_after();
-      const long long tB0 = wp.on ? clock64() : 0;
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        uint32_t d[32];
-        const long long tl0 = wp.on ? clock64() : 0;
-        tmem_ld_x32(tR1 + hh * 32, d);
-        tmem_wait_ld();
-        if (wp.on) wp.acc[6] += clock64() - tl0;
-#pragma unroll
-        for (int c16 = 0; c16 < 4; ++c16) {  // 8 elements (16 B of bf16/fp16) per store
-          float dsv[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            const int c = hh * 32 + c16 * 8 + e;
-            dsv[e] = pr[c] * fmaf(__uint_as_float(d[c16 * 8 + e]), dp_mul, -dl[c]);   // pr already carries ds_mul
-          }
-          const uint4 v4 = kF16 ? make_uint4(pack_f16x2(dsv[0], dsv[1]), pack_f16x2(dsv[2], dsv[3]),
-                                             pack_f16x2(dsv[4], dsv[5]), pack_f16x2(dsv[6], dsv[7]))
-                                : make_uint4(pack_bf16x2(dsv[0], dsv[1]), pack_bf16x2(dsv[2], dsv[3]),
-                                             pack_bf16x2(dsv[4], dsv[5]), pack_bf16x2(dsv[6], dsv[7]));
-          *reinterpret_cast<uint4*>(my_ds + swz128_offset(r, hh * 4 + c16)) = v4;
-        }
-      }
-      fence_proxy_async_smem();
-      mbar_arrive(&bars.ds_ready);
-      if (wp.on) wp.acc[7] += clock64() - tB0;
-    };
-
-    // order: A(0) B(0) A(1) B(1) ... — A(it+1) overlaps the dQ(it), dK(it) UMMAs. One call site per phase keeps
-    // the unrolled code (and the L0 I-cache footprint) small.
-    for (int it = 0; it <= nq; ++it) {
-      if (it > 0) phase_b(it - 1);
-      if (it < nq) phase_a(it);
-    }
-    // prof slots 8..10 waits (q_full, s_full, dp_full); 11,12: A tmem-ld, A st+arrive; 13: A total; 14: B tmem-ld; 15: B total
-    if (wp.on) {
-      for (int i = 0; i < 8; ++i) wp.buf[8 + i] = (unsigned long long)wp.acc[i];
-      wp.buf[20] = (unsigned long long)(clock64() - t_start);
-    }
-    // ------------------------------------------------------------------ epilogue: dK (wg 0) / dV (wg 1)
-    mbar_wait(&bars.final_bar, 0);
-    tc_fence_after();
-    {
-      // dK = (dS*boost)^T Q16 * scale_q / boost ; dV = P^T dO16 * scale_do
-      const float acc_mul = kF16 ? (wg == 0 ? (*p.scale_q) * (1.0f / kDsBoost) : (*p.scale_do) * kPBoostInv) : 1.0f;
-      const uint32_t tAcc = tmem + lane_off + (wg == 0 ? RDK : RDV);
-      float* acc = (wg == 0 ? p.dk_acc : p.dv_acc) +
-                   ((((long long)b * p.Sk + (long long)n * kTile + r) * p.H + h) * kHeadDim);
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t o[32];
-        tmem_ld_x32(tAcc + c * 32, o);
-        tmem_wait_ld();
-        float4* dst = reinterpret_cast<float4*>(acc + c * 32);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          float4 cur = p.dkv_init ? make_float4(0.f, 0.f, 0.f, 0.f) : dst[i];
-          cur.x = fmaf(__uint_as_float(o[4 * i]), acc_mul, cur.x);
-          cur.y = fmaf(__uint_as_float(o[4 * i + 1]), acc_mul, cur.y);
-          cur.z = fmaf(__uint_as_float(o[4 * i + 2]), acc_mul, cur.z);
-          cur.w = fmaf(__uint_as_float(o[4 * i + 3]), acc_mul, cur.w);
-          dst[i] = cur;
-        }
-      }
+      bias_t[hh] = p.mask.bias[(long long)b * p.mask.bias_stride + k_pos[hh]] * kLog2e;
+      key_masked[hh] = bias_t[hh] < kMaskedLogit;
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 9) tmem_dealloc<512>(tmem);
+  // fp16 mode: logits scale picks up scale_q*scale_k; dP = dO V^T picks up scale_do*scale_v
+  const float scale_log2 = p.scale_log2 * (kF16 ? (*p.scale_q) * (*p.scale_k) : 1.0f);
+  const float dp_mul = kF16 ? (*p.scale_do) * (*p.scale_v) : 1.0f;
+  const float ds_mul = p.scale * (kF16 ? kDsBoost * kPBoostInv : 1.0f);   // P holds P * 2^14 in fp16 mode
+  const float dq_mul = kF16 ? (*p.scale_k) * (1.0f / kDsBoost) : 1.0f;   // dQ = (dS*boost) K16 * scale_k / boost
+  const long long wg_k_last = (long long)p.mask.k_pos0 + (long long)n * kTile + wg * 64 + 63;
+
+  const uint32_t aK = smem_u32(smem + kOffK), aV = smem_u32(smem + kOffV), aDS = smem_u32(smem + kOffDS);
+  const uint64_t dK_k = desc_kmajor_sw128(aK + wg * 64 * 128), dV_k = desc_kmajor_sw128(aV + wg * 64 * 128);
+  const uint64_t dK_n = desc_mnmajor_sw128(aK + wg * (kTB / 2), kTB / 2);   // this warpgroup's 64 columns of K
+  const uint64_t dDS_m = desc_mnmajor_sw128(aDS, kTile * 128);
+  uint8_t* sDS = smem + kOffDS;
+
+  float dk[64], dv[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) dk[i] = dv[i] = 0.f;
+
+  mbar_wait(&bars.kv_full, 0);
+  for (int it = 0; it < nq; ++it) {
+    const int st = it & 1;
+    const uint32_t aQ = smem_u32(smem + kOffQ + st * kQB), aDO = smem_u32(smem + kOffDO + st * kQB);
+    const uint64_t dQ_k = desc_kmajor_sw128(aQ), dDO_k = desc_kmajor_sw128(aDO);
+    const uint64_t dQ_n = desc_mnmajor_sw128(aQ, kQB / 2), dDO_n = desc_mnmajor_sw128(aDO, kQB / 2);
+    mbar_wait(&bars.q_full[st], (it >> 1) & 1);
+
+    // ---- S^T = K Q^T, dP^T = V dO^T
+    float sacc[32], dpacc[32];
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < kHeadDim / 16; ++ks) {
+      const uint32_t ka = (ks >> 2) * (kTB / 2) + (ks & 3) * 32, kb = (ks >> 2) * (kQB / 2) + (ks & 3) * 32;
+      wgmma_ss<64, kF16, 0, 0>(sacc, desc_advance(dK_k, ka), desc_advance(dQ_k, kb), ks > 0);
+    }
+#pragma unroll
+    for (int ks = 0; ks < kHeadDim / 16; ++ks) {
+      const uint32_t ka = (ks >> 2) * (kTB / 2) + (ks & 3) * 32, kb = (ks >> 2) * (kQB / 2) + (ks & 3) * 32;
+      wgmma_ss<64, kF16, 0, 0>(dpacc, desc_advance(dV_k, ka), desc_advance(dDO_k, kb), ks > 0);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(sacc);
+    reg_fence(dpacc);
+
+    // ---- P^T = exp2(S^T * scale_log2 (+bias) - lse2), dS^T = P^T o (dP^T - delta) * scale
+    const long long q_tile_pos = (long long)p.mask.q_pos0 + (long long)(i_start + it) * kBQ;
+    const bool need_mask = has_bias || has_seg || (p.mask.causal && q_tile_pos < wg_k_last);
+    uint32_t pk[4][4], dsk[4][4];   // P^T and dS^T as A fragments, one 16-query slice per entry
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      float pr[8], ds[8];
+#pragma unroll
+      for (int t = 0; t < 8; ++t) {
+        const int i = 8 * kk + t;
+        const int hh = (t >> 1) & 1;
+        const int col = (i >> 2) * 8 + quad * 2 + (i & 1);   // query column in the tile
+        const float ls = s_lse[st][col];   // -lse*log2e (or -inf): lwm_attn_bwd_lse
+        if (!need_mask) {
+          pr[t] = ex2f(fmaf(sacc[i], scale_log2, ls));
+        } else {
+          float tv = key_masked[hh] ? kMaskedLogit : fmaf(sacc[i], scale_log2, bias_t[hh]);
+          const int q_pos = int(q_tile_pos) + col;
+          if (has_seg && seg_row[q_pos] != my_seg[hh]) tv = kMaskedLogit;
+          if (p.mask.causal && q_pos < k_pos[hh]) tv = kMaskedLogit;
+          pr[t] = ex2f(tv + ls);
+        }
+      }
+#pragma unroll
+      for (int t = 0; t < 4; ++t) pk[kk][t] = kF16 ? pack_f16x2(pr[2 * t], pr[2 * t + 1]) : pack_bf16x2(pr[2 * t], pr[2 * t + 1]);
+#pragma unroll
+      for (int t = 0; t < 8; ++t) {
+        const int i = 8 * kk + t;
+        const int col = (i >> 2) * 8 + quad * 2 + (i & 1);
+        ds[t] = (pr[t] * ds_mul) * fmaf(dpacc[i], dp_mul, -s_delta[st][col]);
+      }
+#pragma unroll
+      for (int t = 0; t < 4; ++t) dsk[kk][t] = kF16 ? pack_f16x2(ds[2 * t], ds[2 * t + 1]) : pack_bf16x2(ds[2 * t], ds[2 * t + 1]);
+    }
+
+    // ---- dS^T -> shared memory (128B-swizzled, key rows of 64 queries) for the dQ wgmma of both warpgroups.
+    // Barrier 1: the previous tile's dQ wgmmas of both warpgroups (which read this buffer) have completed.
+    named_bar_sync(1, 256);
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+      for (int t = 0; t < 4; ++t) {
+        const uint32_t row = kr0 + 8 * (t & 1);
+        const uint32_t col = kk * 16 + (t >> 1) * 8 + quad * 2;
+        *reinterpret_cast<uint32_t*>(sDS + swz128_offset(row, col >> 3) + (col & 7) * 2) = dsk[kk][t];
+      }
+    fence_proxy_async_smem();
+
+    // ---- dV += P^T dO, dK += dS^T Q
+    reg_fence(dv);
+    reg_fence(dk);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) wgmma_rs128<kF16, 1>(dv, pk[kk], desc_advance(dDO_n, kk * 2048), 1);
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) wgmma_rs128<kF16, 1>(dk, dsk[kk], desc_advance(dQ_n, kk * 2048), 1);
+    wgmma_commit();
+
+    // ---- dQ = dS K over all 128 keys (barrier 2: both halves of dS^T are in shared memory)
+    named_bar_sync(2, 256);
+    float dq[32];
+#pragma unroll
+    for (int ks = 0; ks < kTile / 16; ++ks)
+      wgmma_ss<64, kF16, 1, 1>(dq, desc_advance(dDS_m, ks * 2048), desc_advance(dK_n, ks * 2048), ks > 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(dq);
+    reg_fence(dv);
+    reg_fence(dk);
+    if (lane == 0) mbar_arrive(&bars.q_empty[st]);   // Q, dO, lse and delta of this stage are no longer read
+
+    // dQ tile (64 queries x this warpgroup's 64 columns) -> dq_acc
+    const int q_row0 = (i_start + it) * kBQ + w * 16 + (lane >> 2);
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      float* dst = p.dq_acc + (((long long)b * p.Sq + q_row0 + 8 * hh) * p.H + h) * kHeadDim + wg * 64 + quad * 2;
+#pragma unroll
+      for (int g = 0; g < 8; ++g)
+        atomicAdd(reinterpret_cast<float2*>(dst + g * 8), make_float2(dq[4 * g + 2 * hh] * dq_mul, dq[4 * g + 2 * hh + 1] * dq_mul));
+    }
+  }
+
+  // ------------------------------------------------------------------ epilogue: dK, dV
+  // dK = (dS*boost)^T Q16 * scale_q / boost ; dV = P^T dO16 * scale_do
+  const float dk_mul = kF16 ? (*p.scale_q) * (1.0f / kDsBoost) : 1.0f;
+  const float dv_mul = kF16 ? (*p.scale_do) * kPBoostInv : 1.0f;
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const long long row = ((((long long)b * p.Sk + (long long)n * kTile + kr0 + 8 * hh) * p.H + h) * kHeadDim);
+#pragma unroll
+    for (int g = 0; g < kHeadDim / 8; ++g) {
+      const int c = g * 8 + quad * 2;
+      float2* pk2 = reinterpret_cast<float2*>(p.dk_acc + row + c);
+      float2* pv2 = reinterpret_cast<float2*>(p.dv_acc + row + c);
+      float2 ck = p.dkv_init ? make_float2(0.f, 0.f) : *pk2;
+      float2 cv = p.dkv_init ? make_float2(0.f, 0.f) : *pv2;
+      ck.x = fmaf(dk[4 * g + 2 * hh], dk_mul, ck.x);
+      ck.y = fmaf(dk[4 * g + 2 * hh + 1], dk_mul, ck.y);
+      cv.x = fmaf(dv[4 * g + 2 * hh], dv_mul, cv.x);
+      cv.y = fmaf(dv[4 * g + 2 * hh + 1], dv_mul, cv.y);
+      *pk2 = ck;
+      *pv2 = cv;
+    }
+  }
 }
 
-static bool make_bf16_tmap(CUtensorMap* tm, const void* ptr, int B, int S, int H) {
+static bool make_bf16_tmap(CUtensorMap* tm, const void* ptr, int B, int S, int H, int box_rows) {
   uint64_t dims[4] = {uint64_t(kHeadDim), uint64_t(H), uint64_t(S), uint64_t(B)};
   uint64_t strides[3] = {uint64_t(kHeadDim) * 2, uint64_t(H) * kHeadDim * 2, uint64_t(S) * H * kHeadDim * 2};
-  uint32_t box[4] = {64, 1, uint32_t(kTile), 1};
+  uint32_t box[4] = {64, 1, uint32_t(box_rows), 1};
   return encode_tmap(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, ptr, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
-}
-static bool make_f32_tmap(CUtensorMap* tm, const void* ptr, int B, int S, int H) {
-  // fp32 [B,S,H,128]: one box = 32 columns (128 B) x 128 rows of one head, 128B swizzle
-  uint64_t dims[4] = {uint64_t(kHeadDim), uint64_t(H), uint64_t(S), uint64_t(B)};
-  uint64_t strides[3] = {uint64_t(kHeadDim) * 4, uint64_t(H) * kHeadDim * 4, uint64_t(S) * H * kHeadDim * 4};
-  uint32_t box[4] = {32, 1, uint32_t(kTile), 1};
-  return encode_tmap(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, ptr, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
 }  // namespace lwm
@@ -535,9 +340,9 @@ static int attn_bwd_launch(const void* q, const void* k, const void* v, const vo
   if (segment_ids && (seg_stride < q_pos0 + Sq || seg_stride < k_pos0 + Sk))
     return lwm_fail(LWM_ERR_SHAPE, "attn_bwd: segment_ids is indexed by GLOBAL position: seg_stride < max(q_pos0 + Sq, k_pos0 + Sk)");
   if (!lwm_check_device()) return LWM_ERR_DEVICE;
-  CUtensorMap tq, tk, tv, tdo, tdq;
-  if (!make_bf16_tmap(&tq, q, B, Sq, H) || !make_bf16_tmap(&tk, k, B, Sk, H) || !make_bf16_tmap(&tv, v, B, Sk, H) ||
-      !make_bf16_tmap(&tdo, dout, B, Sq, H) || !make_f32_tmap(&tdq, dq_acc, B, Sq, H))
+  CUtensorMap tq, tk, tv, tdo;
+  if (!make_bf16_tmap(&tq, q, B, Sq, H, kBQ) || !make_bf16_tmap(&tk, k, B, Sk, H, kTile) ||
+      !make_bf16_tmap(&tv, v, B, Sk, H, kTile) || !make_bf16_tmap(&tdo, dout, B, Sq, H, kBQ))
     return lwm_fail(LWM_ERR_CUDA, "attn_bwd: cuTensorMapEncodeTiled failed (pointers must be 16B aligned)");
   BwdParams p;
   p.B = B; p.H = H; p.Sq = Sq; p.Sk = Sk;
@@ -546,8 +351,7 @@ static int attn_bwd_launch(const void* q, const void* k, const void* v, const vo
   p.mask.q_pos0 = int(q_pos0); p.mask.k_pos0 = int(k_pos0); p.mask.causal = causal;
   p.mask.bias = bias; p.mask.bias_stride = bias_stride;
   p.mask.seg = segment_ids; p.mask.seg_stride = seg_stride;
-  p.lse = lse; p.delta = delta; p.dk_acc = dk_acc; p.dv_acc = dv_acc;
-  p.prof = lwm_prof_buffer();
+  p.lse = lse; p.delta = delta; p.dq_acc = dq_acc; p.dk_acc = dk_acc; p.dv_acc = dv_acc;
   p.scale_q = scale_q; p.scale_k = scale_k; p.scale_v = scale_v; p.scale_do = scale_do;
   p.dkv_init = dkv_init ? 1 : 0;
   static bool attr_set_dev[64] = {};
@@ -564,8 +368,8 @@ static int attn_bwd_launch(const void* q, const void* k, const void* v, const vo
   }
   dim3 grid(Sk / kTile, H, B);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (scale_q) attn_bwd_kernel<true><<<grid, kBwdThreads, kBwdSmemBytes, st>>>(tq, tk, tv, tdo, tdq, p);
-  else attn_bwd_kernel<false><<<grid, kBwdThreads, kBwdSmemBytes, st>>>(tq, tk, tv, tdo, tdq, p);
+  if (scale_q) attn_bwd_kernel<true><<<grid, kBwdThreads, kBwdSmemBytes, st>>>(tq, tk, tv, tdo, p);
+  else attn_bwd_kernel<false><<<grid, kBwdThreads, kBwdSmemBytes, st>>>(tq, tk, tv, tdo, p);
   return lwm_check_launch("attn_bwd_kernel");
 }
 

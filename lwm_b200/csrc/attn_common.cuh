@@ -5,7 +5,7 @@
 namespace lwm {
 
 constexpr int kHeadDim = 128;   // LWM-7B: hidden 4096 / 32 heads (lwm/llama.py:70-81)
-constexpr int kTile = 128;      // rows per Q tile and keys per KV tile (one 128xN UMMA)
+constexpr int kTile = 128;      // rows per Q tile (forward) and keys per KV tile
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kLn2 = 0.6931471805599453f;
 // Logit (log2 domain) given to a masked position. The reference adds finfo(dtype).min, which
@@ -24,35 +24,6 @@ struct MaskParams {
   long long bias_stride;
   const int* seg;        // [B, seg_stride] segment ids at global position, or null
   long long seg_stride;
-};
-
-// Debug-only wait-time accounting (lwm_debug_set_prof): a role thread of CTA (0,0,0) accumulates the
-// cycles it spends in each mbarrier wait; slot layout is documented next to each kernel.
-struct WaitProf {
-  unsigned long long* buf;   // null in production
-  bool on;
-  long long acc[12];
-  LWM_DEVICE void init(unsigned long long* b) {
-    buf = b;
-    on = (b != nullptr) && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0;
-#pragma unroll
-    for (int i = 0; i < 12; ++i) acc[i] = 0;
-  }
-  LWM_DEVICE void wait(uint64_t* bar, uint32_t parity, int slot) {
-    if (on) {
-      const long long t0 = clock64();
-      mbar_wait(bar, parity);
-      acc[slot] += clock64() - t0;
-    } else {
-      mbar_wait(bar, parity);
-    }
-  }
-  LWM_DEVICE void flush(int base, int n, long long total) {
-    if (on) {
-      for (int i = 0; i < n; ++i) buf[base + i] = (unsigned long long)acc[i];
-      buf[base + n] = (unsigned long long)total;
-    }
-  }
 };
 
 }  // namespace lwm

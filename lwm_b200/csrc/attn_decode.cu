@@ -2,7 +2,7 @@
 // (bound at lwm/llama.py:601-614; SURVEY.md Appendix A): a few query rows (q_len = 1 while generating)
 // against the sequence-sharded KV cache with an explicit boolean mask [B,1,Q,K_global]:
 //     s = where(mask, q.k / sqrt(D), finfo.min) ; online softmax ; out = num / den.
-// On B200 this is a pure HBM stream (every K and V row is read exactly once, 2 x S_loc x H x 256 B), so
+// This is a pure HBM stream (every K and V row is read exactly once, 2 x S_loc x H x 256 B), so
 // instead of rotating K/V around a ring each rank reduces its own shard to a partial (o, lse) — split
 // over the keys across many CTAs so that all SMs pull on HBM — and the P partials are merged
 // (log-sum-exp weights) after one tiny all-gather. No tensor cores: the GEMV has 1 FLOP per byte.

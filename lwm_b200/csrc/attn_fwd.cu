@@ -1,4 +1,4 @@
-// Ring-attention forward tile kernel for sm_100a.
+// Ring-attention forward tile kernel for sm_90a.
 //
 // One launch = one ring step of SURVEY.md Appendix A `blockwise_fwd`: the local query shard
 // [B,Sq,H,128] attends to the currently held K/V block [B,Sk,H,128]; the running
@@ -6,16 +6,12 @@
 // lwm/llama.py:541) is merged in the epilogue, so the ring loop on the host only rotates K/V.
 //
 // Mapping to the hardware:
-//   * CTA = two 128-row Q tiles of one (batch, head), ping-ponged so that the tensor pipe works
-//     on one tile while the softmax warpgroup of the other tile runs (exp is MUFU-bound).
-//   * warp 8 streams K/V tiles with TMA (128B swizzle) through a 4-slot ring; warp 9 (one lane)
-//     issues tcgen05.mma: S = Q K^T (SS, K-major x K-major) into TMEM, O += P V (TS: P read from
-//     TMEM, V as MN-major B operand straight from the TMA tile, no transpose).
-//   * warps 0-3 / 4-7: one thread per query row; tcgen05.ld the fp32 logits, online softmax in
-//     the log2 domain, write bf16 P back over S in TMEM. O is rescaled lazily (only when the row
-//     max grows by more than 2^8) by the same warps, which is safe without an extra barrier
-//     because the UMMA pipe is in-order: S(j) complete => P V(j-1) complete.
-//   * TMEM: S0 | S1 | O0 | O1 = 4 x 128 fp32 columns = the full 512 columns.
+//   * CTA = one 128-row Q tile of one (batch, head); CTAs are ordered heaviest (latest rows) first.
+//   * warp 8 streams K/V tiles with TMA (128B swizzle) through a 4-slot ring (K0 V0 K1 V1).
+//   * warpgroups 0 and 1 each own 64 query rows: S = Q K^T with wgmma (both operands K-major in
+//     shared memory, fp32 logits in registers), online softmax in the log2 domain on the register
+//     fragment (a row is spread over the 4 lanes of a quad), then O += P V with P taken straight
+//     from registers as the A fragment and V read MN-major from the TMA tile (no transpose).
 //   * causal masking by global token position; KV tiles entirely above the diagonal are never
 //     loaded; only diagonal tiles pay for the mask.
 #include "attn_common.cuh"
@@ -35,35 +31,34 @@ struct FwdParams {
   float* acc_m;        // [B,H,Sq]     running max, log2 domain
   float* acc_l;        // [B,H,Sq]     running denominator
   int first, last;
-  unsigned long long* prof;  // debug wait-time buffer or null
   const float *scale_q, *scale_k, *scale_v;   // fp16 mode: device scalars, x = x16 * scale; null => bf16 operands
 };
 
 constexpr int kFwdStages = 4;
-// Measured (round 1): routing every 4th exp2 through the FMA-pipe polynomial (ex2_poly3) does NOT pay off here —
-// 965 vs 1026 TFLOP/s at S=131072 — the ~10 extra instructions per element make the softmax warps issue-bound
-// before the XU pipe is relieved. Kept as an opt-in (-DLWM_FWD_POLY_EXP=1) for the 64-wide-S-tile redesign.
-#ifndef LWM_FWD_POLY_EXP
-#define LWM_FWD_POLY_EXP 0
-#endif
-constexpr bool kPolyExp = LWM_FWD_POLY_EXP != 0;
 constexpr int kFwdTileBytes = kTile * kHeadDim * 2;  // 32 KB
-constexpr int kFwdThreads = 384;  // 2 softmax warpgroups + 1 producer warpgroup (TMA, UMMA, 2 idle warps)
-constexpr int kFwdSmemBytes = (2 + kFwdStages) * kFwdTileBytes + 1024;
+constexpr int kFwdThreads = 384;  // 2 consumer warpgroups + 1 producer warpgroup (one TMA warp, 3 idle warps)
+constexpr int kFwdConsumerWarps = 8;
+constexpr int kFwdSmemBytes = (1 + kFwdStages) * kFwdTileBytes + 1024;
 
 struct FwdBarriers {
-  uint64_t q_full[2];
+  uint64_t q_full;
   uint64_t kv_full[kFwdStages];
   uint64_t kv_empty[kFwdStages];
-  uint64_t s_full[2];
-  uint64_t p_ready[2];
-  uint64_t o_final[2];
 };
 
 LWM_DEVICE void load_tile(uint8_t* dst, const CUtensorMap* tm, uint64_t* bar, int h, int row0, int b) {
   mbar_arrive_expect_tx(bar, kFwdTileBytes);
   tma_load_4d(dst, tm, bar, 0, h, row0, b);
   tma_load_4d(dst + kFwdTileBytes / 2, tm, bar, 64, h, row0, b);
+}
+
+LWM_DEVICE float quad_max(float x) {
+  x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 1));
+  return fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 2));
+}
+LWM_DEVICE float quad_sum(float x) {
+  x += __shfl_xor_sync(0xffffffffu, x, 1);
+  return x + __shfl_xor_sync(0xffffffffu, x, 2);
 }
 
 // kF16: operands are IEEE fp16 (exact, scaled copies of the bf16 inputs) and P is kept in fp16
@@ -74,61 +69,44 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
                 const __grid_constant__ CUtensorMap tmV, const FwdParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem;                        // 2 x 32 KB
-  uint8_t* sKV = smem + 2 * kFwdTileBytes;   // ring of 32 KB slots: K0 V0 K1 V1 ...
+  uint8_t* sQ = smem;                   // 32 KB: d [0,64) | d [64,128), 128 rows each
+  uint8_t* sKV = smem + kFwdTileBytes;  // ring of 32 KB slots: K0 V0 K1 V1
   __shared__ FwdBarriers bars;
-  __shared__ uint32_t tmem_base_s;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int n_pairs = (p.Sq + 2 * kTile - 1) / (2 * kTile);
-  const int pair = n_pairs - 1 - int(blockIdx.x);  // heaviest (latest rows) first under causal masking
+  const int n_q_tiles = p.Sq / kTile;
+  const int tile = n_q_tiles - 1 - int(blockIdx.x);  // heaviest (latest rows) first under causal masking
   const int h = blockIdx.y, b = blockIdx.z;
-  const int m0 = pair * 2 * kTile;
-  const bool valid1 = (m0 + kTile) < p.Sq;
-  const int rows_here = valid1 ? 2 * kTile : kTile;
+  const int m0 = tile * kTile;
 
   // number of KV tiles any row of this CTA can see
   int n_kv = p.Sk / kTile;
   if (p.mask.causal) {
-    const long long last_q = (long long)p.mask.q_pos0 + m0 + rows_here - 1;
+    const long long last_q = (long long)p.mask.q_pos0 + m0 + kTile - 1;
     const long long vis = last_q - p.mask.k_pos0;  // largest visible local key index
     n_kv = vis < 0 ? 0 : min((long long)n_kv, vis / kTile + 1);
   }
   if (n_kv == 0 && !p.first && !p.last) return;  // nothing visible: the carry is unchanged
 
-  if (warp == 9) {
-    tmem_alloc<512>(&tmem_base_s);
-  } else if (warp == 8 && lane == 0) {
-    mbar_init(&bars.q_full[0], 1);
-    mbar_init(&bars.q_full[1], 1);
+  if (threadIdx.x == 0) {
+    mbar_init(&bars.q_full, 1);
     for (int i = 0; i < kFwdStages; ++i) {
       mbar_init(&bars.kv_full[i], 1);
-      mbar_init(&bars.kv_empty[i], 1);
-    }
-    for (int t = 0; t < 2; ++t) {
-      mbar_init(&bars.s_full[t], 1);
-      mbar_init(&bars.p_ready[t], kTile);
-      mbar_init(&bars.o_final[t], 1);
+      mbar_init(&bars.kv_empty[i], kFwdConsumerWarps);
     }
     fence_mbar_init();
-    tma_prefetch_desc(&tmQ);
-    tma_prefetch_desc(&tmK);
-    tma_prefetch_desc(&tmV);
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_base_s;
 
-  // register re-partitioning: the producer warpgroup gives its registers to the softmax warpgroups
   if (warp >= 8) {
-    setmaxnreg_dec<56>();
-  if (warp == 8) {
     // ------------------------------------------------------------------ TMA producer
-    if (lane == 0 && n_kv > 0) {
-      load_tile(sQ, &tmQ, &bars.q_full[0], h, m0, b);
-      if (valid1) load_tile(sQ + kFwdTileBytes, &tmQ, &bars.q_full[1], h, m0 + kTile, b);
+    setmaxnreg_dec<40>();
+    if (warp == 8 && lane == 0 && n_kv > 0) {
+      tma_prefetch_desc(&tmQ);
+      tma_prefetch_desc(&tmK);
+      tma_prefetch_desc(&tmV);
+      load_tile(sQ, &tmQ, &bars.q_full, h, m0, b);
       for (int i = 0; i < 2 * n_kv; ++i) {
         const int slot = i % kFwdStages;
         const uint32_t ph = (i / kFwdStages) & 1;
@@ -136,259 +114,164 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         load_tile(sKV + slot * kFwdTileBytes, (i & 1) ? &tmV : &tmK, &bars.kv_full[slot], h, (i >> 1) * kTile, b);
       }
     }
-  } else if (warp == 9) {
-    // ------------------------------------------------------------------ UMMA issuer
-    // The whole warp runs this code in uniform control flow (descriptor math stays in uniform
-    // registers); only the elected lane executes the tcgen05 instructions.
-    if (n_kv > 0) {
-      const bool leader = elect_one();
-      constexpr uint32_t kFmt = kF16 ? kFmtF16 : kFmtBF16;
-      constexpr uint32_t idesc_s = make_idesc(kTile, kTile, false, false, kFmt, kFmt);     // S = Q K^T
-      constexpr uint32_t idesc_o = make_idesc(kTile, kHeadDim, false, true, kFmt, kFmt);   // O = P V (V MN-major)
-      const uint64_t q_desc[2] = {desc_kmajor_sw128(smem_u32(sQ)), desc_kmajor_sw128(smem_u32(sQ + kFwdTileBytes))};
-      const uint32_t kv_base = smem_u32(sKV);
-      auto wait_full_p = [&](int i, WaitProf& w, int slot) {
-        w.wait(&bars.kv_full[i % kFwdStages], (i / kFwdStages) & 1, slot);
-        tc_fence_after();
-      };
-      auto issue_s = [&](int t, int i) {  // i = ring index of K(j)
-        const uint64_t kd = desc_kmajor_sw128(kv_base + (i % kFwdStages) * kFwdTileBytes);
-        if (leader) {
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumer warpgroups
+  setmaxnreg_inc<232>();
+  const int wg = warp >> 2;   // rows [64 wg, 64 wg + 64) of the Q tile
+  const int w = warp & 3;
+  const int quad = lane & 3;
+  // this thread's two rows: r0 and r0 + 8 (accumulator fragment of wgmma m64nNk16)
+  const int r0 = m0 + wg * 64 + w * 16 + (lane >> 2);
+  const float scale = p.scale_log2 * (p.scale_q ? (*p.scale_q) * (*p.scale_k) : 1.0f);
+  const bool has_bias = p.mask.bias != nullptr, has_seg = p.mask.seg != nullptr;
+  const float* bias_row = has_bias ? p.mask.bias + (long long)b * p.mask.bias_stride : nullptr;
+  const int* seg_row = has_seg ? p.mask.seg + (long long)b * p.mask.seg_stride : nullptr;
+  long long q_pos[2];
+  int my_seg[2];
 #pragma unroll
-          for (int ks = 0; ks < kHeadDim / 16; ++ks) {
-            const uint32_t off = (ks >> 2) * (kFwdTileBytes / 2) + (ks & 3) * 32;
-            umma_ss(tmem + t * kTile, desc_advance(q_desc[t], off), desc_advance(kd, off), idesc_s, ks > 0);
-          }
-          umma_commit(&bars.s_full[t]);
-        }
-      };
-      auto issue_pv = [&](int t, int i, bool accumulate) {  // i = ring index of V(j)
-        const uint64_t vd = desc_mnmajor_sw128(kv_base + (i % kFwdStages) * kFwdTileBytes, kFwdTileBytes / 2);
-        if (leader) {
+  for (int hh = 0; hh < 2; ++hh) {
+    q_pos[hh] = (long long)p.mask.q_pos0 + r0 + 8 * hh;
+    my_seg[hh] = has_seg ? seg_row[q_pos[hh]] : 0;
+  }
+
+  float o[64];
 #pragma unroll
-          for (int ks = 0; ks < kTile / 16; ++ks)
-            umma_ts(tmem + 2 * kTile + t * kHeadDim, tmem + t * kTile + ks * 8, desc_advance(vd, ks * 2048), idesc_o,
-                    accumulate || ks > 0);
-        }
-      };
-      // prof slots 32..35: kv_full(V), p_ready0, kv_full(K next), p_ready1 ; 36: total
-      WaitProf wp;
-      wp.init(lane == 0 ? p.prof : nullptr);
-      mbar_wait(&bars.q_full[0], 0);
-      if (valid1) mbar_wait(&bars.q_full[1], 0);
-      wait_full_p(0, wp, 0);
-      const long long t_start = clock64();
-      issue_s(0, 0);
-      if (valid1) issue_s(1, 0);
-      if (leader) umma_commit(&bars.kv_empty[0]);
-      for (int j = 0; j < n_kv; ++j) {
-        const int iv = 2 * j + 1, ikn = 2 * j + 2;
-        const bool more = (j + 1) < n_kv;
-        wait_full_p(iv, wp, 0);
-        wp.wait(&bars.p_ready[0], j & 1, 1);
-        tc_fence_after();
-        issue_pv(0, iv, j > 0);
-        if (more) {
-          wait_full_p(ikn, wp, 2);
-          issue_s(0, ikn);
-        } else if (leader) {
-          umma_commit(&bars.o_final[0]);
-        }
-        if (valid1) {
-          wp.wait(&bars.p_ready[1], j & 1, 3);
-          tc_fence_after();
-          issue_pv(1, iv, j > 0);
-          if (more) issue_s(1, ikn);
-          else if (leader) umma_commit(&bars.o_final[1]);
-        }
-        if (leader) {
-          umma_commit(&bars.kv_empty[iv % kFwdStages]);
-          if (more) umma_commit(&bars.kv_empty[ikn % kFwdStages]);
-        }
+  for (int i = 0; i < 64; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+
+  if (n_kv > 0) {
+    mbar_wait(&bars.q_full, 0);
+    const uint64_t q_desc = desc_kmajor_sw128(smem_u32(sQ + wg * 64 * 128));
+    const uint32_t kv_base = smem_u32(sKV);
+    const long long warp_q_pos0 = (long long)p.mask.q_pos0 + m0 + wg * 64 + w * 16;
+    for (int j = 0; j < n_kv; ++j) {
+      const int ik = 2 * j, iv = 2 * j + 1;
+      // ---- S = Q K^T
+      float s[64];
+      mbar_wait(&bars.kv_full[ik % kFwdStages], (ik / kFwdStages) & 1);
+      const uint64_t kd = desc_kmajor_sw128(kv_base + (ik % kFwdStages) * kFwdTileBytes);
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < kHeadDim / 16; ++ks) {
+        const uint32_t off = (ks >> 2) * (kFwdTileBytes / 2) + (ks & 3) * 32;
+        wgmma_ss<128, kF16, 0, 0>(s, desc_advance(q_desc, off), desc_advance(kd, off), ks > 0);
       }
-      wp.flush(32, 4, clock64() - t_start);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(s);
+      if (lane == 0) mbar_arrive(&bars.kv_empty[ik % kFwdStages]);
+
+      // ---- online softmax on the fragment
+      const long long k_tile_pos = (long long)p.mask.k_pos0 + (long long)j * kTile;
+      // warp-uniform: does any row of this warp need a mask on this KV tile?
+      const bool need_mask = has_bias || has_seg || (p.mask.causal && (k_tile_pos + kTile - 1 > warp_q_pos0));
+      float mx[2] = {-INFINITY, -INFINITY};
+      if (!need_mask) {
+#pragma unroll
+        for (int i = 0; i < 64; ++i) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], s[i]);
+        mx[0] = quad_max(mx[0]) * scale;
+        mx[1] = quad_max(mx[1]) * scale;
+      } else {
+#pragma unroll
+        for (int i = 0; i < 64; ++i) {
+          const int hh = (i >> 1) & 1;
+          const int col = (i >> 2) * 8 + quad * 2 + (i & 1);
+          float tv = s[i] * scale;
+          if (has_bias) {
+            const float bt = bias_row[k_tile_pos + col] * kLog2e;
+            tv = (bt < kMaskedLogit) ? kMaskedLogit : tv + bt;
+          }
+          if (has_seg && seg_row[k_tile_pos + col] != my_seg[hh]) tv = kMaskedLogit;
+          if (p.mask.causal && k_tile_pos + col > q_pos[hh]) tv = kMaskedLogit;
+          s[i] = tv;
+          mx[hh] = fmaxf(mx[hh], tv);
+        }
+        mx[0] = quad_max(mx[0]);
+        mx[1] = quad_max(mx[1]);
+      }
+      float alpha[2];
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const float m_new = fmaxf(m_run[hh], mx[hh]);
+        alpha[hh] = (m_run[hh] == -INFINITY) ? 0.f : ex2f(m_run[hh] - m_new);
+        m_run[hh] = m_new;
+        l_run[hh] *= alpha[hh];
+      }
+      if (j > 0) {
+#pragma unroll
+        for (int i = 0; i < 64; ++i) o[i] *= alpha[(i >> 1) & 1];
+      }
+      const float neg_m[2] = {-m_run[0], -m_run[1]};
+      uint32_t pa[8][4];   // P as the A fragment of O += P V, one 16-key slice per entry
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {
+        float e[8];
+#pragma unroll
+        for (int t = 0; t < 8; ++t) {
+          const int i = 8 * kk + t;
+          const int hh = (t >> 1) & 1;
+          e[t] = need_mask ? ex2f(s[i] + neg_m[hh]) : ex2f(fmaf(s[i], scale, neg_m[hh]));
+          l_run[hh] += e[t];
+        }
+#pragma unroll
+        for (int t = 0; t < 4; ++t) pa[kk][t] = kF16 ? pack_f16x2(e[2 * t], e[2 * t + 1]) : pack_bf16x2(e[2 * t], e[2 * t + 1]);
+      }
+
+      // ---- O += P V
+      mbar_wait(&bars.kv_full[iv % kFwdStages], (iv / kFwdStages) & 1);
+      const uint64_t vd = desc_mnmajor_sw128(kv_base + (iv % kFwdStages) * kFwdTileBytes, kFwdTileBytes / 2);
+      reg_fence(o);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < kTile / 16; ++kk) wgmma_rs128<kF16, 1>(o, pa[kk], desc_advance(vd, kk * 2048), 1);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(o);
+      if (lane == 0) mbar_arrive(&bars.kv_empty[iv % kFwdStages]);
     }
   }
-  } else {
-    // ------------------------------------------------------------------ softmax + epilogue warpgroups
-    setmaxnreg_inc<224>();
-    const int t = warp >> 2;                 // Q tile handled by this warpgroup
-    const int r = threadIdx.x & (kTile - 1);  // row inside the tile == TMEM lane
-    if (t == 0 || valid1) {
-      const uint32_t lane_off = uint32_t((warp & 3) * 32) << 16;
-      const uint32_t tS = tmem + lane_off + t * kTile;
-      const uint32_t tO = tmem + lane_off + 2 * kTile + t * kHeadDim;
-      const int q_row = m0 + t * kTile + r;                         // local row
-      const long long q_pos = (long long)p.mask.q_pos0 + q_row;     // global position
-      const float scale = p.scale_log2 * (p.scale_q ? (*p.scale_q) * (*p.scale_k) : 1.0f);
-      const bool has_bias = p.mask.bias != nullptr, has_seg = p.mask.seg != nullptr;
-      const float* bias_row = has_bias ? p.mask.bias + (long long)b * p.mask.bias_stride : nullptr;
-      const int* seg_row = has_seg ? p.mask.seg + (long long)b * p.mask.seg_stride : nullptr;
-      const int my_seg = has_seg ? seg_row[q_pos] : 0;
 
-      float m_run = -INFINITY, l_run = 0.f;
-      WaitProf wp;
-      wp.init(threadIdx.x == 0 ? p.prof : nullptr);
-      const long long t_start = clock64();
-      for (int j = 0; j < n_kv; ++j) {
-        wp.wait(&bars.s_full[t], j & 1, 0);
-        tc_fence_after();
-        uint32_t s[4][32];
+  // ---------------------------------------------------------------- epilogue: merge carry, write
 #pragma unroll
-        for (int c = 0; c < 4; ++c) tmem_ld_x32(tS + c * 32, s[c]);
-        tmem_wait_ld();
-
-        const long long k_tile_pos = (long long)p.mask.k_pos0 + (long long)j * kTile;
-        // warp-uniform: does any row of this tile need a mask on this KV tile?
-        const bool need_mask = has_bias || has_seg ||
-                               (p.mask.causal && (k_tile_pos + kTile - 1 > (long long)p.mask.q_pos0 + m0 + t * kTile));
-        float mx = -INFINITY;
-        if (!need_mask) {
-          // 4 independent chains of 3-input max (FMNMX3): a single 128-long chain costs ~500 cycles
-          float pm0 = -INFINITY, pm1 = -INFINITY, pm2 = -INFINITY, pm3 = -INFINITY;
+  for (int hh = 0; hh < 2; ++hh) {
+    const int q_row = r0 + 8 * hh;
+    const float l_run_row = quad_sum(l_run[hh]);
+    const long long ml_idx = ((long long)b * p.H + h) * p.Sq + q_row;
+    const long long o_idx = (((long long)b * p.Sq + q_row) * p.H + h) * kHeadDim;
+    float m_c = -INFINITY, l_c = 0.f;
+    if (!p.first) {
+      m_c = p.acc_m[ml_idx];
+      l_c = p.acc_l[ml_idx];
+    }
+    const float m_new = fmaxf(m_c, m_run[hh]);
+    float wa = (m_c == -INFINITY) ? 0.f : ex2f(m_c - m_new);          // weight of the carry
+    float wb = (m_run[hh] == -INFINITY) ? 0.f : ex2f(m_run[hh] - m_new);  // weight of this step
+    const float l_new = wa * l_c + wb * l_run_row;
+    if (p.scale_v) wb *= *p.scale_v;   // V was stored as v16 * scale_v
+    if (p.last) {
+      const float inv = l_new > 0.f ? 1.0f / l_new : 0.f;
+      wa *= inv;
+      wb *= inv;
+    }
 #pragma unroll
-          for (int c = 0; c < 4; ++c)
-#pragma unroll
-            for (int i = 0; i < 32; i += 8) {
-              pm0 = fmaxf(fmaxf(pm0, __uint_as_float(s[c][i + 0])), __uint_as_float(s[c][i + 1]));
-              pm1 = fmaxf(fmaxf(pm1, __uint_as_float(s[c][i + 2])), __uint_as_float(s[c][i + 3]));
-              pm2 = fmaxf(fmaxf(pm2, __uint_as_float(s[c][i + 4])), __uint_as_float(s[c][i + 5]));
-              pm3 = fmaxf(fmaxf(pm3, __uint_as_float(s[c][i + 6])), __uint_as_float(s[c][i + 7]));
-            }
-          mx = fmaxf(fmaxf(pm0, pm1), fmaxf(pm2, pm3));
-          mx *= scale;
-        } else {
-          const long long lim = p.mask.causal ? (q_pos - k_tile_pos) : (long long)kTile;  // keys c > lim are masked
-#pragma unroll
-          for (int c = 0; c < 4; ++c)
-#pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              const int col = c * 32 + i;
-              float tv = __uint_as_float(s[c][i]) * scale;
-              if (has_bias) {
-                const float bt = bias_row[k_tile_pos + col] * kLog2e;
-                tv = (bt < kMaskedLogit) ? kMaskedLogit : tv + bt;
-              }
-              if (has_seg && seg_row[k_tile_pos + col] != my_seg) tv = kMaskedLogit;
-              if ((long long)col > lim) tv = kMaskedLogit;
-              s[c][i] = __float_as_uint(tv);
-              mx = fmaxf(mx, tv);
-            }
-        }
-        const float m_new = fmaxf(m_run, mx);
-        if (j == 0) {
-          m_run = m_new;
-        } else if (__any_sync(0xffffffffu, (m_new - m_run) > 8.0f)) {
-          // lazy rescale of the accumulator row (rare after the first few tiles)
-          const float alpha = ex2f(m_run - m_new);
-          l_run *= alpha;
-          m_run = m_new;
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            uint32_t o[32];
-            tmem_ld_x32(tO + c * 32, o);
-            tmem_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st_x32(tO + c * 32, o);
-          }
-        }
-        const float neg_m = -m_run;
-        float sum0 = 0.f, sum1 = 0.f, sum2 = 0.f, sum3 = 0.f;
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          uint32_t pk[16];
-#pragma unroll
-          for (int i = 0; i < 32; i += 4) {
-            float e0, e1, e2, e3;
-            if (!need_mask) {
-              e0 = ex2f(fmaf(__uint_as_float(s[c][i + 0]), scale, neg_m));
-              e1 = ex2f(fmaf(__uint_as_float(s[c][i + 1]), scale, neg_m));
-              e2 = ex2f(fmaf(__uint_as_float(s[c][i + 2]), scale, neg_m));
-              e3 = kPolyExp ? ex2_poly3(fmaf(__uint_as_float(s[c][i + 3]), scale, neg_m))
-                            : ex2f(fmaf(__uint_as_float(s[c][i + 3]), scale, neg_m));
-            } else {
-              e0 = ex2f(__uint_as_float(s[c][i + 0]) + neg_m);
-              e1 = ex2f(__uint_as_float(s[c][i + 1]) + neg_m);
-              e2 = ex2f(__uint_as_float(s[c][i + 2]) + neg_m);
-              e3 = ex2f(__uint_as_float(s[c][i + 3]) + neg_m);
-            }
-            sum0 += e0; sum1 += e1; sum2 += e2; sum3 += e3;
-            pk[i / 2] = kF16 ? pack_f16x2(e0, e1) : pack_bf16x2(e0, e1);
-            pk[i / 2 + 1] = kF16 ? pack_f16x2(e2, e3) : pack_bf16x2(e2, e3);
-          }
-          tmem_st_x16(tS + c * 16, pk);  // P (bf16) aliases the first 64 columns of S
-        }
-        l_run += (sum0 + sum1) + (sum2 + sum3);
-        tmem_wait_st();
-        tc_fence_before();
-        mbar_arrive(&bars.p_ready[t]);
-      }
-
-      wp.flush(40, 1, clock64() - t_start);
-      // ---------------------------------------------------------------- epilogue: merge carry, write
-      if (n_kv > 0) {
-        mbar_wait(&bars.o_final[t], 0);
-        tc_fence_after();
-      }
-      const long long ml_idx = ((long long)b * p.H + h) * p.Sq + q_row;
-      const long long o_idx = (((long long)b * p.Sq + q_row) * p.H + h) * kHeadDim;
-      float m_c = -INFINITY, l_c = 0.f;
+    for (int g = 0; g < kHeadDim / 8; ++g) {
+      const int c = g * 8 + quad * 2;
+      float2 f = make_float2(o[4 * g + 2 * hh] * wb, o[4 * g + 2 * hh + 1] * wb);
       if (!p.first) {
-        m_c = p.acc_m[ml_idx];
-        l_c = p.acc_l[ml_idx];
+        const float2 a2 = *reinterpret_cast<const float2*>(p.acc_o + o_idx + c);
+        f.x = fmaf(a2.x, wa, f.x);
+        f.y = fmaf(a2.y, wa, f.y);
       }
-      const float m_new = fmaxf(m_c, m_run);
-      float wa = (m_c == -INFINITY) ? 0.f : ex2f(m_c - m_new);     // weight of the carry
-      float wb = (m_run == -INFINITY) ? 0.f : ex2f(m_run - m_new);  // weight of this step
-      const float l_new = wa * l_c + wb * l_run;
-      if (p.scale_v) wb *= *p.scale_v;   // V was stored as v16 * scale_v
       if (p.last) {
-        const float inv = l_new > 0.f ? 1.0f / l_new : 0.f;
-        wa *= inv;
-        wb *= inv;
+        *reinterpret_cast<uint32_t*>(p.out + o_idx + c) = pack_bf16x2(f.x, f.y);
+        if (p.out_f32) *reinterpret_cast<float2*>(p.out_f32 + o_idx + c) = f;
+      } else {
+        *reinterpret_cast<float2*>(p.acc_o + o_idx + c) = f;
       }
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t o[32];
-        if (n_kv > 0) {
-          tmem_ld_x32(tO + c * 32, o);
-          tmem_wait_ld();
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) o[i] = 0;
-        }
-        float f[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(o[i]) * wb;
-        if (!p.first) {
-          const float4* src = reinterpret_cast<const float4*>(p.acc_o + o_idx + c * 32);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float4 a4 = src[i];
-            f[4 * i + 0] = fmaf(a4.x, wa, f[4 * i + 0]);
-            f[4 * i + 1] = fmaf(a4.y, wa, f[4 * i + 1]);
-            f[4 * i + 2] = fmaf(a4.z, wa, f[4 * i + 2]);
-            f[4 * i + 3] = fmaf(a4.w, wa, f[4 * i + 3]);
-          }
-        }
-        if (p.last) {
-          uint4* dst = reinterpret_cast<uint4*>(p.out + o_idx + c * 32);
-#pragma unroll
-          for (int i = 0; i < 4; ++i)
-            dst[i] = make_uint4(pack_bf16x2(f[8 * i], f[8 * i + 1]), pack_bf16x2(f[8 * i + 2], f[8 * i + 3]),
-                                pack_bf16x2(f[8 * i + 4], f[8 * i + 5]), pack_bf16x2(f[8 * i + 6], f[8 * i + 7]));
-          if (p.out_f32) {
-            float4* d32 = reinterpret_cast<float4*>(p.out_f32 + o_idx + c * 32);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) d32[i] = make_float4(f[4 * i], f[4 * i + 1], f[4 * i + 2], f[4 * i + 3]);
-          }
-        } else {
-          float4* dst = reinterpret_cast<float4*>(p.acc_o + o_idx + c * 32);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) dst[i] = make_float4(f[4 * i], f[4 * i + 1], f[4 * i + 2], f[4 * i + 3]);
-        }
-      }
+    }
+    if (quad == 0) {
       if (p.last) {
         p.lse[ml_idx] = l_new > 0.f ? (m_new + log2f(l_new)) * kLn2 : -INFINITY;
       } else {
@@ -397,9 +280,6 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 9) tmem_dealloc<512>(tmem);
 }
 
 static bool make_qkv_tmap(CUtensorMap* tm, const void* ptr, int B, int S, int H) {
@@ -446,7 +326,6 @@ static int attn_fwd_launch(const void* q, const void* k, const void* v, void* ou
   p.out = reinterpret_cast<__nv_bfloat16*>(out);
   p.lse = lse; p.acc_o = acc_o; p.acc_m = acc_m; p.acc_l = acc_l;
   p.first = first; p.last = last;
-  p.prof = lwm_prof_buffer();
   p.scale_q = scale_q; p.scale_k = scale_k; p.scale_v = scale_v;
   p.out_f32 = out_f32;
   static bool attr_set_dev[64] = {};
@@ -461,7 +340,7 @@ static int attn_fwd_launch(const void* q, const void* k, const void* v, void* ou
       return lwm_fail(LWM_ERR_CUDA, "attn_fwd: cannot raise dynamic shared memory limit");
     attr_set = true;
   }
-  dim3 grid((Sq + 2 * kTile - 1) / (2 * kTile), H, B);
+  dim3 grid(Sq / kTile, H, B);
   if (scale_q)
     attn_fwd_kernel<true><<<grid, kFwdThreads, kFwdSmemBytes, reinterpret_cast<cudaStream_t>(stream)>>>(tq, tk, tv, p);
   else

@@ -254,7 +254,7 @@ extern "C" int lwm_attn_bwd_lse(const float* lse, float* nlse2, long long n, flo
   if (!lse || !nlse2 || n <= 0) return lwm_fail(LWM_ERR_ARG, "attn_bwd_lse: bad args");
   if (!lwm_check_device()) return LWM_ERR_DEVICE;
   const long long want = (n + 255) / 256;
-  lse_to_nlse2_kernel<<<unsigned(want < 148LL * 8 ? want : 148LL * 8), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+  lse_to_nlse2_kernel<<<unsigned(want < kNumSMs * 8 ? want : kNumSMs * 8), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       lse, nlse2, n, offset_log2);
   return lwm_check_launch("lse_to_nlse2_kernel");
 }
@@ -266,7 +266,7 @@ extern "C" int lwm_cast_f32_to_bf16(const float* src, void* dst, long long n, vo
   const long long n4 = n / 4;
   const int threads = 256;
   const long long want = (n4 + threads - 1) / threads;
-  const unsigned blocks = unsigned(want < 148LL * 16 ? want : 148LL * 16);
+  const unsigned blocks = unsigned(want < kNumSMs * 16 ? want : kNumSMs * 16);
   cast_f32_bf16_kernel<<<blocks, threads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const float4*>(src), reinterpret_cast<uint2*>(dst), n4);
   return lwm_check_launch("cast_f32_bf16_kernel");
@@ -279,7 +279,7 @@ extern "C" int lwm_add_f32(float* dst, const float* src, long long n, void* stre
   const long long n4 = n / 4;
   const int threads = 256;
   const long long want = (n4 + threads - 1) / threads;
-  const unsigned blocks = unsigned(want < 148LL * 16 ? want : 148LL * 16);
+  const unsigned blocks = unsigned(want < kNumSMs * 16 ? want : kNumSMs * 16);
   add_f32_kernel<<<blocks, threads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<float4*>(dst), reinterpret_cast<const float4*>(src), n4);
   return lwm_check_launch("add_f32_kernel");
@@ -295,7 +295,7 @@ extern "C" int lwm_attn_to_f16(const void* src_bf16, void* dst_f16, float* scale
   if (cudaMemsetAsync(workspace, 0, 4, st) != cudaSuccess) return lwm_fail(LWM_ERR_CUDA, "attn_to_f16: memset failed");
   const long long n8 = n / 8;
   const long long want = (n8 + 255) / 256;
-  const unsigned blocks = unsigned(want < 148LL * 8 ? want : 148LL * 8);
+  const unsigned blocks = unsigned(want < kNumSMs * 8 ? want : kNumSMs * 8);
   absmax_bf16_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<const uint4*>(src_bf16), n8,
                                              reinterpret_cast<unsigned*>(workspace));
   bf16_to_scaled_f16_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<const uint4*>(src_bf16),
@@ -307,7 +307,7 @@ extern "C" int lwm_attn_to_f16(const void* src_bf16, void* dst_f16, float* scale
 
 static unsigned grid_for(long long items, int threads, int waves) {
   const long long want = (items + threads - 1) / threads;
-  return unsigned(want < 148LL * waves ? (want > 0 ? want : 1) : 148LL * waves);
+  return unsigned(want < kNumSMs * waves ? (want > 0 ? want : 1) : kNumSMs * waves);
 }
 
 // atomicMax of the |x| bit patterns into *out_bits (the caller zeroes it); dtype 0 = fp32, 1 = bf16.

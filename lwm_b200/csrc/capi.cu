@@ -1,4 +1,4 @@
-// C-ABI plumbing: error reporting and the "sm_100 or fail" device gate. No compute lives here.
+// C-ABI plumbing: error reporting and the "sm_90 or fail" device gate. No compute lives here.
 #include <string.h>
 #include <stdio.h>
 #include "capi_internal.h"
@@ -24,9 +24,9 @@ bool lwm_check_device() {
     int major = 0;
     cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
     checked_dev = dev;
-    ok = (major == 10);
+    ok = (major == 9);
   }
-  if (!ok) lwm_fail(LWM_ERR_DEVICE, "device is not sm_100 (Blackwell B200): lwm_b200 kernels are sm_100a only");
+  if (!ok) lwm_fail(LWM_ERR_DEVICE, "device is not sm_90 (Hopper H100): lwm_b200 kernels are sm_90a only");
   return ok;
 }
 
@@ -40,11 +40,3 @@ int lwm_check_launch(const char* what) {
 
 extern "C" const char* lwm_last_error(void) { return g_last_error; }
 extern "C" int lwm_abi_version(void) { return LWM_B200_ABI_VERSION; }
-
-static unsigned long long* g_prof = nullptr;
-unsigned long long* lwm_prof_buffer() { return g_prof; }
-// debug: device buffer of >= 64 uint64 that the attention kernels fill with barrier-wait cycle counts
-extern "C" int lwm_debug_set_prof(void* device_buffer) {
-  g_prof = reinterpret_cast<unsigned long long*>(device_buffer);
-  return LWM_OK;
-}

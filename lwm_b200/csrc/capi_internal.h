@@ -4,14 +4,15 @@
 
 enum {
   LWM_OK = 0,
-  LWM_ERR_DEVICE = 1,  // not an sm_100 device / no CUDA device: there is no fallback path
+  LWM_ERR_DEVICE = 1,  // not an sm_90 device / no CUDA device: there is no fallback path
   LWM_ERR_SHAPE = 2,
   LWM_ERR_ARG = 3,
   LWM_ERR_CUDA = 4,
 };
 
 int lwm_fail(int code, const char* msg);          // records msg, returns code
-bool lwm_check_device();                          // true iff current device is compute capability 10.x
+bool lwm_check_device();                          // true iff current device is compute capability 9.x
 int lwm_check_launch(const char* what);           // cudaGetLastError -> status
 
-unsigned long long* lwm_prof_buffer();                // debug wait-time buffer (null unless set)
+// SM count of the H100 SXM: cap of the grid-stride launches (one or a few waves of resident blocks)
+constexpr long long kNumSMs = 132;

@@ -1,11 +1,12 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05
-// (alloc / mma / commit / ld / st / fences) and the UMMA shared-memory + instruction descriptors.
-// Everything in this directory is written for sm_100a only; there is no fallback path.
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor) and the wgmma
+// shared-memory descriptors and ordering instructions (the MMA wrappers themselves are in wgmma.cuh).
+// Everything in this directory is written for sm_90a only; there is no fallback path.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <stdint.h>
+#include "wgmma.cuh"
 
 namespace lwm {
 
@@ -16,22 +17,12 @@ LWM_DEVICE uint32_t smem_u32(const void* p) {
 }
 LWM_DEVICE uint32_t lane_id() { return threadIdx.x & 31; }
 
-LWM_DEVICE bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.b32 %0, 1, 0, P;\n\t}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
-
 // ---------------------------------------------------------------- mbarrier
 LWM_DEVICE void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
 }
 LWM_DEVICE void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-// generic-proxy writes to smem -> visible to the async proxy (TMA store / UMMA operand reads)
+// generic-proxy writes to smem -> visible to the async proxy (TMA store / wgmma operand reads)
 LWM_DEVICE void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 LWM_DEVICE void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
@@ -113,37 +104,21 @@ LWM_DEVICE void tma_wait_group() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05: TMEM allocation
-template <uint32_t kCols>
-LWM_DEVICE void tmem_alloc(uint32_t* smem_result) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-LWM_DEVICE void tmem_dealloc(uint32_t taddr) {  // whole warp (the allocating one)
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-LWM_DEVICE void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-LWM_DEVICE void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// ---------------------------------------------------------------- tcgen05: descriptors
-// Shared-memory matrix descriptor (64 bit). Fields (see PTX ISA "tcgen05 matrix descriptor"):
+// ---------------------------------------------------------------- wgmma: descriptors and ordering
+// Shared-memory matrix descriptor (64 bit). Fields (PTX ISA "Matrix Descriptor Format", sm_90):
 //   [0,14)  start address >> 4        [16,30) leading-dim byte offset >> 4
-//   [32,46) stride-dim byte offset>>4 [46,48) version (1 on sm_100)
-//   [49,52) base offset               [61,64) swizzle: 0 none, 2 = 128B, 4 = 64B, 6 = 32B
-constexpr uint64_t kSwz128 = 2;
+//   [32,46) stride-dim byte offset>>4 [49,52) base offset
+//   [62,64) layout: 0 interleave, 1 = 128B swizzle, 2 = 64B, 3 = 32B
+constexpr uint64_t kSwz128 = 1;
 LWM_DEVICE uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= kSwz128 << 61;
+  d |= kSwz128 << 62;
   return d;
 }
-// K-major operand tile stored as rows of 128 B (64 bf16), 128B-swizzled, 8-row groups 1024 B apart.
+// K-major operand tile stored as rows of 128 B (64 16-bit elements), 128B-swizzled, 8-row groups 1024 B apart.
 LWM_DEVICE uint64_t desc_kmajor_sw128(uint32_t saddr) { return make_smem_desc(saddr, 16, 1024); }
 // MN-major operand: 64 contiguous MN elements per 128 B row, 8 K-rows per 1024 B group (SBO),
 // successive 64-wide MN chunks `mn_chunk_stride` bytes apart (LBO).
@@ -153,96 +128,29 @@ LWM_DEVICE uint64_t desc_mnmajor_sw128(uint32_t saddr, uint32_t mn_chunk_stride)
 
 // Advance a descriptor's start address by `bytes` (multiple of 16). The start-address field holds
 // addr >> 4 in bits [0,14); shared memory is < 256 KB so the add never carries out of the field.
-// One 32-bit add instead of re-encoding the descriptor: the UMMA issuer is a single thread and its
-// instruction count per MMA is what bounds the tensor pipe's issue rate.
 LWM_DEVICE uint64_t desc_advance(uint64_t d, uint32_t bytes) {
   const uint32_t lo = static_cast<uint32_t>(d) + (bytes >> 4);
   return (d & 0xFFFFFFFF00000000ull) | lo;
 }
 
-// Instruction descriptor for kind::f16 with bf16 inputs and fp32 accumulation.
-//   [4,6) D fmt (1=f32)  [7,10) A fmt (1=bf16)  [10,13) B fmt  [15] A MN-major  [16] B MN-major
-//   [17,23) N>>3  [24,29) M>>4
-constexpr uint32_t kFmtF16 = 0, kFmtBF16 = 1;
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N, bool a_mn_major, bool b_mn_major, uint32_t a_fmt,
-                                                  uint32_t b_fmt) {
-  return (1u << 4) | (a_fmt << 7) | (b_fmt << 10) | (static_cast<uint32_t>(a_mn_major) << 15) |
-         (static_cast<uint32_t>(b_mn_major) << 16) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
+// Order this warpgroup's register writes before the wgmma instructions that read them (accumulators, A fragments).
+LWM_DEVICE void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+LWM_DEVICE void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+LWM_DEVICE void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, bool a_mn_major, bool b_mn_major) {
-  return make_idesc(M, N, a_mn_major, b_mn_major, kFmtBF16, kFmtBF16);
+// Keeps the compiler from moving accesses of accumulator registers across wgmma issue / wait points.
+template <int N>
+LWM_DEVICE void reg_fence(float (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
 }
-
-// ---------------------------------------------------------------- tcgen05: MMA + commit (one thread)
-LWM_DEVICE void umma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+template <int N>
+LWM_DEVICE void reg_fence(uint32_t (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+r"(r[i])::"memory");
 }
-// A operand read from TMEM (lane = M row, two bf16 per 32-bit column)
-LWM_DEVICE void umma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05 ops of this thread have completed.
-LWM_DEVICE void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// ---------------------------------------------------------------- tcgen05: TMEM <-> registers
-// 32x32b: thread t of the warp touches TMEM lane (32*(warp%4) + t); x16 / x32 = consecutive columns.
-LWM_DEVICE void tmem_ld_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]),
-        "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]),
-        "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-LWM_DEVICE void tmem_ld_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-LWM_DEVICE void tmem_st_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-      "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]),
-      "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]),
-      "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-LWM_DEVICE void tmem_st_x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-      "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-LWM_DEVICE void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-LWM_DEVICE void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // ---------------------------------------------------------------- misc
 LWM_DEVICE uint32_t pack_bf16x2(float lo, float hi) {
@@ -259,19 +167,6 @@ LWM_DEVICE float ex2f(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
-}
-// 2^x on the FMA/ALU pipes (no MUFU): round-to-nearest split x = n + f, f in [-0.5, 0.5], degree-3 polynomial
-// for 2^f (max relative error 1.03e-4, below the bf16/fp16 rounding of P), exponent patched in by integer add.
-// The forward softmax is bound by the 16-lane/clk XU pipe (ncu: XU 51 % busy while the tensor pipe is 51 %);
-// routing a quarter of the exponentials here balances XU against the issue slots.
-LWM_DEVICE float ex2_poly3(float x) {
-  x = fmaxf(x, -126.0f);
-  const float xr = x + 12582912.0f;
-  const float f = x - (xr - 12582912.0f);
-  float p = fmaf(f, 0.05592203565f, 0.24264008283f);
-  p = fmaf(f, p, 0.69312103399f);
-  p = fmaf(f, p, 0.99992448146f);
-  return __int_as_float(__float_as_int(p) + ((__float_as_int(xr) - 0x4B400000) << 23));
 }
 template <int kRegs>
 LWM_DEVICE void setmaxnreg_inc() {

@@ -1,6 +1,6 @@
 // VQGAN convolutions (flax nn.Conv of lwm/vqgan.py: ResnetBlock 3x3, 1x1 shortcuts, Downsample
 // stride-2, Upsample conv, conv_out, quant/post_quant 1x1) as a persistent implicit GEMM on the
-// 5th-gen tensor cores.
+// Hopper tensor cores (wgmma).
 //
 //   GEMM view  M = N*Ho*Wo output pixels, N = Cout, K = taps * Cin.
 //   A operand  the activation plane [N,Hin,Win,Cpad] (bf16, written by lwm_vq_prep) is never
@@ -12,25 +12,24 @@
 //   B operand  weights pre-packed [tap][Cout_pad][Cpad] bf16 (K-major), 3-D TMA box (64, BN, 1).
 //   precision  n_pass = 1: bf16 x bf16 (fast). n_pass = 3: both operands split x = hi + lo (two bf16)
 //              and D += A_hi B_hi + A_lo B_hi + A_hi B_lo — fp32-class accuracy (2^-16 products,
-//              fp32 accumulation in TMEM), which is what the reference's fp32 convs need.
+//              fp32 accumulation), which is what the reference's fp32 convs need.
 //              n_pass = 2 ("fp16x2"): the activation is ONE fp16 plane and the weights are split w = hi + lo (two fp16,
 //              pre-scaled by a power of two); both halves are stacked along N ([BN hi rows | BN lo rows]) so a single
-//              128 x 2BN x 16 UMMA produces A.hi and A.lo side by side in TMEM and the epilogue adds the two halves:
-//              2x the algorithmic MMA work instead of 3x, wide-N instructions (the measured SS issue rate is 171
-//              cycles at N=256 vs 2 x 107 at N=128), one operand plane to write and read instead of two, and
-//              8.9e-4 end-to-end relative error on the encoder (activation rounding to 11 bits is all that is left).
+//              64 x 2BN x 16 wgmma per warpgroup produces A.hi and A.lo side by side and the epilogue adds the two
+//              halves: 2x the algorithmic MMA work instead of 3x and one operand plane to write and read instead of two.
 //   GN stats   optional epilogue: per-(sample, group) sum / sum of squares of the conv OUTPUT (bias and residual
 //              included) — the statistics the next GroupNorm needs — so no separate pass re-reads the activation.
-//   pipeline   warp 4: TMA producer; warp 5: UMMA issuer; warps 0-3: epilogue (TMEM -> registers
-//              -> + bias (+ residual) -> fp32 NHWC). Accumulators are double-buffered in TMEM so the
-//              epilogue of tile i overlaps the main loop of tile i+1. Grid = #SMs, tiles strided.
+//   pipeline   warp 8: TMA producer through a ring of `stages` slots; warpgroups 0 / 1: pixels [0,64) / [64,128)
+//              of the 8x16 tile, fp32 accumulators in registers, epilogue (+ bias (+ residual) -> fp32 NHWC)
+//              straight from the accumulator fragment. Grid = #SMs, tiles strided.
 #include "ptx.cuh"
 #include "tmap.h"
 #include "capi_internal.h"
 
 namespace lwm {
 
-constexpr int kConvThreads = 192;
+constexpr int kConvThreads = 384;
+constexpr int kConvConsumerWarps = 8;
 constexpr int kATile = 128 * 128;  // 16 KB: 128 pixels x 64 bf16
 
 struct ConvParams {
@@ -49,20 +48,19 @@ struct ConvParams {
   float* out;                     // [N,Ho,Wo,Cout]
 };
 
+// NI: the wgmma N (BN, or 2*BN for the stacked fp16x2 weights); kF16: fp16 operands (n_pass 2), else bf16.
+template <int NI, bool kF16>
 __global__ void __launch_bounds__(kConvThreads, 1)
-conv_umma_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant__ CUtensorMap tmAlo,
-                 const __grid_constant__ CUtensorMap tmBhi, const __grid_constant__ CUtensorMap tmBlo,
-                 const ConvParams p) {
+conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant__ CUtensorMap tmAlo,
+                  const __grid_constant__ CUtensorMap tmBhi, const __grid_constant__ CUtensorMap tmBlo,
+                  const ConvParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   if (smem_u32(smem) & 1023u) __trap();
   const int b_bytes = (p.n_pass == 2 ? 2 : 1) * p.BN * 128;
   const int stage_bytes = (p.n_pass == 3 ? 2 : 1) * (kATile + b_bytes);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.stages * stage_bytes);
   uint64_t* empty = full + 8;
-  uint64_t* tmem_full = empty + 8;   // [2]
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_base_s = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  float* s_stats = reinterpret_cast<float*>(tmem_base_s + 2);   // [64][2] per-group partials of the current tile
+  float* s_stats = reinterpret_cast<float*>(empty + 8);   // [64][2] per-group partials of the current tile
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_w = p.Wo / 16, tiles_h = p.Ho / 8;
@@ -71,30 +69,15 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constan
   const int k_chunks = p.Cpad / 64;
   const int k_iters = p.taps * k_chunks;
 
-  if (warp == 5) {
-    tmem_alloc<512>(tmem_base_s);
-  } else if (warp == 4 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int i = 0; i < p.stages; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 128);
+      mbar_init(&empty[i], kConvConsumerWarps);
     }
     fence_mbar_init();
     for (int i = 0; i < 128; ++i) s_stats[i] = 0.f;
-    tma_prefetch_desc(&tmAhi);
-    tma_prefetch_desc(&tmBhi);
-    if (p.n_pass == 3) {
-      tma_prefetch_desc(&tmAlo);
-      tma_prefetch_desc(&tmBlo);
-    }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_base_s;
 
   // every CTA owns a CONTIGUOUS range of tiles, ordered N-tile-major then image-major: consecutive tiles share the
   // activation halo in L2, and (image, N tile) — the key of the GroupNorm-statistics accumulators — changes at most a
@@ -110,9 +93,16 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constan
     n = m / tiles_h;
   };
 
-  if (warp == 4) {
+  if (warp >= 8) {
     // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
+    setmaxnreg_dec<40>();
+    if (warp == 8 && lane == 0) {
+      tma_prefetch_desc(&tmAhi);
+      tma_prefetch_desc(&tmBhi);
+      if (p.n_pass == 3) {
+        tma_prefetch_desc(&tmAlo);
+        tma_prefetch_desc(&tmBlo);
+      }
       int it = 0;
       for (int tile = tile_begin; tile < tile_end; ++tile) {
         int n, oh0, ow0, nt;
@@ -135,153 +125,153 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constan
         }
       }
     }
-  } else if (warp == 5) {
-    // ------------------------------------------------------------------ UMMA issuer
-    // whole warp, uniform control flow; descriptors advanced by one add per k-step; elected lane issues
-    {
-      const bool leader = elect_one();
-      const uint32_t idesc = p.n_pass == 2 ? make_idesc(128, 2 * p.BN, false, false, kFmtF16, kFmtF16)
-                                           : make_idesc_bf16(128, p.BN, false, false);
-      int it = 0, local = 0;
-      for (int tile = tile_begin; tile < tile_end; ++tile, ++local) {
-        const int acc = local & 1;
-        mbar_wait(&tmem_empty[acc], ((local >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t d = tmem + acc * 256;
-        for (int ki = 0; ki < k_iters; ++ki, ++it) {
-          const int s = it % p.stages;
-          mbar_wait(&full[s], (it / p.stages) & 1);
-          tc_fence_after();
-          const uint32_t a_hi = smem_u32(smem + s * stage_bytes);
-          const uint64_t dAh = desc_kmajor_sw128(a_hi), dBh = desc_kmajor_sw128(a_hi + kATile);
-          const uint64_t dAl = desc_kmajor_sw128(a_hi + kATile + b_bytes), dBl = desc_kmajor_sw128(a_hi + 2 * kATile + b_bytes);
-          if (leader) {
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumer warpgroups
+  setmaxnreg_inc<232>();
+  const int wg = warp >> 2, w = warp & 3, quad = lane & 3;
+  const int ncols = kF16 ? NI / 2 : NI;   // output channels per tile (hi | lo halves are summed for fp16x2)
+  // GroupNorm statistics of the output: per-thread running sums for every 8-channel group of the current N tile, kept
+  // in registers across tiles and folded (warp shuffle -> shared -> double atomics) only when the (image, N tile) pair
+  // changes — a handful of times per CTA thanks to the contiguous tile ranges.
+  constexpr int kStatG = kF16 ? NI / 16 : 1;
+  float st1[kStatG], st2[kStatG];
 #pragma unroll
-            for (int ks = 0; ks < 4; ++ks) {
-              const uint32_t o = ks * 32;
-              umma_ss(d, desc_advance(dAh, o), desc_advance(dBh, o), idesc, (ki | ks) != 0);
-              if (p.n_pass == 3) {
-                umma_ss(d, desc_advance(dAl, o), desc_advance(dBh, o), idesc, 1);
-                umma_ss(d, desc_advance(dAh, o), desc_advance(dBl, o), idesc, 1);
-              }
-            }
-            umma_commit(&empty[s]);
-          }
-        }
-        if (leader) umma_commit(&tmem_full[acc]);
+  for (int i = 0; i < kStatG; ++i) st1[i] = st2[i] = 0.f;
+  int st_n = -1, st_nt = -1;
+  const int cpg = p.stats ? p.Cout / p.groups : 1;
+  auto flush_stats = [&]() {
+    if (st_n < 0) return;
+#pragma unroll
+    for (int g = 0; g < kStatG; ++g) {
+      float s1 = st1[g], s2 = st2[g];
+#pragma unroll
+      for (int sh = 4; sh < 32; sh <<= 1) {
+        s1 += __shfl_xor_sync(0xffffffffu, s1, sh);
+        s2 += __shfl_xor_sync(0xffffffffu, s2, sh);
       }
+      const int c = st_nt * p.BN + g * 8 + lane * 2;   // lanes 0..3: a channel pair, never straddling a group
+      if (lane < 4 && g * 8 < ncols && c < p.Cout) {
+        atomicAdd(&s_stats[2 * (c / cpg)], s1);
+        atomicAdd(&s_stats[2 * (c / cpg) + 1], s2);
+      }
+      st1[g] = st2[g] = 0.f;
     }
-  } else {
-    // ------------------------------------------------------------------ epilogue warps (0..3)
-    const int r = threadIdx.x;  // TMEM lane = pixel inside the 8x16 tile
-    const uint32_t lane_off = uint32_t(warp * 32) << 16;
-    int local = 0;
-    // GroupNorm statistics of the output: per-thread (= per-pixel-slot) running sums for every channel quad of the
-    // current N tile, kept in registers across tiles and folded (warp shuffle -> shared -> double atomics) only when
-    // the (image, N tile) pair changes — a handful of times per CTA thanks to the contiguous tile ranges.
-    float st1[32], st2[32];
+    named_bar_sync(1, 256);
+    if (threadIdx.x < 2 * p.groups) {
+      const float t = s_stats[threadIdx.x];
+      if (t != 0.f) atomicAdd(&p.stats[(size_t)st_n * p.groups * 2 + threadIdx.x], (double)t);
+      s_stats[threadIdx.x] = 0.f;
+    }
+    named_bar_sync(1, 256);
+  };
+
+  int it = 0;
+  for (int tile = tile_begin; tile < tile_end; ++tile) {
+    int n, oh0, ow0, nt;
+    decode_tile(tile, n, oh0, ow0, nt);
+    if (p.stats && (n != st_n || nt != st_nt)) {
+      flush_stats();
+      st_n = n;
+      st_nt = nt;
+    }
+    float acc[NI / 2];
+    int prev_s = -1;
+    for (int ki = 0; ki < k_iters; ++ki, ++it) {
+      const int s = it % p.stages;
+      mbar_wait(&full[s], (it / p.stages) & 1);
+      const uint32_t a_hi = smem_u32(smem + s * stage_bytes);
+      const uint64_t dAh = desc_kmajor_sw128(a_hi + wg * 64 * 128), dBh = desc_kmajor_sw128(a_hi + kATile);
+      const uint64_t dAl = desc_kmajor_sw128(a_hi + kATile + b_bytes + wg * 64 * 128);
+      const uint64_t dBl = desc_kmajor_sw128(a_hi + 2 * kATile + b_bytes);
+      wgmma_fence();
 #pragma unroll
-    for (int i = 0; i < 32; ++i) st1[i] = st2[i] = 0.f;
-    int st_n = -1, st_nt = -1;
-    const int cpg = p.stats ? p.Cout / p.groups : 1;
-    auto flush_stats = [&]() {
-      if (st_n < 0) return;
-#pragma unroll
-      for (int qd = 0; qd < 32; ++qd) {
-        if (qd * 4 >= p.BN) break;
-        float s1 = st1[qd], s2 = st2[qd];
-#pragma unroll
-        for (int sh = 16; sh > 0; sh >>= 1) {
-          s1 += __shfl_xor_sync(0xffffffffu, s1, sh);
-          s2 += __shfl_xor_sync(0xffffffffu, s2, sh);
+      for (int ks = 0; ks < 4; ++ks) {
+        const uint32_t o = ks * 32;
+        wgmma_ss<NI, kF16, 0, 0>(acc, desc_advance(dAh, o), desc_advance(dBh, o), (ki | ks) != 0);
+        if (!kF16 && p.n_pass == 3) {
+          wgmma_ss<NI, kF16, 0, 0>(acc, desc_advance(dAl, o), desc_advance(dBh, o), 1);
+          wgmma_ss<NI, kF16, 0, 0>(acc, desc_advance(dAh, o), desc_advance(dBl, o), 1);
         }
-        const int c = st_nt * p.BN + qd * 4;
-        if (lane == 0 && c < p.Cout) {
-          atomicAdd(&s_stats[2 * (c / cpg)], s1);
-          atomicAdd(&s_stats[2 * (c / cpg) + 1], s2);
-        }
-        st1[qd] = st2[qd] = 0.f;
       }
-      named_bar_sync(2, 128);
-      if (r < 2 * p.groups) {
-        const float t = s_stats[r];
-        if (t != 0.f) atomicAdd(&p.stats[(size_t)st_n * p.groups * 2 + r], (double)t);
-        s_stats[r] = 0.f;
-      }
-      named_bar_sync(2, 128);
-    };
-    for (int tile = tile_begin; tile < tile_end; ++tile, ++local) {
-      int n, oh0, ow0, nt;
-      decode_tile(tile, n, oh0, ow0, nt);
-      if (p.stats && (n != st_n || nt != st_nt)) {
-        flush_stats();
-        st_n = n;
-        st_nt = nt;
-      }
-      const int acc = local & 1;
-      mbar_wait(&tmem_full[acc], (local >> 1) & 1);
-      tc_fence_after();
-      const size_t pix = ((size_t)n * p.Ho + oh0 + (r >> 4)) * p.Wo + ow0 + (r & 15);
+      wgmma_commit();
+      wgmma_wait<1>();   // the previous k-step's wgmmas are done: its slot may be refilled
+      if (prev_s >= 0 && lane == 0) mbar_arrive(&empty[prev_s]);
+      prev_s = s;
+    }
+    wgmma_wait<0>();
+    reg_fence(acc);
+    if (lane == 0) mbar_arrive(&empty[prev_s]);
+
+    // ---- epilogue: this thread's pixels are rows r and r + 8 of its warp's 16 (one image row of the 8x16 tile)
+    const int c_base = nt * p.BN;
+    const bool vec = (p.Cout & 1) == 0;
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const size_t pix = ((size_t)n * p.Ho + oh0 + wg * 4 + w) * p.Wo + ow0 + (lane >> 2) + 8 * hh;
       float* dst = p.out + pix * p.Cout;
       const float* res = p.residual ? p.residual + pix * p.Cout : nullptr;
-      const int c_base = nt * p.BN;
 #pragma unroll
-      for (int ci = 0; ci < 16; ++ci) {
-        const int c0 = ci * 16;
-        if (c0 >= p.BN) break;
-        uint32_t v[16];
-        tmem_ld_x16(tmem + lane_off + acc * 256 + c0, v);
-        if (p.n_pass == 2) {
-          uint32_t w[16];
-          tmem_ld_x16(tmem + lane_off + acc * 256 + p.BN + c0, w);
-          tmem_wait_ld();
-#pragma unroll
-          for (int j = 0; j < 16; ++j)
-            v[j] = __float_as_uint((__uint_as_float(v[j]) + __uint_as_float(w[j])) * p.w_scale_inv);
-        } else {
-          tmem_wait_ld();
+      for (int g = 0; g < NI / 8; ++g) {
+        if (g * 8 >= ncols) break;
+        const int c = c_base + g * 8 + quad * 2;
+        float v0 = acc[4 * g + 2 * hh], v1 = acc[4 * g + 2 * hh + 1];
+        if (kF16) {
+          v0 = (v0 + acc[4 * g + 2 * hh + NI / 4]) * p.w_scale_inv;
+          v1 = (v1 + acc[4 * g + 2 * hh + 1 + NI / 4]) * p.w_scale_inv;
         }
-        const int c = c_base + c0;
-        if (c + 16 <= p.Cout && (p.Cout & 3) == 0) {
-#pragma unroll
-          for (int j = 0; j < 16; j += 4) {
-            const float4 b4 = *reinterpret_cast<const float4*>(p.bias + c + j);
-            float4 o = make_float4(__uint_as_float(v[j]) + b4.x, __uint_as_float(v[j + 1]) + b4.y,
-                                   __uint_as_float(v[j + 2]) + b4.z, __uint_as_float(v[j + 3]) + b4.w);
-            if (res) {
-              const float4 r4 = *reinterpret_cast<const float4*>(res + c + j);
-              o.x += r4.x; o.y += r4.y; o.z += r4.z; o.w += r4.w;
-            }
-            if (p.clip) {
-              o.x = fminf(fmaxf(o.x, -1.f), 1.f); o.y = fminf(fmaxf(o.y, -1.f), 1.f);
-              o.z = fminf(fmaxf(o.z, -1.f), 1.f); o.w = fminf(fmaxf(o.w, -1.f), 1.f);
-            }
-            *reinterpret_cast<float4*>(dst + c + j) = o;
-            if (p.stats && ci < 8) {   // stats need BN <= 128 (checked on the host); a quad never straddles a group
-              st1[ci * 4 + j / 4] += (o.x + o.y) + (o.z + o.w);
-              st2[ci * 4 + j / 4] += (o.x * o.x + o.y * o.y) + (o.z * o.z + o.w * o.w);
-            }
+        if (vec && c + 1 < p.Cout) {
+          const float2 b2 = *reinterpret_cast<const float2*>(p.bias + c);
+          float2 o2 = make_float2(v0 + b2.x, v1 + b2.y);
+          if (res) {
+            const float2 r2 = *reinterpret_cast<const float2*>(res + c);
+            o2.x += r2.x;
+            o2.y += r2.y;
+          }
+          if (p.clip) {
+            o2.x = fminf(fmaxf(o2.x, -1.f), 1.f);
+            o2.y = fminf(fmaxf(o2.y, -1.f), 1.f);
+          }
+          *reinterpret_cast<float2*>(dst + c) = o2;
+          if (kF16 && p.stats) {   // stats need Cout % 16 == 0 (checked on the host): always this path
+            st1[g < kStatG ? g : 0] += o2.x + o2.y;
+            st2[g < kStatG ? g : 0] += o2.x * o2.x + o2.y * o2.y;
           }
         } else {
+          const float vv[2] = {v0, v1};
 #pragma unroll
-          for (int j = 0; j < 16; ++j)
-            if (c + j < p.Cout) {
-              float o = __uint_as_float(v[j]) + p.bias[c + j];
-              if (res) o += res[c + j];
+          for (int e = 0; e < 2; ++e)
+            if (c + e < p.Cout) {
+              float o = vv[e] + p.bias[c + e];
+              if (res) o += res[c + e];
               if (p.clip) o = fminf(fmaxf(o, -1.f), 1.f);
-              dst[c + j] = o;
+              dst[c + e] = o;
             }
         }
       }
-      tc_fence_before();
-      mbar_arrive(&tmem_empty[acc]);
     }
-    if (p.stats) flush_stats();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) tmem_dealloc<512>(tmem);
+  if (p.stats) flush_stats();
 }
+
+typedef void (*ConvKernel)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const ConvParams);
+
+// the instantiated wgmma widths: bf16 (n_pass 1 / 3) BN in {16, 32, 64, 128, 256}; fp16x2 2*BN in {32, 64, ..., 256}
+static ConvKernel conv_kernel_for(int NI, bool f16, int* variant) {
+#define LWM_CONV_CASE(n, f, idx) \
+  if (NI == n && f16 == f) {     \
+    *variant = idx;              \
+    return conv_wgmma_kernel<n, f>; \
+  }
+  LWM_CONV_CASE(16, false, 0) LWM_CONV_CASE(32, false, 1) LWM_CONV_CASE(64, false, 2) LWM_CONV_CASE(128, false, 3)
+  LWM_CONV_CASE(256, false, 4)
+  LWM_CONV_CASE(32, true, 5) LWM_CONV_CASE(64, true, 6) LWM_CONV_CASE(96, true, 7) LWM_CONV_CASE(128, true, 8)
+  LWM_CONV_CASE(160, true, 9) LWM_CONV_CASE(192, true, 10) LWM_CONV_CASE(224, true, 11) LWM_CONV_CASE(256, true, 12)
+#undef LWM_CONV_CASE
+  return nullptr;
+}
+constexpr int kConvVariants = 13;
 
 }  // namespace lwm
 
@@ -303,15 +293,18 @@ static int conv_launch(const void* a_hi, const void* a_lo, const void* w_hi, con
     return lwm_fail(LWM_ERR_ARG, "vq_conv2d: output statistics are an epilogue of the fp16x2 scheme (N tile <= 128)");
   if (!lwm_check_device()) return LWM_ERR_DEVICE;
   int BN = Cout_pad;
-  if (n_pass == 2) {      // fp16x2 stacks hi|lo: the UMMA is 2*BN wide -> BN = largest multiple of 16 <= 128 dividing Cout_pad
+  if (n_pass == 2) {      // fp16x2 stacks hi|lo: the wgmma is 2*BN wide -> BN = largest multiple of 16 <= 128 dividing Cout_pad
     for (BN = 128; BN >= 16; BN -= 16)
       if (Cout_pad % BN == 0) break;
-  } else if (BN > 256) {
-    if (Cout_pad % 256 == 0) BN = 256;
-    else if (Cout_pad % 192 == 0) BN = 192;
-    else if (Cout_pad % 128 == 0) BN = 128;
-    else return lwm_fail(LWM_ERR_SHAPE, "vq_conv2d: Cout_pad > 256 must be a multiple of 128");
+  } else {
+    if (Cout_pad > 256 && Cout_pad % 128)
+      return lwm_fail(LWM_ERR_SHAPE, "vq_conv2d: Cout_pad > 256 must be a multiple of 128");
+    for (BN = 256; BN > 16; BN >>= 1)      // the widest instantiated wgmma N that divides Cout_pad
+      if (Cout_pad % BN == 0) break;
   }
+  int variant = 0;
+  const ConvKernel kern = conv_kernel_for(n_pass == 2 ? 2 * BN : BN, n_pass == 2, &variant);
+  if (!kern) return lwm_fail(LWM_ERR_SHAPE, "vq_conv2d: no kernel for this N tile");
   const int taps = ksize * ksize;
   const CUtensorMapDataType dt = n_pass == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   const int wrows = (n_pass == 2 ? 2 : 1);
@@ -350,19 +343,19 @@ static int conv_launch(const void* a_hi, const void* a_lo, const void* w_hi, con
   if (stages < 2) return lwm_fail(LWM_ERR_SHAPE, "vq_conv2d: tile does not fit in shared memory");
   p.stages = stages;
   const int smem_bytes = stages * stage_bytes + 1024;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 0;
   cudaGetDevice(&dev);
-  static bool attr_set_dev[64] = {};      // function attributes are per device
-  if (!attr_set_dev[dev & 63]) {
-    if (cudaFuncSetAttribute(conv_umma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
+  static bool attr_set_dev[64][kConvVariants] = {};      // function attributes are per device
+  if (!attr_set_dev[dev & 63][variant]) {
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
       return lwm_fail(LWM_ERR_CUDA, "vq_conv2d: cannot raise dynamic shared memory limit");
-    attr_set_dev[dev & 63] = true;
+    attr_set_dev[dev & 63][variant] = true;
   }
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int total_tiles = N * (Ho / 8) * (Wo / 16) * p.n_tiles;
   const int grid = total_tiles < sms ? total_tiles : sms;
-  conv_umma_kernel<<<grid, kConvThreads, smem_bytes, reinterpret_cast<cudaStream_t>(stream)>>>(tAh, tAl, tBh, tBl, p);
-  return lwm_check_launch("conv_umma_kernel");
+  kern<<<grid, kConvThreads, smem_bytes, reinterpret_cast<cudaStream_t>(stream)>>>(tAh, tAl, tBh, tBl, p);
+  return lwm_check_launch("conv_wgmma_kernel");
 }
 
 // a_hi/a_lo: [N,Hin,Win,Cpad] bf16 planes; w_hi/w_lo: [taps][Cout_pad][Cpad] bf16; out/residual fp32 NHWC.

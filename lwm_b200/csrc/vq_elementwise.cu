@@ -334,7 +334,7 @@ extern "C" int lwm_vq_prep(const float* x, const double* gn_stats, const float* 
   const size_t total = (size_t)N * (H << upsample2x) * (W << upsample2x) * (C_pad / 8);
   const int threads = 256;
   const size_t want = (total + threads - 1) / threads;
-  const unsigned blocks = unsigned(want < 148u * 32 ? want : 148u * 32);
+  const unsigned blocks = unsigned(want < kNumSMs * 32 ? want : kNumSMs * 32);
   prep_kernel<false><<<blocks, threads, gn_stats ? size_t(N) * groups * 8 : 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       x, gn_stats, gamma, beta, reinterpret_cast<__nv_bfloat16*>(hi), reinterpret_cast<__nv_bfloat16*>(lo), N, H, W,
       C, C_pad, groups, upsample2x ? 1 : 0, eps, lo != nullptr);
@@ -354,7 +354,7 @@ extern "C" int lwm_vq_prep_f16(const float* x, const double* gn_stats, const flo
   const size_t total = (size_t)N * (H << upsample2x) * (W << upsample2x) * (C_pad / 8);
   const int threads = 256;
   const size_t want = (total + threads - 1) / threads;
-  const unsigned blocks = unsigned(want < 148u * 32 ? want : 148u * 32);
+  const unsigned blocks = unsigned(want < kNumSMs * 32 ? want : kNumSMs * 32);
   prep_kernel<true><<<blocks, threads, gn_stats ? size_t(N) * groups * 8 : 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       x, gn_stats, gamma, beta, reinterpret_cast<__nv_bfloat16*>(out), nullptr, N, H, W, C, C_pad, groups,
       upsample2x ? 1 : 0, eps, 0);
@@ -395,7 +395,7 @@ extern "C" int lwm_vq_gather(const int* idx, const float* codebook, float* out, 
   if (N == 0) return LWM_OK;
   const int quads = e_dim / 4;
   const long long total = N * quads;
-  const unsigned blocks = unsigned((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+  const unsigned blocks = unsigned((total + 255) / 256 < kNumSMs * 16 ? (total + 255) / 256 : kNumSMs * 16);
   vq_gather_kernel<<<blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       idx, reinterpret_cast<const float4*>(codebook), reinterpret_cast<float4*>(out), N, quads, n_e);
   return lwm_check_launch("vq_gather_kernel");

@@ -35,7 +35,7 @@ __global__ void unframe_tokens_kernel(const int* __restrict__ tokens, int* __res
 
 static unsigned grid_for(long long total) {
   const long long want = (total + 255) / 256;
-  return unsigned(want < 148LL * 16 ? want : 148LL * 16);
+  return unsigned(want < kNumSMs * 16 ? want : kNumSMs * 16);
 }
 
 }  // namespace lwm

@@ -3,7 +3,7 @@ stream while the tile kernels of step idx run, and sequences the per-(q chunk, k
 kernel launches with their first/last carry flags.
 
 The step functions are injected (`ops`), so the very same sequencing code is exercised on CPU
-with the gloo backend and an oracle-backed `ops` in tests/test_ring_gloo.py, and on B200s with
+with the gloo backend and an oracle-backed `ops` in tests/test_ring_gloo.py, and on H100s with
 the CUDA C-ABI calls of lwm_b200.ringattention.
 """
 import os

@@ -105,8 +105,7 @@ def step_kv(world, rank, idx, Sk, layout, sub=(0, 1)):
 def auto_sub(world, Sk, layout, min_piece=2048):
     """How many pieces to cut the first / last step's blocks into so that their transfer pipelines with the
     tile kernels instead of being exposed (nothing precedes step 0; nothing follows the last dK/dV return)."""
-    # measured (profiles/ring_timeline_n2_substeps_r01.log): at N=2 the extra, smaller launches cost more than the
-    # ~3 ms of exposed transfer they hide, so sub-stepping is opt-in (LWM_RING_SUBSTEPS=1)
+    # sub-stepping trades extra, smaller launches for less exposed transfer; it is opt-in (LWM_RING_SUBSTEPS=1)
     if world == 1 or os.environ.get("LWM_RING_SUBSTEPS", "0") != "1":
         return 1
     block = Sk if layout == "contiguous" else Sk // 2

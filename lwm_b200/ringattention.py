@@ -1,4 +1,4 @@
-"""Host side of the B200 RingAttention operator — same call signature as the reference's
+"""Host side of the H100 RingAttention operator — same call signature as the reference's
 `ringattention(q, k, v, attn_bias, segment_ids, *, axis_name, float32_logits, cache_idx,
 blockwise_kwargs)` bound with functools.partial at lwm/llama.py:540-557 and called at
 lwm/llama.py:569 on per-device shards inside shard_map.
@@ -13,7 +13,7 @@ Translation of the execution model (SURVEY.md §8b):
     epilogue (include/lwm_b200.h: lwm_attn_fwd_step).
 
 Everything numeric happens in liblwm_b200.so; this file only sequences launches and NCCL calls.
-There is no fallback: without the library / an sm_100 GPU the op raises.
+There is no fallback: without the library / an sm_90 GPU the op raises.
 """
 import math
 import os
@@ -161,7 +161,7 @@ def ringattention(q, k, v, attn_bias=None, segment_ids=None, *, axis_name="sp", 
     if cache_idx is not None:
         raise NotImplementedError("cache_idx is always None at the reference call site (lwm/llama.py:544)")
     if not q.is_cuda:
-        raise _lib.LwmError("ringattention: tensors must live on an sm_100 GPU (no CPU fallback)")
+        raise _lib.LwmError("ringattention: tensors must live on an sm_90 GPU (no CPU fallback)")
     in_dtype = q.dtype
     if not (k.dtype == in_dtype and v.dtype == in_dtype and in_dtype in (torch.bfloat16, torch.float32)):
         raise TypeError("ringattention: q, k, v must all be bfloat16 or all float32 (fp32 logits and accumulation "
@@ -575,7 +575,7 @@ def ringattention_inference(q, k, v, attn_mask, axis_name="sp"):
     reduces its own shard (K/V are read once, from local HBM) and the P partial (o, lse) pairs — a few KB — are
     all-gathered and merged."""
     if not q.is_cuda:
-        raise _lib.LwmError("ringattention_inference: tensors must live on an sm_100 GPU (no CPU fallback)")
+        raise _lib.LwmError("ringattention_inference: tensors must live on an sm_90 GPU (no CPU fallback)")
     if q.dtype != torch.bfloat16 or k.dtype != torch.bfloat16 or v.dtype != torch.bfloat16:
         raise TypeError("ringattention_inference: q, k, v must be bfloat16")
     group, rank, world = _resolve_group(axis_name)

@@ -4,7 +4,7 @@
 The reference precomputes a complex64 table [max_position, 64] on the host and gathers it by position_ids; the kernel
 rebuilds the same float32 angles on the fly, so only the 64 inverse frequencies are kept on the device.
 Differentiable: the VJP of a rotation is the rotation by the conjugate, done by the same kernel (conj=1).
-No CPU path: tensors must live on a B200."""
+No CPU path: tensors must live on an H100."""
 import numpy as np
 import torch
 

@@ -11,7 +11,7 @@ def _rel(x, ref):
 
 
 def sampled_parity(S_total, H, check_heads, op, device, rank=0, world=1, base_seed=1234, shards=None):
-    """Parity of the attention op at BASELINE sizes (32K .. 128K tokens), where the dense oracle does not fit: this
+    """Parity of the attention op at 32K .. 128K tokens, where the dense oracle does not fit: this
     rank's shards of the seeded synthetic q/k/v (lwm_b200/synthetic.py) go through `op` (forward + backward) with a dO
     that is zero outside one sampled query row per 128-row tile (+ the last 128 rows of the sequence); the float64
     row-wise oracle (oracle/attn_rows.py) then gives, for each head in `check_heads`, the exact out / dq of the sampled
@@ -95,7 +95,7 @@ def smoke(verbose=True):
     res["attn_bf16_out_rel_err"] = _rel(n(ob), ref)
     res["attn_bf16_dq_rel_err"] = _rel(n(qb.grad), rq)
     assert res["attn_bf16_out_rel_err"] < 3e-3 and res["attn_bf16_dq_rel_err"] < 3e-3, res
-    # ---- VQGAN: GroupNorm+SiLU prep -> tcgen05 conv, and the nearest-code search (bit-exact)
+    # ---- VQGAN: GroupNorm+SiLU prep -> wgmma conv, and the nearest-code search (bit-exact)
     ops = Ops("bf16x3")
     x = torch.randn(1, 16, 16, 128, generator=g)
     gn = vr._gn_p(g, 128)

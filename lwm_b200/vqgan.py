@@ -1,4 +1,4 @@
-"""Host side of the B200 VQGAN tokenizer — mirrors the reference's public surface
+"""Host side of the H100 VQGAN tokenizer — mirrors the reference's public surface
 (lwm/vqgan.py): `VQGAN(vqgan_checkpoint, replicate=False).encode(pixel_values)` ->
 (quantized_states, codebook_indices), `.decode(encoding)` -> pixels in [-1, 1], `VQGANConfig`
 defaults (vqgan.py:62-77), and the sub-modules north_star names (`ResnetBlock`, `Downsample`,
@@ -12,8 +12,8 @@ weights are re-packed once into the conv kernel's layout ([tap][Cout_pad][Cin_pa
 All arithmetic happens in liblwm_b200.so (include/lwm_b200.h: lwm_vq_*). torch only owns memory.
 precision (the reference computes these convs in fp32):
   'fp16x2' (default)  activation = one fp16 plane, weights split hi + lo (two fp16) stacked along Cout so that one wide
-                      UMMA does both halves; GroupNorm statistics come out of the producing conv's epilogue. 8.9e-4
-                      end-to-end relative error on the encoder latents (<= 1e-3), 2x the algorithmic tensor work.
+                      wgmma does both halves; GroupNorm statistics come out of the producing conv's epilogue. Within
+                      1e-3 end-to-end relative error on the encoder latents, 2x the algorithmic tensor work.
   'bf16x3'            both operands split into two bf16, three MMAs: fp32-class accuracy (1e-5), 3x the tensor work.
   'bf16'              single pass (≈1e-2 end-to-end relative error, 99.6 % code agreement on synthetic weights).
 """
@@ -362,7 +362,7 @@ class VQGANModel:
 
     def _to_dev(self, x):
         if not torch.cuda.is_available():
-            raise _lib.LwmError("VQGAN needs an sm_100 GPU: lwm_b200 has no CPU fallback")
+            raise _lib.LwmError("VQGAN needs an sm_90 GPU: lwm_b200 has no CPU fallback")
         return torch.as_tensor(np.asarray(x) if not torch.is_tensor(x) else x).to(self.device, torch.float32)
 
 

@@ -6,7 +6,7 @@ lwm_b200/ may import this package: the product path is the CUDA library or a lou
 
 PARITY STATUS
   * VQGAN: PINNED (structure) — tests/golden/vqgan_reference_small.npz is produced by executing the UNMODIFIED
-    reference module /root/reference/lwm/vqgan.py over a numpy-backed shim of its jax/flax/tux imports
+    reference module lwm/vqgan.py over a numpy-backed shim of its jax/flax/tux imports
     (oracle/flax_shim, tools/make_golden_vqgan_from_reference.py); oracle/vqgan_ref.py reproduces it (indices
     bit-exact, floats to 1e-6). The semantics of the flax primitives themselves (nn.Conv SAME/HWIO, nn.GroupNorm
     defaults, nearest resize) are this repo's reading of flax 0.8.4 — not executable offline.

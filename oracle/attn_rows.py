@@ -1,5 +1,5 @@
 """Float64 oracle for SAMPLED query rows of a long causal sequence — the row-wise restatement of oracle/attn_dense.py
-(same semantics: lwm/llama.py:525-570 call-site contract, SURVEY.md Appendix A), usable at the BASELINE sizes
+(same semantics: lwm/llama.py:525-570 call-site contract, SURVEY.md Appendix A), usable at 32K .. 128K tokens
 (S = 32768 .. 131072) where the dense S x S oracle does not fit: a query row only needs its own logits row.
 
 With a dO that is zero outside the sampled rows the gradients are exact too and cheap:

@@ -1,5 +1,5 @@
 """Import shim: `from ringattention import ringattention, blockwise_feedforward, ringattention_jax,
-ringattention_inference` (lwm/llama.py:30) resolves to the B200 ops."""
+ringattention_inference` (lwm/llama.py:30) resolves to the H100 ops."""
 from lwm_b200.blockwise_ffn import blockwise_feedforward  # noqa: F401
 from lwm_b200.ringattention import ringattention, ringattention_inference, set_axis_group  # noqa: F401
 

@@ -9,19 +9,19 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90) GPU")
 
 
 def pytest_collection_modifyitems(config, items):
-    """gpu-marked tests are skipped (not failed) on a machine without an sm_100 device"""
+    """gpu-marked tests are skipped (not failed) on a machine without an sm_90 device"""
     try:
         import torch
-        ok = torch.cuda.is_available() and torch.cuda.get_device_capability(0)[0] == 10
+        ok = torch.cuda.is_available() and torch.cuda.get_device_capability(0)[0] == 9
     except Exception:
         ok = False
     if ok:
         return
-    skip = pytest.mark.skip(reason="needs a B200 (sm_100) GPU")
+    skip = pytest.mark.skip(reason="needs an H100 (sm_90) GPU")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

@@ -1,5 +1,5 @@
 """CPU emulation of the peer-memory transport and of the step functions, so that lwm_b200/ring_peer.py — the very
-executor that runs on the B200s — is exercised in the CPU test-suite: P rank THREADS of one process share P uint8
+executor that runs on the GPUs — is exercised in the CPU test-suite: P rank THREADS of one process share P uint8
 "heaps" and a flag table; pulls / puts are tensor copies, remote flag writes take effect immediately, waits block on a
 condition variable. Streams do not exist here (every operation completes before the next one is issued), which is a
 stricter ordering than the GPU's, so a protocol that deadlocks here may still be correct — but one that passes here has

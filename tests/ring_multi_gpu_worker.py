@@ -106,7 +106,7 @@ def main():
 
 
 def sampled(rank, world, dev):
-    """BASELINE-size parity (configs[1]: 32K tokens over 2 GPUs; configs[2]: 128K over 8): sampled query rows and every
+    """Benchmark-size parity (32K tokens over 2 GPUs; 128K over 8): sampled query rows and every
     key row against the float64 row-wise oracle — lwm_b200/selftest.py::sampled_parity."""
     from lwm_b200.ringattention import ringattention
     from lwm_b200.selftest import sampled_parity

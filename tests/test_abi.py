@@ -1,5 +1,5 @@
 """The C-ABI library loads without a GPU and exports every symbol include/lwm_b200.h declares;
-compute entry points refuse to run without an sm_100 device (no CPU fallback)."""
+compute entry points refuse to run without an sm_90 device (no CPU fallback)."""
 import ctypes
 import os
 import re
@@ -35,7 +35,7 @@ def test_compute_calls_fail_loudly_without_gpu(lib):
     from lwm_b200 import _lib
     with pytest.raises(_lib.LwmError):
         _lib.call("lwm_cast_f32_to_bf16", None, None, 4, None)
-    assert b"no CPU fallback" in lib.lwm_last_error() or b"sm_100" in lib.lwm_last_error()
+    assert b"no CPU fallback" in lib.lwm_last_error() or b"sm_90" in lib.lwm_last_error()
     from lwm_b200.ringattention import ringattention
     q = torch.zeros(1, 128, 1, 128, dtype=torch.bfloat16)
     with pytest.raises(_lib.LwmError):

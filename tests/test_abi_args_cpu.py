@@ -1,6 +1,6 @@
 """Argument validation of the C ABI, checked without a GPU: every entry point validates its pure arguments (shapes,
 null pointers, flags) BEFORE it looks for a device, so wrong calls get LWM_ERR_SHAPE (2) / LWM_ERR_ARG (3) with a message,
-and well-formed calls on a machine without an sm_100 GPU get LWM_ERR_DEVICE (1) — never a silent fallback.
+and well-formed calls on a machine without an sm_90 GPU get LWM_ERR_DEVICE (1) — never a silent fallback.
 Pointers are fake non-null addresses: nothing dereferences them before the device check."""
 import ctypes
 
@@ -85,4 +85,4 @@ GOOD_CALLS = [
 def test_well_formed_calls_fail_with_device_error_without_gpu(lib, name, args):
     status, msg = _status(lib, name, *args)
     assert status == DEVICE, (status, msg)
-    assert "no CPU fallback" in msg or "sm_100" in msg, msg
+    assert "no CPU fallback" in msg or "sm_90" in msg, msg

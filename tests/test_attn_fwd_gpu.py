@@ -158,7 +158,7 @@ def test_fwd_fp32_readout_structured_values_1e3():
 
 
 def test_fwd_ring_order_invariance_at_shard_size():
-    """Size-independent property at BASELINE config-2/3's shard size (S_loc = 16384): attending to the
+    """Size-independent property at an 8-way shard of 128K tokens (S_loc = 16384): attending to the
     diagonal block first and the earlier block second (ring order, carry merged in the epilogue) equals one
     launch over the concatenated K/V."""
     from lwm_b200 import ringattention as ra

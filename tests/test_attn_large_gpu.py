@@ -1,4 +1,4 @@
-"""Oracle parity at the BASELINE sequence lengths (BASELINE.json configs[1..2]: 32K and 128K tokens, LWM-7B head
+"""Oracle parity at the benchmark sequence lengths (32K and 128K tokens, LWM-7B head
 geometry) on one GPU: the public op in its default precision mode against the float64 row-wise oracle
 (oracle/attn_rows.py) on one sampled query row of every 128-row tile plus the last 128 rows (out, dq) and on EVERY key
 row (dk, dv) — see lwm_b200/selftest.py::sampled_parity. Tolerance: 1e-3 relative Frobenius (north_star) on the

@@ -32,32 +32,3 @@ def test_gpu_arm_fails_loudly_without_gpu():
                        capture_output=True, text=True, timeout=300)
     assert r.returncode != 0
     assert "no CPU fallback" in (r.stdout + r.stderr)
-
-
-def test_committed_bench_lines_carry_the_contract():
-    """the round's measured lines under profiles/ (written by bench.py on the B200 boxes) have every key the bench
-    contract names — metric / value / e2e with copy bytes / gpu_launches / clocks / roofline at N=1 / parity at every N —
-    and the VQGAN record is a full second record"""
-    prof = os.path.join(ROOT, "profiles")
-    for n in (1, 2, 4, 8):
-        d = json.load(open(os.path.join(prof, "bench_r02_n%d.json" % n)))
-        assert d["metric"] == "ring_attn_fwd_bwd_tokens_per_s_attention_only_7B_128K" and d["n_gpus"] == n
-        assert d["unit"] == "tokens/s" and d["higher_is_better"] is True and d["scaling"] == "strong"
-        assert d["config"]["precision"] == "fp16" and "S=131072" in d["config"]["workload"]
-        assert abs(d["value"] - 131072 / (32 * d["ms_per_step"] * 1e-3)) < 1e-6 * d["value"]
-        assert d["e2e"]["h2d_bytes_per_step"] == 4 * 131072 // n * 4096 * 2 and d["e2e"]["d2h_bytes_per_step"] > 0
-        assert d["e2e"]["ms_per_step"] >= d["ms_per_step"]
-        assert d["gpu_launches"] > 0
-        assert d["clocks"]["sm_mhz"] and not set(d["clocks"]["reasons"]) & {"hw_slowdown", "hw_thermal_slowdown",
-                                                                             "sw_thermal_slowdown"}
-        p = d["parity"]
-        assert p["ok"] is True and p["max_rel"] < 1e-3 and p["rows"] >= 1024 and p["key_rows"] == 131072
-    d1 = json.load(open(os.path.join(prof, "bench_r02_n1.json")))
-    r = d1["roofline"]
-    assert r["bound"] == "tensor" and abs(r["frac"] - r["achieved"] / r["peak"]) < 1e-9 and r["traffic"] > 1e10
-    assert d1["cpu_baseline"]["kind"] == "port" and d1["cpu_baseline"]["cores"] >= 1
-    vq = d1["vqgan"]
-    assert vq["unit"] == "frames/s" and vq["roofline"]["bound"] == "hbm" and vq["roofline"]["traffic"] > 1e10
-    assert abs(vq["roofline"]["frac"] - vq["roofline"]["achieved"] / vq["roofline"]["peak"]) < 1e-9
-    assert vq["e2e"]["h2d_bytes_per_step"] == 16 * 256 * 256 * 3 * 4 and vq["e2e"]["d2h_bytes_per_step"] == 16 * 256 * 4
-    assert vq["parity"]["latent_rel"] < 1e-3 and vq["cpu_baseline"]["kind"] == "port" and vq["decode"]["ms_per_clip"] > 0

@@ -97,7 +97,7 @@ def test_frame_tokens_bit_exact_vs_reference_fixture(tag):
 
 
 def test_frame_tokens_batched_clip_of_vqgan_size():
-    """[B,T,16,16] clips (BASELINE config 4: 16 frames): round trip + delimiter positions, and chaining from VQGAN.encode"""
+    """[B,T,16,16] clips (16 frames, as in the benchmark clip): round trip + delimiter positions, and chaining from VQGAN.encode"""
     from lwm_b200.vision_tokens import EOF_TOKEN, EOV_TOKEN, frame_tokens, unframe_tokens
     from oracle import vision_tokens as V
     g = torch.Generator().manual_seed(9)

@@ -1,6 +1,6 @@
 """Multi-GPU parity of the sequence-parallel attention op (skipped unless >= 2 GPUs are visible), against the float64
 ORACLE: (1) dense oracle at a small size — forward and all gradients, both work assignments, masks, fp32 and bf16
-inputs, decode op; (2) the row-wise oracle at the BASELINE length of the visible GPU count (32K tokens on 2 GPUs =
+inputs, decode op; (2) the row-wise oracle at the benchmark length of the visible GPU count (32K tokens on 2 GPUs =
 configs[1]; 128K on 8 = configs[2])."""
 import os
 import subprocess

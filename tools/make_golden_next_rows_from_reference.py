@@ -1,8 +1,9 @@
 """Generate tests/golden/rope_reference.npz and tests/golden/vision_tokens_reference.npz by EXECUTING REFERENCE CODE
-(unmodified source text, extracted with `ast` from /root/reference at run time — nothing is copied into this repo):
+(unmodified source text, extracted with `ast` from a checkout of LargeWorldModel/LWM at run time — nothing is copied
+into this repo; the checkout's root is $LWM_REFERENCE):
   * lwm/llama.py `precompute_freqs_cis` and `apply_rotary_emb` over the numpy-backed jax shim (oracle/flax_shim);
   * lwm/data.py `VisionTextProcessor` with a stub tokenizer (only `<vision>` / `</vision>` / bos / eos ids matter).
-Runs only in the build container (the reference tree is not on the GPU box); the fixtures are committed."""
+The fixtures are committed, so the tests need no reference checkout."""
 import ast
 import os
 import random
@@ -13,7 +14,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "oracle", "flax_shim"))
-REF = "/root/reference/lwm"
+REF = os.path.join(os.environ.get("LWM_REFERENCE", "reference"), "lwm")
 
 
 def extract(path, names):
@@ -91,7 +92,7 @@ def make_process_frame_fixture(path="tests/golden/process_frame_reference.npz"):
     import numpy as np
     sys.path.insert(0, "tests")
     from test_next_rows2_cpu import _images
-    src = open("/root/reference/lwm/vision_chat.py").read()
+    src = open(os.path.join(REF, "vision_chat.py")).read()
     fn = next(n for n in ast.walk(ast.parse(src)) if isinstance(n, ast.FunctionDef) and n.name == "_process_frame")
     ns = {"np": np}
     exec("def _process_frame" + ast.get_source_segment(src, fn).split("def _process_frame", 1)[1], ns)

@@ -1,6 +1,6 @@
-"""Generate tests/golden/vqgan_reference_small.npz by EXECUTING THE REFERENCE MODULE /root/reference/lwm/vqgan.py
-(unmodified) over the numpy-backed flax/jax shim in oracle/flax_shim (see its README for what this does and does not
-pin). Runs only in the build container (the reference tree is not on the GPU box); the fixture is committed.
+"""Generate tests/golden/vqgan_reference_small.npz by EXECUTING THE REFERENCE MODULE lwm/vqgan.py of a
+LargeWorldModel/LWM checkout (its root is $LWM_REFERENCE; unmodified) over the numpy-backed flax/jax shim in oracle/flax_shim (see its README for what this does and does not
+pin). The fixture is committed, so the tests need no reference checkout.
 
 Config: a down-scaled VQGANConfig (resolution 64, hidden 32, codebook 512) so that the fixture stays small; layer
 structure, naming and every code path of encode()/decode() are those of the default config."""
@@ -23,7 +23,8 @@ def to_np_tree(t):
 
 
 def main():
-    spec = importlib.util.spec_from_file_location("lwm_ref_vqgan", "/root/reference/lwm/vqgan.py")
+    spec = importlib.util.spec_from_file_location(
+        "lwm_ref_vqgan", os.path.join(os.environ.get("LWM_REFERENCE", "reference"), "lwm", "vqgan.py"))
     ref = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(ref)
     from oracle import vqgan_ref as vr

@@ -99,7 +99,7 @@ int main(int argc, char** argv) {
   for (int busy = 0; busy < 2; ++busy) {
     for (int it = 0; it < 3; ++it) {
       host_barrier(sh, n, &phase);
-      if (busy) spin_kernel<<<148 * 2, 1024, 0, s_main>>>(100000000LL);   // ~50 ms, every SM fully occupied
+      if (busy) spin_kernel<<<132 * 2, 1024, 0, s_main>>>(100000000LL);   // ~50 ms, every SM fully occupied
       CK(cudaEventRecord(e0, s_copy));
       CK(cudaMemcpyAsync(land, peer_heap[src] + kFlagBytes, kData, cudaMemcpyDeviceToDevice, s_copy));
       CK(cudaEventRecord(e1, s_copy));

@@ -1,5 +1,7 @@
 """On-GPU self-check used by __graft_entry__.smoke(): one small invocation of each hot path,
 compared against the CPU oracle (the oracle is only ever the checker — see oracle/__init__.py)."""
+import math
+
 import numpy as np
 import torch
 
@@ -10,7 +12,7 @@ def _rel(x, ref):
     return float(np.linalg.norm(x - ref) / max(np.linalg.norm(ref), 1e-30))
 
 
-def sampled_parity(S_total, H, check_heads, op, device, rank=0, world=1, base_seed=1234, shards=None):
+def sampled_parity(S_total, H, check_heads, op, device, rank=0, world=1, base_seed=1234, shards=None, do_scale=1.0):
     """Parity of the attention op at 32K .. 128K tokens, where the dense oracle does not fit: this
     rank's shards of the seeded synthetic q/k/v (lwm_b200/synthetic.py) go through `op` (forward + backward) with a dO
     that is zero outside one sampled query row per 128-row tile (+ the last 128 rows of the sequence); the float64
@@ -19,7 +21,11 @@ def sampled_parity(S_total, H, check_heads, op, device, rank=0, world=1, base_se
     its un-rounded fp32 results. Returns {name: relative Frobenius error over this rank's rows}.
     op(q, k, v) -> out must be differentiable (the public ringattention op bound to the caller's process group).
     shards: optional dict(q, k, v, do) of this rank's DEVICE tensors [1, S_total/world, H, 128] already built with
-    synthetic.shard(name, rank, ...) and the same base_seed (bench.py passes its timed inputs)."""
+    synthetic.shard(name, rank, ...) and the same base_seed (bench.py passes its timed inputs).
+    do_scale: a power of two that multiplies dO (exactly, in both the op's input and the oracle's), to check the
+    gradients at the magnitudes a loss averaged over many tokens produces; the relative errors are unchanged by it."""
+    if do_scale <= 0 or math.frexp(do_scale)[0] != 0.5:
+        raise ValueError("do_scale must be a power of two")
     from oracle.attn_rows import attention_rows, sample_rows
     from . import synthetic as syn
     D = 128
@@ -31,7 +37,7 @@ def sampled_parity(S_total, H, check_heads, op, device, rank=0, world=1, base_se
         shards = {n_: syn.shard(n_, rank, Sl, H, D, base_seed, torch.bfloat16).to(device) for n_ in ("q", "k", "v", "do")}
     keep = torch.zeros(Sl, dtype=torch.bool)
     keep[mine - lo] = True
-    do = shards["do"].float()
+    do = shards["do"].float() * do_scale
     do[0, (~keep).to(device)] = 0
     qd, kd, vd = [shards[n_].float().requires_grad_(True) for n_ in ("q", "k", "v")]
     out = op(qd, kd, vd)
@@ -42,7 +48,7 @@ def sampled_parity(S_total, H, check_heads, op, device, rank=0, world=1, base_se
     errs = {}
     for h in check_heads:
         kg, vg = syn.head_global("k", world, h, Sl, D, base_seed), syn.head_global("v", world, h, Sl, D, base_seed)
-        qg, dg = syn.head_global("q", world, h, Sl, D, base_seed), syn.head_global("do", world, h, Sl, D, base_seed)
+        qg, dg = syn.head_global("q", world, h, Sl, D, base_seed), syn.head_global("do", world, h, Sl, D, base_seed) * do_scale
         ref = attention_rows(qg[rows], rows, kg, vg, dg[rows], causal=True)
         sel = (rows >= lo) & (rows < hi)
         pairs = dict(out=(got["out"][mine - lo, h], ref["out"][sel]), dq=(got["dq"][mine - lo, h], ref["dq"][sel]),

@@ -4,6 +4,15 @@ executor that runs on the GPUs — is exercised in the CPU test-suite: P rank TH
 condition variable. Streams do not exist here (every operation completes before the next one is issued), which is a
 stricter ordering than the GPU's, so a protocol that deadlocks here may still be correct — but one that passes here has
 no circular cross-rank wait. Numerics come from the oracle-backed step functions (oracle/step_ops.py).
+
+EmuWorld(world, device=cuda_device) puts the heaps on one GPU instead, so that the executor can run with the real CUDA
+step functions (ringattention.PeerOpsF16 / PeerOpsBf16; tests/test_ring_peer_emulated_gpu.py). Pulls and puts are then
+device-to-device copies, while the flags stay on the host. This is sound because every rank thread issues ALL of its
+device work — staging, copies, kernels — on the one default stream of that device: the host order of the enqueues is
+their device order. A rank signals a flag only after it has enqueued the work the flag announces, and the consumer
+enqueues its dependent copies or kernels only after it has seen the flag on the host, so they run after the producer's
+work on the device. There is no device-side wait anywhere in the emulation: a protocol mistake ends as a host timeout
+and a failed assertion, never as a stalled GPU.
 TEST INFRASTRUCTURE ONLY."""
 import contextlib
 import threading
@@ -14,9 +23,10 @@ from oracle.step_ops import CpuOps
 
 
 class EmuWorld:
-    def __init__(self, world, n_flags=4096):
+    def __init__(self, world, n_flags=4096, device=None):
         self.world = world
-        self.heaps = [torch.zeros(0, dtype=torch.uint8) for _ in range(world)]
+        self.device = torch.device("cpu") if device is None else torch.device(device)
+        self.heaps = [torch.zeros(0, dtype=torch.uint8, device=self.device) for _ in range(world)]
         self.flags = [[0] * n_flags for _ in range(world)]
         self.cv = threading.Condition()
         self.barrier = threading.Barrier(world)
@@ -31,7 +41,7 @@ class EmuTransport:
     def ensure(self, nbytes):
         if self.emu.heaps[self.rank].numel() < nbytes:
             self.emu.barrier.wait()
-            self.emu.heaps[self.rank] = torch.zeros(nbytes + 256, dtype=torch.uint8)
+            self.emu.heaps[self.rank] = torch.zeros(nbytes + 256, dtype=torch.uint8, device=self.emu.device)
             self.pass_id = 0
             self.emu.barrier.wait()
 

@@ -66,18 +66,21 @@ def test_fp16_mode_meets_1e3_on_white_noise(S, H, causal):
 
 
 def test_fp16_mode_scale_robustness():
-    """operands far from unit scale (tiny upstream gradients, large keys) must neither overflow nor lose bits"""
+    """operands far from unit scale (tiny upstream gradients, large keys, large or small values) must neither overflow
+    nor lose bits: the V and dO scales vary independently, so their product ranges over 3e-10 .. 9e4"""
     from oracle.attn_dense import attention_dense_grads
-    q, k, v, do = make_qkv(1, 512, 512, 2, n_extra=1, seed=43)
-    k = (k.float() * 24.0).to(torch.bfloat16)
-    q = (q.float() / 24.0).to(torch.bfloat16)
-    v = (v.float() * 300.0).to(torch.bfloat16)
-    do = (do.float() * 1e-7).to(torch.bfloat16)
-    o32, out, lse, dq, dk, dv = _run(q, k, v, do)
-    rq, rk, rv = attention_dense_grads(to_np(q), to_np(k), to_np(v), to_np(do), causal=True)
-    for got, ref in ((dq, rq), (dk, rk), (dv, rv)):
-        assert np.isfinite(got).all()
-        assert rel_fro(got, ref) < TOL
+    q0, k0, v0, do0 = make_qkv(1, 512, 512, 2, n_extra=1, seed=43)
+    k = (k0.float() * 24.0).to(torch.bfloat16)
+    q = (q0.float() / 24.0).to(torch.bfloat16)
+    for v_scale in (1.0 / 300.0, 1.0, 300.0):
+        for do_scale in (1e-7, 1.0, 300.0):
+            v = (v0.float() * v_scale).to(torch.bfloat16)
+            do = (do0.float() * do_scale).to(torch.bfloat16)
+            o32, out, lse, dq, dk, dv = _run(q, k, v, do)
+            rq, rk, rv = attention_dense_grads(to_np(q), to_np(k), to_np(v), to_np(do), causal=True)
+            for name, got, ref in (("dq", dq, rq), ("dk", dk, rk), ("dv", dv, rv)):
+                assert np.isfinite(got).all(), (v_scale, do_scale, name)
+                assert rel_fro(got, ref) < TOL, (v_scale, do_scale, name, rel_fro(got, ref))
 
 
 def test_fp16_mode_bias_segments_and_public_op():

@@ -15,9 +15,13 @@
 //     dV  += P^T dO     m64n128  A = P^T from registers, dO read MN-major
 //     dK  += dS^T Q     m64n128  A = dS^T from registers, Q read MN-major
 //     dQ   = dS  K      m64n64   A = the shared dS^T tile read MN-major (all 128 keys), B = this
-//                                warpgroup's 64 columns of K read MN-major; added to dq_acc with
-//                                vector fp32 atomics.
+//                                warpgroup's 64 columns of K read MN-major; staged in shared memory
+//                                as fp32 and added to dq_acc by a TMA reduction.
 //   warp 8: TMA loads (K, V once; Q + dO + lse + delta double-buffered).
+//   warp 9: dQ reductions (cp.reduce.async.bulk.tensor add, from a double-buffered fp32 staging tile).
+//   warps 10, 11: idle.
+// Inside an iteration each wgmma group is waited for only where its result is needed: exp(S^T) runs under
+// dP^T, dS^T under dV, and the dS^T handoff between the warpgroups under dK.
 // The softmax scale is folded into dS before it is rounded, so dK and dQ need no epilogue scaling.
 // dk_acc / dv_acc are accumulated read-modify-write by the one CTA that owns the tile.
 #include "attn_common.cuh"
@@ -46,14 +50,21 @@ constexpr int kBwdThreads = 384;                // 2 consumer warpgroups + 1 pro
 constexpr int kBwdConsumerWarps = 8;
 constexpr int kTB = kTile * kHeadDim * 2;       // 32 KB: a 128-row bf16 tile
 constexpr int kQB = kBQ * kHeadDim * 2;         // 16 KB: a 64-row bf16 tile
-// smem map (bytes): K | V | Q0 Q1 | dO0 dO1 | dS^T (128 keys x 64 queries) | lse[2] | delta[2] | barriers
+constexpr int kDSB = kTile * kBQ * 2;           // 16 KB: dS^T of one Q tile (128 keys x 64 queries, 16 bit)
+constexpr int kDQB = kBQ * kHeadDim * 4;        // 32 KB: fp32 dQ tile (64 queries x 128 columns)
+constexpr int kDQBox = kBQ * 32 * 4;            // 8 KB: one 32-column box of the dQ tile (128 B rows, swizzled)
+// smem map (bytes): K | V | Q0 Q1 | dO0 dO1 | dS^T 0 1 | dQ 0 1 | lse[2] | delta[2] | barriers
 constexpr int kOffK = 0, kOffV = kTB, kOffQ = 2 * kTB, kOffDO = kOffQ + 2 * kQB, kOffDS = kOffDO + 2 * kQB;
-constexpr int kOffLse = kOffDS + kTile * kBQ * 2, kOffDelta = kOffLse + 2 * kBQ * 4, kOffBars = kOffDelta + 2 * kBQ * 4;
+constexpr int kOffDQ = kOffDS + 2 * kDSB;
+constexpr int kOffLse = kOffDQ + 2 * kDQB, kOffDelta = kOffLse + 2 * kBQ * 4, kOffBars = kOffDelta + 2 * kBQ * 4;
 constexpr int kBwdSmemBytes = kOffBars + 128;
+static_assert(kBwdSmemBytes <= 227 * 1024, "attn_bwd: shared memory over the sm_90 per-block limit");
+static_assert(kOffDQ % 1024 == 0, "128B-swizzled TMA tiles need 1024-byte alignment");
 
 struct BwdBarriers {
   uint64_t kv_full;
   uint64_t q_full[2], q_empty[2];   // Q + dO + lse + delta of one Q tile
+  uint64_t dq_full[2], dq_empty[2]; // fp32 dQ staging tile: written by the consumers, reduced by warp 9
 };
 
 LWM_DEVICE void load_tile_nb(uint8_t* dst, const CUtensorMap* tm, uint64_t* bar, int h, int row0, int b, int half_bytes) {
@@ -77,7 +88,8 @@ constexpr float kPBoostInv = 1.0f / 16384.0f;
 template <bool kF16>
 __global__ void __launch_bounds__(kBwdThreads, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO, const BwdParams p) {
+                const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
+                const __grid_constant__ CUtensorMap tmDQ, const BwdParams p) {
   // no static shared memory in this kernel: the dynamic window starts 1024-aligned (checked below)
   extern __shared__ __align__(1024) uint8_t smem[];
   float (*s_lse)[kBQ] = reinterpret_cast<float (*)[kBQ]>(smem + kOffLse);
@@ -114,6 +126,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     for (int s = 0; s < 2; ++s) {
       mbar_init(&bars.q_full[s], 1);
       mbar_init(&bars.q_empty[s], kBwdConsumerWarps);
+      mbar_init(&bars.dq_full[s], kBwdConsumerWarps * 32);
+      mbar_init(&bars.dq_empty[s], 1);
     }
     fence_mbar_init();
   }
@@ -121,7 +135,23 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 
   if (warp >= 8) {
     // ------------------------------------------------------------------ TMA producer
-    setmaxnreg_dec<40>();
+    setmaxnreg_dec<24>();
+    if (warp == 9 && lane == 0) {
+      // dQ reductions: one fp32 add per dQ element per (key tile, Q tile), four 32-column boxes per tile
+      tma_prefetch_desc(&tmDQ);
+      for (int it = 0; it < nq; ++it) {
+        const int st = it & 1;
+        const int row0 = (i_start + it) * kBQ;
+        mbar_wait(&bars.dq_full[st], (it >> 1) & 1);
+#pragma unroll
+        for (int j = 0; j < kHeadDim / 32; ++j)
+          tma_reduce_add_4d(&tmDQ, smem + kOffDQ + st * kDQB + j * kDQBox, 32 * j, h, row0, b);
+        tma_commit_group();
+        tma_wait_group_read<0>();
+        mbar_arrive(&bars.dq_empty[st]);
+      }
+      tma_wait_group<0>();
+    }
     if (warp == 8 && lane == 0) {
       tma_prefetch_desc(&tmQ);
       tma_prefetch_desc(&tmK);
@@ -146,39 +176,24 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   }
 
   // -------------------------------------------------------------------- consumer warpgroups
-  setmaxnreg_inc<232>();
+  setmaxnreg_inc<240>();
   const int wg = warp >> 2;      // keys [64 wg, 64 wg + 64) of the tile
   const int w = warp & 3;
   const int quad = lane & 3;
   const int kr0 = wg * 64 + w * 16 + (lane >> 2);   // this thread's key rows in the tile: kr0, kr0 + 8
   const bool has_bias = p.mask.bias != nullptr, has_seg = p.mask.seg != nullptr;
-  const int* seg_row = has_seg ? p.mask.seg + (long long)b * p.mask.seg_stride : nullptr;
-  int k_pos[2], my_seg[2];
-  float bias_t[2] = {0.f, 0.f};
-  bool key_masked[2] = {false, false};
-#pragma unroll
-  for (int hh = 0; hh < 2; ++hh) {
-    k_pos[hh] = p.mask.k_pos0 + n * kTile + kr0 + 8 * hh;
-    my_seg[hh] = has_seg ? seg_row[k_pos[hh]] : 0;
-    if (has_bias) {
-      bias_t[hh] = p.mask.bias[(long long)b * p.mask.bias_stride + k_pos[hh]] * kLog2e;
-      key_masked[hh] = bias_t[hh] < kMaskedLogit;
-    }
-  }
   // fp16 mode: logits scale picks up scale_q*scale_k; dP = dO16 V16^T stays in operand units (the absolute delta is
   // brought into them instead) and the dS scale dp_mul = scale_do*scale_v is undone with the dQ / dK scales
   const float scale_log2 = p.scale_log2 * (kF16 ? (*p.scale_q) * (*p.scale_k) : 1.0f);
-  const float dp_mul = kF16 ? (*p.scale_do) * (*p.scale_v) : 1.0f;
-  const float delta_mul = kF16 ? 1.0f / dp_mul : 1.0f;                   // exact: a power of two
+  const float delta_mul = kF16 ? 1.0f / ((*p.scale_do) * (*p.scale_v)) : 1.0f;   // exact: a power of two
   const float ds_mul = p.scale * (kF16 ? kDsNorm * kPBoostInv : 1.0f);    // P holds P * 2^14 in fp16 mode
-  const float dq_mul = kF16 ? (*p.scale_k) * dp_mul * (1.0f / kDsNorm) : 1.0f;   // dQ = dS16 K16 * scale_k * dp_mul / norm
-  const long long wg_k_last = (long long)p.mask.k_pos0 + (long long)n * kTile + wg * 64 + 63;
+  // positions fit in int32 (checked on the host); int keeps the loop under the register budget
+  const int wg_k_last = p.mask.k_pos0 + n * kTile + wg * 64 + 63;
 
   const uint32_t aK = smem_u32(smem + kOffK), aV = smem_u32(smem + kOffV), aDS = smem_u32(smem + kOffDS);
   const uint64_t dK_k = desc_kmajor_sw128(aK + wg * 64 * 128), dV_k = desc_kmajor_sw128(aV + wg * 64 * 128);
   const uint64_t dK_n = desc_mnmajor_sw128(aK + wg * (kTB / 2), kTB / 2);   // this warpgroup's 64 columns of K
-  const uint64_t dDS_m = desc_mnmajor_sw128(aDS, kTile * 128);
-  uint8_t* sDS = smem + kOffDS;
+  uint8_t* sDQ = smem + kOffDQ;
 
   float dk[64], dv[64];
 #pragma unroll
@@ -190,9 +205,11 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     const uint32_t aQ = smem_u32(smem + kOffQ + st * kQB), aDO = smem_u32(smem + kOffDO + st * kQB);
     const uint64_t dQ_k = desc_kmajor_sw128(aQ), dDO_k = desc_kmajor_sw128(aDO);
     const uint64_t dQ_n = desc_mnmajor_sw128(aQ, kQB / 2), dDO_n = desc_mnmajor_sw128(aDO, kQB / 2);
+    const uint64_t dDS_m = desc_mnmajor_sw128(aDS + st * kDSB, kDSB);
+    uint8_t* sDS = smem + kOffDS + st * kDSB;
     mbar_wait(&bars.q_full[st], (it >> 1) & 1);
 
-    // ---- S^T = K Q^T, dP^T = V dO^T
+    // ---- S^T = K Q^T, dP^T = V dO^T: two groups, so that exp(S^T) runs while dP^T is on the tensor cores
     float sacc[32], dpacc[32];
     wgmma_fence();
 #pragma unroll
@@ -200,54 +217,86 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       const uint32_t ka = (ks >> 2) * (kTB / 2) + (ks & 3) * 32, kb = (ks >> 2) * (kQB / 2) + (ks & 3) * 32;
       wgmma_ss<64, kF16, 0, 0>(sacc, desc_advance(dK_k, ka), desc_advance(dQ_k, kb), ks > 0);
     }
+    wgmma_commit();
 #pragma unroll
     for (int ks = 0; ks < kHeadDim / 16; ++ks) {
       const uint32_t ka = (ks >> 2) * (kTB / 2) + (ks & 3) * 32, kb = (ks >> 2) * (kQB / 2) + (ks & 3) * 32;
       wgmma_ss<64, kF16, 0, 0>(dpacc, desc_advance(dV_k, ka), desc_advance(dDO_k, kb), ks > 0);
     }
     wgmma_commit();
-    wgmma_wait<0>();
+    wgmma_wait<1>();
     reg_fence(sacc);
-    reg_fence(dpacc);
 
-    // ---- P^T = exp2(S^T * scale_log2 (+bias) - lse2), dS^T = P^T o (dP^T - delta) * scale
-    const long long q_tile_pos = (long long)p.mask.q_pos0 + (long long)(i_start + it) * kBQ;
+    // ---- P^T = exp2(S^T * scale_log2 (+bias) - lse2)
+    const int q_tile_pos = p.mask.q_pos0 + (i_start + it) * kBQ;
     const bool need_mask = has_bias || has_seg || (p.mask.causal && q_tile_pos < wg_k_last);
     uint32_t pk[4][4], dsk[4][4];   // P^T and dS^T as A fragments, one 16-query slice per entry
+    float pr[4][8];
+    // the mask test is hoisted out of the element loop: one branch per tile keeps the fragment in registers
+    if (!need_mask) {
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-      float pr[8], ds[8];
-#pragma unroll
-      for (int t = 0; t < 8; ++t) {
-        const int i = 8 * kk + t;
-        const int hh = (t >> 1) & 1;
+      for (int i = 0; i < 32; ++i) {
         const int col = (i >> 2) * 8 + quad * 2 + (i & 1);   // query column in the tile
-        const float ls = s_lse[st][col];   // -lse*log2e (or -inf): lwm_attn_bwd_lse
-        if (!need_mask) {
-          pr[t] = ex2f(fmaf(sacc[i], scale_log2, ls));
-        } else {
-          float tv = key_masked[hh] ? kMaskedLogit : fmaf(sacc[i], scale_log2, bias_t[hh]);
-          const int q_pos = int(q_tile_pos) + col;
-          if (has_seg && seg_row[q_pos] != my_seg[hh]) tv = kMaskedLogit;
-          if (p.mask.causal && q_pos < k_pos[hh]) tv = kMaskedLogit;
-          pr[t] = ex2f(tv + ls);
+        pr[i >> 3][i & 7] = ex2f(fmaf(sacc[i], scale_log2, s_lse[st][col]));   // -lse*log2e (or -inf): lwm_attn_bwd_lse
+      }
+    } else {
+      // per-key mask inputs, reloaded per masked tile (L1 hits) rather than held in registers across the loop
+      const int* seg_row = has_seg ? p.mask.seg + (long long)b * p.mask.seg_stride : nullptr;
+      const int k_pos = p.mask.k_pos0 + n * kTile + kr0;   // this thread's keys: k_pos, k_pos + 8
+      int my_seg[2];
+      float bias_t[2] = {0.f, 0.f};
+      bool key_masked[2] = {false, false};
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        my_seg[hh] = has_seg ? seg_row[k_pos + 8 * hh] : 0;
+        if (has_bias) {
+          bias_t[hh] = p.mask.bias[(long long)b * p.mask.bias_stride + k_pos + 8 * hh] * kLog2e;
+          key_masked[hh] = bias_t[hh] < kMaskedLogit;
         }
       }
 #pragma unroll
-      for (int t = 0; t < 4; ++t) pk[kk][t] = kF16 ? pack_f16x2(pr[2 * t], pr[2 * t + 1]) : pack_bf16x2(pr[2 * t], pr[2 * t + 1]);
+      for (int i = 0; i < 32; ++i) {
+        const int hh = (i >> 1) & 1;
+        const int col = (i >> 2) * 8 + quad * 2 + (i & 1);
+        float tv = key_masked[hh] ? kMaskedLogit : fmaf(sacc[i], scale_log2, bias_t[hh]);
+        const int q_pos = q_tile_pos + col;
+        if (has_seg && seg_row[q_pos] != my_seg[hh]) tv = kMaskedLogit;
+        if (p.mask.causal && q_pos < k_pos + 8 * hh) tv = kMaskedLogit;
+        pr[i >> 3][i & 7] = ex2f(tv + s_lse[st][col]);
+      }
+    }
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+      for (int t = 0; t < 4; ++t)
+        pk[kk][t] = kF16 ? pack_f16x2(pr[kk][2 * t], pr[kk][2 * t + 1]) : pack_bf16x2(pr[kk][2 * t], pr[kk][2 * t + 1]);
+
+    // ---- dV += P^T dO, on the tensor cores while dS^T is computed
+    reg_fence(dv);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) wgmma_rs128<kF16, 1>(dv, pk[kk], desc_advance(dDO_n, kk * 2048), 1);
+    wgmma_commit();
+
+    // ---- dS^T = P^T o (dP^T - delta) * scale (waits for dP^T only)
+    wgmma_wait<1>();
+    reg_fence(dpacc);
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      float ds[8];
 #pragma unroll
       for (int t = 0; t < 8; ++t) {
         const int i = 8 * kk + t;
         const int col = (i >> 2) * 8 + quad * 2 + (i & 1);
-        ds[t] = (pr[t] * ds_mul) * fmaf(-s_delta[st][col], delta_mul, dpacc[i]);
+        ds[t] = (pr[kk][t] * ds_mul) * fmaf(-s_delta[st][col], delta_mul, dpacc[i]);
       }
 #pragma unroll
       for (int t = 0; t < 4; ++t) dsk[kk][t] = kF16 ? pack_f16x2(ds[2 * t], ds[2 * t + 1]) : pack_bf16x2(ds[2 * t], ds[2 * t + 1]);
     }
 
-    // ---- dS^T -> shared memory (128B-swizzled, key rows of 64 queries) for the dQ wgmma of both warpgroups.
-    // Barrier 1: the previous tile's dQ wgmmas of both warpgroups (which read this buffer) have completed.
-    named_bar_sync(1, 256);
+    // ---- dS^T -> shared memory stage st (128B-swizzled, key rows of 64 queries) for the dQ wgmma of both
+    // warpgroups. The stage was last read by the dQ wgmmas of tile it - 2, which both warpgroups waited for
+    // before they passed the barrier of tile it - 1.
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk)
 #pragma unroll
@@ -258,43 +307,48 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       }
     fence_proxy_async_smem();
 
-    // ---- dV += P^T dO, dK += dS^T Q
-    reg_fence(dv);
+    // ---- dK += dS^T Q, running while the other warpgroup's half of dS^T arrives
     reg_fence(dk);
     wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) wgmma_rs128<kF16, 1>(dv, pk[kk], desc_advance(dDO_n, kk * 2048), 1);
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) wgmma_rs128<kF16, 1>(dk, dsk[kk], desc_advance(dQ_n, kk * 2048), 1);
     wgmma_commit();
 
-    // ---- dQ = dS K over all 128 keys (barrier 2: both halves of dS^T are in shared memory)
-    named_bar_sync(2, 256);
+    // ---- dQ = dS K over all 128 keys (the barrier: both halves of dS^T are in shared memory)
+    named_bar_sync(1, 256);
     float dq[32];
 #pragma unroll
     for (int ks = 0; ks < kTile / 16; ++ks)
       wgmma_ss<64, kF16, 1, 1>(dq, desc_advance(dDS_m, ks * 2048), desc_advance(dK_n, ks * 2048), ks > 0);
     wgmma_commit();
-    wgmma_wait<0>();
-    reg_fence(dq);
+    wgmma_wait<1>();   // dV and dK: the last reads of Q, dO, lse and delta of this stage
     reg_fence(dv);
     reg_fence(dk);
-    if (lane == 0) mbar_arrive(&bars.q_empty[st]);   // Q, dO, lse and delta of this stage are no longer read
+    if (lane == 0) mbar_arrive(&bars.q_empty[st]);
 
-    // dQ tile (64 queries x this warpgroup's 64 columns) -> dq_acc
-    const int q_row0 = (i_start + it) * kBQ + w * 16 + (lane >> 2);
+    // dQ tile (64 queries x this warpgroup's 64 columns, scaled to fp32 gradient units) -> staging tile st, as
+    // two 32-column boxes of 128-byte rows, 16-byte chunks XOR-swizzled by row (conflict-free float2 stores)
+    mbar_wait(&bars.dq_empty[st], ((it >> 1) & 1) ^ 1);
+    wgmma_wait<0>();
+    reg_fence(dq);
+    // dQ = dS16 K16 * scale_k * dp_mul / norm with dp_mul = scale_do * scale_v (re-read here: no register held across the loop)
+    const float dq_mul = kF16 ? (*p.scale_k) * ((*p.scale_do) * (*p.scale_v)) * (1.0f / kDsNorm) : 1.0f;
+    uint8_t* sdq = sDQ + st * kDQB + wg * 2 * kDQBox + (quad & 1) * 8;
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
-      float* dst = p.dq_acc + (((long long)b * p.Sq + q_row0 + 8 * hh) * p.H + h) * kHeadDim + wg * 64 + quad * 2;
+      const uint32_t row = w * 16 + (lane >> 2) + 8 * hh;
 #pragma unroll
       for (int g = 0; g < 8; ++g)
-        atomicAdd(reinterpret_cast<float2*>(dst + g * 8), make_float2(dq[4 * g + 2 * hh] * dq_mul, dq[4 * g + 2 * hh + 1] * dq_mul));
+        *reinterpret_cast<float2*>(sdq + (g >> 2) * kDQBox + swz128_offset(row, (g & 3) * 2 + (quad >> 1))) =
+            make_float2(dq[4 * g + 2 * hh] * dq_mul, dq[4 * g + 2 * hh + 1] * dq_mul);
     }
+    fence_proxy_async_smem();
+    mbar_arrive(&bars.dq_full[st]);
   }
 
   // ------------------------------------------------------------------ epilogue: dK, dV
   // dK = dS16^T Q16 * scale_q * dp_mul / norm ; dV = P^T dO16 * scale_do
-  const float dk_mul = kF16 ? (*p.scale_q) * dp_mul * (1.0f / kDsNorm) : 1.0f;
+  const float dk_mul = kF16 ? (*p.scale_q) * ((*p.scale_do) * (*p.scale_v)) * (1.0f / kDsNorm) : 1.0f;
   const float dv_mul = kF16 ? (*p.scale_do) * kPBoostInv : 1.0f;
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
@@ -323,6 +377,14 @@ static bool make_bf16_tmap(CUtensorMap* tm, const void* ptr, int B, int S, int H
   return encode_tmap(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, ptr, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
+// fp32 [B, S, H, 128] accumulator, boxes of 32 columns (128 B, swizzled) x box_rows rows: the dQ reduction target
+static bool make_f32_tmap(CUtensorMap* tm, const void* ptr, int B, int S, int H, int box_rows) {
+  uint64_t dims[4] = {uint64_t(kHeadDim), uint64_t(H), uint64_t(S), uint64_t(B)};
+  uint64_t strides[3] = {uint64_t(kHeadDim) * 4, uint64_t(H) * kHeadDim * 4, uint64_t(S) * H * kHeadDim * 4};
+  uint32_t box[4] = {32, 1, uint32_t(box_rows), 1};
+  return encode_tmap(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, ptr, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
+}
+
 }  // namespace lwm
 
 using namespace lwm;
@@ -345,9 +407,10 @@ static int attn_bwd_launch(const void* q, const void* k, const void* v, const vo
   if (segment_ids && (seg_stride < q_pos0 + Sq || seg_stride < k_pos0 + Sk))
     return lwm_fail(LWM_ERR_SHAPE, "attn_bwd: segment_ids is indexed by GLOBAL position: seg_stride < max(q_pos0 + Sq, k_pos0 + Sk)");
   if (!lwm_check_device()) return LWM_ERR_DEVICE;
-  CUtensorMap tq, tk, tv, tdo;
+  CUtensorMap tq, tk, tv, tdo, tdq;
   if (!make_bf16_tmap(&tq, q, B, Sq, H, kBQ) || !make_bf16_tmap(&tk, k, B, Sk, H, kTile) ||
-      !make_bf16_tmap(&tv, v, B, Sk, H, kTile) || !make_bf16_tmap(&tdo, dout, B, Sq, H, kBQ))
+      !make_bf16_tmap(&tv, v, B, Sk, H, kTile) || !make_bf16_tmap(&tdo, dout, B, Sq, H, kBQ) ||
+      !make_f32_tmap(&tdq, dq_acc, B, Sq, H, kBQ))
     return lwm_fail(LWM_ERR_CUDA, "attn_bwd: cuTensorMapEncodeTiled failed (pointers must be 16B aligned)");
   BwdParams p;
   p.B = B; p.H = H; p.Sq = Sq; p.Sk = Sk;
@@ -373,8 +436,8 @@ static int attn_bwd_launch(const void* q, const void* k, const void* v, const vo
   }
   dim3 grid(Sk / kTile, H, B);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (scale_q) attn_bwd_kernel<true><<<grid, kBwdThreads, kBwdSmemBytes, st>>>(tq, tk, tv, tdo, p);
-  else attn_bwd_kernel<false><<<grid, kBwdThreads, kBwdSmemBytes, st>>>(tq, tk, tv, tdo, p);
+  if (scale_q) attn_bwd_kernel<true><<<grid, kBwdThreads, kBwdSmemBytes, st>>>(tq, tk, tv, tdo, tdq, p);
+  else attn_bwd_kernel<false><<<grid, kBwdThreads, kBwdSmemBytes, st>>>(tq, tk, tv, tdo, tdq, p);
   return lwm_check_launch("attn_bwd_kernel");
 }
 

@@ -12,6 +12,9 @@
 //     shared memory, fp32 logits in registers), online softmax in the log2 domain on the register
 //     fragment (a row is spread over the 4 lanes of a quad), then O += P V with P taken straight
 //     from registers as the A fragment and V read MN-major from the TMA tile (no transpose).
+//   * the consumer loop is software-pipelined: iteration j issues S_j = Q K_j^T and O += P_{j-1} V_{j-1} as two
+//     commit groups, waits for S_j only, and runs tile j's softmax while the PV group is on the tensor cores. The
+//     two warpgroups take turns issuing (named barriers 1 and 2), so one's softmax also runs under the other's GEMMs.
 //   * causal masking by global token position; KV tiles entirely above the diagonal are never
 //     loaded; only diagonal tiles pay for the mask.
 #include "attn_common.cuh"
@@ -101,7 +104,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 
   if (warp >= 8) {
     // ------------------------------------------------------------------ TMA producer
-    setmaxnreg_dec<40>();
+    setmaxnreg_dec<24>();
     if (warp == 8 && lane == 0 && n_kv > 0) {
       tma_prefetch_desc(&tmQ);
       tma_prefetch_desc(&tmK);
@@ -118,7 +121,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   }
 
   // -------------------------------------------------------------------- consumer warpgroups
-  setmaxnreg_inc<232>();
+  setmaxnreg_inc<240>();
   const int wg = warp >> 2;   // rows [64 wg, 64 wg + 64) of the Q tile
   const int w = warp & 3;
   const int quad = lane & 3;
@@ -126,15 +129,6 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const int r0 = m0 + wg * 64 + w * 16 + (lane >> 2);
   const float scale = p.scale_log2 * (p.scale_q ? (*p.scale_q) * (*p.scale_k) : 1.0f);
   const bool has_bias = p.mask.bias != nullptr, has_seg = p.mask.seg != nullptr;
-  const float* bias_row = has_bias ? p.mask.bias + (long long)b * p.mask.bias_stride : nullptr;
-  const int* seg_row = has_seg ? p.mask.seg + (long long)b * p.mask.seg_stride : nullptr;
-  long long q_pos[2];
-  int my_seg[2];
-#pragma unroll
-  for (int hh = 0; hh < 2; ++hh) {
-    q_pos[hh] = (long long)p.mask.q_pos0 + r0 + 8 * hh;
-    my_seg[hh] = has_seg ? seg_row[q_pos[hh]] : 0;
-  }
 
   float o[64];
 #pragma unroll
@@ -145,26 +139,45 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     mbar_wait(&bars.q_full, 0);
     const uint64_t q_desc = desc_kmajor_sw128(smem_u32(sQ + wg * 64 * 128));
     const uint32_t kv_base = smem_u32(sKV);
-    const long long warp_q_pos0 = (long long)p.mask.q_pos0 + m0 + wg * 64 + w * 16;
-    for (int j = 0; j < n_kv; ++j) {
-      const int ik = 2 * j, iv = 2 * j + 1;
-      // ---- S = Q K^T
-      float s[64];
-      mbar_wait(&bars.kv_full[ik % kFwdStages], (ik / kFwdStages) & 1);
-      const uint64_t kd = desc_kmajor_sw128(kv_base + (ik % kFwdStages) * kFwdTileBytes);
-      wgmma_fence();
+    // positions fit in int32 (checked on the host); int keeps the loop under the register budget
+    const int warp_q_pos0 = p.mask.q_pos0 + m0 + wg * 64 + w * 16;
+    float s[64];         // logits of tile j, then their exponentials (fp32) until they are packed into pa
+    uint32_t pa[8][4];   // P as the A fragment of O += P V, one 16-key slice per entry
+    float alpha[2];      // rescale of o and l_run from tile j - 1's row max to tile j's
+
+    // Ring item i: K of tile i / 2 (even i) or V of tile i / 2 (odd i), in slot i % kFwdStages.
+    auto wait_full = [&](int i) { mbar_wait(&bars.kv_full[i % kFwdStages], (i / kFwdStages) & 1); };
+    auto release = [&](int i) {
+      if (lane == 0) mbar_arrive(&bars.kv_empty[i % kFwdStages]);
+    };
+    // The two warpgroups take turns issuing their GEMMs (named barrier 1 + wg: "warpgroup wg may issue"), so
+    // that one warpgroup's softmax runs while the other's GEMMs are on the tensor cores. Warpgroup 0 goes first.
+    // Each warpgroup passes the turn n_kv + 1 times; warpgroup 1 skips its last hand-over, which nobody waits for.
+    auto turn_begin = [&]() { named_bar_sync(1 + wg, 256); };
+    auto turn_end = [&](bool last) {
+      if (!(last && wg == 1)) named_bar_arrive(2 - wg, 256);
+    };
+    if (wg == 1) named_bar_arrive(1, 256);
+    // S = Q K_j^T, one commit group
+    auto issue_s = [&](int j) {
+      const uint64_t kd = desc_kmajor_sw128(kv_base + ((2 * j) % kFwdStages) * kFwdTileBytes);
 #pragma unroll
       for (int ks = 0; ks < kHeadDim / 16; ++ks) {
         const uint32_t off = (ks >> 2) * (kFwdTileBytes / 2) + (ks & 3) * 32;
         wgmma_ss<128, kF16, 0, 0>(s, desc_advance(q_desc, off), desc_advance(kd, off), ks > 0);
       }
       wgmma_commit();
-      wgmma_wait<0>();
-      reg_fence(s);
-      if (lane == 0) mbar_arrive(&bars.kv_empty[ik % kFwdStages]);
-
-      // ---- online softmax on the fragment
-      const long long k_tile_pos = (long long)p.mask.k_pos0 + (long long)j * kTile;
+    };
+    // O += P_j V_j, one commit group (P from registers, V read MN-major)
+    auto issue_pv = [&](int j) {
+      const uint64_t vd = desc_mnmajor_sw128(kv_base + ((2 * j + 1) % kFwdStages) * kFwdTileBytes, kFwdTileBytes / 2);
+#pragma unroll
+      for (int kk = 0; kk < kTile / 16; ++kk) wgmma_rs128<kF16, 1>(o, pa[kk], desc_advance(vd, kk * 2048), 1);
+      wgmma_commit();
+    };
+    // online softmax of tile j on the fragment: row max, alpha, m_run / l_run update, s <- exp2(s * scale - m)
+    auto softmax = [&](int j) {
+      const int k_tile_pos = p.mask.k_pos0 + j * kTile;
       // warp-uniform: does any row of this warp need a mask on this KV tile?
       const bool need_mask = has_bias || has_seg || (p.mask.causal && (k_tile_pos + kTile - 1 > warp_q_pos0));
       float mx[2] = {-INFINITY, -INFINITY};
@@ -174,6 +187,16 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         mx[0] = quad_max(mx[0]) * scale;
         mx[1] = quad_max(mx[1]) * scale;
       } else {
+        // per-row mask inputs, reloaded per masked tile (L1 hits) rather than held in registers across the loop
+        const float* bias_row = has_bias ? p.mask.bias + (long long)b * p.mask.bias_stride : nullptr;
+        const int* seg_row = has_seg ? p.mask.seg + (long long)b * p.mask.seg_stride : nullptr;
+        int q_pos[2];
+        int my_seg[2];
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          q_pos[hh] = p.mask.q_pos0 + r0 + 8 * hh;
+          my_seg[hh] = has_seg ? seg_row[q_pos[hh]] : 0;
+        }
 #pragma unroll
         for (int i = 0; i < 64; ++i) {
           const int hh = (i >> 1) & 1;
@@ -191,46 +214,76 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         mx[0] = quad_max(mx[0]);
         mx[1] = quad_max(mx[1]);
       }
-      float alpha[2];
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
         const float m_new = fmaxf(m_run[hh], mx[hh]);
         alpha[hh] = (m_run[hh] == -INFINITY) ? 0.f : ex2f(m_run[hh] - m_new);
         m_run[hh] = m_new;
-        l_run[hh] *= alpha[hh];
-      }
-      if (j > 0) {
-#pragma unroll
-        for (int i = 0; i < 64; ++i) o[i] *= alpha[(i >> 1) & 1];
+        // rounded on its own, never fused with the first += below: l_run keeps its multiply-then-add rounding
+        l_run[hh] = __fmul_rn(l_run[hh], alpha[hh]);
       }
       const float neg_m[2] = {-m_run[0], -m_run[1]};
-      uint32_t pa[8][4];   // P as the A fragment of O += P V, one 16-key slice per entry
 #pragma unroll
-      for (int kk = 0; kk < 8; ++kk) {
-        float e[8];
-#pragma unroll
-        for (int t = 0; t < 8; ++t) {
-          const int i = 8 * kk + t;
-          const int hh = (t >> 1) & 1;
-          e[t] = need_mask ? ex2f(s[i] + neg_m[hh]) : ex2f(fmaf(s[i], scale, neg_m[hh]));
-          l_run[hh] += e[t];
-        }
-#pragma unroll
-        for (int t = 0; t < 4; ++t) pa[kk][t] = kF16 ? pack_f16x2(e[2 * t], e[2 * t + 1]) : pack_bf16x2(e[2 * t], e[2 * t + 1]);
+      for (int i = 0; i < 64; ++i) {
+        const int hh = (i >> 1) & 1;
+        s[i] = need_mask ? ex2f(s[i] + neg_m[hh]) : ex2f(fmaf(s[i], scale, neg_m[hh]));
+        l_run[hh] += s[i];
       }
+    };
+    auto pack_p = [&]() {
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk)
+#pragma unroll
+        for (int t = 0; t < 4; ++t) {
+          const int i = 8 * kk + 2 * t;
+          pa[kk][t] = kF16 ? pack_f16x2(s[i], s[i + 1]) : pack_bf16x2(s[i], s[i + 1]);
+        }
+    };
 
-      // ---- O += P V
-      mbar_wait(&bars.kv_full[iv % kFwdStages], (iv / kFwdStages) & 1);
-      const uint64_t vd = desc_mnmajor_sw128(kv_base + (iv % kFwdStages) * kFwdTileBytes, kFwdTileBytes / 2);
+    // Software pipeline: iteration j issues S_j and O += P_{j-1} V_{j-1} back to back, then runs tile j's
+    // softmax while the PV group is still on the tensor cores.
+    // ---- prologue: S_0, softmax_0 (o is still zero: no rescale)
+    wait_full(0);
+    turn_begin();
+    wgmma_fence();
+    issue_s(0);
+    turn_end(false);
+    wgmma_wait<0>();
+    reg_fence(s);
+    release(0);
+    softmax(0);
+    pack_p();
+    // ---- steady state
+    for (int j = 1; j < n_kv; ++j) {
+      wait_full(2 * j);
+      wait_full(2 * j - 1);
+      turn_begin();
       reg_fence(o);
       wgmma_fence();
-#pragma unroll
-      for (int kk = 0; kk < kTile / 16; ++kk) wgmma_rs128<kF16, 1>(o, pa[kk], desc_advance(vd, kk * 2048), 1);
-      wgmma_commit();
+      issue_s(j);
+      issue_pv(j - 1);
+      turn_end(false);
+      wgmma_wait<1>();   // S_j done; PV_{j-1} may still run
+      reg_fence(s);
+      release(2 * j);
+      softmax(j);
       wgmma_wait<0>();
       reg_fence(o);
-      if (lane == 0) mbar_arrive(&bars.kv_empty[iv % kFwdStages]);
+      release(2 * j - 1);
+#pragma unroll
+      for (int i = 0; i < 64; ++i) o[i] *= alpha[(i >> 1) & 1];
+      pack_p();
     }
+    // ---- epilogue: the last O += P V
+    wait_full(2 * n_kv - 1);
+    turn_begin();
+    reg_fence(o);
+    wgmma_fence();
+    issue_pv(n_kv - 1);
+    turn_end(true);
+    wgmma_wait<0>();
+    reg_fence(o);
+    release(2 * n_kv - 1);
   }
 
   // ---------------------------------------------------------------- epilogue: merge carry, write

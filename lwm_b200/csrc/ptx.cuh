@@ -179,6 +179,9 @@ LWM_DEVICE void setmaxnreg_dec() {
 LWM_DEVICE void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+LWM_DEVICE void named_bar_arrive(uint32_t id, uint32_t nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
 
 // Byte offset of element (row, 16-byte chunk c in [0,8)) inside a 128B-swizzled tile whose base is
 // 1024-byte aligned and whose rows are 128 B: chunk index is XORed with (row % 8).

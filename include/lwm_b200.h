@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define LWM_B200_ABI_VERSION 2
+#define LWM_B200_ABI_VERSION 3
 
 #define LWM_OK 0
 #define LWM_ERR_DEVICE 1
@@ -250,7 +250,8 @@ int lwm_ring_layout(int B, long long Sq, long long Sk, int H, int D, int world, 
  * lwm_vq_conv_cin3 Encoder conv_in (3 -> Cout, 3x3 SAME, vqgan.py:155) on the CUDA cores; w is HWIO.
  * lwm_vq_argmin    VectorQuantizer (vqgan.py:207-215): idx = argmin_n (sum z^2 + sum e_n^2 - 2 z.e_n) with the
  *                  first index on ties, fp32 with a pinned operation order (bit-exact vs oracle/vqgan_ref.py);
- *                  zq_st (optional) = z + (e[idx] - z). workspace: 8 * N * 8 bytes.
+ *                  zq_st (optional) = z + (e[idx] - z). workspace: 8 * N * 8 bytes. Non-finite distances follow
+ *                  np.argmin: the first NaN wins and an all-+inf row gives index 0, so idx is always in [0, n_e).
  * lwm_vq_gather    out[i] = codebook[idx[i]] (decode path, vqgan.py:193-195).
  */
 int lwm_vq_gn_stats(const float* x, double* stats, int N, int H, int W, int C, int groups, void* stream);
@@ -263,20 +264,29 @@ int lwm_vq_conv_cin3(const float* x, const float* w_hwio, const float* bias, flo
                      void* stream);
 /* "fp16x2" precision mode of the conv stack (the default: <= 1e-3 vs the fp32 reference at 2x instead of 3x the
  * algorithmic tensor work and half the operand bytes):
- * lwm_vq_prep_f16    like lwm_vq_prep, but ONE fp16 operand plane [N,H',W',C_pad].
- * lwm_vq_conv2d_f16  activation = that plane; weights split w = hi + lo (two fp16, pre-multiplied by the power of two
+ * lwm_vq_prep_f16    like lwm_vq_prep, but ONE fp16 operand plane [N,H',W',C_pad] holding y / s, with a power of two s
+ *                    written to the device float *scale_out. Without GroupNorm s = 2^(e-12), e the exponent of |x|max:
+ *                    x_absmax (required then) holds |x|max's bit pattern when x_absmax_given (lwm_vq_conv2d_f16's
+ *                    absmax_out of the conv that produced x), else it is computed into it; with GroupNorm s brings a bound on
+ *                    |y| derived from gn_stats, gamma and beta into [1, 2^13) (s = 1 for ordinary layers). The plane is
+ *                    then never inf nor fp16-subnormal because of the activation's magnitude.
+ * lwm_vq_conv2d_f16  activation = that plane, a_scale = its scale (device float; NULL = 1, multiplied back in fp32
+ *                    in the epilogue); weights split w = hi + lo (two fp16, pre-multiplied by the power of two
  *                    1/w_scale_inv so that lo stays a normal fp16) and STACKED along Cout: w_stacked
  *                    [taps][Cout_pad/BN][2*BN][C_pad], BN = largest multiple of 16 <= 128 dividing Cout_pad, rows [0,BN) = hi, [BN,2BN) = lo. One
  *                    64 x 2BN wgmma per warpgroup yields A.hi | A.lo side by side; the epilogue adds them, applies w_scale_inv, bias,
  *                    residual, clip. gn_stats_out (optional; zeroed by the caller; [N, groups, 2] float64): the epilogue
  *                    also accumulates (sum, sum of squares) of the OUTPUT per (sample, group) — the statistics of the
  *                    GroupNorm that consumes this tensor (vqgan.py:251,254,161,181), so lwm_vq_gn_stats' extra pass
- *                    over the activation disappears. */
-int lwm_vq_prep_f16(const float* x, const double* gn_stats, const float* gamma, const float* beta, void* out, int N, int H,
-                    int W, int C, int C_pad, int groups, int upsample2x, float eps, void* stream);
-int lwm_vq_conv2d_f16(const void* a, const void* w_stacked, const float* bias, const float* residual, float* out,
-                      double* gn_stats_out, int N, int Hin, int Win, int Cpad, int Ho, int Wo, int Cout, int Cout_pad,
-                      int ksize, int stride, int pad, float w_scale_inv, int groups, int clip, void* stream);
+ *                    over the activation disappears. absmax_out (optional; zeroed by the caller): atomicMax of the
+ *                    output's |value| bit patterns, the x_absmax of an lwm_vq_prep_f16 that reads this tensor. */
+int lwm_vq_prep_f16(const float* x, const double* gn_stats, const float* gamma, const float* beta, void* out,
+                    float* scale_out, unsigned* x_absmax, int x_absmax_given, int N, int H, int W, int C, int C_pad,
+                    int groups, int upsample2x, float eps, void* stream);
+int lwm_vq_conv2d_f16(const void* a, const float* a_scale, const void* w_stacked, const float* bias,
+                      const float* residual, float* out, double* gn_stats_out, unsigned* absmax_out, int N, int Hin,
+                      int Win, int Cpad, int Ho, int Wo, int Cout, int Cout_pad, int ksize, int stride, int pad,
+                      float w_scale_inv, int groups, int clip, void* stream);
 int lwm_vq_argmin(const float* z, const float* codebook, int* idx, float* zq_st, void* workspace, int N, int n_e,
                   int e_dim, void* stream);
 int lwm_vq_gather(const int* idx, const float* codebook, float* out, long long N, int n_e, int e_dim, void* stream);

@@ -17,8 +17,10 @@
 //              pre-scaled by a power of two); both halves are stacked along N ([BN hi rows | BN lo rows]) so a single
 //              64 x 2BN x 16 wgmma per warpgroup produces A.hi and A.lo side by side and the epilogue adds the two
 //              halves: 2x the algorithmic MMA work instead of 3x and one operand plane to write and read instead of two.
+//              The plane holds x / a_scale (a power of two, lwm_vq_prep_f16), restored with w_scale_inv in fp32.
 //   GN stats   optional epilogue: per-(sample, group) sum / sum of squares of the conv OUTPUT (bias and residual
-//              included) — the statistics the next GroupNorm needs — so no separate pass re-reads the activation.
+//              included) — the statistics the next GroupNorm needs — so no separate pass re-reads the activation;
+//              likewise |output|max, the scale of a raw fp16 plane of the output (Downsample, 1x1 shortcut).
 //   pipeline   warp 8: TMA producer through a ring of `stages` slots; warpgroups 0 / 1: pixels [0,64) / [64,128)
 //              of the 8x16 tile, fp32 accumulators in registers, epilogue (+ bias (+ residual) -> fp32 NHWC)
 //              straight from the accumulator fragment. Grid = #SMs, tiles strided.
@@ -39,7 +41,10 @@ struct ConvParams {
   int BN, n_tiles;                // N-tile width (<= 256, multiple of 16) and count
   int n_pass;                     // 1 (bf16), 3 (bf16x3) or 2 (fp16 activation x stacked fp16 hi|lo weights)
   float w_scale_inv;              // n_pass 2: the weights were packed multiplied by 1/w_scale_inv (a power of two)
+  const float* a_scale;           // n_pass 2, optional: the activation plane holds x / *a_scale (a power of two)
   double* stats;                  // optional [N, groups, 2] (sum, sumsq) of the output, accumulated with atomics
+  unsigned* absmax;               // n_pass 2, optional: atomicMax of the output's |value| bit patterns (the next
+                                  // fp16 plane's scale, without another pass over the tensor)
   int groups;
   int stages;
   int clip;                       // 1: clamp the result to [-1, 1] (VQGANModel.decode, vqgan.py:141)
@@ -141,6 +146,9 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_consta
   for (int i = 0; i < kStatG; ++i) st1[i] = st2[i] = 0.f;
   int st_n = -1, st_nt = -1;
   const int cpg = p.stats ? p.Cout / p.groups : 1;
+  // fp16x2: accumulator units -> output units, w_scale_inv * a_scale (a product of powers of two: exact)
+  const float out_scale = (kF16 && p.a_scale) ? p.w_scale_inv * *p.a_scale : p.w_scale_inv;
+  float amax = 0.f;     // |output| max (fmaxf skips a NaN output, which the next plane keeps as NaN anyway)
   auto flush_stats = [&]() {
     if (st_n < 0) return;
 #pragma unroll
@@ -218,8 +226,8 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_consta
         const int c = c_base + g * 8 + quad * 2;
         float v0 = acc[4 * g + 2 * hh], v1 = acc[4 * g + 2 * hh + 1];
         if (kF16) {
-          v0 = (v0 + acc[4 * g + 2 * hh + NI / 4]) * p.w_scale_inv;
-          v1 = (v1 + acc[4 * g + 2 * hh + 1 + NI / 4]) * p.w_scale_inv;
+          v0 = (v0 + acc[4 * g + 2 * hh + NI / 4]) * out_scale;
+          v1 = (v1 + acc[4 * g + 2 * hh + 1 + NI / 4]) * out_scale;
         }
         if (vec && c + 1 < p.Cout) {
           const float2 b2 = *reinterpret_cast<const float2*>(p.bias + c);
@@ -234,6 +242,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_consta
             o2.y = fminf(fmaxf(o2.y, -1.f), 1.f);
           }
           *reinterpret_cast<float2*>(dst + c) = o2;
+          if (kF16 && p.absmax) amax = fmaxf(amax, fmaxf(fabsf(o2.x), fabsf(o2.y)));
           if (kF16 && p.stats) {   // stats need Cout % 16 == 0 (checked on the host): always this path
             st1[g < kStatG ? g : 0] += o2.x + o2.y;
             st2[g < kStatG ? g : 0] += o2.x * o2.x + o2.y * o2.y;
@@ -247,12 +256,18 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_consta
               if (res) o += res[c + e];
               if (p.clip) o = fminf(fmaxf(o, -1.f), 1.f);
               dst[c + e] = o;
+              if (kF16 && p.absmax) amax = fmaxf(amax, fabsf(o));
             }
         }
       }
     }
   }
   if (p.stats) flush_stats();
+  if (kF16 && p.absmax) {
+    // non-negative floats order like their bit patterns
+    const unsigned m = __reduce_max_sync(0xffffffffu, __float_as_uint(amax));
+    if (lane == 0 && m) atomicMax(p.absmax, m);
+  }
 }
 
 typedef void (*ConvKernel)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const ConvParams);
@@ -280,7 +295,7 @@ using namespace lwm;
 static int conv_launch(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo, const float* bias,
                        const float* residual, float* out, int N, int Hin, int Win, int Cpad, int Ho, int Wo, int Cout,
                        int Cout_pad, int ksize, int stride, int pad, int n_pass, int clip, float w_scale_inv,
-                       double* stats, int groups, void* stream) {
+                       const float* a_scale, double* stats, unsigned* absmax, int groups, void* stream) {
   if (!a_hi || !w_hi || !bias || !out) return lwm_fail(LWM_ERR_ARG, "vq_conv2d: null pointer");
   if (n_pass < 1 || n_pass > 3) return lwm_fail(LWM_ERR_ARG, "vq_conv2d: n_pass must be 1 (bf16), 2 (fp16x2) or 3 (bf16x3)");
   if (n_pass == 3 && (!a_lo || !w_lo)) return lwm_fail(LWM_ERR_ARG, "vq_conv2d: n_pass=3 needs the lo planes");
@@ -336,7 +351,7 @@ static int conv_launch(const void* a_hi, const void* a_lo, const void* w_hi, con
   p.taps_w = ksize; p.taps = taps; p.stride = stride; p.pad = pad;
   p.BN = BN; p.n_tiles = Cout_pad / BN; p.n_pass = n_pass;
   p.bias = bias; p.residual = residual; p.out = out; p.clip = clip;
-  p.w_scale_inv = w_scale_inv; p.stats = stats; p.groups = groups;
+  p.w_scale_inv = w_scale_inv; p.a_scale = a_scale; p.stats = stats; p.absmax = absmax; p.groups = groups;
   const int stage_bytes = (n_pass == 3 ? 2 : 1) * (kATile + wrows * BN * 128);
   int stages = (227 * 1024 - 2048) / stage_bytes;
   if (stages > 6) stages = 6;
@@ -365,17 +380,19 @@ extern "C" int lwm_vq_conv2d(const void* a_hi, const void* a_lo, const void* w_h
                              int n_pass, int clip, void* stream) {
   if (n_pass != 1 && n_pass != 3) return lwm_fail(LWM_ERR_ARG, "vq_conv2d: n_pass must be 1 (bf16) or 3 (bf16x3)");
   return conv_launch(a_hi, a_lo, w_hi, w_lo, bias, residual, out, N, Hin, Win, Cpad, Ho, Wo, Cout, Cout_pad, ksize,
-                     stride, pad, n_pass, clip, 1.0f, nullptr, 0, stream);
+                     stride, pad, n_pass, clip, 1.0f, nullptr, nullptr, nullptr, 0, stream);
 }
 
-// fp16x2 mode: a [N,Hin,Win,Cpad] fp16 plane (lwm_vq_prep_f16); w_stacked [taps][Cout_pad/BN][2*BN][Cpad] fp16 with
+// fp16x2 mode: a [N,Hin,Win,Cpad] fp16 plane (lwm_vq_prep_f16) holding x / *a_scale (a device float; NULL = 1);
+// w_stacked [taps][Cout_pad/BN][2*BN][Cpad] fp16 with
 // BN = the largest multiple of 16 <= 128 that divides Cout_pad: rows [0,BN) = fp16(w / w_scale_inv), rows [BN,2BN) = fp16(w / w_scale_inv - hi).
 // gn_stats_out (optional, zeroed by the caller): [N, groups, 2] double (sum, sumsq) of the OUTPUT tensor.
-extern "C" int lwm_vq_conv2d_f16(const void* a, const void* w_stacked, const float* bias, const float* residual,
-                                 float* out, double* gn_stats_out, int N, int Hin, int Win, int Cpad, int Ho, int Wo,
-                                 int Cout, int Cout_pad, int ksize, int stride, int pad, float w_scale_inv, int groups,
-                                 int clip, void* stream) {
+// absmax_out (optional, zeroed by the caller): atomicMax of the output's |value| bit patterns.
+extern "C" int lwm_vq_conv2d_f16(const void* a, const float* a_scale, const void* w_stacked, const float* bias,
+                                 const float* residual, float* out, double* gn_stats_out, unsigned* absmax_out,
+                                 int N, int Hin, int Win, int Cpad, int Ho, int Wo, int Cout, int Cout_pad, int ksize,
+                                 int stride, int pad, float w_scale_inv, int groups, int clip, void* stream) {
   if (!(w_scale_inv > 0.f)) return lwm_fail(LWM_ERR_ARG, "vq_conv2d_f16: w_scale_inv must be positive");
   return conv_launch(a, nullptr, w_stacked, nullptr, bias, residual, out, N, Hin, Win, Cpad, Ho, Wo, Cout, Cout_pad,
-                     ksize, stride, pad, 2, clip, w_scale_inv, gn_stats_out, groups, stream);
+                     ksize, stride, pad, 2, clip, w_scale_inv, a_scale, gn_stats_out, absmax_out, groups, stream);
 }

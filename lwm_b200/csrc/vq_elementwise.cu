@@ -13,6 +13,9 @@
 
 namespace lwm {
 
+// |x| max of an fp32 tensor as raw bits, atomicMax into *out_bits (attn_misc.cu)
+__global__ void absmax_f32_kernel(const uint4* __restrict__ x, long long n4, unsigned* __restrict__ out_bits);
+
 // ------------------------------------------------------------------------------------------------
 // GroupNorm statistics: stats[n][g] = (sum, sumsq) in double (atomics; zeroed by the caller).
 // Thread t owns channel quad (t % (C/4)) and strides over pixels, so a warp reads whole 128 B lines.
@@ -51,12 +54,22 @@ __global__ void gn_stats_kernel(const float* __restrict__ x, double* __restrict_
 // prep: y = [silu(gn(x))] at (h>>up, w>>up); hi = bf16(y); lo = bf16(y - hi). Output planes have
 // C_pad >= C channels (multiple of 64 for the conv's 128-byte TMA rows); padding channels are zero.
 // ------------------------------------------------------------------------------------------------
-// kF16: ONE fp16 plane (the fp16x2 conv mode: 11 significant bits, half the bytes of the hi+lo pair) instead.
+// kF16: ONE fp16 plane (the fp16x2 conv mode: 11 significant bits, half the bytes of the hi+lo pair) instead, written
+// as y / s with a power-of-two scale s (block 0 stores s to *scale_out; the conv multiplies it back in fp32), so that
+// the plane is neither inf nor fp16-subnormal whatever the activation's magnitude:
+//   no GroupNorm  s = 2^(e-12), e the exponent of |x|max (*absmax_bits: from the producing conv's epilogue, or from
+//                 an absmax pass over x): the largest element lands in [2^12, 2^13), as for the attention operands.
+//                 Scaling x by 2^k gives the same plane.
+//   GroupNorm     |silu(t)| <= |t| <= max|gamma| * (sqrt(n_g * E[x^2]) + |mean|) * rstd + max|beta| over every
+//                 (sample, group), n_g the group's element count (|x - mean| <= |x| + |mean| and x^2 <= n_g E[x^2]).
+//                 Every block derives the same bound B from the statistics; s = 1 while B lies in [1, 2^13), which
+//                 is every ordinary layer, and otherwise the power of two that brings B into that range.
 template <bool kF16>
 __global__ void prep_kernel(const float* __restrict__ x, const double* __restrict__ stats,
                             const float* __restrict__ gamma, const float* __restrict__ beta,
                             __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo, int N, int H, int W,
-                            int C, int C_pad, int groups, int up, float eps, int write_lo) {
+                            int C, int C_pad, int groups, int up, float eps, int write_lo,
+                            const unsigned* __restrict__ absmax_bits, float* __restrict__ scale_out) {
   // one thread = 8 channels of one output pixel: 2 x 16 B loads, 16 B stores per plane.
   // (mean, rstd) of every (sample, group) are derived once per block from the float64 sums into shared memory: the
   // element loop is then pure fp32 (FFMA + 2 MUFU per element), no float64 arithmetic per quad.
@@ -65,16 +78,55 @@ __global__ void prep_kernel(const float* __restrict__ x, const double* __restric
   const int octs = C_pad / 8;
   const size_t total = (size_t)N * Ho * Wo * octs;
   const int cpg = stats ? C / groups : 1;
+  __shared__ unsigned s_bound[3];    // kF16 with GroupNorm: bit patterns of max over (sample, group) of
+                                     // (sqrt(n_g E[x^2]) + |mean|) * rstd, of max|gamma| and of max|beta|
   if (stats) {
+    if (kF16 && threadIdx.x < 3) s_bound[threadIdx.x] = 0u;
+    if (kF16) __syncthreads();
     const double inv_cnt = 1.0 / ((double)H * W * cpg);
+    const float n_g = float((double)H * W * cpg);
+    float dev_max = 0.f;
     for (int i = threadIdx.x; i < N * groups; i += blockDim.x) {
       const float mean = float(stats[2 * i] * inv_cnt);
-      float var = float(stats[2 * i + 1] * inv_cnt) - mean * mean;   // flax fast variance, clamped at 0
+      const float msq = float(stats[2 * i + 1] * inv_cnt);
+      float var = msq - mean * mean;   // flax fast variance, clamped at 0
       var = fmaxf(var, 0.f);
       s_mr[2 * i] = mean;
       s_mr[2 * i + 1] = rsqrtf(var + eps);
+      if (kF16) dev_max = fmaxf(dev_max, (sqrtf(n_g * msq) + fabsf(mean)) * s_mr[2 * i + 1]);
+    }
+    if (kF16) {
+      float g_max = 0.f, b_max = 0.f;
+      for (int c = threadIdx.x; c < C; c += blockDim.x) {
+        g_max = fmaxf(g_max, fabsf(gamma[c]));
+        b_max = fmaxf(b_max, fabsf(beta[c]));
+      }
+      // non-negative floats order like their bit patterns (a NaN sorts above +inf)
+      const unsigned m0 = __reduce_max_sync(0xffffffffu, __float_as_uint(dev_max));
+      const unsigned m1 = __reduce_max_sync(0xffffffffu, __float_as_uint(g_max));
+      const unsigned m2 = __reduce_max_sync(0xffffffffu, __float_as_uint(b_max));
+      if ((threadIdx.x & 31) == 0) {
+        atomicMax(&s_bound[0], m0);
+        atomicMax(&s_bound[1], m1);
+        atomicMax(&s_bound[2], m2);
+      }
     }
     __syncthreads();
+  }
+  float inv_scale = 1.f;   // kF16: 1 / s
+  if constexpr (kF16) {
+    int shift;             // s = 2^shift
+    if (stats) {
+      const float bound = __uint_as_float(s_bound[1]) * __uint_as_float(s_bound[0]) + __uint_as_float(s_bound[2]);
+      const unsigned bits = __float_as_uint(bound);
+      const int e = max(int((bits >> 23) & 0xffu) - 127, -114);
+      shift = bits ? min(e, 0) + max(e - 12, 0) : 0;
+    } else {
+      const unsigned bits = *absmax_bits;
+      shift = bits ? max(int((bits >> 23) & 0xffu) - 127, -114) - 12 : 0;
+    }
+    inv_scale = __uint_as_float(unsigned(127 - shift) << 23);
+    if (blockIdx.x == 0 && threadIdx.x == 0) *scale_out = __uint_as_float(unsigned(127 + shift) << 23);
   }
 #pragma unroll 2
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
@@ -112,7 +164,7 @@ __global__ void prep_kernel(const float* __restrict__ x, const double* __restric
     const size_t o = (((size_t)n * Ho + ho) * Wo + wo) * C_pad + c0;
     if constexpr (kF16) {
 #pragma unroll
-      for (int e = 0; e < 4; ++e) h4[e] = pack_f16x2(y[2 * e], y[2 * e + 1]);
+      for (int e = 0; e < 4; ++e) h4[e] = pack_f16x2(y[2 * e] * inv_scale, y[2 * e + 1] * inv_scale);
       *reinterpret_cast<uint4*>(hi + o) = make_uint4(h4[0], h4[1], h4[2], h4[3]);
     } else {
 #pragma unroll
@@ -195,7 +247,15 @@ constexpr int kVqSplits = 8;   // the codebook is scanned in 8 slices so that 40
 
 // thread = one row of z (held in registers); the block's codebook slice streams through shared memory
 // in tiles of 128 codes (broadcast reads). Every thread visits codes in ascending order, so a strict
-// '<' keeps the first minimal index. Partial (distance, index) per slice go to `part_*`.
+// '<' keeps the first minimal index. Partial (distance, index) per slice go to `part_*`; an empty slice
+// (n_e < 8) reports index -1.
+// Non-finite distances follow np.argmin over the oracle's float32 distances: the first NaN wins, and a row whose
+// distances are all +inf keeps its first code (|z| >~ 1.8e19 overflows sum z^2; a NaN pixel makes every distance
+// NaN). The first code of a slice is therefore always taken, whatever its distance.
+__device__ __forceinline__ bool vq_better(float d, float best_d, int best_i) {
+  return best_i < 0 || (!isnan(best_d) && (isnan(d) || d < best_d));
+}
+
 __global__ void __launch_bounds__(128)
 vq_argmin_partial_kernel(const float* __restrict__ z, const float* __restrict__ emb, float* __restrict__ part_d,
                          int* __restrict__ part_i, int N, int n_e) {
@@ -215,7 +275,7 @@ vq_argmin_partial_kernel(const float* __restrict__ z, const float* __restrict__ 
 #pragma unroll
   for (int d = 0; d < kVqDim; ++d) zz = __fadd_rn(zz, __fmul_rn(zr[d], zr[d]));
   float best_d = INFINITY;
-  int best_i = 0x7fffffff;
+  int best_i = -1;
   for (int c0 = c_begin; c0 < c_end; c0 += 128) {
     __syncthreads();
     {
@@ -248,7 +308,7 @@ vq_argmin_partial_kernel(const float* __restrict__ z, const float* __restrict__ 
         dot = __fadd_rn(dot, __fmul_rn(zr[4 * d4 + 3], e4.w));
       }
       const float dist = __fadd_rn(__fadd_rn(zz, s_ee[j]), -__fmul_rn(2.0f, dot));
-      if (dist < best_d) {
+      if (vq_better(dist, best_d, best_i)) {
         best_d = dist;
         best_i = c0 + j;
       }
@@ -260,7 +320,8 @@ vq_argmin_partial_kernel(const float* __restrict__ z, const float* __restrict__ 
   }
 }
 
-// merge the slices in ascending order (strict '<' => first index), emit idx and the straight-through value
+// merge the slices in ascending order (same rule as within a slice => first index), emit idx and the
+// straight-through value. idx is always in [0, n_e): at least slice 0 is non-empty.
 __global__ void vq_argmin_final_kernel(const float* __restrict__ z, const float* __restrict__ emb,
                                        const float* __restrict__ part_d, const int* __restrict__ part_i,
                                        int* __restrict__ idx, float* __restrict__ zq_st, int N) {
@@ -268,12 +329,13 @@ __global__ void vq_argmin_final_kernel(const float* __restrict__ z, const float*
   const int q = threadIdx.x % 16;
   if (row >= N) return;
   float bd = INFINITY;
-  int bi = 0x7fffffff;
+  int bi = -1;
   for (int s = 0; s < kVqSplits; ++s) {
+    const int i = part_i[(size_t)s * N + row];
     const float d = part_d[(size_t)s * N + row];
-    if (d < bd) {
+    if (i >= 0 && vq_better(d, bd, bi)) {
       bd = d;
-      bi = part_i[(size_t)s * N + row];
+      bi = i;
     }
   }
   if (q == 0) idx[row] = bi;
@@ -337,27 +399,38 @@ extern "C" int lwm_vq_prep(const float* x, const double* gn_stats, const float* 
   const unsigned blocks = unsigned(want < kNumSMs * 32 ? want : kNumSMs * 32);
   prep_kernel<false><<<blocks, threads, gn_stats ? size_t(N) * groups * 8 : 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       x, gn_stats, gamma, beta, reinterpret_cast<__nv_bfloat16*>(hi), reinterpret_cast<__nv_bfloat16*>(lo), N, H, W,
-      C, C_pad, groups, upsample2x ? 1 : 0, eps, lo != nullptr);
+      C, C_pad, groups, upsample2x ? 1 : 0, eps, lo != nullptr, nullptr, nullptr);
   return lwm_check_launch("prep_kernel");
 }
 
-// fp16x2 conv mode: y = [silu(groupnorm(x))] (optionally nearest-2x upsampled) as ONE fp16 plane [N,H',W',C_pad].
+// fp16x2 conv mode: y = [silu(groupnorm(x))] (optionally nearest-2x upsampled) as ONE fp16 plane [N,H',W',C_pad]
+// holding y / *scale_out (prep_kernel). Without GroupNorm the scale comes from x_absmax (|x|max bits): read as given
+// (x_absmax_given, e.g. from lwm_vq_conv2d_f16's absmax_out), or computed into it here.
 extern "C" int lwm_vq_prep_f16(const float* x, const double* gn_stats, const float* gamma, const float* beta, void* out,
-                               int N, int H, int W, int C, int C_pad, int groups, int upsample2x, float eps,
-                               void* stream) {
-  if (!x || !out) return lwm_fail(LWM_ERR_ARG, "vq_prep_f16: null pointer");
+                               float* scale_out, unsigned* x_absmax, int x_absmax_given, int N, int H, int W, int C,
+                               int C_pad, int groups, int upsample2x, float eps, void* stream) {
+  if (!x || !out || !scale_out) return lwm_fail(LWM_ERR_ARG, "vq_prep_f16: null pointer");
+  if (!gn_stats && !x_absmax) return lwm_fail(LWM_ERR_ARG, "vq_prep_f16: the plane without GroupNorm needs x_absmax");
   if (C % 4 || C_pad % 8 || C_pad < C) return lwm_fail(LWM_ERR_SHAPE, "vq_prep_f16: C % 4 and C_pad % 8 required");
   if (gn_stats && (!gamma || !beta || C % groups || (C / groups) % 4))
     return lwm_fail(LWM_ERR_SHAPE, "vq_prep_f16: GroupNorm needs gamma/beta and C/groups % 4 == 0");
   if (gn_stats && (size_t)N * groups * 8 > 40 * 1024) return lwm_fail(LWM_ERR_SHAPE, "vq_prep_f16: N * groups too large (<= 5120)");
   if (!lwm_check_device()) return LWM_ERR_DEVICE;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (!gn_stats && !x_absmax_given) {
+    if (cudaMemsetAsync(x_absmax, 0, 4, st) != cudaSuccess) return lwm_fail(LWM_ERR_CUDA, "vq_prep_f16: memset failed");
+    const long long n4 = (long long)N * H * W * C / 4;
+    const long long want4 = (n4 + 255) / 256;
+    absmax_f32_kernel<<<unsigned(want4 < kNumSMs * 8 ? (want4 > 0 ? want4 : 1) : kNumSMs * 8), 256, 0, st>>>(
+        reinterpret_cast<const uint4*>(x), n4, x_absmax);
+  }
   const size_t total = (size_t)N * (H << upsample2x) * (W << upsample2x) * (C_pad / 8);
   const int threads = 256;
   const size_t want = (total + threads - 1) / threads;
   const unsigned blocks = unsigned(want < kNumSMs * 32 ? want : kNumSMs * 32);
-  prep_kernel<true><<<blocks, threads, gn_stats ? size_t(N) * groups * 8 : 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+  prep_kernel<true><<<blocks, threads, gn_stats ? size_t(N) * groups * 8 : 0, st>>>(
       x, gn_stats, gamma, beta, reinterpret_cast<__nv_bfloat16*>(out), nullptr, N, H, W, C, C_pad, groups,
-      upsample2x ? 1 : 0, eps, 0);
+      upsample2x ? 1 : 0, eps, 0, x_absmax, scale_out);
   return lwm_check_launch("prep_kernel<f16>");
 }
 

@@ -198,9 +198,15 @@ class Ops:
                 st = self.gn_stats(x)
             g, b = gn["scale"], gn["bias"]
         if n_pass == 2:
+            # the plane holds y / s for a power of two s (device float, hi._plane_scale) that keeps it finite and normal
+            # without GroupNorm, |x|max comes from the producing conv's epilogue when it computed one
             hi = torch.empty(N, H * s, W * s, cpad, dtype=torch.float16, device=x.device)
-            _lib.call("lwm_vq_prep_f16", _lib.ptr(x), _lib.ptr(st), _lib.ptr(g), _lib.ptr(b), _lib.ptr(hi), N, H, W, C,
-                      cpad, GN_GROUPS, int(upsample), GN_EPS, _lib.stream_ptr())
+            sc = torch.empty(2, dtype=torch.float32, device=x.device)        # [s, |x|max workspace]
+            amax = getattr(x, "_absmax_bits", None) if gn is None else None
+            _lib.call("lwm_vq_prep_f16", _lib.ptr(x), _lib.ptr(st), _lib.ptr(g), _lib.ptr(b), _lib.ptr(hi), _lib.ptr(sc),
+                      _lib.ptr(sc[1:] if amax is None else amax), int(amax is not None), N, H, W, C, cpad, GN_GROUPS,
+                      int(upsample), GN_EPS, _lib.stream_ptr())
+            hi._plane_scale = sc[:1]
             return hi, None
         hi = torch.empty(N, H * s, W * s, cpad, dtype=torch.bfloat16, device=x.device)
         lo = torch.empty_like(hi) if n_pass == 3 else None
@@ -209,7 +215,8 @@ class Ops:
         return hi, lo
 
     def conv(self, planes, pc, stride=1, residual=None, clip=False, want_stats=False):
-        """want_stats: the output feeds a GroupNorm — have the epilogue accumulate its statistics (fp16x2 mode)."""
+        """want_stats: the output feeds a GroupNorm (or a raw fp16 plane) — have the epilogue accumulate its statistics
+        and its |max| (fp16x2 mode)."""
         hi, lo = planes
         N, Hin, Win, cpad = hi.shape
         assert cpad == pc.cpad, (cpad, pc.cpad)
@@ -218,14 +225,21 @@ class Ops:
         out = torch.empty(N, Ho, Wo, pc.cout, dtype=torch.float32, device=hi.device)
         n_pass = 2 if hi.dtype == torch.float16 else (3 if lo is not None else 1)
         if n_pass == 2:
-            st = None
-            if want_stats and pc.cout % 16 == 0 and pc.cout % GN_GROUPS == 0 and (pc.cout // GN_GROUPS) % 4 == 0:
-                st = torch.zeros(N, GN_GROUPS, 2, dtype=torch.float64, device=hi.device)
-            _lib.call("lwm_vq_conv2d_f16", _lib.ptr(hi), _lib.ptr(pc.w_stack), _lib.ptr(pc.bias), _lib.ptr(residual),
-                      _lib.ptr(out), _lib.ptr(st), N, Hin, Win, cpad, Ho, Wo, pc.cout, pc.cout_pad, pc.k, stride, pad,
+            st = amax = None
+            if want_stats:         # |out|max too: the scale of a raw fp16 plane of this tensor (Downsample, shortcut)
+                # one zero-filled buffer: [N, groups, 2] float64 statistics, then the |max| bit pattern
+                buf = torch.zeros(N * GN_GROUPS * 2 + 1, dtype=torch.float64, device=hi.device)
+                amax = buf[-1:].view(torch.int32)[:1]
+                if pc.cout % 16 == 0 and pc.cout % GN_GROUPS == 0 and (pc.cout // GN_GROUPS) % 4 == 0:
+                    st = buf[:-1].view(N, GN_GROUPS, 2)
+            _lib.call("lwm_vq_conv2d_f16", _lib.ptr(hi), _lib.ptr(getattr(hi, "_plane_scale", None)),
+                      _lib.ptr(pc.w_stack), _lib.ptr(pc.bias), _lib.ptr(residual), _lib.ptr(out), _lib.ptr(st),
+                      _lib.ptr(amax), N, Hin, Win, cpad, Ho, Wo, pc.cout, pc.cout_pad, pc.k, stride, pad,
                       pc.w_scale_inv, GN_GROUPS, int(clip), _lib.stream_ptr())
             if st is not None:
                 out._gn_stats = st
+            if amax is not None:
+                out._absmax_bits = amax
             return out
         _lib.call("lwm_vq_conv2d", _lib.ptr(hi), _lib.ptr(lo), _lib.ptr(pc.w_hi),
                   _lib.ptr(pc.w_lo if n_pass == 3 else None), _lib.ptr(pc.bias), _lib.ptr(residual),

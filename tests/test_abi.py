@@ -16,12 +16,16 @@ def _declared():
     return sorted(set(re.findall(r"\b(lwm_[a-z0-9_]+)\s*\(", src)))
 
 
-def test_library_exports_every_declared_symbol(lib):
+def test_library_exports_every_declared_symbol_and_its_abi_version(lib):
     names = _declared()
     assert len(names) >= 13
     for n in names:
         assert hasattr(lib, n), "liblwm_b200.so does not export %s" % n
-    assert lib.lwm_abi_version() == 2
+    # version 3: lwm_vq_prep_f16 writes a scaled fp16 plane (scale_out, x_absmax) and lwm_vq_conv2d_f16 reads its scale
+    # (a_scale) and can return the output's |max| (absmax_out)
+    src = open(os.path.join(ROOT, "include", "lwm_b200.h")).read()
+    assert re.search(r"#define LWM_B200_ABI_VERSION 3\b", src)
+    assert lib.lwm_abi_version() == 3
 
 
 def test_python_binding_covers_header():

@@ -50,6 +50,11 @@ BAD_CALLS = [
     ("lwm_vq_conv2d", (P, N, P, N, P, N, P, 1, 16, 16, 64, 16, 16, 64, 64, 3, 1, 1, 2, 0, N), ARG, "n_pass"),
     ("lwm_vq_conv2d", (P, N, P, N, P, N, P, 1, 16, 16, 64, 12, 16, 64, 64, 3, 1, 1, 1, 0, N), SHAPE, "8 x 16"),
     ("lwm_vq_conv2d", (P, N, P, N, P, N, P, 1, 16, 16, 64, 16, 16, 64, 64, 5, 1, 2, 1, 0, N), SHAPE, "ksize"),
+    ("lwm_vq_prep_f16", (P, N, N, N, P, N, P, 0, 1, 8, 8, 64, 64, 32, 0, 1e-6, N), ARG, "null pointer"),
+    ("lwm_vq_prep_f16", (P, N, N, N, P, P, N, 0, 1, 8, 8, 64, 64, 32, 0, 1e-6, N), ARG, "x_absmax"),
+    ("lwm_vq_prep_f16", (P, N, N, N, P, P, P, 1, 1, 8, 8, 6, 64, 32, 0, 1e-6, N), SHAPE, "C % 4"),
+    ("lwm_vq_conv2d_f16", (P, P, P, P, N, P, N, N, 1, 16, 16, 64, 16, 16, 64, 64, 3, 1, 1, 0.0, 32, 0, N), ARG, "w_scale_inv"),
+    ("lwm_vq_conv2d_f16", (P, N, P, P, N, P, P, P, 1, 16, 16, 64, 16, 16, 64, 64, 3, 1, 1, 1.0, 32, 0, N), SHAPE, "statistics"),
     ("lwm_vq_conv_cin3", (P, P, P, P, 1, 16, 16, 64, N), SHAPE, "Cout == 128"),
     ("lwm_vq_argmin", (P, P, P, N, P, 16, 8192, 32, N), SHAPE, "e_dim"),
     ("lwm_vq_argmin", (P, P, P, N, N, 16, 8192, 64, N), ARG, "null"),
@@ -75,6 +80,11 @@ GOOD_CALLS = [
     ("lwm_attn_rope", (P, P, 1, P, P, 1, P, P, 1, 8, 2, 2, 128, 0, N)),
     ("lwm_vq_conv2d", (P, P, P, P, P, N, P, 1, 16, 16, 64, 16, 16, 64, 64, 3, 1, 1, 3, 0, N)),
     ("lwm_vq_argmin", (P, P, P, N, P, 16, 8192, 64, N)),
+    ("lwm_vq_prep_f16", (P, N, N, N, P, P, P, 0, 1, 8, 8, 64, 64, 32, 0, 1e-6, N)),
+    ("lwm_vq_prep_f16", (P, N, N, N, P, P, P, 1, 1, 8, 8, 64, 64, 32, 0, 1e-6, N)),
+    ("lwm_vq_prep_f16", (P, P, P, P, P, P, N, 0, 1, 8, 8, 128, 128, 32, 1, 1e-6, N)),
+    ("lwm_vq_conv2d_f16", (P, P, P, P, N, P, P, P, 1, 16, 16, 64, 16, 16, 128, 128, 3, 1, 1, 0.25, 32, 0, N)),
+    ("lwm_vq_conv2d_f16", (P, N, P, P, P, P, N, N, 1, 16, 16, 64, 16, 16, 64, 64, 3, 2, 0, 0.25, 32, 1, N)),
     ("lwm_vq_frame_tokens", (P, N, P, 1, 4, 4, 256, 8192, 8193, N)),
     ("lwm_cast_f32_to_bf16", (P, P, 0, N)),           # even an empty call does not succeed without a device
 ]

@@ -143,6 +143,35 @@ int lwm_attn_decode_partial(const void* q, const void* k, const void* v, const u
                             void* stream);
 int lwm_attn_decode_merge(const float* o_parts, const float* ml_parts, int n_part, void* out, float* lse,
                           long long rows, void* stream);
+/* fp32 inputs / fp32 output: lwm_attn_decode_partial_f32 reads fp32 q, k, v directly (same arguments, same partial
+ * layout); lwm_attn_decode_merge_f32 writes the un-rounded fp32 output. */
+int lwm_attn_decode_partial_f32(const float* q, const float* k, const float* v, const unsigned char* mask,
+                                float* o_part, float* ml_part, void* workspace, int B, int H, int Q, int Sk, int D,
+                                long long k_pos0, long long mask_stride_b, long long mask_stride_q, int splits,
+                                float softmax_scale, void* stream);
+int lwm_attn_decode_merge_f32(const float* o_parts, const float* ml_parts, int n_part, float* out, float* lse,
+                              long long rows, void* stream);
+
+/* Tensor-core inference path (multi-row queries). The mask becomes bits and a per-(b, 128-row Q tile) list of KV tiles:
+ * lwm_attn_mask_pack      mask element (b, q, k) at mask[b*stride_b + q*stride_q + k*stride_k] (uint8/bool, nonzero =
+ *                         attend; stride_b = 0 broadcasts over the batch) -> bits [n_slabs][B][Q][ceil(ncols/128)*4]
+ *                         uint32 for the key columns [col0 + s*ncols, col0 + (s+1)*ncols) of slab s (bit j of word w
+ *                         <=> column 32w + j; zero padded), and row_any [B][Q] int32 = the row has a true entry.
+ * lwm_attn_infer_tilemap  bits [B][Q][ceil(Sk/128)*4] (null: every key visible), row_any [B][Q] over ALL keys of the
+ *                         ring (null: no row is fully masked) -> tiles [B][ceil(Q/128)][ceil(Sk/128)] (kt*2 + mixed)
+ *                         and tile_count [B][ceil(Q/128)].
+ * lwm_attn_infer_partial  q16 [B,Q,H,128], k16/v16 [B,Sk,H,128] power-of-two-scaled fp16 copies (lwm_attn_to_f16_scaled)
+ *                         with their device scales; fp32 logits, softmax and accumulation on the tensor cores. Writes
+ *                         the decode partial layout o_part [B*Q*H,128], ml_part [B*Q*H,2]; splits > 1 CTAs per Q tile
+ *                         need workspace >= splits * B*Q*H * 130 floats. Keys >= Sk enter no sum. */
+int lwm_attn_mask_pack(const unsigned char* mask, long long stride_b, long long stride_q, long long stride_k, int B,
+                       int Q, long long col0, int ncols, int n_slabs, unsigned* bits, int* row_any, void* stream);
+int lwm_attn_infer_tilemap(const unsigned* bits, const int* row_any, int B, int Q, int Sk, int* tiles, int* tile_count,
+                           void* stream);
+int lwm_attn_infer_partial(const void* q16, const void* k16, const void* v16, const float* scale_q,
+                           const float* scale_k, const float* scale_v, const unsigned* bits, const int* tiles,
+                           const int* tile_count, float* o_part, float* ml_part, void* workspace, int B, int H, int Q,
+                           int Sk, int D, int splits, float softmax_scale, void* stream);
 
 /* Attention prologue: rotary position embedding (lwm/llama.py:344-375 precompute_freqs_cis / apply_rotary_emb, applied
  * at llama.py:517-519 on the head-split projections right before the ring-attention call; SURVEY.md §8f next-row 2).

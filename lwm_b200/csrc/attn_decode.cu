@@ -8,53 +8,70 @@
 // (log-sum-exp weights) after one tiny all-gather. No tensor cores: the GEMV has 1 FLOP per byte.
 //   decode_partial_kernel  grid (splits, H, B*Q): warp = one key at a time per lane-quad layout:
 //                          lane l owns dims [4l, 4l+4) of q, k, v rows (one coalesced 256 B row per load)
-//   decode_merge_kernel    merges `n_part` partials per (b, q, h): used for the key splits and, after the
-//                          all-gather, for the ranks.
+//                          bf16 or fp32 rows (one uint2 / float4 per lane and row). Below INFER_MIN_Q query
+//                          rows only; longer queries go to the tensor-core inference mode of attn_fwd_kernel.
+//   decode_merge_kernel    merges `n_part` partials per (b, q, h): used for the key splits (of both kernels) and,
+//                          after the exchange, for the ranks; writes bf16 or fp32.
 #include "attn_common.cuh"
 #include "capi_internal.h"
+
+#include <type_traits>
 
 namespace lwm {
 
 constexpr int kDecWarps = 4;
 
+template <typename T>
 __global__ void __launch_bounds__(kDecWarps * 32)
-decode_partial_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
-                      const __nv_bfloat16* __restrict__ v, const unsigned char* __restrict__ mask,
+decode_partial_kernel(const T* __restrict__ q, const T* __restrict__ k,
+                      const T* __restrict__ v, const unsigned char* __restrict__ mask,
                       float* __restrict__ o_part, float* __restrict__ ml_part, int B, int H, int Q, int Sk,
                       long long k_pos0, long long mask_stride_b, long long mask_stride_q, int splits,
                       float scale_log2) {
+  constexpr bool kF32 = std::is_same<T, float>::value;   // fp32 rows: one float4 per lane, bf16 rows: one uint2
+  using Raw = typename std::conditional<kF32, float4, uint2>::type;
   const int split = blockIdx.x, h = blockIdx.y;
   const int b = blockIdx.z / Q, qi = blockIdx.z % Q;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int per = (Sk + splits - 1) / splits;
   const int k_begin = split * per, k_end = min(Sk, k_begin + per);
 
-  const uint2 qraw = reinterpret_cast<const uint2*>(q + (((size_t)b * Q + qi) * H + h) * kHeadDim)[lane];
-  const __nv_bfloat162 q01 = *reinterpret_cast<const __nv_bfloat162*>(&qraw.x);
-  const __nv_bfloat162 q23 = *reinterpret_cast<const __nv_bfloat162*>(&qraw.y);
-  const float q0 = __low2float(q01) * scale_log2, q1 = __high2float(q01) * scale_log2;
-  const float q2 = __low2float(q23) * scale_log2, q3 = __high2float(q23) * scale_log2;
+  float q0, q1, q2, q3;
+  if constexpr (kF32) {
+    const float4 qf = reinterpret_cast<const float4*>(q + (((size_t)b * Q + qi) * H + h) * kHeadDim)[lane];
+    q0 = qf.x * scale_log2; q1 = qf.y * scale_log2; q2 = qf.z * scale_log2; q3 = qf.w * scale_log2;
+  } else {
+    const uint2 qraw = reinterpret_cast<const uint2*>(q + (((size_t)b * Q + qi) * H + h) * kHeadDim)[lane];
+    const __nv_bfloat162 q01 = *reinterpret_cast<const __nv_bfloat162*>(&qraw.x);
+    const __nv_bfloat162 q23 = *reinterpret_cast<const __nv_bfloat162*>(&qraw.y);
+    q0 = __low2float(q01) * scale_log2; q1 = __high2float(q01) * scale_log2;
+    q2 = __low2float(q23) * scale_log2; q3 = __high2float(q23) * scale_log2;
+  }
   const unsigned char* mrow = mask ? mask + (size_t)b * mask_stride_b + (size_t)qi * mask_stride_q + k_pos0 : nullptr;
 
   float m = -INFINITY, l = 0.f, a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
   const size_t row_stride = (size_t)H * kHeadDim;   // elements between consecutive keys of one head
-  const __nv_bfloat16* kb = k + ((size_t)b * Sk) * row_stride + (size_t)h * kHeadDim;
-  const __nv_bfloat16* vb = v + ((size_t)b * Sk) * row_stride + (size_t)h * kHeadDim;
+  const T* kb = k + ((size_t)b * Sk) * row_stride + (size_t)h * kHeadDim;
+  const T* vb = v + ((size_t)b * Sk) * row_stride + (size_t)h * kHeadDim;
   // each warp strides over the CTA's key range, 4 keys in flight per iteration
   for (int j0 = k_begin + warp * 4; j0 < k_end; j0 += kDecWarps * 4) {
     float s[4];
-    uint2 vr[4];
+    Raw vr[4];
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
       const int j = j0 + u;
       float part = 0.f;
-      vr[u] = make_uint2(0, 0);
+      vr[u] = Raw{};
       if (j < k_end) {
-        const uint2 kr = reinterpret_cast<const uint2*>(kb + (size_t)j * row_stride)[lane];
-        vr[u] = reinterpret_cast<const uint2*>(vb + (size_t)j * row_stride)[lane];
-        const __nv_bfloat162 k01 = *reinterpret_cast<const __nv_bfloat162*>(&kr.x);
-        const __nv_bfloat162 k23 = *reinterpret_cast<const __nv_bfloat162*>(&kr.y);
-        part = q0 * __low2float(k01) + q1 * __high2float(k01) + q2 * __low2float(k23) + q3 * __high2float(k23);
+        const Raw kr = reinterpret_cast<const Raw*>(kb + (size_t)j * row_stride)[lane];
+        vr[u] = reinterpret_cast<const Raw*>(vb + (size_t)j * row_stride)[lane];
+        if constexpr (kF32) {
+          part = q0 * kr.x + q1 * kr.y + q2 * kr.z + q3 * kr.w;
+        } else {
+          const __nv_bfloat162 k01 = *reinterpret_cast<const __nv_bfloat162*>(&kr.x);
+          const __nv_bfloat162 k23 = *reinterpret_cast<const __nv_bfloat162*>(&kr.y);
+          part = q0 * __low2float(k01) + q1 * __high2float(k01) + q2 * __low2float(k23) + q3 * __high2float(k23);
+        }
       }
       s[u] = part;
     }
@@ -71,13 +88,19 @@ decode_partial_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* 
         if (mrow && !mrow[j]) t = kMaskedLogit;
         const float m_new = fmaxf(m, t);
         const float c = ex2f(m - m_new), p = ex2f(t - m_new);
-        const __nv_bfloat162 v01 = *reinterpret_cast<const __nv_bfloat162*>(&vr[u].x);
-        const __nv_bfloat162 v23 = *reinterpret_cast<const __nv_bfloat162*>(&vr[u].y);
+        float4 vf;
+        if constexpr (kF32) {
+          vf = vr[u];
+        } else {
+          const __nv_bfloat162 v01 = *reinterpret_cast<const __nv_bfloat162*>(&vr[u].x);
+          const __nv_bfloat162 v23 = *reinterpret_cast<const __nv_bfloat162*>(&vr[u].y);
+          vf = make_float4(__low2float(v01), __high2float(v01), __low2float(v23), __high2float(v23));
+        }
         l = l * c + p;
-        a0 = a0 * c + p * __low2float(v01);
-        a1 = a1 * c + p * __high2float(v01);
-        a2 = a2 * c + p * __low2float(v23);
-        a3 = a3 * c + p * __high2float(v23);
+        a0 = a0 * c + p * vf.x;
+        a1 = a1 * c + p * vf.y;
+        a2 = a2 * c + p * vf.z;
+        a3 = a3 * c + p * vf.w;
         m = m_new;
       }
     }
@@ -112,9 +135,11 @@ decode_partial_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* 
 }
 
 // partials: o_part [rows][n_part][128] (un-normalised numerators), ml_part [rows][n_part][2] (max in log2 domain,
-// denominator). normalise != 0: write out (bf16) = num/den and lse (natural log); else write one merged partial.
+// denominator). out != null: write out = num/den (bf16, or fp32 when kF32Out) and lse (natural log); else write one
+// merged partial. The layout is the one decode_partial_kernel's splits and attn_fwd_kernel's inference mode write.
+template <bool kF32Out>
 __global__ void decode_merge_kernel(const float* __restrict__ o_part, const float* __restrict__ ml_part, int n_part,
-                                    __nv_bfloat16* __restrict__ out, float* __restrict__ lse,
+                                    void* __restrict__ out, float* __restrict__ lse,
                                     float* __restrict__ o_merged, float* __restrict__ ml_merged, long long rows) {
   const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= rows) return;
@@ -132,8 +157,12 @@ __global__ void decode_merge_kernel(const float* __restrict__ o_part, const floa
   }
   if (out) {
     const float inv = ll > 0.f ? 1.0f / ll : 0.f;
-    *reinterpret_cast<uint2*>(out + row * kHeadDim + lane * 4) =
-        make_uint2(pack_bf16x2(acc.x * inv, acc.y * inv), pack_bf16x2(acc.z * inv, acc.w * inv));
+    if constexpr (kF32Out)
+      *reinterpret_cast<float4*>(reinterpret_cast<float*>(out) + row * kHeadDim + lane * 4) =
+          make_float4(acc.x * inv, acc.y * inv, acc.z * inv, acc.w * inv);
+    else
+      *reinterpret_cast<uint2*>(reinterpret_cast<__nv_bfloat16*>(out) + row * kHeadDim + lane * 4) =
+          make_uint2(pack_bf16x2(acc.x * inv, acc.y * inv), pack_bf16x2(acc.z * inv, acc.w * inv));
     if (lse && lane == 0) lse[row] = ll > 0.f ? (mm + log2f(ll)) * kLn2 : -INFINITY;
   } else {
     *reinterpret_cast<float4*>(o_merged + row * kHeadDim + lane * 4) = acc;
@@ -148,14 +177,18 @@ __global__ void decode_merge_kernel(const float* __restrict__ o_part, const floa
 
 using namespace lwm;
 
-// q [B,Q,H,128] bf16 ; k,v [B,Sk,H,128] bf16 (this rank's KV shard) ; mask uint8 [B, ., Q, .] addressed as
-// mask[b*mask_stride_b + q*mask_stride_q + k_pos0 + j] (nonzero = attend) or NULL ;
-// o_part [B*Q*H, 128] fp32 + ml_part [B*Q*H, 2] fp32 : this rank's partial (numerator, (max_log2, denominator));
-// workspace: splits * B*Q*H * (128 + 2) floats.
-extern "C" int lwm_attn_decode_partial(const void* q, const void* k, const void* v, const unsigned char* mask,
-                                       float* o_part, float* ml_part, void* workspace, int B, int H, int Q, int Sk,
-                                       int D, long long k_pos0, long long mask_stride_b, long long mask_stride_q,
-                                       int splits, float softmax_scale, void* stream) {
+// merge n_part partials per row into one partial (o_merged, ml_merged); shared with attn_fwd.cu's inference mode.
+void lwm_decode_merge_partials(const float* o_parts, const float* ml_parts, int n_part, float* o_merged,
+                               float* ml_merged, long long rows, cudaStream_t st) {
+  decode_merge_kernel<false><<<unsigned((rows + 3) / 4), 128, 0, st>>>(o_parts, ml_parts, n_part, nullptr, nullptr,
+                                                                       o_merged, ml_merged, rows);
+}
+
+template <typename T>
+static int decode_partial_launch(const void* q, const void* k, const void* v, const unsigned char* mask,
+                                 float* o_part, float* ml_part, void* workspace, int B, int H, int Q, int Sk, int D,
+                                 long long k_pos0, long long mask_stride_b, long long mask_stride_q, int splits,
+                                 float softmax_scale, void* stream) {
   if (D != kHeadDim) return lwm_fail(LWM_ERR_SHAPE, "attn_decode: head_dim must be 128");
   if (!q || !k || !v || !o_part || !ml_part || !workspace) return lwm_fail(LWM_ERR_ARG, "attn_decode: null pointer");
   if (B <= 0 || H <= 0 || Q <= 0 || Sk <= 0 || splits <= 0 || (long long)B * Q > 65535)
@@ -166,13 +199,32 @@ extern "C" int lwm_attn_decode_partial(const void* q, const void* k, const void*
   float* ws_o = reinterpret_cast<float*>(workspace);
   float* ws_ml = ws_o + rows * splits * kHeadDim;
   dim3 grid(splits, H, B * Q);
-  decode_partial_kernel<<<grid, kDecWarps * 32, 0, st>>>(
-      reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(k),
-      reinterpret_cast<const __nv_bfloat16*>(v), mask, ws_o, ws_ml, B, H, Q, Sk, k_pos0, mask_stride_b, mask_stride_q,
-      splits, softmax_scale * kLog2e);
-  decode_merge_kernel<<<unsigned((rows + 3) / 4), 128, 0, st>>>(ws_o, ws_ml, splits, nullptr, nullptr, o_part, ml_part,
-                                                                rows);
+  decode_partial_kernel<T><<<grid, kDecWarps * 32, 0, st>>>(
+      reinterpret_cast<const T*>(q), reinterpret_cast<const T*>(k), reinterpret_cast<const T*>(v), mask, ws_o, ws_ml,
+      B, H, Q, Sk, k_pos0, mask_stride_b, mask_stride_q, splits, softmax_scale * kLog2e);
+  lwm_decode_merge_partials(ws_o, ws_ml, splits, o_part, ml_part, rows, st);
   return lwm_check_launch("attn_decode kernels");
+}
+
+// q [B,Q,H,128] bf16 ; k,v [B,Sk,H,128] bf16 (this rank's KV shard) ; mask uint8 [B, ., Q, .] addressed as
+// mask[b*mask_stride_b + q*mask_stride_q + k_pos0 + j] (nonzero = attend) or NULL ;
+// o_part [B*Q*H, 128] fp32 + ml_part [B*Q*H, 2] fp32 : this rank's partial (numerator, (max_log2, denominator));
+// workspace: splits * B*Q*H * (128 + 2) floats.
+extern "C" int lwm_attn_decode_partial(const void* q, const void* k, const void* v, const unsigned char* mask,
+                                       float* o_part, float* ml_part, void* workspace, int B, int H, int Q, int Sk,
+                                       int D, long long k_pos0, long long mask_stride_b, long long mask_stride_q,
+                                       int splits, float softmax_scale, void* stream) {
+  return decode_partial_launch<__nv_bfloat16>(q, k, v, mask, o_part, ml_part, workspace, B, H, Q, Sk, D, k_pos0,
+                                              mask_stride_b, mask_stride_q, splits, softmax_scale, stream);
+}
+
+// the same with fp32 q, k, v (read directly: one float4 per lane and row)
+extern "C" int lwm_attn_decode_partial_f32(const float* q, const float* k, const float* v, const unsigned char* mask,
+                                           float* o_part, float* ml_part, void* workspace, int B, int H, int Q, int Sk,
+                                           int D, long long k_pos0, long long mask_stride_b, long long mask_stride_q,
+                                           int splits, float softmax_scale, void* stream) {
+  return decode_partial_launch<float>(q, k, v, mask, o_part, ml_part, workspace, B, H, Q, Sk, D, k_pos0,
+                                      mask_stride_b, mask_stride_q, splits, softmax_scale, stream);
 }
 
 // merge n_part partials per row (e.g. the all-gathered per-rank partials) into out (bf16) and lse.
@@ -180,7 +232,18 @@ extern "C" int lwm_attn_decode_merge(const float* o_parts, const float* ml_parts
                                      long long rows, void* stream) {
   if (!o_parts || !ml_parts || !out || n_part <= 0 || rows <= 0) return lwm_fail(LWM_ERR_ARG, "attn_decode_merge: bad args");
   if (!lwm_check_device()) return LWM_ERR_DEVICE;
-  decode_merge_kernel<<<unsigned((rows + 3) / 4), 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      o_parts, ml_parts, n_part, reinterpret_cast<__nv_bfloat16*>(out), lse, nullptr, nullptr, rows);
+  decode_merge_kernel<false><<<unsigned((rows + 3) / 4), 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      o_parts, ml_parts, n_part, out, lse, nullptr, nullptr, rows);
+  return lwm_check_launch("decode_merge_kernel");
+}
+
+// the same, writing the un-rounded fp32 output
+extern "C" int lwm_attn_decode_merge_f32(const float* o_parts, const float* ml_parts, int n_part, float* out,
+                                         float* lse, long long rows, void* stream) {
+  if (!o_parts || !ml_parts || !out || n_part <= 0 || rows <= 0)
+    return lwm_fail(LWM_ERR_ARG, "attn_decode_merge_f32: bad args");
+  if (!lwm_check_device()) return LWM_ERR_DEVICE;
+  decode_merge_kernel<true><<<unsigned((rows + 3) / 4), 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      o_parts, ml_parts, n_part, out, lse, nullptr, nullptr, rows);
   return lwm_check_launch("decode_merge_kernel");
 }

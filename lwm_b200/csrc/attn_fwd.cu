@@ -35,6 +35,13 @@ struct FwdParams {
   float* acc_l;        // [B,H,Sq]     running denominator
   int first, last;
   const float *scale_q, *scale_k, *scale_v;   // fp16 mode: device scalars, x = x16 * scale; null => bf16 operands
+  // inference mode only (ringattention_inference, Sq = Q rows, any Q and Sk): the (b, Q tile) lists of KV tiles
+  const uint32_t* bits;   // [B, Sq, n_kt * 4] mask bits (bit j of word w <=> key 32 w + j; 1 = attend) or null
+  const int* tiles;       // [B, ceil(Sq/128), n_kt]: kt * 2 + mixed, ascending kt
+  const int* tile_count;  // [B, ceil(Sq/128)]
+  int n_kt, splits;       // KV tiles of the shard; CTAs per Q tile, each takes a contiguous slice of the list
+  float* o_part;          // [B*Sq*H, splits, 128] un-normalised numerators (in V's units)
+  float* ml_part;         // [B*Sq*H, splits, 2] (max in the log2 domain, denominator)
 };
 
 constexpr int kFwdStages = 4;
@@ -66,7 +73,10 @@ LWM_DEVICE float quad_sum(float x) {
 
 // kF16: operands are IEEE fp16 (exact, scaled copies of the bf16 inputs) and P is kept in fp16
 // (11 significant bits instead of 8) — the precision mode that meets 1e-3 on white-noise inputs.
-template <bool kF16>
+// kInfer: the inference mode. A CTA walks its slice of its Q tile's KV tile list (built from a bit mask by
+// attn_infer.cu); only tiles marked mixed read mask bits, keys >= Sk get -inf, rows >= Sq are padding. The epilogue
+// writes the CTA's un-normalised partial for decode_merge_kernel instead of a carry.
+template <bool kF16, bool kInfer = false>
 __global__ void __launch_bounds__(kFwdThreads, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const FwdParams p) {
@@ -78,14 +88,23 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int n_q_tiles = p.Sq / kTile;
-  const int tile = n_q_tiles - 1 - int(blockIdx.x);  // heaviest (latest rows) first under causal masking
+  const int n_q_tiles = kInfer ? (p.Sq + kTile - 1) / kTile : p.Sq / kTile;
+  // heaviest (latest rows) first under causal masking
+  const int tile = n_q_tiles - 1 - int(kInfer ? blockIdx.x / p.splits : blockIdx.x);
   const int h = blockIdx.y, b = blockIdx.z;
   const int m0 = tile * kTile;
 
   // number of KV tiles any row of this CTA can see
   int n_kv = p.Sk / kTile;
-  if (p.mask.causal) {
+  const int* list = nullptr;   // kInfer: this CTA's slice of the tile list
+  if constexpr (kInfer) {
+    const long long lt = (long long)b * n_q_tiles + tile;
+    const int cnt = p.tile_count[lt];
+    const int per = (cnt + p.splits - 1) / p.splits;
+    const int beg = min(cnt, int(blockIdx.x % p.splits) * per);
+    n_kv = min(cnt, beg + per) - beg;
+    list = p.tiles + lt * p.n_kt + beg;
+  } else if (p.mask.causal) {
     const long long last_q = (long long)p.mask.q_pos0 + m0 + kTile - 1;
     const long long vis = last_q - p.mask.k_pos0;  // largest visible local key index
     n_kv = vis < 0 ? 0 : min((long long)n_kv, vis / kTile + 1);
@@ -114,7 +133,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         const int slot = i % kFwdStages;
         const uint32_t ph = (i / kFwdStages) & 1;
         mbar_wait(&bars.kv_empty[slot], ph ^ 1);
-        load_tile(sKV + slot * kFwdTileBytes, (i & 1) ? &tmV : &tmK, &bars.kv_full[slot], h, (i >> 1) * kTile, b);
+        const int kt = kInfer ? (list[i >> 1] >> 1) : (i >> 1);
+        load_tile(sKV + slot * kFwdTileBytes, (i & 1) ? &tmV : &tmK, &bars.kv_full[slot], h, kt * kTile, b);
       }
     }
     return;
@@ -177,15 +197,45 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     };
     // online softmax of tile j on the fragment: row max, alpha, m_run / l_run update, s <- exp2(s * scale - m)
     auto softmax = [&](int j) {
-      const int k_tile_pos = p.mask.k_pos0 + j * kTile;
-      // warp-uniform: does any row of this warp need a mask on this KV tile?
-      const bool need_mask = has_bias || has_seg || (p.mask.causal && (k_tile_pos + kTile - 1 > warp_q_pos0));
+      int k_tile_pos;
+      bool need_mask;   // warp-uniform: does any row of this warp need a mask on this KV tile?
+      if constexpr (kInfer) {
+        const int e = list[j];
+        k_tile_pos = (e >> 1) * kTile;
+        need_mask = e & 1;
+      } else {
+        k_tile_pos = p.mask.k_pos0 + j * kTile;
+        need_mask = has_bias || has_seg || (p.mask.causal && (k_tile_pos + kTile - 1 > warp_q_pos0));
+      }
       float mx[2] = {-INFINITY, -INFINITY};
       if (!need_mask) {
 #pragma unroll
         for (int i = 0; i < 64; ++i) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], s[i]);
         mx[0] = quad_max(mx[0]) * scale;
         mx[1] = quad_max(mx[1]) * scale;
+      } else if constexpr (kInfer) {
+        // this thread's two rows: 4 mask words each (the tile's 128 keys); padding rows read none (all visible)
+        uint32_t mw[2][4];
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int row = r0 + 8 * hh;
+          uint4 w4 = make_uint4(~0u, ~0u, ~0u, ~0u);
+          if (p.bits && row < p.Sq)
+            w4 = *reinterpret_cast<const uint4*>(p.bits + ((long long)b * p.Sq + row) * (p.n_kt * 4) + k_tile_pos / 32);
+          mw[hh][0] = w4.x; mw[hh][1] = w4.y; mw[hh][2] = w4.z; mw[hh][3] = w4.w;
+        }
+#pragma unroll
+        for (int i = 0; i < 64; ++i) {
+          const int hh = (i >> 1) & 1;
+          const int col = (i >> 2) * 8 + quad * 2 + (i & 1);   // col >> 5 == i >> 4
+          float tv = s[i] * scale;
+          if (!((mw[hh][i >> 4] >> (col & 31)) & 1u)) tv = kMaskedLogit;
+          if (k_tile_pos + col >= p.Sk) tv = -INFINITY;       // past the cache: in no sum, not even a masked one
+          s[i] = tv;
+          mx[hh] = fmaxf(mx[hh], tv);
+        }
+        mx[0] = quad_max(mx[0]);
+        mx[1] = quad_max(mx[1]);
       } else {
         // per-row mask inputs, reloaded per masked tile (L1 hits) rather than held in registers across the loop
         const float* bias_row = has_bias ? p.mask.bias + (long long)b * p.mask.bias_stride : nullptr;
@@ -286,6 +336,29 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     release(2 * n_kv - 1);
   }
 
+  if constexpr (kInfer) {
+    // ---------------------------------------------------------------- epilogue: this CTA's partial
+    const int split = blockIdx.x % p.splits;
+    const float l_rows[2] = {quad_sum(l_run[0]), quad_sum(l_run[1])};
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int q_row = r0 + 8 * hh;
+      const float l_run_row = l_rows[hh];
+      if (q_row >= p.Sq) continue;
+      const long long pidx = (((long long)b * p.Sq + q_row) * p.H + h) * p.splits + split;
+      const float wv = *p.scale_v;   // V was stored as v16 * scale_v
+#pragma unroll
+      for (int g = 0; g < kHeadDim / 8; ++g) {
+        const int c = g * 8 + quad * 2;
+        *reinterpret_cast<float2*>(p.o_part + pidx * kHeadDim + c) =
+            make_float2(o[4 * g + 2 * hh] * wv, o[4 * g + 2 * hh + 1] * wv);
+      }
+      if (quad == 0) {
+        p.ml_part[pidx * 2] = m_run[hh];
+        p.ml_part[pidx * 2 + 1] = l_run_row;
+      }
+    }
+  } else {
   // ---------------------------------------------------------------- epilogue: merge carry, write
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
@@ -332,6 +405,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         p.acc_l[ml_idx] = l_new;
       }
     }
+  }
   }
 }
 
@@ -421,4 +495,52 @@ extern "C" int lwm_attn_fwd_step_f16(const void* q16, const void* k16, const voi
   return attn_fwd_launch(q16, k16, v16, out, lse, acc_o, acc_m, acc_l, B, H, Sq, Sk, D, q_pos0, k_pos0, causal, bias,
                          bias_stride, segment_ids, seg_stride, softmax_scale, first, last, scale_q, scale_k, scale_v,
                          out_f32, stream);
+}
+
+// Inference mode (ringattention_inference with Q >= kInferMinQ rows): q16 [B,Q,H,128], k16/v16 [B,Sk,H,128] scaled fp16
+// copies, any Q and Sk; bits / tiles / tile_count from lwm_attn_mask_pack + lwm_attn_infer_tilemap. Writes one
+// partial per (b, q, h) row: o_part [B*Q*H,128], ml_part [B*Q*H,2] (the decode partial layout). splits > 1: CTAs per
+// Q tile, each over a slice of its tile list; their partials go through workspace (splits * B*Q*H * 130 floats) and
+// are merged here.
+extern "C" int lwm_attn_infer_partial(const void* q16, const void* k16, const void* v16, const float* scale_q,
+                                      const float* scale_k, const float* scale_v, const unsigned* bits,
+                                      const int* tiles, const int* tile_count, float* o_part, float* ml_part,
+                                      void* workspace, int B, int H, int Q, int Sk, int D, int splits,
+                                      float softmax_scale, void* stream) {
+  if (D != kHeadDim) return lwm_fail(LWM_ERR_SHAPE, "attn_infer_partial: head_dim must be 128");
+  if (!q16 || !k16 || !v16 || !scale_q || !scale_k || !scale_v || !tiles || !tile_count || !o_part || !ml_part)
+    return lwm_fail(LWM_ERR_ARG, "attn_infer_partial: null pointer");
+  if (splits > 1 && !workspace) return lwm_fail(LWM_ERR_ARG, "attn_infer_partial: workspace required when splits > 1");
+  if (B <= 0 || H <= 0 || Q <= 0 || Sk <= 0 || B > 65535 || H > 65535 || splits <= 0 || splits > 1024)
+    return lwm_fail(LWM_ERR_SHAPE, "attn_infer_partial: bad shape (B, H <= 65535; 1 <= splits <= 1024)");
+  if (!lwm_check_device()) return LWM_ERR_DEVICE;
+  CUtensorMap tq, tk, tv;
+  if (!make_qkv_tmap(&tq, q16, B, Q, H) || !make_qkv_tmap(&tk, k16, B, Sk, H) || !make_qkv_tmap(&tv, v16, B, Sk, H))
+    return lwm_fail(LWM_ERR_CUDA, "attn_infer_partial: cuTensorMapEncodeTiled failed (pointers must be 16B aligned)");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const long long rows = (long long)B * Q * H;
+  FwdParams p{};
+  p.B = B; p.H = H; p.Sq = Q; p.Sk = Sk;
+  p.scale_log2 = softmax_scale * kLog2e;
+  p.first = 1; p.last = 0;
+  p.scale_q = scale_q; p.scale_k = scale_k; p.scale_v = scale_v;
+  p.bits = bits; p.tiles = tiles; p.tile_count = tile_count;
+  p.n_kt = (Sk + kTile - 1) / kTile;
+  p.splits = splits;
+  p.o_part = splits > 1 ? reinterpret_cast<float*>(workspace) : o_part;
+  p.ml_part = splits > 1 ? reinterpret_cast<float*>(workspace) + rows * splits * kHeadDim : ml_part;
+  static bool attr_set_dev[64] = {};
+  int cur_dev = 0;
+  cudaGetDevice(&cur_dev);
+  bool& attr_set = attr_set_dev[cur_dev & 63];
+  if (!attr_set) {
+    if (cudaFuncSetAttribute(attn_fwd_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             kFwdSmemBytes) != cudaSuccess)
+      return lwm_fail(LWM_ERR_CUDA, "attn_infer_partial: cannot raise dynamic shared memory limit");
+    attr_set = true;
+  }
+  dim3 grid(unsigned((Q + kTile - 1) / kTile * splits), H, B);
+  attn_fwd_kernel<true, true><<<grid, kFwdThreads, kFwdSmemBytes, st>>>(tq, tk, tv, p);
+  if (splits > 1) lwm_decode_merge_partials(p.o_part, p.ml_part, splits, o_part, ml_part, rows, st);
+  return lwm_check_launch("attn_fwd_kernel (inference)");
 }

@@ -547,10 +547,23 @@ def ring_backward(res, k, v, dout, bias, seg, causal, group, rank, world, layout
 
 
 # ------------------------------------------------------------------------------------------------
-# decode path: ringattention_inference (lwm/llama.py:601-614)
+# inference path: ringattention_inference (lwm/llama.py:601-614)
 # ------------------------------------------------------------------------------------------------
+# Query rows at which the tensor-core kernel (attn_fwd_kernel's inference mode) takes over from the GEMV kernel, which
+# streams K/V once per query row. From tools/perf_infer.py (H100, H = 32): at K = 131072 the tensor-core path is faster
+# from Q = 8 in fp32 and bf16 (bf16 Q = 4: 3.6 vs 3.1 ms); with short caches the GEMV kernel stays ahead up to
+# Q = 64, by at most 0.15 ms per call.
+INFER_MIN_Q = 8
+
+
+def _check_infer_dtypes(q, k, v):
+    if not (q.dtype == k.dtype == v.dtype and q.dtype in (torch.bfloat16, torch.float32)):
+        raise TypeError("ringattention_inference: q, k, v must all be bfloat16 or all float32")
+
+
 def decode_partial(q, k, v, mask_u8, k_pos0, stream=None):
-    """This rank's partial over its KV shard -> (o_part [B*Q*H,128] fp32, ml_part [B*Q*H,2] fp32)."""
+    """This rank's partial over its KV shard with the GEMV kernel (bf16 or fp32 q/k/v, read as they are)
+    -> (o_part [B*Q*H,128] fp32, ml_part [B*Q*H,2] fp32)."""
     B, Q, H, D = q.shape
     Sk = k.shape[1]
     rows = B * Q * H
@@ -561,38 +574,179 @@ def decode_partial(q, k, v, mask_u8, k_pos0, stream=None):
     sb = sq = 0
     if mask_u8 is not None:
         sb, sq = mask_u8.stride(0), mask_u8.stride(-2)
-    _lib.call("lwm_attn_decode_partial", _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(mask_u8), _lib.ptr(o_part),
+    fn = "lwm_attn_decode_partial_f32" if q.dtype == torch.float32 else "lwm_attn_decode_partial"
+    _lib.call(fn, _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(mask_u8), _lib.ptr(o_part),
               _lib.ptr(ml_part), _lib.ptr(ws), B, H, Q, Sk, D, int(k_pos0), int(sb), int(sq), splits,
               1.0 / math.sqrt(D), _lib.stream_ptr(stream))
     return o_part, ml_part
 
 
+def decode_merge(o_parts, ml_parts, n_part, out_shape, dtype):
+    """merge n_part partials per row ([rows][n_part][128], [rows][n_part][2]) into the normalised output"""
+    out = torch.empty(out_shape, dtype=dtype, device=o_parts.device)
+    rows = o_parts.shape[0]
+    lse = torch.empty(rows, dtype=torch.float32, device=o_parts.device)
+    fn = "lwm_attn_decode_merge_f32" if dtype == torch.float32 else "lwm_attn_decode_merge"
+    _lib.call(fn, _lib.ptr(o_parts), _lib.ptr(ml_parts), n_part, _lib.ptr(out), _lib.ptr(lse), rows,
+              _lib.stream_ptr())
+    return out
+
+
+def mask_pack(mask, B, n_slabs, ncols):
+    """bool/uint8 mask [Bm,1,Q,K] (Bm in {1, B}; read through its strides) -> (bits [n_slabs,B,Q,kw] int32 for the
+    key columns [s*ncols, (s+1)*ncols) of slab s, row_any [B,Q] int32)."""
+    Q = mask.shape[2]
+    m = mask.view(torch.uint8) if mask.dtype == torch.bool else mask
+    if m.dtype != torch.uint8:
+        m = (m != 0).view(torch.uint8)
+    kw = (ncols + 127) // 128 * 4
+    bits = torch.empty(n_slabs, B, Q, kw, dtype=torch.int32, device=m.device)
+    row_any = torch.empty(B, Q, dtype=torch.int32, device=m.device)
+    sb = m.stride(0) if m.shape[0] > 1 else 0
+    _lib.call("lwm_attn_mask_pack", _lib.ptr(m), sb, m.stride(2), m.stride(3), B, Q, 0, ncols, n_slabs,
+              _lib.ptr(bits), _lib.ptr(row_any), _lib.stream_ptr())
+    return bits, row_any
+
+
+def _scaled_f16(x):
+    scale = torch.empty(1, dtype=torch.float32, device=x.device)
+    PeerOpsF16.scale_of(x, scale)
+    return _stage_local(PeerOpsF16, x, scale), scale
+
+
+def infer_partial(q, k, v, bits, row_any):
+    """This rank's partial with the tensor-core kernel: q [B,Q,H,128] against k/v [B,Sk,H,128] (bf16 or fp32, staged
+    to scaled fp16 here), bits [B,Q,kw] / row_any [B,Q] (row_any over the whole ring) or None
+    -> (o_part [B*Q*H,128], ml_part [B*Q*H,2])."""
+    B, Q, H, D = q.shape
+    Sk = k.shape[1]
+    dev = q.device
+    n_qt, n_kt = (Q + 127) // 128, (Sk + 127) // 128
+    tiles = torch.empty(B, n_qt, n_kt, dtype=torch.int32, device=dev)
+    counts = torch.empty(B, n_qt, dtype=torch.int32, device=dev)
+    _lib.call("lwm_attn_infer_tilemap", _lib.ptr(bits), _lib.ptr(row_any), B, Q, Sk, _lib.ptr(tiles),
+              _lib.ptr(counts), _lib.stream_ptr())
+    (q16, sq), (k16, sk), (v16, sv) = _scaled_f16(q), _scaled_f16(k), _scaled_f16(v)
+    ctas = n_qt * H * B
+    splits = 1 if ctas >= 132 else min(n_kt, -(-132 // ctas))     # key splits: fill the 132 SMs
+    rows = B * Q * H
+    o_part = torch.empty(rows, D, dtype=torch.float32, device=dev)
+    ml_part = torch.empty(rows, 2, dtype=torch.float32, device=dev)
+    ws = torch.empty(splits * rows * (D + 2), dtype=torch.float32, device=dev) if splits > 1 else None
+    _lib.call("lwm_attn_infer_partial", _lib.ptr(q16), _lib.ptr(k16), _lib.ptr(v16), _lib.ptr(sq), _lib.ptr(sk),
+              _lib.ptr(sv), _lib.ptr(bits), _lib.ptr(tiles), _lib.ptr(counts), _lib.ptr(o_part), _lib.ptr(ml_part),
+              _lib.ptr(ws), B, H, Q, Sk, D, splits, 1.0 / math.sqrt(D), _lib.stream_ptr())
+    return o_part, ml_part
+
+
+class InferOps:
+    """The kernels of the q-sharded protocol (_infer_sharded); tests substitute stand-ins."""
+    mask_pack = staticmethod(mask_pack)
+    merge = staticmethod(decode_merge)
+
+    @staticmethod
+    def partial(q, k, v, mask, row_any, tensor_cores):
+        """mask: bits [B,Q,kw] when tensor_cores, else uint8 [B,Q,Sk] (or None)"""
+        if tensor_cores:
+            return infer_partial(q, k, v, mask, row_any)
+        return decode_partial(q, k, v, mask, 0)
+
+
+class TorchComm:
+    """The collectives of the q-sharded protocol over a torch.distributed group (tests substitute a fake)."""
+
+    def __init__(self, group, world):
+        self.group, self.world = group, world
+
+    def all_gather(self, x):
+        """-> [world, *x.shape], rank-major"""
+        out = torch.empty((self.world * x.shape[0],) + tuple(x.shape[1:]), dtype=x.dtype, device=x.device)
+        dist.all_gather_into_tensor(out, x.contiguous(), group=self.group)
+        return out.view((self.world,) + tuple(x.shape))
+
+    def all_to_all(self, x):
+        """x [world, ...]: slab s goes to rank s; -> [world, ...], slab r came from rank r"""
+        x = x.contiguous()
+        out = torch.empty(x.shape, dtype=x.dtype, device=x.device)
+        dist.all_to_all_single(out, x, group=self.group)
+        return out
+
+
+def _infer_sharded(q, k, v, mask, comm, ops=InferOps):
+    """q-sharded protocol (query length > 1 on a ring of comm.world ranks): q [B,Q_loc,H,D] and mask [Bm,1,Q_loc,K]
+    are this rank's query rows, k/v [B,S_loc,H,D] its KV shard (K = world*S_loc). Each rank computes the partials of
+    ALL world*Q_loc rows over its own keys, so K/V never move; per rank the traffic is world*Q_loc*H*D words of q and
+    of partials plus Q_loc*K/8 bytes of mask. Returns this rank's [B,Q_loc,H,D] output."""
+    B, Ql, H, D = q.shape
+    Sk = k.shape[1]
+    W = comm.world
+    qls = comm.all_gather(torch.tensor([Ql], dtype=torch.int64, device=q.device))
+    if bool((qls != Ql).any()):
+        raise ValueError("ringattention_inference: every rank must hold the same number of query rows, got %s"
+                         % qls.flatten().tolist())
+    Qg = W * Ql
+    # 1. every rank gets all query rows (it stages them with one scale, from the same data)
+    q_all = comm.all_gather(q).transpose(0, 1).reshape(B, Qg, H, D)
+    tc = Qg >= INFER_MIN_Q
+    m = row_any = None
+    if mask is not None:
+        if tc:
+            # 2./3. bits of my rows, one slab per key owner, and the rows' global "any true" flags
+            bits, any_loc = ops.mask_pack(mask, B, W, Sk)                         # [W,B,Ql,kw], [B,Ql]
+            row_any = comm.all_gather(any_loc).transpose(0, 1).reshape(B, Qg)
+            m = comm.all_to_all(bits).transpose(0, 1).reshape(B, Qg, -1)
+        else:
+            m8 = mask.view(torch.uint8) if mask.dtype == torch.bool else (mask != 0).view(torch.uint8)
+            slabs = m8[:, 0, :, :W * Sk].expand(B, Ql, W * Sk).reshape(B, Ql, W, Sk).permute(2, 0, 1, 3)
+            m = comm.all_to_all(slabs).transpose(0, 1).reshape(B, Qg, Sk)
+    # 4. partials of all rows over my keys (key splits merged locally)
+    o, ml = ops.partial(q_all, k, v, m, row_any, tc)
+    # 5. each owner gets its rows' partials back
+    o = comm.all_to_all(o.view(B, W, Ql, H, D).transpose(0, 1))
+    ml = comm.all_to_all(ml.view(B, W, Ql, H, 2).transpose(0, 1))
+    # 6. merge the world partials
+    o = o.permute(1, 2, 3, 0, 4).reshape(B * Ql * H, W, D)
+    ml = ml.permute(1, 2, 3, 0, 4).reshape(B * Ql * H, W, 2)
+    return ops.merge(o.contiguous(), ml.contiguous(), W, (B, Ql, H, D), q.dtype)
+
+
 def ringattention_inference(q, k, v, attn_mask, axis_name="sp"):
-    """Drop-in for the reference's decode-time op (bound at lwm/llama.py:601-614 inside shard_map):
-    q [B,Q,H,D] (replicated along the ring when Q == 1, lwm/llama.py:598), k/v [B,S_loc,H,D] = this rank's
-    contiguous shard of the KV cache, attn_mask boolean [B,1,Q,K_global] (not sharded). Returns [B,Q,H,D].
-    The reference rotates K/V around the ring for one un-chunked online-softmax tile per step; here every rank
-    reduces its own shard (K/V are read once, from local HBM) and the P partial (o, lse) pairs — a few KB — are
-    all-gathered and merged."""
+    """Drop-in for the reference's inference-time op (bound at lwm/llama.py:601-614 inside shard_map).
+    q, k, v all bfloat16 or all float32; the output has their dtype (fp32: the un-rounded fp32 result).
+    k/v [B,S_loc,H,D] = this rank's contiguous shard of the KV cache.
+      * Q = 1 (generation): q [B,1,H,D] and attn_mask [B,1,1,K_global] are replicated along the ring. Every rank
+        reduces its own shard with the GEMV kernel and the (o, lse) partials, a few KB, are all-gathered and merged.
+      * Q > 1 on a ring: q [B,Q_loc,H,D] and attn_mask [B,1,Q_loc,K_global] are sharded on the query dimension
+        (q_sp_dim, lwm/llama.py:598); returns this rank's rows. See _infer_sharded.
+    Below INFER_MIN_Q query rows the GEMV kernel runs; from there on the tensor-core kernel over scaled fp16 copies
+    of q, k, v with fp32 logits, softmax and accumulation, visiting only the KV tiles the mask leaves visible.
+    attn_mask: bool/uint8 [B or 1,1,Q,K_global] (nonzero = attend) or None (every key visible). A row with no true
+    entry in all of K_global averages V over all keys (the reference's finfo.min semantics)."""
     if not q.is_cuda:
         raise _lib.LwmError("ringattention_inference: tensors must live on an sm_90 GPU (no CPU fallback)")
-    if q.dtype != torch.bfloat16 or k.dtype != torch.bfloat16 or v.dtype != torch.bfloat16:
-        raise TypeError("ringattention_inference: q, k, v must be bfloat16")
+    _check_infer_dtypes(q, k, v)
     group, rank, world = _resolve_group(axis_name)
     B, Q, H, D = q.shape
     Sk = k.shape[1]
-    if world > 1 and Q != 1:
-        # the reference shards q along 'sp' when q_len > 1 (q_sp_dim, lwm/llama.py:598); that short-sequence
-        # prefill variant needs a q all-gather + per-row partial exchange and is not built (q_len == 1 decode is)
-        raise NotImplementedError("ringattention_inference across a ring supports q_len == 1 (decode) only")
+    if attn_mask is not None:
+        if attn_mask.dim() != 4 or attn_mask.shape[1] != 1 or attn_mask.shape[2] != Q or attn_mask.shape[0] not in (1, B):
+            raise ValueError("attn_mask must be [B,1,Q,K_global] (lwm/llama.py:585-590)")
+        if attn_mask.shape[-1] < (world if Q > 1 else rank + 1) * Sk:
+            raise ValueError("attn_mask covers %d keys but the ring holds %d" % (attn_mask.shape[-1], world * Sk))
+    q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
+    if world > 1 and Q > 1:
+        return _infer_sharded(q, k, v, attn_mask, TorchComm(group, world))
+    if Q >= INFER_MIN_Q:
+        bits = row_any = None
+        if attn_mask is not None:
+            bits, row_any = mask_pack(attn_mask, B, 1, Sk)
+            bits = bits[0]
+        o_part, ml_part = infer_partial(q, k, v, bits, row_any)
+        return decode_merge(o_part, ml_part, 1, (B, Q, H, D), q.dtype)
     mask = None
     if attn_mask is not None:
-        if attn_mask.dim() != 4 or attn_mask.shape[1] != 1 or attn_mask.shape[2] != Q:
-            raise ValueError("attn_mask must be [B,1,Q,K_global] (lwm/llama.py:585-590)")
-        if attn_mask.shape[-1] < (rank + 1) * Sk:
-            raise ValueError("attn_mask covers %d keys but the ring holds %d" % (attn_mask.shape[-1], world * Sk))
         mask = attn_mask.to(torch.uint8).expand(B, 1, Q, attn_mask.shape[-1]).contiguous()
-    o_part, ml_part = decode_partial(q.contiguous(), k.contiguous(), v.contiguous(), mask, rank * Sk)
+    o_part, ml_part = decode_partial(q, k, v, mask, rank * Sk)
     rows = B * Q * H
     if world > 1:
         o_all = torch.empty(world, rows, D, dtype=torch.float32, device=q.device)
@@ -601,8 +755,4 @@ def ringattention_inference(q, k, v, attn_mask, axis_name="sp"):
         dist.all_gather_into_tensor(ml_all, ml_part, group=group)
         o_part = o_all.permute(1, 0, 2).contiguous()       # [row][rank][D]
         ml_part = ml_all.permute(1, 0, 2).contiguous()
-    out = torch.empty(B, Q, H, D, dtype=torch.bfloat16, device=q.device)
-    lse = torch.empty(rows, dtype=torch.float32, device=q.device)
-    _lib.call("lwm_attn_decode_merge", _lib.ptr(o_part), _lib.ptr(ml_part), world, _lib.ptr(out), _lib.ptr(lse), rows,
-              _lib.stream_ptr())
-    return out
+    return decode_merge(o_part, ml_part, world, (B, Q, H, D), q.dtype)

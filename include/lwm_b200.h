@@ -329,6 +329,20 @@ int lwm_vq_frame_tokens(const int* codes, const int* frame_idx, int* tokens, int
                         int tokens_per_frame, int eof_token, int eov_token, void* stream);
 int lwm_vq_unframe_tokens(const int* tokens, int* codes, long long n_frames, int tokens_per_frame, void* stream);
 
+/* Frame preprocessing in front of the encoder (lwm/vision_chat.py:59-74 `Sampler._process_frame`): PIL's default
+ * bicubic resize of uint8 RGB frames, the crop, and x / 127.5 - 1 in fp32 — bit-identical to Pillow's 8-bit path.
+ *   frames     [T, H, W, C] uint8, C == 3 (RGB)
+ *   x_bounds   [out_w, 2] int32 (first input column, tap count) and x_coeffs [out_w, kx] int32: Pillow's fixed-point
+ *              (2^22) coefficients of the horizontal pass W -> out_w; a pass that keeps the size is given as the
+ *              identity (one tap of 2^22). y_bounds / y_coeffs [out_h, ky]: the vertical pass H -> out_h.
+ *              The host builder is lwm_b200/vision_frames.py::pass_tables.
+ *   left, top, crop_w, crop_h   the crop window inside the out_w x out_h resized frame (integer: after PIL's rounding)
+ *   out        [T, crop_h, crop_w, 3] fp32 in [-1, 1]
+ * Only the crop window is computed. One launch per call. */
+int lwm_vq_frames_prep(const unsigned char* frames, int T, int H, int W, int C, const int* x_bounds, const int* x_coeffs,
+                       int out_w, int kx, const int* y_bounds, const int* y_coeffs, int out_h, int ky, int left, int top,
+                       int crop_w, int crop_h, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

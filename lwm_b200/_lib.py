@@ -61,6 +61,8 @@ _SIGNATURES = {
     "lwm_attn_rope": [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p] + [c_int] * 6 + [c_void_p],
     "lwm_vq_frame_tokens": [c_void_p] * 3 + [c_int] * 6 + [c_void_p],
     "lwm_vq_unframe_tokens": [c_void_p, c_void_p, c_ll, c_int, c_void_p],
+    "lwm_vq_frames_prep": [c_void_p] + [c_int] * 4 + [c_void_p] * 2 + [c_int] * 2 + [c_void_p] * 2 + [c_int] * 6
+                          + [c_void_p, c_void_p],
 }
 
 

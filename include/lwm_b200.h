@@ -111,6 +111,46 @@ int lwm_attn_bwd_step_f16(const void* q16, const void* k16, const void* v16, con
                           long long bias_stride, const int* segment_ids, long long seg_stride, float softmax_scale,
                           int dkv_init, void* stream);
 
+/* Block map of a training step with a padding bias and/or segment ids (packed or padded sequences): the tile kernels
+ * then visit only the (Q tile, KV tile) pairs that hold a visible entry, and read the mask only where it varies.
+ * lwm_attn_step_tilemap  bias / segment_ids as for lwm_attn_fwd_step (at least one non-null), the step's B, Sq, Sk,
+ *                        q_pos0, k_pos0, causal -> forward map fwd_tiles [B][Sq/128][Sk/128] (per 128-row Q tile the
+ *                        ascending KV tiles kt*2 + mixed), fwd_count [B][Sq/128], and backward map bwd_tiles
+ *                        [B][Sk/128][Sq/64] (per 128-key K tile the ascending 64-row Q tiles qt*2 + mixed), bwd_count
+ *                        [B][Sk/128]. Either map may be omitted (both of its pointers null). workspace >=
+ *                        B * (Sq/64 + Sk/128) * 16 bytes. A pair is left out when every entry is masked (bias below the
+ *                        masked level, or disjoint segment ids); in the forward only for Q tiles whose every row sees its
+ *                        own key in this step. mixed = the pair reads bias / segment ids per element.
+ * lwm_attn_{fwd,bwd}_step_map[_f16]  lwm_attn_{fwd,bwd}_step[_f16] with the matching map of lwm_attn_step_tilemap
+ *                        (built from the same arguments) appended; bias or segment_ids required. out, lse, the carries,
+ *                        dK and dV are bit-identical to the calls without a map; dQ differs only by the order of its
+ *                        fp32 reductions, which already varies from run to run. */
+int lwm_attn_step_tilemap(const float* bias, long long bias_stride, const int* segment_ids, long long seg_stride, int B,
+                          int Sq, int Sk, long long q_pos0, long long k_pos0, int causal, int* fwd_tiles, int* fwd_count,
+                          int* bwd_tiles, int* bwd_count, void* workspace, void* stream);
+int lwm_attn_fwd_step_map(const void* q, const void* k, const void* v, void* out, float* lse, float* acc_o,
+                          float* acc_m, float* acc_l, int B, int H, int Sq, int Sk, int D, long long q_pos0,
+                          long long k_pos0, int causal, const float* bias, long long bias_stride,
+                          const int* segment_ids, long long seg_stride, float softmax_scale, int first, int last,
+                          const int* tiles, const int* tile_count, void* stream);
+int lwm_attn_fwd_step_map_f16(const void* q16, const void* k16, const void* v16, const float* scale_q,
+                              const float* scale_k, const float* scale_v, float* out_f32_or_null, void* out, float* lse,
+                              float* acc_o, float* acc_m, float* acc_l, int B, int H, int Sq, int Sk, int D,
+                              long long q_pos0, long long k_pos0, int causal, const float* bias, long long bias_stride,
+                              const int* segment_ids, long long seg_stride, float softmax_scale, int first, int last,
+                              const int* tiles, const int* tile_count, void* stream);
+int lwm_attn_bwd_step_map(const void* q, const void* k, const void* v, const void* dout, const float* lse,
+                          const float* delta, float* dq_acc, float* dk_acc, float* dv_acc, int B, int H, int Sq,
+                          int Sk, int D, long long q_pos0, long long k_pos0, int causal, const float* bias,
+                          long long bias_stride, const int* segment_ids, long long seg_stride, float softmax_scale,
+                          int dkv_init, const int* tiles, const int* tile_count, void* stream);
+int lwm_attn_bwd_step_map_f16(const void* q16, const void* k16, const void* v16, const void* dout16,
+                              const float* scale_q, const float* scale_k, const float* scale_v, const float* scale_do,
+                              const float* lse, const float* delta, float* dq_acc, float* dk_acc, float* dv_acc, int B,
+                              int H, int Sq, int Sk, int D, long long q_pos0, long long k_pos0, int causal,
+                              const float* bias, long long bias_stride, const int* segment_ids, long long seg_stride,
+                              float softmax_scale, int dkv_init, const int* tiles, const int* tile_count, void* stream);
+
 /* Sharded-tensor variant of the fp16 operand conversion (ring executor): every rank publishes the |max| bit pattern of
  * its shard (lwm_attn_absmax: atomicMax into *out_bits, caller zeroes it; dtype 0 = fp32, 1 = bf16), all ranks derive
  * the SAME power-of-two scale from the gathered patterns (lwm_attn_scale_from_absmax over bits[i*stride], i < n), and

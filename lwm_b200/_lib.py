@@ -26,6 +26,16 @@ _SIGNATURES = {
                                                              c_float, c_int, c_int, c_void_p],
     "lwm_attn_bwd_step_f16": [c_void_p] * 13 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll,
                                                              c_float, c_int, c_void_p],
+    "lwm_attn_step_tilemap": [c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_ll, c_ll, c_int]
+                             + [c_void_p] * 6,
+    "lwm_attn_fwd_step_map": [c_void_p] * 8 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll,
+                                                           c_float, c_int, c_int, c_void_p, c_void_p, c_void_p],
+    "lwm_attn_fwd_step_map_f16": [c_void_p] * 12 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll,
+                                                                 c_float, c_int, c_int, c_void_p, c_void_p, c_void_p],
+    "lwm_attn_bwd_step_map": [c_void_p] * 9 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll,
+                                                           c_float, c_int, c_void_p, c_void_p, c_void_p],
+    "lwm_attn_bwd_step_map_f16": [c_void_p] * 13 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll,
+                                                                 c_float, c_int, c_void_p, c_void_p, c_void_p],
     "lwm_attn_absmax": [c_void_p, c_int, c_ll, c_void_p, c_void_p],
     "lwm_attn_absmax_scale": [c_void_p, c_int, c_ll, c_void_p, c_void_p, c_void_p],
     "lwm_attn_scale_from_absmax": [c_void_p, c_int, c_int, c_void_p, c_void_p],

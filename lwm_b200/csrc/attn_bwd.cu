@@ -43,6 +43,10 @@ struct BwdParams {
   float* dv_acc;       // [B,Sk,H,D] fp32
   const float *scale_q, *scale_k, *scale_v, *scale_do;   // fp16 mode: device scalars (x = x16 * scale); else null
   int dkv_init;        // 1: dk_acc/dv_acc rows of this launch are WRITTEN (first visit of the block), 0: accumulated
+  // kMap (a bias or segment ids): the backward map of lwm_attn_step_tilemap, per (b, K tile) the ascending list of
+  // 64-row Q tiles, entries qt * 2 + mixed
+  const int* tiles;       // [B, Sk/128, Sq/64]
+  const int* tile_count;  // [B, Sk/128]
 };
 
 constexpr int kBQ = 64;                         // query rows per inner iteration
@@ -66,6 +70,10 @@ struct BwdBarriers {
   uint64_t q_full[2], q_empty[2];   // Q + dO + lse + delta of one Q tile
   uint64_t dq_full[2], dq_empty[2]; // fp32 dQ staging tile: written by the consumers, reduced by warp 9
 };
+// kMap: the list entry of the Q tile in stage st, written by the producer before it arms q_full[st] (the consumers read
+// it there instead of holding a pointer into the list across their loop)
+constexpr int kOffEntry = kOffBars + 96;
+static_assert(sizeof(BwdBarriers) <= 96 && 96 + 2 * 4 <= 128, "attn_bwd: barrier block layout");
 
 LWM_DEVICE void load_tile_nb(uint8_t* dst, const CUtensorMap* tm, uint64_t* bar, int h, int row0, int b, int half_bytes) {
   tma_load_4d(dst, tm, bar, 0, h, row0, b);
@@ -85,7 +93,10 @@ constexpr float kDsNorm = 1.0f / 32768.0f;
 // offset_log2 = LWM_ATTN_F16_P_BOOST_LOG2) and the factor is undone in fp32 in the dV epilogue and in the dS scale.
 constexpr float kPBoostInv = 1.0f / 16384.0f;
 
-template <bool kF16>
+// kMap: the CTA walks its K tile's list of Q tiles instead of i_start .. n_q_tiles (pairs whose entries are all masked
+// are not in it: they would add exact zeros); mixed tiles run the per-element mask, clean tiles the same branch with no
+// bias or segment read.
+template <bool kF16, bool kMap = false>
 __global__ void __launch_bounds__(kBwdThreads, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
@@ -108,7 +119,18 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     const long long diff = (long long)p.mask.k_pos0 + (long long)n * kTile - p.mask.q_pos0;
     i_start = diff <= 0 ? 0 : int(min(diff / kBQ, (long long)n_q_tiles));
   }
-  const int nq = n_q_tiles - i_start;
+  int nq = n_q_tiles - i_start;
+  int list0 = 0;   // kMap: offset of this K tile's list in p.tiles (B * Sk/128 * Sq/64 < 2^31: checked on the host)
+  if constexpr (kMap) {
+    const int lt = b * gridDim.x + n;
+    nq = p.tile_count[lt];
+    list0 = lt * n_q_tiles;
+  }
+  int* s_entry = reinterpret_cast<int*>(smem + kOffEntry);
+  // Q tile of list position it (producer warps)
+  auto q_tile = [&](int it) { return kMap ? (p.tiles[list0 + it] >> 1) : i_start + it; };
+  // kMap: the count is re-read where each role starts its loop rather than held across setmaxnreg (no spill)
+  auto loop_count = [&]() { return kMap ? p.tile_count[b * gridDim.x + n] : nq; };
   if (nq <= 0) {  // this key tile is invisible to the whole q shard: dk/dv unchanged (zero when this launch initialises them)
     if (p.dkv_init) {
       const long long base = (((long long)b * p.Sk + (long long)n * kTile) * p.H + h) * kHeadDim;
@@ -139,9 +161,10 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     if (warp == 9 && lane == 0) {
       // dQ reductions: one fp32 add per dQ element per (key tile, Q tile), four 32-column boxes per tile
       tma_prefetch_desc(&tmDQ);
-      for (int it = 0; it < nq; ++it) {
+      const int nql = loop_count();
+      for (int it = 0; it < nql; ++it) {
         const int st = it & 1;
-        const int row0 = (i_start + it) * kBQ;
+        const int row0 = q_tile(it) * kBQ;
         mbar_wait(&bars.dq_full[st], (it >> 1) & 1);
 #pragma unroll
         for (int j = 0; j < kHeadDim / 32; ++j)
@@ -161,10 +184,12 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       load_tile_nb(smem + kOffK, &tmK, &bars.kv_full, h, n * kTile, b, kTB / 2);
       load_tile_nb(smem + kOffV, &tmV, &bars.kv_full, h, n * kTile, b, kTB / 2);
       const long long ml_base = ((long long)b * p.H + h) * p.Sq;
-      for (int it = 0; it < nq; ++it) {
+      const int nql = loop_count();
+      for (int it = 0; it < nql; ++it) {
         const int st = it & 1;
-        const int row0 = (i_start + it) * kBQ;
+        const int row0 = q_tile(it) * kBQ;
         mbar_wait(&bars.q_empty[st], ((it >> 1) & 1) ^ 1);
+        if constexpr (kMap) s_entry[st] = p.tiles[list0 + it];
         mbar_arrive_expect_tx(&bars.q_full[st], 2 * kQB + 2 * kBQ * 4);
         load_tile_nb(smem + kOffQ + st * kQB, &tmQ, &bars.q_full[st], h, row0, b, kQB / 2);
         load_tile_nb(smem + kOffDO + st * kQB, &tmDO, &bars.q_full[st], h, row0, b, kQB / 2);
@@ -200,7 +225,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   for (int i = 0; i < 64; ++i) dk[i] = dv[i] = 0.f;
 
   mbar_wait(&bars.kv_full, 0);
-  for (int it = 0; it < nq; ++it) {
+  const int nql = loop_count();
+  for (int it = 0; it < nql; ++it) {
     const int st = it & 1;
     const uint32_t aQ = smem_u32(smem + kOffQ + st * kQB), aDO = smem_u32(smem + kOffDO + st * kQB);
     const uint64_t dQ_k = desc_kmajor_sw128(aQ), dDO_k = desc_kmajor_sw128(aDO);
@@ -208,6 +234,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     const uint64_t dDS_m = desc_mnmajor_sw128(aDS + st * kDSB, kDSB);
     uint8_t* sDS = smem + kOffDS + st * kDSB;
     mbar_wait(&bars.q_full[st], (it >> 1) & 1);
+    const int entry = kMap ? s_entry[st] : 0;
 
     // ---- S^T = K Q^T, dP^T = V dO^T: two groups, so that exp(S^T) runs while dP^T is on the tensor cores
     float sacc[32], dpacc[32];
@@ -228,8 +255,10 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     reg_fence(sacc);
 
     // ---- P^T = exp2(S^T * scale_log2 (+bias) - lse2)
-    const int q_tile_pos = p.mask.q_pos0 + (i_start + it) * kBQ;
-    const bool need_mask = has_bias || has_seg || (p.mask.causal && q_tile_pos < wg_k_last);
+    const int q_tile_pos = p.mask.q_pos0 + (kMap ? entry >> 1 : i_start + it) * kBQ;
+    // kMap: clean tiles keep the masked path's rounding (fmaf(s, scale, 0)): bit-identical to the step without a map
+    const bool need_mask = kMap || has_bias || has_seg || (p.mask.causal && q_tile_pos < wg_k_last);
+    const bool mixed = kMap ? (entry & 1) : true;   // the tile reads bias and segment ids
     uint32_t pk[4][4], dsk[4][4];   // P^T and dS^T as A fragments, one 16-query slice per entry
     float pr[4][8];
     // the mask test is hoisted out of the element loop: one branch per tile keeps the fragment in registers
@@ -241,15 +270,16 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       }
     } else {
       // per-key mask inputs, reloaded per masked tile (L1 hits) rather than held in registers across the loop
-      const int* seg_row = has_seg ? p.mask.seg + (long long)b * p.mask.seg_stride : nullptr;
+      const bool use_bias = has_bias && mixed, use_seg = has_seg && mixed;
+      const int* seg_row = use_seg ? p.mask.seg + (long long)b * p.mask.seg_stride : nullptr;
       const int k_pos = p.mask.k_pos0 + n * kTile + kr0;   // this thread's keys: k_pos, k_pos + 8
       int my_seg[2];
       float bias_t[2] = {0.f, 0.f};
       bool key_masked[2] = {false, false};
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
-        my_seg[hh] = has_seg ? seg_row[k_pos + 8 * hh] : 0;
-        if (has_bias) {
+        my_seg[hh] = use_seg ? seg_row[k_pos + 8 * hh] : 0;
+        if (use_bias) {
           bias_t[hh] = p.mask.bias[(long long)b * p.mask.bias_stride + k_pos + 8 * hh] * kLog2e;
           key_masked[hh] = bias_t[hh] < kMaskedLogit;
         }
@@ -260,7 +290,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         const int col = (i >> 2) * 8 + quad * 2 + (i & 1);
         float tv = key_masked[hh] ? kMaskedLogit : fmaf(sacc[i], scale_log2, bias_t[hh]);
         const int q_pos = q_tile_pos + col;
-        if (has_seg && seg_row[q_pos] != my_seg[hh]) tv = kMaskedLogit;
+        if (use_seg && seg_row[q_pos] != my_seg[hh]) tv = kMaskedLogit;
         if (p.mask.causal && q_pos < k_pos + 8 * hh) tv = kMaskedLogit;
         pr[i >> 3][i & 7] = ex2f(tv + s_lse[st][col]);
       }
@@ -394,7 +424,7 @@ static int attn_bwd_launch(const void* q, const void* k, const void* v, const vo
                            int Sk, int D, long long q_pos0, long long k_pos0, int causal, const float* bias,
                            long long bias_stride, const int* segment_ids, long long seg_stride, float softmax_scale,
                            const float* scale_q, const float* scale_k, const float* scale_v, const float* scale_do,
-                           int dkv_init, void* stream) {
+                           int dkv_init, const int* tiles, const int* tile_count, void* stream) {
   if (D != kHeadDim) return lwm_fail(LWM_ERR_SHAPE, "attn_bwd: head_dim must be 128");
   if (B <= 0 || H <= 0 || Sq <= 0 || Sk <= 0 || Sq % kTile || Sk % kTile)
     return lwm_fail(LWM_ERR_SHAPE, "attn_bwd: Sq and Sk must be positive multiples of 128");
@@ -406,6 +436,8 @@ static int attn_bwd_launch(const void* q, const void* k, const void* v, const vo
     return lwm_fail(LWM_ERR_SHAPE, "attn_bwd: bias is indexed by GLOBAL key position: bias_stride < k_pos0 + Sk");
   if (segment_ids && (seg_stride < q_pos0 + Sq || seg_stride < k_pos0 + Sk))
     return lwm_fail(LWM_ERR_SHAPE, "attn_bwd: segment_ids is indexed by GLOBAL position: seg_stride < max(q_pos0 + Sq, k_pos0 + Sk)");
+  if (tiles && (long long)B * (Sk / kTile) * (Sq / kBQ) > 0x7fffffffLL)
+    return lwm_fail(LWM_ERR_SHAPE, "attn_bwd_map: B * Sk/128 * Sq/64 must fit in int32");
   if (!lwm_check_device()) return LWM_ERR_DEVICE;
   CUtensorMap tq, tk, tv, tdo, tdq;
   if (!make_bf16_tmap(&tq, q, B, Sq, H, kBQ) || !make_bf16_tmap(&tk, k, B, Sk, H, kTile) ||
@@ -422,6 +454,7 @@ static int attn_bwd_launch(const void* q, const void* k, const void* v, const vo
   p.lse = lse; p.delta = delta; p.dq_acc = dq_acc; p.dk_acc = dk_acc; p.dv_acc = dv_acc;
   p.scale_q = scale_q; p.scale_k = scale_k; p.scale_v = scale_v; p.scale_do = scale_do;
   p.dkv_init = dkv_init ? 1 : 0;
+  p.tiles = tiles; p.tile_count = tile_count;
   static bool attr_set_dev[64] = {};
   int cur_dev = 0;
   cudaGetDevice(&cur_dev);
@@ -430,12 +463,21 @@ static int attn_bwd_launch(const void* q, const void* k, const void* v, const vo
     if (cudaFuncSetAttribute(attn_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBwdSmemBytes) !=
             cudaSuccess ||
         cudaFuncSetAttribute(attn_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBwdSmemBytes) !=
-            cudaSuccess)
+            cudaSuccess ||
+        cudaFuncSetAttribute(attn_bwd_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             kBwdSmemBytes) != cudaSuccess ||
+        cudaFuncSetAttribute(attn_bwd_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             kBwdSmemBytes) != cudaSuccess)
       return lwm_fail(LWM_ERR_CUDA, "attn_bwd: cannot raise dynamic shared memory limit");
     attr_set = true;
   }
   dim3 grid(Sk / kTile, H, B);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (tiles) {
+    if (scale_q) attn_bwd_kernel<true, true><<<grid, kBwdThreads, kBwdSmemBytes, st>>>(tq, tk, tv, tdo, tdq, p);
+    else attn_bwd_kernel<false, true><<<grid, kBwdThreads, kBwdSmemBytes, st>>>(tq, tk, tv, tdo, tdq, p);
+    return lwm_check_launch("attn_bwd_kernel (block map)");
+  }
   if (scale_q) attn_bwd_kernel<true><<<grid, kBwdThreads, kBwdSmemBytes, st>>>(tq, tk, tv, tdo, tdq, p);
   else attn_bwd_kernel<false><<<grid, kBwdThreads, kBwdSmemBytes, st>>>(tq, tk, tv, tdo, tdq, p);
   return lwm_check_launch("attn_bwd_kernel");
@@ -448,7 +490,7 @@ extern "C" int lwm_attn_bwd_step(const void* q, const void* k, const void* v, co
                                  long long seg_stride, float softmax_scale, int dkv_init, void* stream) {
   return attn_bwd_launch(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, B, H, Sq, Sk, D, q_pos0, k_pos0, causal,
                          bias, bias_stride, segment_ids, seg_stride, softmax_scale, nullptr, nullptr, nullptr, nullptr,
-                         dkv_init, stream);
+                         dkv_init, nullptr, nullptr, stream);
 }
 
 // fp16-operand variant: scale_* = device scalars of the four fp16 operand copies (lwm_attn_to_f16).
@@ -462,5 +504,41 @@ extern "C" int lwm_attn_bwd_step_f16(const void* q16, const void* k16, const voi
   if (!scale_q || !scale_k || !scale_v || !scale_do) return lwm_fail(LWM_ERR_ARG, "attn_bwd_f16: scales required");
   return attn_bwd_launch(q16, k16, v16, dout16, lse, delta, dq_acc, dk_acc, dv_acc, B, H, Sq, Sk, D, q_pos0, k_pos0,
                          causal, bias, bias_stride, segment_ids, seg_stride, softmax_scale, scale_q, scale_k, scale_v,
-                         scale_do, dkv_init, stream);
+                         scale_do, dkv_init, nullptr, nullptr, stream);
+}
+
+// Block-map variants (a bias or segment ids given): tiles / tile_count are the backward map of lwm_attn_step_tilemap,
+// built with the same (bias, segment_ids, B, Sq, Sk, q_pos0, k_pos0, causal). dK and dV are bit-identical to
+// lwm_attn_bwd_step / lwm_attn_bwd_step_f16; dQ differs only by the order of its reductions.
+static int bwd_map_args(const float* bias, const int* segment_ids, const int* tiles, const int* tile_count) {
+  if (!bias && !segment_ids) return lwm_fail(LWM_ERR_ARG, "attn_bwd_map: bias or segment_ids required");
+  if (!tiles || !tile_count) return lwm_fail(LWM_ERR_ARG, "attn_bwd_map: null tiles / tile_count");
+  return LWM_OK;
+}
+
+extern "C" int lwm_attn_bwd_step_map(const void* q, const void* k, const void* v, const void* dout, const float* lse,
+                                     const float* delta, float* dq_acc, float* dk_acc, float* dv_acc, int B, int H,
+                                     int Sq, int Sk, int D, long long q_pos0, long long k_pos0, int causal,
+                                     const float* bias, long long bias_stride, const int* segment_ids,
+                                     long long seg_stride, float softmax_scale, int dkv_init, const int* tiles,
+                                     const int* tile_count, void* stream) {
+  if (int e = bwd_map_args(bias, segment_ids, tiles, tile_count)) return e;
+  return attn_bwd_launch(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, B, H, Sq, Sk, D, q_pos0, k_pos0, causal,
+                         bias, bias_stride, segment_ids, seg_stride, softmax_scale, nullptr, nullptr, nullptr, nullptr,
+                         dkv_init, tiles, tile_count, stream);
+}
+
+extern "C" int lwm_attn_bwd_step_map_f16(const void* q16, const void* k16, const void* v16, const void* dout16,
+                                         const float* scale_q, const float* scale_k, const float* scale_v,
+                                         const float* scale_do, const float* lse, const float* delta, float* dq_acc,
+                                         float* dk_acc, float* dv_acc, int B, int H, int Sq, int Sk, int D,
+                                         long long q_pos0, long long k_pos0, int causal, const float* bias,
+                                         long long bias_stride, const int* segment_ids, long long seg_stride,
+                                         float softmax_scale, int dkv_init, const int* tiles, const int* tile_count,
+                                         void* stream) {
+  if (!scale_q || !scale_k || !scale_v || !scale_do) return lwm_fail(LWM_ERR_ARG, "attn_bwd_map_f16: scales required");
+  if (int e = bwd_map_args(bias, segment_ids, tiles, tile_count)) return e;
+  return attn_bwd_launch(q16, k16, v16, dout16, lse, delta, dq_acc, dk_acc, dv_acc, B, H, Sq, Sk, D, q_pos0, k_pos0,
+                         causal, bias, bias_stride, segment_ids, seg_stride, softmax_scale, scale_q, scale_k, scale_v,
+                         scale_do, dkv_init, tiles, tile_count, stream);
 }

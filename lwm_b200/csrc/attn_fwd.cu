@@ -35,11 +35,12 @@ struct FwdParams {
   float* acc_l;        // [B,H,Sq]     running denominator
   int first, last;
   const float *scale_q, *scale_k, *scale_v;   // fp16 mode: device scalars, x = x16 * scale; null => bf16 operands
-  // inference mode only (ringattention_inference, Sq = Q rows, any Q and Sk): the (b, Q tile) lists of KV tiles
-  const uint32_t* bits;   // [B, Sq, n_kt * 4] mask bits (bit j of word w <=> key 32 w + j; 1 = attend) or null
+  // list modes: the (b, Q tile) lists of KV tiles. Inference (ringattention_inference, Sq = Q rows, any Q and Sk):
+  // from the mask bits (attn_infer.cu). Training with a bias or segment ids: from lwm_attn_step_tilemap (attn_tiles.cu).
+  const uint32_t* bits;   // inference: [B, Sq, n_kt * 4] mask bits (bit j of word w <=> key 32 w + j; 1 = attend) or null
   const int* tiles;       // [B, ceil(Sq/128), n_kt]: kt * 2 + mixed, ascending kt
   const int* tile_count;  // [B, ceil(Sq/128)]
-  int n_kt, splits;       // KV tiles of the shard; CTAs per Q tile, each takes a contiguous slice of the list
+  int n_kt, splits;       // KV tiles of the shard; inference: CTAs per Q tile, each takes a contiguous slice of the list
   float* o_part;          // [B*Sq*H, splits, 128] un-normalised numerators (in V's units)
   float* ml_part;         // [B*Sq*H, splits, 2] (max in the log2 domain, denominator)
 };
@@ -76,7 +77,10 @@ LWM_DEVICE float quad_sum(float x) {
 // kInfer: the inference mode. A CTA walks its slice of its Q tile's KV tile list (built from a bit mask by
 // attn_infer.cu); only tiles marked mixed read mask bits, keys >= Sk get -inf, rows >= Sq are padding. The epilogue
 // writes the CTA's un-normalised partial for decode_merge_kernel instead of a carry.
-template <bool kF16, bool kInfer = false>
+// kMap: the training step with a bias or segment ids, over the block map of lwm_attn_step_tilemap: the CTA walks its
+// Q tile's list of KV tiles (masked ones are not in it); mixed tiles run the per-element mask, clean tiles the same
+// branch with no bias or segment read (the causal compare stays). The epilogue is the training one.
+template <bool kF16, bool kInfer = false, bool kMap = false>
 __global__ void __launch_bounds__(kFwdThreads, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const FwdParams p) {
@@ -104,6 +108,10 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     const int beg = min(cnt, int(blockIdx.x % p.splits) * per);
     n_kv = min(cnt, beg + per) - beg;
     list = p.tiles + lt * p.n_kt + beg;
+  } else if constexpr (kMap) {
+    const long long lt = (long long)b * n_q_tiles + tile;
+    n_kv = p.tile_count[lt];
+    list = p.tiles + lt * p.n_kt;
   } else if (p.mask.causal) {
     const long long last_q = (long long)p.mask.q_pos0 + m0 + kTile - 1;
     const long long vis = last_q - p.mask.k_pos0;  // largest visible local key index
@@ -133,7 +141,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         const int slot = i % kFwdStages;
         const uint32_t ph = (i / kFwdStages) & 1;
         mbar_wait(&bars.kv_empty[slot], ph ^ 1);
-        const int kt = kInfer ? (list[i >> 1] >> 1) : (i >> 1);
+        const int kt = (kInfer || kMap) ? (list[i >> 1] >> 1) : (i >> 1);
         load_tile(sKV + slot * kFwdTileBytes, (i & 1) ? &tmV : &tmK, &bars.kv_full[slot], h, kt * kTile, b);
       }
     }
@@ -199,10 +207,17 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     auto softmax = [&](int j) {
       int k_tile_pos;
       bool need_mask;   // warp-uniform: does any row of this warp need a mask on this KV tile?
+      bool mixed = true;  // kMap: the tile reads bias and segment ids
       if constexpr (kInfer) {
         const int e = list[j];
         k_tile_pos = (e >> 1) * kTile;
         need_mask = e & 1;
+      } else if constexpr (kMap) {
+        const int e = list[j];
+        k_tile_pos = p.mask.k_pos0 + (e >> 1) * kTile;
+        // clean tiles keep the rounding of the masked path (s * scale, then - m): bit-identical to the step without a map
+        need_mask = true;
+        mixed = e & 1;
       } else {
         k_tile_pos = p.mask.k_pos0 + j * kTile;
         need_mask = has_bias || has_seg || (p.mask.causal && (k_tile_pos + kTile - 1 > warp_q_pos0));
@@ -238,25 +253,26 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         mx[1] = quad_max(mx[1]);
       } else {
         // per-row mask inputs, reloaded per masked tile (L1 hits) rather than held in registers across the loop
-        const float* bias_row = has_bias ? p.mask.bias + (long long)b * p.mask.bias_stride : nullptr;
-        const int* seg_row = has_seg ? p.mask.seg + (long long)b * p.mask.seg_stride : nullptr;
+        const bool use_bias = has_bias && mixed, use_seg = has_seg && mixed;
+        const float* bias_row = use_bias ? p.mask.bias + (long long)b * p.mask.bias_stride : nullptr;
+        const int* seg_row = use_seg ? p.mask.seg + (long long)b * p.mask.seg_stride : nullptr;
         int q_pos[2];
         int my_seg[2];
 #pragma unroll
         for (int hh = 0; hh < 2; ++hh) {
           q_pos[hh] = p.mask.q_pos0 + r0 + 8 * hh;
-          my_seg[hh] = has_seg ? seg_row[q_pos[hh]] : 0;
+          my_seg[hh] = use_seg ? seg_row[q_pos[hh]] : 0;
         }
 #pragma unroll
         for (int i = 0; i < 64; ++i) {
           const int hh = (i >> 1) & 1;
           const int col = (i >> 2) * 8 + quad * 2 + (i & 1);
           float tv = s[i] * scale;
-          if (has_bias) {
+          if (use_bias) {
             const float bt = bias_row[k_tile_pos + col] * kLog2e;
             tv = (bt < kMaskedLogit) ? kMaskedLogit : tv + bt;
           }
-          if (has_seg && seg_row[k_tile_pos + col] != my_seg[hh]) tv = kMaskedLogit;
+          if (use_seg && seg_row[k_tile_pos + col] != my_seg[hh]) tv = kMaskedLogit;
           if (p.mask.causal && k_tile_pos + col > q_pos[hh]) tv = kMaskedLogit;
           s[i] = tv;
           mx[hh] = fmaxf(mx[hh], tv);
@@ -426,7 +442,7 @@ static int attn_fwd_launch(const void* q, const void* k, const void* v, void* ou
                            long long k_pos0, int causal, const float* bias, long long bias_stride,
                            const int* segment_ids, long long seg_stride, float softmax_scale, int first, int last,
                            const float* scale_q, const float* scale_k, const float* scale_v, float* out_f32,
-                           void* stream) {
+                           const int* tiles, const int* tile_count, void* stream) {
   if (D != kHeadDim) return lwm_fail(LWM_ERR_SHAPE, "attn_fwd: head_dim must be 128");
   if (B <= 0 || H <= 0 || Sq <= 0 || Sk <= 0 || Sq % kTile || Sk % kTile)
     return lwm_fail(LWM_ERR_SHAPE, "attn_fwd: Sq and Sk must be positive multiples of 128");
@@ -455,6 +471,8 @@ static int attn_fwd_launch(const void* q, const void* k, const void* v, void* ou
   p.first = first; p.last = last;
   p.scale_q = scale_q; p.scale_k = scale_k; p.scale_v = scale_v;
   p.out_f32 = out_f32;
+  p.bits = nullptr; p.tiles = tiles; p.tile_count = tile_count;
+  p.n_kt = Sk / kTile; p.splits = 1;
   static bool attr_set_dev[64] = {};
   int cur_dev = 0;
   cudaGetDevice(&cur_dev);
@@ -463,15 +481,23 @@ static int attn_fwd_launch(const void* q, const void* k, const void* v, void* ou
     if (cudaFuncSetAttribute(attn_fwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFwdSmemBytes) !=
             cudaSuccess ||
         cudaFuncSetAttribute(attn_fwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFwdSmemBytes) !=
-            cudaSuccess)
+            cudaSuccess ||
+        cudaFuncSetAttribute(attn_fwd_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             kFwdSmemBytes) != cudaSuccess ||
+        cudaFuncSetAttribute(attn_fwd_kernel<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             kFwdSmemBytes) != cudaSuccess)
       return lwm_fail(LWM_ERR_CUDA, "attn_fwd: cannot raise dynamic shared memory limit");
     attr_set = true;
   }
   dim3 grid(Sq / kTile, H, B);
-  if (scale_q)
-    attn_fwd_kernel<true><<<grid, kFwdThreads, kFwdSmemBytes, reinterpret_cast<cudaStream_t>(stream)>>>(tq, tk, tv, p);
-  else
-    attn_fwd_kernel<false><<<grid, kFwdThreads, kFwdSmemBytes, reinterpret_cast<cudaStream_t>(stream)>>>(tq, tk, tv, p);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (tiles) {
+    if (scale_q) attn_fwd_kernel<true, false, true><<<grid, kFwdThreads, kFwdSmemBytes, st>>>(tq, tk, tv, p);
+    else attn_fwd_kernel<false, false, true><<<grid, kFwdThreads, kFwdSmemBytes, st>>>(tq, tk, tv, p);
+    return lwm_check_launch("attn_fwd_kernel (block map)");
+  }
+  if (scale_q) attn_fwd_kernel<true><<<grid, kFwdThreads, kFwdSmemBytes, st>>>(tq, tk, tv, p);
+  else attn_fwd_kernel<false><<<grid, kFwdThreads, kFwdSmemBytes, st>>>(tq, tk, tv, p);
   return lwm_check_launch("attn_fwd_kernel");
 }
 
@@ -481,7 +507,8 @@ extern "C" int lwm_attn_fwd_step(const void* q, const void* k, const void* v, vo
                                  long long bias_stride, const int* segment_ids, long long seg_stride,
                                  float softmax_scale, int first, int last, void* stream) {
   return attn_fwd_launch(q, k, v, out, lse, acc_o, acc_m, acc_l, B, H, Sq, Sk, D, q_pos0, k_pos0, causal, bias,
-                         bias_stride, segment_ids, seg_stride, softmax_scale, first, last, nullptr, nullptr, nullptr, nullptr, stream);
+                         bias_stride, segment_ids, seg_stride, softmax_scale, first, last, nullptr, nullptr, nullptr, nullptr,
+                         nullptr, nullptr, stream);
 }
 
 // fp16-operand variant: q/k/v are the fp16 copies made by lwm_attn_to_f16, scale_* their device scalars.
@@ -494,7 +521,42 @@ extern "C" int lwm_attn_fwd_step_f16(const void* q16, const void* k16, const voi
   if (!scale_q || !scale_k || !scale_v) return lwm_fail(LWM_ERR_ARG, "attn_fwd_f16: scales required");
   return attn_fwd_launch(q16, k16, v16, out, lse, acc_o, acc_m, acc_l, B, H, Sq, Sk, D, q_pos0, k_pos0, causal, bias,
                          bias_stride, segment_ids, seg_stride, softmax_scale, first, last, scale_q, scale_k, scale_v,
-                         out_f32, stream);
+                         out_f32, nullptr, nullptr, stream);
+}
+
+// Block-map variants (a bias or segment ids given): tiles / tile_count are the forward map of lwm_attn_step_tilemap,
+// built with the same (bias, segment_ids, B, Sq, Sk, q_pos0, k_pos0, causal). Results are bit-identical to
+// lwm_attn_fwd_step / lwm_attn_fwd_step_f16.
+static int fwd_map_args(const float* bias, const int* segment_ids, const int* tiles, const int* tile_count) {
+  if (!bias && !segment_ids) return lwm_fail(LWM_ERR_ARG, "attn_fwd_map: bias or segment_ids required");
+  if (!tiles || !tile_count) return lwm_fail(LWM_ERR_ARG, "attn_fwd_map: null tiles / tile_count");
+  return LWM_OK;
+}
+
+extern "C" int lwm_attn_fwd_step_map(const void* q, const void* k, const void* v, void* out, float* lse, float* acc_o,
+                                     float* acc_m, float* acc_l, int B, int H, int Sq, int Sk, int D,
+                                     long long q_pos0, long long k_pos0, int causal, const float* bias,
+                                     long long bias_stride, const int* segment_ids, long long seg_stride,
+                                     float softmax_scale, int first, int last, const int* tiles,
+                                     const int* tile_count, void* stream) {
+  if (int e = fwd_map_args(bias, segment_ids, tiles, tile_count)) return e;
+  return attn_fwd_launch(q, k, v, out, lse, acc_o, acc_m, acc_l, B, H, Sq, Sk, D, q_pos0, k_pos0, causal, bias,
+                         bias_stride, segment_ids, seg_stride, softmax_scale, first, last, nullptr, nullptr, nullptr, nullptr,
+                         tiles, tile_count, stream);
+}
+
+extern "C" int lwm_attn_fwd_step_map_f16(const void* q16, const void* k16, const void* v16, const float* scale_q,
+                                         const float* scale_k, const float* scale_v, float* out_f32,
+                                         void* out, float* lse, float* acc_o, float* acc_m, float* acc_l, int B, int H,
+                                         int Sq, int Sk, int D, long long q_pos0, long long k_pos0, int causal,
+                                         const float* bias, long long bias_stride, const int* segment_ids,
+                                         long long seg_stride, float softmax_scale, int first, int last,
+                                         const int* tiles, const int* tile_count, void* stream) {
+  if (!scale_q || !scale_k || !scale_v) return lwm_fail(LWM_ERR_ARG, "attn_fwd_map_f16: scales required");
+  if (int e = fwd_map_args(bias, segment_ids, tiles, tile_count)) return e;
+  return attn_fwd_launch(q16, k16, v16, out, lse, acc_o, acc_m, acc_l, B, H, Sq, Sk, D, q_pos0, k_pos0, causal, bias,
+                         bias_stride, segment_ids, seg_stride, softmax_scale, first, last, scale_q, scale_k, scale_v,
+                         out_f32, tiles, tile_count, stream);
 }
 
 // Inference mode (ringattention_inference with Q >= kInferMinQ rows): q16 [B,Q,H,128], k16/v16 [B,Sk,H,128] scaled fp16

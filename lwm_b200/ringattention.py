@@ -195,10 +195,42 @@ def to_f16(x, stream=None):
     return x16, scale
 
 
+def step_tilemap(B, Sq, Sk, q_pos0, k_pos0, causal, bias, seg, fwd=True, bwd=True, stream=None):
+    """Block map of one training step with a bias and/or segment ids (include/lwm_b200.h: lwm_attn_step_tilemap)
+    -> (fwd_tiles, fwd_count, bwd_tiles, bwd_count); the maps not asked for are None."""
+    dev = (bias if bias is not None else seg).device
+    n_qt, n_q64, n_kt = Sq // 128, Sq // 64, Sk // 128
+    ft = torch.empty((B, n_qt, n_kt), dtype=torch.int32, device=dev) if fwd else None
+    fc = torch.empty((B, n_qt), dtype=torch.int32, device=dev) if fwd else None
+    bt = torch.empty((B, n_kt, n_q64), dtype=torch.int32, device=dev) if bwd else None
+    bc = torch.empty((B, n_kt), dtype=torch.int32, device=dev) if bwd else None
+    ws = torch.empty(B * (n_q64 + n_kt) * 4, dtype=torch.int32, device=dev)
+    _lib.call("lwm_attn_step_tilemap", _lib.ptr(bias), 0 if bias is None else bias.shape[1], _lib.ptr(seg),
+              0 if seg is None else seg.shape[1], B, Sq, Sk, int(q_pos0), int(k_pos0), int(bool(causal)), _lib.ptr(ft),
+              _lib.ptr(fc), _lib.ptr(bt), _lib.ptr(bc), _lib.ptr(ws), _lib.stream_ptr(stream))
+    return ft, fc, bt, bc
+
+
 def fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last,
-             stream=None, scales=None, out_f32=None):
+             stream=None, scales=None, out_f32=None, tilemap=None):
+    """tilemap: None, or the forward map (tiles, counts) of step_tilemap for these arguments: the tile kernel then
+    visits only the KV tiles in it (same results, bit for bit)."""
     B, Sq, H, D = q.shape
     Sk = k.shape[1]
+    if tilemap is not None:
+        tail = (_lib.ptr(tilemap[0]), _lib.ptr(tilemap[1]), _lib.stream_ptr(stream))
+        if scales is not None:
+            _lib.call("lwm_attn_fwd_step_map_f16", _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(scales[0]),
+                      _lib.ptr(scales[1]), _lib.ptr(scales[2]), _lib.ptr(out_f32), _lib.ptr(out), _lib.ptr(lse),
+                      _lib.ptr(acc_o), _lib.ptr(acc_m), _lib.ptr(acc_l), B, H, Sq, Sk, D, int(q_pos0), int(k_pos0),
+                      int(bool(causal)), _lib.ptr(bias), 0 if bias is None else bias.shape[1], _lib.ptr(seg),
+                      0 if seg is None else seg.shape[1], 1.0 / math.sqrt(D), int(first), int(last), *tail)
+        else:
+            _lib.call("lwm_attn_fwd_step_map", _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(out), _lib.ptr(lse),
+                      _lib.ptr(acc_o), _lib.ptr(acc_m), _lib.ptr(acc_l), B, H, Sq, Sk, D, int(q_pos0), int(k_pos0),
+                      int(bool(causal)), _lib.ptr(bias), 0 if bias is None else bias.shape[1], _lib.ptr(seg),
+                      0 if seg is None else seg.shape[1], 1.0 / math.sqrt(D), int(first), int(last), *tail)
+        return
     if scales is not None:   # fp16-operand kernels: q/k/v are fp16 copies, scales = (sq, sk, sv) device scalars
         _lib.call("lwm_attn_fwd_step_f16", _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(scales[0]),
                   _lib.ptr(scales[1]), _lib.ptr(scales[2]), _lib.ptr(out_f32), _lib.ptr(out), _lib.ptr(lse),
@@ -238,10 +270,26 @@ def lse_for_bwd(lse, stream=None, f16=False):
 
 
 def bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg, stream=None,
-             scales=None, init=False):
-    """`lse` is the PRE-SCALED array returned by lse_for_bwd. init=True: dk_acc/dv_acc rows are written, not accumulated."""
+             scales=None, init=False, tilemap=None):
+    """`lse` is the PRE-SCALED array returned by lse_for_bwd. init=True: dk_acc/dv_acc rows are written, not accumulated.
+    tilemap: None, or the backward map (tiles, counts) of step_tilemap for these arguments (dK, dV bit-identical; dQ
+    up to the order of its reductions)."""
     B, Sq, H, D = q.shape
     Sk = k.shape[1]
+    if tilemap is not None:
+        tail = (_lib.ptr(tilemap[0]), _lib.ptr(tilemap[1]), _lib.stream_ptr(stream))
+        if scales is not None:
+            _lib.call("lwm_attn_bwd_step_map_f16", _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(dout),
+                      _lib.ptr(scales[0]), _lib.ptr(scales[1]), _lib.ptr(scales[2]), _lib.ptr(scales[3]), _lib.ptr(lse),
+                      _lib.ptr(delta), _lib.ptr(dq_acc), _lib.ptr(dk_acc), _lib.ptr(dv_acc), B, H, Sq, Sk, D,
+                      int(q_pos0), int(k_pos0), int(bool(causal)), _lib.ptr(bias), 0 if bias is None else bias.shape[1],
+                      _lib.ptr(seg), 0 if seg is None else seg.shape[1], 1.0 / math.sqrt(D), int(bool(init)), *tail)
+        else:
+            _lib.call("lwm_attn_bwd_step_map", _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(dout), _lib.ptr(lse),
+                      _lib.ptr(delta), _lib.ptr(dq_acc), _lib.ptr(dk_acc), _lib.ptr(dv_acc), B, H, Sq, Sk, D,
+                      int(q_pos0), int(k_pos0), int(bool(causal)), _lib.ptr(bias), 0 if bias is None else bias.shape[1],
+                      _lib.ptr(seg), 0 if seg is None else seg.shape[1], 1.0 / math.sqrt(D), int(bool(init)), *tail)
+        return
     if scales is not None:   # (sq, sk, sv, sdo)
         _lib.call("lwm_attn_bwd_step_f16", _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(dout), _lib.ptr(scales[0]),
                   _lib.ptr(scales[1]), _lib.ptr(scales[2]), _lib.ptr(scales[3]), _lib.ptr(lse), _lib.ptr(delta),
@@ -256,6 +304,26 @@ def bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, 
               1.0 / math.sqrt(D), int(bool(init)), _lib.stream_ptr(stream))
 
 
+def _map_kw(q, k, q_pos0, k_pos0, causal, bias, seg, fwd):
+    """{} without a bias and segment ids, else {"tilemap": this step's forward (fwd) or backward map}"""
+    if bias is None and seg is None:
+        return {}
+    m = step_tilemap(q.shape[0], q.shape[1], k.shape[1], q_pos0, k_pos0, causal, bias, seg, fwd=fwd, bwd=not fwd)
+    return {"tilemap": m[:2] if fwd else m[2:]}
+
+
+def mapped_fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last, **kw):
+    """fwd_step over the step's block map whenever a bias or segment ids are given: the step the ring executors run"""
+    fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last, **kw,
+             **_map_kw(q, k, q_pos0, k_pos0, causal, bias, seg, True))
+
+
+def mapped_bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg, **kw):
+    """bwd_step over the step's block map whenever a bias or segment ids are given"""
+    bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg, **kw,
+             **_map_kw(q, k, q_pos0, k_pos0, causal, bias, seg, False))
+
+
 def cast_f32_to_bf16(src, dst, stream=None):
     _lib.call("lwm_cast_f32_to_bf16", _lib.ptr(src), _lib.ptr(dst), src.numel(), _lib.stream_ptr(stream))
 
@@ -265,10 +333,10 @@ def cast_f32_to_bf16(src, dst, stream=None):
 # ------------------------------------------------------------------------------------------------
 class CudaOps:
     """The injected step functions of ring_exec: thin calls into liblwm_b200.so."""
-    fwd_step = staticmethod(fwd_step)
+    fwd_step = staticmethod(mapped_fwd_step)
     bwd_prep = staticmethod(bwd_prep)
     lse_for_bwd = staticmethod(lse_for_bwd)
-    bwd_step = staticmethod(bwd_step)
+    bwd_step = staticmethod(mapped_bwd_step)
     cast = staticmethod(cast_f32_to_bf16)
 
     @staticmethod
@@ -301,8 +369,8 @@ class CudaOpsF16(CudaOps):
         if last:
             o32 = torch.empty(out.shape, dtype=torch.float32, device=out.device)
             self.out_f32[out.data_ptr()] = o32
-        fwd_step(q16, k16, v16, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last,
-                 scales=(sq, sk, sv), out_f32=o32)
+        mapped_fwd_step(q16, k16, v16, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last,
+                        scales=(sq, sk, sv), out_f32=o32)
 
     @staticmethod
     def lse_for_bwd(lse):
@@ -310,8 +378,8 @@ class CudaOpsF16(CudaOps):
 
     def bwd_step(self, q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg):
         (q16, sq), (k16, sk), (v16, sv), (d16, sd) = self._f16(q), self._f16(k), self._f16(v), self._f16(dout)
-        bwd_step(q16, k16, v16, d16, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg,
-                 scales=(sq, sk, sv, sd))
+        mapped_bwd_step(q16, k16, v16, d16, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg,
+                        scales=(sq, sk, sv, sd))
 
 
 def _f32_residuals(ops, res):
@@ -361,8 +429,8 @@ class PeerOpsF16:
 
     @staticmethod
     def fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last, scales, out_f32):
-        fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last, scales=scales,
-                 out_f32=out_f32)
+        mapped_fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last,
+                        scales=scales, out_f32=out_f32)
 
     @staticmethod
     def bwd_prep(out, dout16, sdo, delta):
@@ -376,8 +444,8 @@ class PeerOpsF16:
 
     @staticmethod
     def bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg, scales, init):
-        bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg, scales=scales,
-                 init=init)
+        mapped_bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg,
+                        scales=scales, init=init)
 
     @staticmethod
     def reduce_cast(srcs, dst):
@@ -398,7 +466,7 @@ class PeerOpsBf16(PeerOpsF16):
 
     @staticmethod
     def fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last, scales, out_f32):
-        fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last)
+        mapped_fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last)
         if last and out_f32 is not None:
             out_f32.copy_(out)
 
@@ -412,7 +480,7 @@ class PeerOpsBf16(PeerOpsF16):
 
     @staticmethod
     def bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg, scales, init):
-        bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg, init=init)
+        mapped_bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg, init=init)
 
 
 _PEER_BROKEN = {}      # process group id -> reason: the peer-memory heaps could not be set up for this group

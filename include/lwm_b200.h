@@ -213,6 +213,26 @@ int lwm_attn_infer_partial(const void* q16, const void* k16, const void* v16, co
                            const int* tile_count, float* o_part, float* ml_part, void* workspace, int B, int H, int Q,
                            int Sk, int D, int splits, float softmax_scale, void* stream);
 
+/* Backward of the inference op (the VJP of s = where(mask, q.k/sqrt(D), finfo.min), softmax(s) v):
+ * lwm_attn_infer_bwd_tilemap  bits [B][Q][ceil(Sk/128)*4] (null: every key visible), row_any [B][Q] over ALL keys of the
+ *                         ring (null: every row live) -> per (b, 128-key tile) the ascending list of 64-row Q tiles,
+ *                         tiles [B][ceil(Sk/128)][ceil(Q/64)] (t*2 + mixed) and tile_count [B][ceil(Sk/128)]. A pair is
+ *                         left out when no live row (row < Q, row_any set) has a true bit in it, and clean (no mask
+ *                         read) when every live row's bits are all true and every key is < Sk.
+ * lwm_attn_infer_bwd      q16 / dout16 [B,Q,H,128], k16 / v16 [B,Sk,H,128] scaled fp16 copies with their device scales,
+ *                         any Q and Sk. lse: lwm_attn_bwd_lse of the forward's lse with offset LWM_ATTN_F16_P_BOOST_LOG2,
+ *                         -inf for rows with no visible key, and delta = rowsum(dout o out), both [B,H,Qp] with
+ *                         Qp = Q rounded up to 64 (rows >= Q: lse -inf). dq_acc [B,Q,H,128] fp32 is accumulated into;
+ *                         dk_acc / dv_acc [B,Sk,H,128] fp32 are written. Masked entries and keys >= Sk contribute
+ *                         nothing; nothing outside the tensors' rows is read or written. */
+int lwm_attn_infer_bwd_tilemap(const unsigned* bits, const int* row_any, int B, int Q, int Sk, int* tiles,
+                               int* tile_count, void* stream);
+int lwm_attn_infer_bwd(const void* q16, const void* k16, const void* v16, const void* dout16, const float* scale_q,
+                       const float* scale_k, const float* scale_v, const float* scale_do, const float* lse,
+                       const float* delta, const unsigned* bits, const int* tiles, const int* tile_count,
+                       float* dq_acc, float* dk_acc, float* dv_acc, int B, int H, int Q, int Sk, int D,
+                       float softmax_scale, void* stream);
+
 /* Attention prologue: rotary position embedding (lwm/llama.py:344-375 precompute_freqs_cis / apply_rotary_emb, applied
  * at llama.py:517-519 on the head-split projections right before the ring-attention call; SURVEY.md §8f next-row 2).
  * xq [B,S,Hq,128], xk [B,S,Hk,128] (= the [B,S,H*128] projection outputs: the head split is a view), dtype codes

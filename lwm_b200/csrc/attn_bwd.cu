@@ -47,6 +47,11 @@ struct BwdParams {
   // 64-row Q tiles, entries qt * 2 + mixed
   const int* tiles;       // [B, Sk/128, Sq/64]
   const int* tile_count;  // [B, Sk/128]
+  // kBits (the backward of ringattention_inference): Sq is the query length rounded up to 64 (the row stride of lse,
+  // delta and the lists), q_rows the real one; Sk is the real key length (any value, K tiles = gridDim.x). bits is the
+  // forward's mask, [B, q_rows, gridDim.x * 4] words (bit j of word w <=> key 32 w + j; 1 = attend), or null.
+  const uint32_t* bits;
+  int q_rows;
 };
 
 constexpr int kBQ = 64;                         // query rows per inner iteration
@@ -96,7 +101,11 @@ constexpr float kPBoostInv = 1.0f / 16384.0f;
 // kMap: the CTA walks its K tile's list of Q tiles instead of i_start .. n_q_tiles (pairs whose entries are all masked
 // are not in it: they would add exact zeros); mixed tiles run the per-element mask, clean tiles the same branch with no
 // bias or segment read.
-template <bool kF16, bool kMap = false>
+// kBits (with kMap): the backward of the inference op. The lists come from lwm_attn_infer_bwd_tilemap; clean tiles take
+// the unmasked path, mixed tiles read one mask word per query column and give masked entries and keys >= Sk P = 0.
+// Rows >= q_rows and rows without any visible key carry lse = -inf (P = 0, dS = 0). Q / dO rows past q_rows and K / V
+// rows past Sk are zero-filled by TMA, the dQ reduction clips rows >= q_rows, and dK / dV rows >= Sk are not written.
+template <bool kF16, bool kMap = false, bool kBits = false>
 __global__ void __launch_bounds__(kBwdThreads, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
@@ -135,6 +144,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     if (p.dkv_init) {
       const long long base = (((long long)b * p.Sk + (long long)n * kTile) * p.H + h) * kHeadDim;
       for (int i = threadIdx.x; i < kTile * kHeadDim / 4; i += kBwdThreads) {
+        if (kBits && n * kTile + i / (kHeadDim / 4) >= p.Sk) break;   // rows past the cache: not ours to write
         const long long off = base + (long long)(i / (kHeadDim / 4)) * p.H * kHeadDim + (i % (kHeadDim / 4)) * 4;
         *reinterpret_cast<float4*>(p.dk_acc + off) = make_float4(0.f, 0.f, 0.f, 0.f);
         *reinterpret_cast<float4*>(p.dv_acc + off) = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -257,7 +267,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     // ---- P^T = exp2(S^T * scale_log2 (+bias) - lse2)
     const int q_tile_pos = p.mask.q_pos0 + (kMap ? entry >> 1 : i_start + it) * kBQ;
     // kMap: clean tiles keep the masked path's rounding (fmaf(s, scale, 0)): bit-identical to the step without a map
-    const bool need_mask = kMap || has_bias || has_seg || (p.mask.causal && q_tile_pos < wg_k_last);
+    const bool need_mask =
+        kBits ? bool(entry & 1) : (kMap || has_bias || has_seg || (p.mask.causal && q_tile_pos < wg_k_last));
     const bool mixed = kMap ? (entry & 1) : true;   // the tile reads bias and segment ids
     uint32_t pk[4][4], dsk[4][4];   // P^T and dS^T as A fragments, one 16-query slice per entry
     float pr[4][8];
@@ -268,6 +279,27 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         const int col = (i >> 2) * 8 + quad * 2 + (i & 1);   // query column in the tile
         pr[i >> 3][i & 7] = ex2f(fmaf(sacc[i], scale_log2, s_lse[st][col]));   // -lse*log2e (or -inf): lwm_attn_bwd_lse
       }
+    } else if constexpr (kBits) {
+      // keys kr0 and kr0 + 8 sit in one 32-bit word of every query row's bits (bits sh and sh + 8). Rows past q_rows
+      // read the last row instead: their lse is -inf, whatever the bits say. Masked entries and keys >= Sk get P = 0.
+      const int key0 = n * kTile + kr0;
+      const int sh = key0 & 31;
+      const int kw = gridDim.x * 4;
+      const uint32_t* wcol = p.bits ? p.bits + (long long)b * p.q_rows * kw + (key0 >> 5) : nullptr;
+      const bool key_in[2] = {key0 < p.Sk, key0 + 8 < p.Sk};
+#pragma unroll
+      for (int g = 0; g < 8; ++g)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int col = g * 8 + quad * 2 + e;
+          const uint32_t word = wcol ? wcol[(long long)min(q_tile_pos + col, p.q_rows - 1) * kw] : ~0u;
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            const int i = 4 * g + 2 * hh + e;
+            const bool vis = key_in[hh] && ((word >> (sh + 8 * hh)) & 1u);
+            pr[i >> 3][i & 7] = vis ? ex2f(fmaf(sacc[i], scale_log2, s_lse[st][col])) : 0.f;
+          }
+        }
     } else {
       // per-key mask inputs, reloaded per masked tile (L1 hits) rather than held in registers across the loop
       const bool use_bias = has_bias && mixed, use_seg = has_seg && mixed;
@@ -382,6 +414,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const float dv_mul = kF16 ? (*p.scale_do) * kPBoostInv : 1.0f;
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
+    if (kBits && n * kTile + kr0 + 8 * hh >= p.Sk) continue;   // key rows past the cache are not written
     const long long row = ((((long long)b * p.Sk + (long long)n * kTile + kr0 + 8 * hh) * p.H + h) * kHeadDim);
 #pragma unroll
     for (int g = 0; g < kHeadDim / 8; ++g) {
@@ -541,4 +574,53 @@ extern "C" int lwm_attn_bwd_step_map_f16(const void* q16, const void* k16, const
   return attn_bwd_launch(q16, k16, v16, dout16, lse, delta, dq_acc, dk_acc, dv_acc, B, H, Sq, Sk, D, q_pos0, k_pos0,
                          causal, bias, bias_stride, segment_ids, seg_stride, softmax_scale, scale_q, scale_k, scale_v,
                          scale_do, dkv_init, tiles, tile_count, stream);
+}
+
+// Backward of ringattention_inference (attn_bwd_kernel<true, true, true>): any Q and Sk. q16 / dout16 [B,Q,H,128],
+// k16 / v16 [B,Sk,H,128] scaled fp16 copies with their device scales; lse (pre-scaled by lwm_attn_bwd_lse with the fp16
+// offset, -inf for rows without a visible key) and delta [B,H,Qp], Qp = Q rounded up to 64, rows >= Q: lse = -inf;
+// bits [B,Q,ceil(Sk/128)*4] or null; tiles / tile_count from lwm_attn_infer_bwd_tilemap. dq_acc [B,Q,H,128] fp32 is
+// accumulated into (zero it first); dk_acc / dv_acc [B,Sk,H,128] fp32 are written.
+extern "C" int lwm_attn_infer_bwd(const void* q16, const void* k16, const void* v16, const void* dout16,
+                                  const float* scale_q, const float* scale_k, const float* scale_v,
+                                  const float* scale_do, const float* lse, const float* delta, const unsigned* bits,
+                                  const int* tiles, const int* tile_count, float* dq_acc, float* dk_acc, float* dv_acc,
+                                  int B, int H, int Q, int Sk, int D, float softmax_scale, void* stream) {
+  if (D != kHeadDim) return lwm_fail(LWM_ERR_SHAPE, "attn_infer_bwd: head_dim must be 128");
+  if (!q16 || !k16 || !v16 || !dout16 || !scale_q || !scale_k || !scale_v || !scale_do || !lse || !delta || !tiles ||
+      !tile_count || !dq_acc || !dk_acc || !dv_acc)
+    return lwm_fail(LWM_ERR_ARG, "attn_infer_bwd: null pointer");
+  if (B <= 0 || H <= 0 || Q <= 0 || Sk <= 0 || B > 65535 || H > 65535)
+    return lwm_fail(LWM_ERR_SHAPE, "attn_infer_bwd: bad shape (B, H <= 65535; Q, Sk >= 1)");
+  const int n_kt = (Sk + kTile - 1) / kTile, qp = (Q + kBQ - 1) / kBQ * kBQ;
+  if ((long long)B * n_kt * (qp / kBQ) > 0x7fffffffLL || (long long)Q + kBQ > 0x7fffffffLL)
+    return lwm_fail(LWM_ERR_SHAPE, "attn_infer_bwd: B * ceil(Sk/128) * ceil(Q/64) must fit in int32");
+  if (!lwm_check_device()) return LWM_ERR_DEVICE;
+  CUtensorMap tq, tk, tv, tdo, tdq;
+  if (!make_bf16_tmap(&tq, q16, B, Q, H, kBQ) || !make_bf16_tmap(&tk, k16, B, Sk, H, kTile) ||
+      !make_bf16_tmap(&tv, v16, B, Sk, H, kTile) || !make_bf16_tmap(&tdo, dout16, B, Q, H, kBQ) ||
+      !make_f32_tmap(&tdq, dq_acc, B, Q, H, kBQ))
+    return lwm_fail(LWM_ERR_CUDA, "attn_infer_bwd: cuTensorMapEncodeTiled failed (pointers must be 16B aligned)");
+  BwdParams p{};
+  p.B = B; p.H = H; p.Sq = qp; p.Sk = Sk;
+  p.scale = softmax_scale;
+  p.scale_log2 = softmax_scale * kLog2e;
+  p.lse = lse; p.delta = delta; p.dq_acc = dq_acc; p.dk_acc = dk_acc; p.dv_acc = dv_acc;
+  p.scale_q = scale_q; p.scale_k = scale_k; p.scale_v = scale_v; p.scale_do = scale_do;
+  p.dkv_init = 1;
+  p.tiles = tiles; p.tile_count = tile_count;
+  p.bits = bits; p.q_rows = Q;
+  static bool attr_set_dev[64] = {};
+  int cur_dev = 0;
+  cudaGetDevice(&cur_dev);
+  bool& attr_set = attr_set_dev[cur_dev & 63];
+  if (!attr_set) {
+    if (cudaFuncSetAttribute(attn_bwd_kernel<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             kBwdSmemBytes) != cudaSuccess)
+      return lwm_fail(LWM_ERR_CUDA, "attn_infer_bwd: cannot raise dynamic shared memory limit");
+    attr_set = true;
+  }
+  attn_bwd_kernel<true, true, true><<<dim3(n_kt, H, B), kBwdThreads, kBwdSmemBytes,
+                                      reinterpret_cast<cudaStream_t>(stream)>>>(tq, tk, tv, tdo, tdq, p);
+  return lwm_check_launch("attn_bwd_kernel (inference)");
 }

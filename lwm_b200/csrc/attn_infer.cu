@@ -62,6 +62,35 @@ infer_tilemap_kernel(const uint32_t* __restrict__ bits, const int* __restrict__ 
   if (threadIdx.x == 0) tile_count[(long long)b * n_qt + qt] = n;
 }
 
+// The backward's map, transposed: per (b, 128-key tile) the ascending list of 64-row Q tiles, entries t * 2 + mixed.
+// Only live rows count (row < Q and row_any set): a fully masked row contributes nothing to any gradient, so it forces
+// no visit and does not stop a tile from being clean. A pair is skipped when no live row has a true bit in the tile,
+// clean when every live row's bits are all true and every key is < Sk, mixed otherwise.
+constexpr int kBwdMapRows = 64;
+
+__global__ void __launch_bounds__(kBwdMapRows)
+infer_bwd_tilemap_kernel(const uint32_t* __restrict__ bits, const int* __restrict__ row_any, int Q, int Sk, int n_kt,
+                         int n_qt, int* __restrict__ tiles, int* __restrict__ tile_count) {
+  const int kt = blockIdx.x, b = blockIdx.y;
+  const bool tail = (kt + 1) * kTile > Sk;
+  int* out = tiles + ((long long)b * n_kt + kt) * n_qt;
+  int n = 0;
+  for (int t = 0; t < n_qt; ++t) {
+    const int row = t * kBwdMapRows + threadIdx.x;
+    const bool live = row < Q && (!row_any || row_any[(long long)b * Q + row] != 0);
+    int any_t = live, all_t = 1;      // no mask: every live row sees every key
+    if (live && bits) {
+      const uint4 w = *reinterpret_cast<const uint4*>(bits + ((long long)b * Q + row) * (n_kt * 4) + kt * 4);
+      any_t = (w.x | w.y | w.z | w.w) != 0u;
+      all_t = (w.x & w.y & w.z & w.w) == ~0u;
+    }
+    const int any = __syncthreads_or(any_t);
+    const int all = __syncthreads_and(all_t);
+    if (threadIdx.x == 0 && any) out[n++] = t * 2 + ((tail || !all) ? 1 : 0);
+  }
+  if (threadIdx.x == 0) tile_count[(long long)b * n_kt + kt] = n;
+}
+
 }  // namespace lwm
 
 using namespace lwm;
@@ -96,4 +125,18 @@ extern "C" int lwm_attn_infer_tilemap(const unsigned* bits, const int* row_any, 
   infer_tilemap_kernel<<<dim3((Q + kTile - 1) / kTile, B), kTile, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       bits, row_any, Q, Sk, (Sk + kTile - 1) / kTile, tiles, tile_count);
   return lwm_check_launch("infer_tilemap_kernel");
+}
+
+// bits [B][Q][ceil(Sk/128)*4] or null (every key visible); row_any [B][Q] (global over the ring) or null (every row
+// live) -> tiles [B][ceil(Sk/128)][ceil(Q/64)], tile_count [B][ceil(Sk/128)] for lwm_attn_infer_bwd.
+extern "C" int lwm_attn_infer_bwd_tilemap(const unsigned* bits, const int* row_any, int B, int Q, int Sk, int* tiles,
+                                          int* tile_count, void* stream) {
+  if (!tiles || !tile_count) return lwm_fail(LWM_ERR_ARG, "attn_infer_bwd_tilemap: null pointer");
+  if (B <= 0 || Q <= 0 || Sk <= 0 || B > 65535 || Q > 0x7fffffff - kBwdMapRows)
+    return lwm_fail(LWM_ERR_SHAPE, "attn_infer_bwd_tilemap: bad shape");
+  if (!lwm_check_device()) return LWM_ERR_DEVICE;
+  const int n_kt = (Sk + kTile - 1) / kTile, n_qt = (Q + kBwdMapRows - 1) / kBwdMapRows;
+  infer_bwd_tilemap_kernel<<<dim3(n_kt, B), kBwdMapRows, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      bits, row_any, Q, Sk, n_kt, n_qt, tiles, tile_count);
+  return lwm_check_launch("infer_bwd_tilemap_kernel");
 }

@@ -66,6 +66,20 @@ def decode_attention_mask(attention_mask, query_length, cache_index, max_decoder
     return (attention_mask[:, None, None, :K] > 0) & causal[None, None]
 
 
+def causal_attention_mask(attention_mask, segment_ids=None, query_length=None):
+    """Boolean mask [B,1,Q,Q] for `ringattention_inference` without a KV cache (lwm/llama.py:580-592), the branch
+    training takes for short sequences: causal (key j <= query i) AND padding (attention_mask [B,S] > 0 at the key)
+    AND, with segment_ids [B,S], same segment (combine_masks). Q = query_length, default S."""
+    Q = attention_mask.shape[-1] if query_length is None else int(query_length)
+    dev = attention_mask.device
+    causal = torch.ones(Q, Q, dtype=torch.bool, device=dev).tril_()
+    m = (attention_mask[:, None, None, :Q] > 0) & causal[None, None]
+    if segment_ids is not None:
+        seg = segment_ids[:, :Q]
+        m = m & (seg[:, :, None] == seg[:, None, :])[:, None]
+    return m
+
+
 def _resolve_group(axis_name):
     if not (dist.is_available() and dist.is_initialized()):
         return None, 0, 1
@@ -258,6 +272,7 @@ def bwd_prep(out, dout, delta, stream=None):
 
 
 F16_P_BOOST_LOG2 = 14.0      # include/lwm_b200.h: LWM_ATTN_F16_P_BOOST_LOG2
+LWM_REDUCE_MAX_SRCS = 16     # include/lwm_b200.h: sources per lwm_reduce_cast_f32 call
 
 
 def lse_for_bwd(lse, stream=None, f16=False):
@@ -649,15 +664,16 @@ def decode_partial(q, k, v, mask_u8, k_pos0, stream=None):
     return o_part, ml_part
 
 
-def decode_merge(o_parts, ml_parts, n_part, out_shape, dtype):
-    """merge n_part partials per row ([rows][n_part][128], [rows][n_part][2]) into the normalised output"""
+def decode_merge(o_parts, ml_parts, n_part, out_shape, dtype, with_lse=False):
+    """merge n_part partials per row ([rows][n_part][128], [rows][n_part][2]) into the normalised output;
+    with_lse: -> (out, lse [rows], natural log)"""
     out = torch.empty(out_shape, dtype=dtype, device=o_parts.device)
     rows = o_parts.shape[0]
     lse = torch.empty(rows, dtype=torch.float32, device=o_parts.device)
     fn = "lwm_attn_decode_merge_f32" if dtype == torch.float32 else "lwm_attn_decode_merge"
     _lib.call(fn, _lib.ptr(o_parts), _lib.ptr(ml_parts), n_part, _lib.ptr(out), _lib.ptr(lse), rows,
               _lib.stream_ptr())
-    return out
+    return (out, lse) if with_lse else out
 
 
 def mask_pack(mask, B, n_slabs, ncols):
@@ -682,10 +698,11 @@ def _scaled_f16(x):
     return _stage_local(PeerOpsF16, x, scale), scale
 
 
-def infer_partial(q, k, v, bits, row_any):
+def infer_partial(q, k, v, bits, row_any, staged=None):
     """This rank's partial with the tensor-core kernel: q [B,Q,H,128] against k/v [B,Sk,H,128] (bf16 or fp32, staged
     to scaled fp16 here), bits [B,Q,kw] / row_any [B,Q] (row_any over the whole ring) or None
-    -> (o_part [B*Q*H,128], ml_part [B*Q*H,2])."""
+    -> (o_part [B*Q*H,128], ml_part [B*Q*H,2]). staged: the caller's ((q16, sq), (k16, sk), (v16, sv)) of
+    _scaled_f16, used instead of staging q, k, v again."""
     B, Q, H, D = q.shape
     Sk = k.shape[1]
     dev = q.device
@@ -694,7 +711,9 @@ def infer_partial(q, k, v, bits, row_any):
     counts = torch.empty(B, n_qt, dtype=torch.int32, device=dev)
     _lib.call("lwm_attn_infer_tilemap", _lib.ptr(bits), _lib.ptr(row_any), B, Q, Sk, _lib.ptr(tiles),
               _lib.ptr(counts), _lib.stream_ptr())
-    (q16, sq), (k16, sk), (v16, sv) = _scaled_f16(q), _scaled_f16(k), _scaled_f16(v)
+    if staged is None:
+        staged = _scaled_f16(q), _scaled_f16(k), _scaled_f16(v)
+    (q16, sq), (k16, sk), (v16, sv) = staged
     ctas = n_qt * H * B
     splits = 1 if ctas >= 132 else min(n_kt, -(-132 // ctas))     # key splits: fill the 132 SMs
     rows = B * Q * H
@@ -707,17 +726,76 @@ def infer_partial(q, k, v, bits, row_any):
     return o_part, ml_part
 
 
+def infer_backward(q16, k16, v16, do16, scales, lse, delta, bits, row_any):
+    """One backward launch of the inference op over this rank's keys: q16 / do16 [B,Q,H,128], k16 / v16 [B,Sk,H,128]
+    scaled fp16 copies, scales = (sq, sk, sv, sdo); lse [B,H,Q] (natural log, -inf for rows with no visible key),
+    delta [B,H,Q] = rowsum(dO o O); bits [B,Q,kw] / row_any [B,Q] (over the whole ring) or None
+    -> fp32 (dq [B,Q,H,128], dk, dv [B,Sk,H,128])."""
+    B, Q, H, D = q16.shape
+    Sk = k16.shape[1]
+    dev = q16.device
+    n_kt, Qp = (Sk + 127) // 128, (Q + 63) // 64 * 64
+    tiles = torch.empty(B, n_kt, Qp // 64, dtype=torch.int32, device=dev)
+    counts = torch.empty(B, n_kt, dtype=torch.int32, device=dev)
+    _lib.call("lwm_attn_infer_bwd_tilemap", _lib.ptr(bits), _lib.ptr(row_any), B, Q, Sk, _lib.ptr(tiles),
+              _lib.ptr(counts), _lib.stream_ptr())
+    # lse / delta padded to whole 64-row tiles: the padding rows get P = 0
+    lse_p = torch.full((B, H, Qp), -math.inf, dtype=torch.float32, device=dev)
+    lse_p[..., :Q] = lse
+    delta_p = torch.zeros((B, H, Qp), dtype=torch.float32, device=dev)
+    delta_p[..., :Q] = delta
+    nlse = lse_for_bwd(lse_p, f16=True)
+    dq = torch.zeros((B, Q, H, D), dtype=torch.float32, device=dev)
+    dk = torch.empty((B, Sk, H, D), dtype=torch.float32, device=dev)
+    dv = torch.empty((B, Sk, H, D), dtype=torch.float32, device=dev)
+    sq, sk, sv, sdo = scales
+    _lib.call("lwm_attn_infer_bwd", _lib.ptr(q16), _lib.ptr(k16), _lib.ptr(v16), _lib.ptr(do16), _lib.ptr(sq),
+              _lib.ptr(sk), _lib.ptr(sv), _lib.ptr(sdo), _lib.ptr(nlse), _lib.ptr(delta_p), _lib.ptr(bits),
+              _lib.ptr(tiles), _lib.ptr(counts), _lib.ptr(dq), _lib.ptr(dk), _lib.ptr(dv), B, H, Q, Sk, D,
+              1.0 / math.sqrt(D), _lib.stream_ptr())
+    return dq, dk, dv
+
+
 class InferOps:
-    """The kernels of the q-sharded protocol (_infer_sharded); tests substitute stand-ins."""
+    """The kernels of the q-sharded protocol (_infer_sharded, _infer_sharded_bwd); tests substitute stand-ins."""
     mask_pack = staticmethod(mask_pack)
     merge = staticmethod(decode_merge)
+    stage = staticmethod(_scaled_f16)
+    backward = staticmethod(infer_backward)
+    reduce_cast = staticmethod(PeerOpsF16.reduce_cast)
 
     @staticmethod
-    def partial(q, k, v, mask, row_any, tensor_cores):
-        """mask: bits [B,Q,kw] when tensor_cores, else uint8 [B,Q,Sk] (or None)"""
+    def partial(q, k, v, mask, row_any, tensor_cores, staged=None):
+        """mask: bits [B,Q,kw] when tensor_cores, else uint8 [B,Q,Sk] (or None); staged: see infer_partial"""
         if tensor_cores:
-            return infer_partial(q, k, v, mask, row_any)
+            return infer_partial(q, k, v, mask, row_any, staged)
         return decode_partial(q, k, v, mask, 0)
+
+    @staticmethod
+    def merge_lse(o, ml, n_part, out_shape):
+        """-> (fp32 output, lse [rows], natural log)"""
+        return decode_merge(o, ml, n_part, out_shape, torch.float32, with_lse=True)
+
+    @staticmethod
+    def stage_by(x, scale):
+        """scaled fp16 copy of x with a given scale"""
+        return _stage_local(PeerOpsF16, x, scale)
+
+    @staticmethod
+    def delta(o32, do16, sdo):
+        """rowsum(dO o O) [B,H,Q] from the fp32 output and the staged dO"""
+        B, Q, H, D = o32.shape
+        d = torch.empty((B, H, Q), dtype=torch.float32, device=o32.device)
+        PeerOpsF16.bwd_prep(o32, do16, sdo, d)
+        return d
+
+    @staticmethod
+    def cast(x32, dtype):
+        if dtype == torch.float32:
+            return x32
+        y = torch.empty(x32.shape, dtype=dtype, device=x32.device)
+        cast_f32_to_bf16(x32, y)
+        return y
 
 
 class TorchComm:
@@ -740,11 +818,35 @@ class TorchComm:
         return out
 
 
-def _infer_sharded(q, k, v, mask, comm, ops=InferOps):
+class _LocalComm:
+    """The collectives of a ring of one: the single-GPU backward runs the q-sharded backward with world = 1."""
+    world = 1
+
+    @staticmethod
+    def all_gather(x):
+        return x[None]
+
+    @staticmethod
+    def all_to_all(x):
+        return x
+
+
+def _return_partials(o, ml, comm, B, Ql, H, D):
+    """partials of all world*Q_loc rows over my keys -> each owner's rows' partials, [B*Q_loc*H, world, D / 2]"""
+    W = comm.world
+    o = comm.all_to_all(o.view(B, W, Ql, H, D).transpose(0, 1))
+    ml = comm.all_to_all(ml.view(B, W, Ql, H, 2).transpose(0, 1))
+    o = o.permute(1, 2, 3, 0, 4).reshape(B * Ql * H, W, D)
+    ml = ml.permute(1, 2, 3, 0, 4).reshape(B * Ql * H, W, 2)
+    return o.contiguous(), ml.contiguous()
+
+
+def _infer_sharded(q, k, v, mask, comm, ops=InferOps, saved=None):
     """q-sharded protocol (query length > 1 on a ring of comm.world ranks): q [B,Q_loc,H,D] and mask [Bm,1,Q_loc,K]
     are this rank's query rows, k/v [B,S_loc,H,D] its KV shard (K = world*S_loc). Each rank computes the partials of
     ALL world*Q_loc rows over its own keys, so K/V never move; per rank the traffic is world*Q_loc*H*D words of q and
-    of partials plus Q_loc*K/8 bytes of mask. Returns this rank's [B,Q_loc,H,D] output."""
+    of partials plus Q_loc*K/8 bytes of mask. Returns this rank's [B,Q_loc,H,D] output.
+    saved: None, or a dict that receives what _infer_sharded_bwd needs (the output is the same either way)."""
     B, Ql, H, D = q.shape
     Sk = k.shape[1]
     W = comm.world
@@ -768,14 +870,87 @@ def _infer_sharded(q, k, v, mask, comm, ops=InferOps):
             slabs = m8[:, 0, :, :W * Sk].expand(B, Ql, W * Sk).reshape(B, Ql, W, Sk).permute(2, 0, 1, 3)
             m = comm.all_to_all(slabs).transpose(0, 1).reshape(B, Qg, Sk)
     # 4. partials of all rows over my keys (key splits merged locally)
-    o, ml = ops.partial(q_all, k, v, m, row_any, tc)
+    if saved is None:
+        o, ml = ops.partial(q_all, k, v, m, row_any, tc)
+    elif tc:
+        staged = ops.stage(q_all), ops.stage(k), ops.stage(v)
+        o, ml = ops.partial(q_all, k, v, m, row_any, tc, staged=staged)
+        saved.update(staged=staged, bits=m, row_any=row_any)
+    else:
+        # the backward recomputes the row statistics on tensor cores (_infer_sharded_bwd)
+        o, ml = ops.partial(q_all, k, v, m, row_any, tc)
+        saved.update(q_all=q_all, k=k, v=v, slabs=m)
     # 5. each owner gets its rows' partials back
-    o = comm.all_to_all(o.view(B, W, Ql, H, D).transpose(0, 1))
-    ml = comm.all_to_all(ml.view(B, W, Ql, H, 2).transpose(0, 1))
+    o, ml = _return_partials(o, ml, comm, B, Ql, H, D)
     # 6. merge the world partials
-    o = o.permute(1, 2, 3, 0, 4).reshape(B * Ql * H, W, D)
-    ml = ml.permute(1, 2, 3, 0, 4).reshape(B * Ql * H, W, 2)
-    return ops.merge(o.contiguous(), ml.contiguous(), W, (B, Ql, H, D), q.dtype)
+    out = ops.merge(o, ml, W, (B, Ql, H, D), q.dtype)
+    if saved is not None and tc:
+        # the fp32 output and lse of my rows, from a second merge of the same partials
+        saved["o32"], saved["lse"] = ops.merge_lse(o, ml, W, (B, Ql, H, D))
+    return out
+
+
+def _row_stats_tc(q_all, k, v, slabs, comm, ops):
+    """A forward that ran the GEMV kernel (world*Q_loc < INFER_MIN_Q): its uint8 mask slabs [B,Qg,S_loc] (or None)
+    become bits, row_any is made global, and the fp32 output and lse of my rows are recomputed with one tensor-core
+    partial and merge on the staged operands, so that the backward's P sums to one over each row.
+    -> (staged, bits, row_any, o32, lse)"""
+    B, Qg, H, D = q_all.shape
+    W = comm.world
+    bits = row_any = None
+    if slabs is not None:
+        bits, any_loc = ops.mask_pack(slabs[:, None], B, 1, k.shape[1])
+        bits = bits[0]
+        row_any = comm.all_gather(any_loc).amax(0)
+    staged = ops.stage(q_all), ops.stage(k), ops.stage(v)
+    o, ml = ops.partial(q_all, k, v, bits, row_any, True, staged=staged)
+    o, ml = _return_partials(o, ml, comm, B, Qg // W, H, D)
+    o32, lse = ops.merge_lse(o, ml, W, (B, Qg // W, H, D))
+    return staged, bits, row_any, o32, lse
+
+
+def _infer_sharded_bwd(saved, dout, comm, ops=InferOps):
+    """Backward of _infer_sharded (and, with world = 1, of the single-GPU op), mirroring its protocol: K and V never
+    move. dout [B,Q_loc,H,D] is the gradient of this rank's rows; saved is what the forward recorded.
+      1. all-gather dO; every rank stages all world*Q_loc rows with one shared scale;
+      2. the owner computes delta = rowsum(dO o O) of its rows (its dO staged with that scale, its fp32 O);
+      3. all-gather lse and delta;
+      4. one backward launch of all rows against the local K/V: dK and dV come out complete on their owner;
+      5. the fp32 dQ partials go back to the row owners (all_to_all), which sum them in rank order.
+    Per rank the traffic is world*Q_loc*H*D words of dO and of fp32 dQ partials, plus world*Q_loc*H*2 floats of lse
+    and delta. -> (dq, dk, dv) in dout's dtype."""
+    B, Ql, H, D = dout.shape
+    W = comm.world
+    Qg = W * Ql
+    if "o32" in saved:
+        staged, bits, row_any, o32, lse = (saved[n] for n in ("staged", "bits", "row_any", "o32", "lse"))
+    else:
+        staged, bits, row_any, o32, lse = _row_stats_tc(saved["q_all"], saved["k"], saved["v"], saved["slabs"],
+                                                        comm, ops)
+    (q16, sq), (k16, sk), (v16, sv) = staged
+    # 1.
+    do_all = comm.all_gather(dout).transpose(0, 1).reshape(B, Qg, H, D)
+    do16, sdo = ops.stage(do_all)
+    # 2. (the owner's rows of do16, staged again from its own dout: the same values)
+    delta = ops.delta(o32, ops.stage_by(dout, sdo), sdo)                         # [B,H,Ql]
+    # 3.
+    stats = torch.stack([lse.view(B, Ql, H).permute(0, 2, 1).to(delta.dtype), delta])
+    stats = comm.all_gather(stats).permute(1, 2, 3, 0, 4).reshape(2, B, H, Qg)
+    lse_all, delta_all = stats[0], stats[1]
+    if row_any is not None:       # rows with no visible key over the whole ring contribute nothing
+        lse_all = torch.where(row_any[:, None, :] != 0, lse_all, torch.full_like(lse_all, -math.inf))
+    # 4.
+    dq, dk, dv = ops.backward(q16, k16, v16, do16, (sq, sk, sv, sdo), lse_all, delta_all, bits, row_any)
+    # 5.
+    parts = comm.all_to_all(dq.view(B, W, Ql, H, D).transpose(0, 1))
+    dq = torch.empty((B, Ql, H, D), dtype=dout.dtype, device=dout.device)
+    srcs = [parts[r] for r in range(W)]
+    while len(srcs) > LWM_REDUCE_MAX_SRCS:      # fold the first 16 in fp32, keep the rank order
+        acc = torch.empty(srcs[0].shape, dtype=srcs[0].dtype, device=srcs[0].device)
+        ops.reduce_cast(srcs[:LWM_REDUCE_MAX_SRCS], acc)
+        srcs = [acc] + srcs[LWM_REDUCE_MAX_SRCS:]
+    ops.reduce_cast([s.contiguous() for s in srcs], dq)
+    return dq, ops.cast(dk, dout.dtype), ops.cast(dv, dout.dtype)
 
 
 def ringattention_inference(q, k, v, attn_mask, axis_name="sp"):
@@ -802,15 +977,32 @@ def ringattention_inference(q, k, v, attn_mask, axis_name="sp"):
         if attn_mask.shape[-1] < (world if Q > 1 else rank + 1) * Sk:
             raise ValueError("attn_mask covers %d keys but the ring holds %d" % (attn_mask.shape[-1], world * Sk))
     q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
+    if torch.is_grad_enabled() and (q.requires_grad or k.requires_grad or v.requires_grad):
+        return _InferAttnFn.apply(q, k, v, attn_mask, axis_name)
+    return _infer_forward(q, k, v, attn_mask, group, rank, world)
+
+
+def _infer_forward(q, k, v, attn_mask, group, rank, world, saved=None):
+    """the forward of ringattention_inference; saved: None, or a dict that receives what the backward needs (the
+    output is bit-identical either way)"""
+    B, Q, H, D = q.shape
+    Sk = k.shape[1]
     if world > 1 and Q > 1:
-        return _infer_sharded(q, k, v, attn_mask, TorchComm(group, world))
+        return _infer_sharded(q, k, v, attn_mask, TorchComm(group, world), saved=saved)
     if Q >= INFER_MIN_Q:
         bits = row_any = None
         if attn_mask is not None:
             bits, row_any = mask_pack(attn_mask, B, 1, Sk)
             bits = bits[0]
-        o_part, ml_part = infer_partial(q, k, v, bits, row_any)
-        return decode_merge(o_part, ml_part, 1, (B, Q, H, D), q.dtype)
+        if saved is None:
+            o_part, ml_part = infer_partial(q, k, v, bits, row_any)
+            return decode_merge(o_part, ml_part, 1, (B, Q, H, D), q.dtype)
+        staged = _scaled_f16(q), _scaled_f16(k), _scaled_f16(v)
+        o_part, ml_part = infer_partial(q, k, v, bits, row_any, staged)
+        out = decode_merge(o_part, ml_part, 1, (B, Q, H, D), q.dtype)
+        o32, lse = decode_merge(o_part, ml_part, 1, (B, Q, H, D), torch.float32, with_lse=True)
+        saved.update(staged=staged, bits=bits, row_any=row_any, o32=o32, lse=lse)
+        return out
     mask = None
     if attn_mask is not None:
         mask = attn_mask.to(torch.uint8).expand(B, 1, Q, attn_mask.shape[-1]).contiguous()
@@ -823,4 +1015,50 @@ def ringattention_inference(q, k, v, attn_mask, axis_name="sp"):
         dist.all_gather_into_tensor(ml_all, ml_part, group=group)
         o_part = o_all.permute(1, 0, 2).contiguous()       # [row][rank][D]
         ml_part = ml_all.permute(1, 0, 2).contiguous()
+    elif saved is not None:
+        # GEMV forward: the backward recomputes the row statistics on tensor cores (_row_stats_tc)
+        saved.update(q_all=q, k=k, v=v, slabs=None if attn_mask is None else attn_mask[:, 0])
     return decode_merge(o_part, ml_part, world, (B, Q, H, D), q.dtype)
+
+
+_INFER_SAVED = ("bits", "row_any", "o32", "lse", "q_all", "k", "v", "slabs")
+
+
+class _InferAttnFn(torch.autograd.Function):
+    """ringattention_inference with a backward w.r.t. q, k, v (the mask gets none). Saves the staged fp16 operands
+    with their scales, the fp32 output and lse of this rank's rows and the mask bits with row_any (tensor-core
+    forward), or the operands and mask slabs (GEMV forward: the backward recomputes the row statistics)."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, attn_mask, axis_name):
+        group, rank, world = _resolve_group(axis_name)
+        saved = {}
+        out = _infer_forward(q, k, v, attn_mask, group, rank, world, saved)
+        ctx.axis_name, ctx.replicated = axis_name, world > 1 and q.shape[1] == 1
+        # a ring whose world*Q_loc rows run the GEMV kernel: not validated on real kernels yet (see DESIGN §3.6)
+        ctx.small_ring = world > 1 and 1 < q.shape[1] and world * q.shape[1] < INFER_MIN_Q
+        staged = saved.pop("staged", None)
+        ctx.staged = staged is not None
+        flat = [t for pair in staged for t in pair] if staged is not None else []
+        ctx.keys = [n for n in _INFER_SAVED if n in saved]
+        ctx.save_for_backward(*flat, *[saved[n] for n in ctx.keys])
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        if ctx.replicated:
+            raise NotImplementedError("ringattention_inference: no backward for a single query row replicated along "
+                                      "a ring of more than one rank (the generation call); shard the query rows instead")
+        if ctx.small_ring:
+            raise NotImplementedError("ringattention_inference: no backward on a ring with world * Q_loc < INFER_MIN_Q "
+                                      "(%d) query rows yet" % INFER_MIN_Q)
+        t = ctx.saved_tensors
+        saved = {}
+        if ctx.staged:
+            saved["staged"] = (t[0], t[1]), (t[2], t[3]), (t[4], t[5])
+            t = t[6:]
+        saved.update(zip(ctx.keys, t))
+        group, rank, world = _resolve_group(ctx.axis_name)
+        comm = TorchComm(group, world) if world > 1 else _LocalComm()
+        dq, dk, dv = _infer_sharded_bwd(saved, dout.contiguous(), comm)
+        return dq, dk, dv, None, None

@@ -890,6 +890,22 @@ def _infer_sharded(q, k, v, mask, comm, ops=InferOps, saved=None):
     return out
 
 
+def _infer_replicated(q, k, v, mask, rank, comm, ops=InferOps):
+    """Replicated protocol (one query row, the generation call, on a ring of comm.world ranks): q [B,1,H,D] and mask
+    [Bm,1,1,K] are the same on every rank, k/v [B,S_loc,H,D] are this rank's KV shard (keys [rank*S_loc,
+    (rank+1)*S_loc) of K). Each rank reduces its shard to an (o, max, sum) partial with the GEMV kernel, the partials
+    (a few KB) are all-gathered rank-major and merged. Returns the [B,1,H,D] output, the same on every rank."""
+    B, Q, H, D = q.shape
+    Sk = k.shape[1]
+    m = None
+    if mask is not None:
+        m = mask[:, 0, :, rank * Sk:(rank + 1) * Sk].to(torch.uint8).expand(B, Q, Sk).contiguous()
+    o, ml = ops.partial(q, k, v, m, None, False)
+    o = comm.all_gather(o).transpose(0, 1).contiguous()           # [row][rank][D]
+    ml = comm.all_gather(ml).transpose(0, 1).contiguous()
+    return ops.merge(o, ml, comm.world, (B, Q, H, D), q.dtype)
+
+
 def _row_stats_tc(q_all, k, v, slabs, comm, ops):
     """A forward that ran the GEMV kernel (world*Q_loc < INFER_MIN_Q): its uint8 mask slabs [B,Qg,S_loc] (or None)
     become bits, row_any is made global, and the fp32 output and lse of my rows are recomputed with one tensor-core
@@ -987,8 +1003,10 @@ def _infer_forward(q, k, v, attn_mask, group, rank, world, saved=None):
     output is bit-identical either way)"""
     B, Q, H, D = q.shape
     Sk = k.shape[1]
-    if world > 1 and Q > 1:
-        return _infer_sharded(q, k, v, attn_mask, TorchComm(group, world), saved=saved)
+    if world > 1:
+        if Q > 1:
+            return _infer_sharded(q, k, v, attn_mask, TorchComm(group, world), saved=saved)
+        return _infer_replicated(q, k, v, attn_mask, rank, TorchComm(group, world))
     if Q >= INFER_MIN_Q:
         bits = row_any = None
         if attn_mask is not None:
@@ -1006,19 +1024,11 @@ def _infer_forward(q, k, v, attn_mask, group, rank, world, saved=None):
     mask = None
     if attn_mask is not None:
         mask = attn_mask.to(torch.uint8).expand(B, 1, Q, attn_mask.shape[-1]).contiguous()
-    o_part, ml_part = decode_partial(q, k, v, mask, rank * Sk)
-    rows = B * Q * H
-    if world > 1:
-        o_all = torch.empty(world, rows, D, dtype=torch.float32, device=q.device)
-        ml_all = torch.empty(world, rows, 2, dtype=torch.float32, device=q.device)
-        dist.all_gather_into_tensor(o_all, o_part, group=group)
-        dist.all_gather_into_tensor(ml_all, ml_part, group=group)
-        o_part = o_all.permute(1, 0, 2).contiguous()       # [row][rank][D]
-        ml_part = ml_all.permute(1, 0, 2).contiguous()
-    elif saved is not None:
+    o_part, ml_part = decode_partial(q, k, v, mask, 0)
+    if saved is not None:
         # GEMV forward: the backward recomputes the row statistics on tensor cores (_row_stats_tc)
         saved.update(q_all=q, k=k, v=v, slabs=None if attn_mask is None else attn_mask[:, 0])
-    return decode_merge(o_part, ml_part, world, (B, Q, H, D), q.dtype)
+    return decode_merge(o_part, ml_part, 1, (B, Q, H, D), q.dtype)
 
 
 _INFER_SAVED = ("bits", "row_any", "o32", "lse", "q_all", "k", "v", "slabs")

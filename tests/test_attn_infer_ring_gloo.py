@@ -3,7 +3,9 @@ lwm_b200.ringattention._infer_sharded with its collectives on torch.distributed 
 all_to_all_single), and numpy stand-ins for the mask-packing, partial and merge kernels that follow the kernels'
 contracts (mask bits, fully masked rows, log2-domain partials). Compared against the dense float64 oracle on the
 whole query and cache, with Q_loc not a multiple of 128, fully masked rows, a left-padded decode mask and a
-batch-broadcast mask, on both sides of INFER_MIN_Q."""
+batch-broadcast mask, on both sides of INFER_MIN_Q. The replicated protocol of the generation call
+(lwm_b200.ringattention._infer_replicated, Q = 1) runs the same way under the generation masks of
+tests/test_attn_decode_ring_gpu.py: whole ranks unfilled or padded, a fully masked batch row, a broadcast mask."""
 import os
 import socket
 import sys
@@ -102,6 +104,36 @@ def _worker(rank, world, port, Ql, B, broadcast, use_mask, ret):
         dist.destroy_process_group()
 
 
+def _replicated_worker(rank, world, port, ret):
+    """the replicated (Q = 1, generation) protocol under every generation mask of the GPU test"""
+    sys.path.insert(0, ROOT)
+    os.environ["MASTER_ADDR"] = "127.0.0.1"
+    os.environ["MASTER_PORT"] = str(port)
+    dist.init_process_group("gloo", rank=rank, world_size=world)
+    try:
+        from lwm_b200 import ringattention as ra
+        from oracle.attn_dense import attention_inference_dense
+        from test_attn_decode_ring_gpu import MASK_KINDS, generation_mask
+        B, H, D, Sl = 2, 2, 16, 50
+        K = world * Sl
+        g = torch.Generator().manual_seed(11)
+        q = torch.randn(B, 1, H, D, generator=g)
+        # every rank's shard has its own magnitudes: keys 2^-r, values 2^(6r), 2^(-6r) alternately
+        r_of = torch.arange(K) // Sl
+        k = torch.randn(B, K, H, D, generator=g) * (2.0 ** -r_of)[None, :, None, None]
+        v = torch.randn(B, K, H, D, generator=g) * (2.0 ** (6 * r_of * (-1) ** r_of))[None, :, None, None]
+        keys = slice(rank * Sl, (rank + 1) * Sl)
+        for kind in MASK_KINDS:
+            mask = generation_mask(kind, B, Sl, world)
+            out = ra._infer_replicated(q, k[:, keys].contiguous(), v[:, keys].contiguous(), mask, rank,
+                                       ra.TorchComm(None, world), NumpyInferOps).numpy()
+            full = None if mask is None else np.broadcast_to(mask.numpy(), (B,) + mask.shape[1:])
+            ref = attention_inference_dense(q.numpy(), k.numpy(), v.numpy(), full)
+            ret[(rank, kind)] = float((np.linalg.norm(out - ref, axis=-1) / np.linalg.norm(ref, axis=-1)).max())
+    finally:
+        dist.destroy_process_group()
+
+
 def _free_port():
     with socket.socket() as s:
         s.bind(("127.0.0.1", 0))
@@ -122,3 +154,15 @@ def test_q_sharded_protocol_matches_dense_oracle(world, Ql, B, broadcast, use_ma
     assert len(ret) == world
     for r in range(world):
         assert ret[r] < 1e-12, (r, ret[r])
+
+
+@pytest.mark.parametrize("world", [2, 4])
+def test_replicated_protocol_matches_dense_oracle(world):
+    """Q = 1 replicated along the ring: each rank's partial over its shard, all-gathered and merged in rank order,
+    under masks that leave whole ranks unfilled, padded or fully masked"""
+    from test_attn_decode_ring_gpu import MASK_KINDS
+    ret = mp.Manager().dict()
+    mp.spawn(_replicated_worker, args=(world, _free_port(), ret), nprocs=world, join=True)
+    assert len(ret) == world * len(MASK_KINDS)
+    for (r, kind), err in sorted(ret.items()):
+        assert err < 1e-12, (r, kind, err)

@@ -245,6 +245,24 @@ int lwm_attn_rope(const void* xq, const void* xk, int in_dtype, void* out_q, voi
                   const int* position_ids, const float* inv_freq, int B, int S, int Hq, int Hk, int D, int conj,
                   void* stream);
 
+/* The operand passes of the attention op with the rotary embedding folded in (`ringattention(..., freqs_cis,
+ * position_ids)`): x [B,S,H,128] fp32 (0) or bf16 (1) holds UN-rotated q or k, position_ids int32 [B,S], inv_freq [64]
+ * as for lwm_attn_rope. Every pass works on rope(x) rounded to x's dtype — bit for bit what lwm_attn_rope writes — so
+ * each equals lwm_attn_rope followed by the plain pass, without the rotated tensor in memory.
+ * lwm_attn_absmax_rope      atomicMax of the |rope(x)| bit patterns into *out_bits (caller zeroes it), as lwm_attn_absmax.
+ * lwm_attn_stage_rope       dst_dtype 2: dst = fp16(rope(x) / *scale), as lwm_attn_to_f16_scaled; dst_dtype 1: dst =
+ *                           bf16(rope(x)), the bf16 operand mode's copy (scale unused, may be null).
+ * lwm_reduce_cast_rope_f32  dst [B,S,H,128] = T(rope*(T(sum of n_src <= 16 fp32 arrays, fixed order))), T = fp32 (0) or
+ *                           bf16 (1), rope* the conjugate rotation: lwm_reduce_cast_f32 followed by lwm_attn_rope(conj=1)
+ *                           in one pass (the gradient w.r.t. the un-rotated q / k). host_srcs: HOST array of device
+ *                           pointers; dst may be one of them (in place). */
+int lwm_attn_absmax_rope(const void* x, int dtype, const int* position_ids, const float* inv_freq, int B, int S, int H,
+                         unsigned* out_bits, void* stream);
+int lwm_attn_stage_rope(const void* x, int dtype, void* dst, int dst_dtype, const float* scale, const int* position_ids,
+                        const float* inv_freq, int B, int S, int H, void* stream);
+int lwm_reduce_cast_rope_f32(const float* const* host_srcs, int n_src, void* dst, int dst_dtype,
+                             const int* position_ids, const float* inv_freq, int B, int S, int H, void* stream);
+
 /* Element-wise helpers used by the ring host loop. */
 int lwm_cast_f32_to_bf16(const float* src, void* dst, long long n, void* stream);
 /* dst[i] += src[i] (fp32, n % 4 == 0): folds a dK/dV partial received from a peer into the owner's accumulator. */

@@ -71,6 +71,9 @@ _SIGNATURES = {
     "lwm_vq_argmin": [c_void_p] * 5 + [c_int] * 3 + [c_void_p],
     "lwm_vq_gather": [c_void_p] * 3 + [c_ll, c_int, c_int, c_void_p],
     "lwm_attn_rope": [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p] + [c_int] * 6 + [c_void_p],
+    "lwm_attn_absmax_rope": [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p],
+    "lwm_attn_stage_rope": [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p],
+    "lwm_reduce_cast_rope_f32": [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p],
     "lwm_vq_frame_tokens": [c_void_p] * 3 + [c_int] * 6 + [c_void_p],
     "lwm_vq_unframe_tokens": [c_void_p, c_void_p, c_ll, c_int, c_void_p],
     "lwm_vq_frames_prep": [c_void_p] + [c_int] * 4 + [c_void_p] * 2 + [c_int] * 2 + [c_void_p] * 2 + [c_int] * 6

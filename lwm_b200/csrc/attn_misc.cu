@@ -2,9 +2,12 @@
 //   lwm_attn_bwd_prep     delta[b,h,s] = sum_d dout*out  (the rowsum(g∘out) term of the reference's
 //                         custom_vjp bwd, SURVEY.md Appendix A `bwd`)
 //   lwm_cast_f32_to_bf16  final cast of the fp32 gradient accumulators to the input dtype
+//   lwm_attn_*_rope       the operand passes with the rotary embedding of q / k applied on the fly
 #include "attn_common.cuh"
 #include <cuda_fp16.h>
+#include <cstdio>
 #include "capi_internal.h"
+#include "rope_common.cuh"
 #include "../../include/lwm_b200.h"
 
 namespace lwm {
@@ -222,6 +225,132 @@ __global__ void reduce_cast_kernel(const ReduceSrcs srcs, int n_src, void* __res
   }
 }
 
+
+// ---- the same passes over q / k with the rotary embedding applied on the fly (rope_common.cuh) ----
+// x [n_tok, H, 128] with one position per token: the value every pass below works on is rope(x) rounded to x's
+// dtype, bit for bit what lwm_attn_rope(x -> x's dtype) writes, so each pass equals "rotate, then the plain pass".
+// A CTA of 256 threads walks token groups of kRopePos (grid stride); per group it builds the (cos, sin) table once,
+// under the group's first loads, and then streams the group's H*16 vectors of 8 elements.
+
+// One token group of the rotating passes: the group's first batch of loads is issued, then the (cos, sin) table of its
+// kRopePos tokens is built (its double-precision sincos runs under those loads), and then f(element offset, y[8]) is
+// called for every 8-element vector of the group, y = rope(x) rounded to TIn. Every thread of the CTA calls it.
+template <typename TIn, typename F>
+__device__ __forceinline__ void rope_group_apply(const TIn* __restrict__ x, const int* __restrict__ pos,
+                                                 const float* __restrict__ inv_freq, long long tok0, long long n_tok,
+                                                 int H, float2 (*cs)[kRopePairs], F&& f) {
+  const int vt = H * (kRopeDim / 8);
+  const long long left = n_tok - tok0;
+  const int total = (left < kRopePos ? int(left) : kRopePos) * vt;
+  const long long e0 = tok0 * H * kRopeDim;
+  constexpr int kBatch = Raw8<TIn>::kBatch;
+  Raw8<TIn> raw[kBatch];
+  auto load = [&](int base) {
+#pragma unroll
+    for (int u = 0; u < kBatch; ++u) {
+      const int v = base + u * blockDim.x;
+      if (v < total) raw[u].load(x + e0 + (long long)v * 8);
+    }
+  };
+  auto use = [&](int base) {
+#pragma unroll
+    for (int u = 0; u < kBatch; ++u) {
+      const int v = base + u * blockDim.x;
+      if (v >= total) continue;
+      const int p = v / vt, r = v - p * vt;
+      float xv[8], y[8];
+      raw[u].unpack(xv);
+      rope_rotate8(xv, y, &cs[0][0], p * kRopePairs + (r & 15) * 4);
+      round8<TIn>(y);
+      f(e0 + (long long)v * 8, y);
+    }
+  };
+  load(threadIdx.x);
+  __syncthreads();                      // the previous group's table is no longer read
+  rope_fill_table(cs, pos, inv_freq, tok0, n_tok, 1.0f);
+  __syncthreads();
+  use(threadIdx.x);
+  for (int base = threadIdx.x + kBatch * blockDim.x; base < total; base += kBatch * blockDim.x) {
+    load(base);
+    use(base);
+  }
+}
+
+// absmax_*_kernel of rope(x): atomicMax of the |value| bit patterns into *out_bits
+template <typename TIn>
+__global__ void __launch_bounds__(256) absmax_rope_kernel(const TIn* __restrict__ x, const int* __restrict__ pos,
+                                                          const float* __restrict__ inv_freq, long long n_tok, int H,
+                                                          unsigned* __restrict__ out_bits) {
+  __shared__ float2 cs[kRopePos][kRopePairs];
+  unsigned m = 0;
+  for (long long tok0 = (long long)blockIdx.x * kRopePos; tok0 < n_tok; tok0 += (long long)gridDim.x * kRopePos) {
+    rope_group_apply<TIn>(x, pos, inv_freq, tok0, n_tok, H, cs, [&](long long, const float (&y)[8]) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) m = max(m, __float_as_uint(y[i]) & 0x7fffffffu);
+    });
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0 && m) atomicMax(out_bits, m);
+}
+
+// *_to_f16_by_scale_kernel of rope(x) (kF16: fp16(value / *scale)), or the bf16 operand mode's copy (bf16(value))
+template <typename TIn, bool kF16>
+__global__ void __launch_bounds__(256) stage_rope_kernel(const TIn* __restrict__ x, uint4* __restrict__ dst,
+                                                         const float* __restrict__ scale, const int* __restrict__ pos,
+                                                         const float* __restrict__ inv_freq, long long n_tok, int H) {
+  __shared__ float2 cs[kRopePos][kRopePairs];
+  const float inv = kF16 ? 1.0f / *scale : 1.0f;
+  for (long long tok0 = (long long)blockIdx.x * kRopePos; tok0 < n_tok; tok0 += (long long)gridDim.x * kRopePos) {
+    rope_group_apply<TIn>(x, pos, inv_freq, tok0, n_tok, H, cs, [&](long long e, const float (&y)[8]) {
+      unsigned o[4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        o[k] = kF16 ? pack_f16x2(y[2 * k] * inv, y[2 * k + 1] * inv) : pack_bf16x2(y[2 * k], y[2 * k + 1]);
+      dst[e / 8] = make_uint4(o[0], o[1], o[2], o[3]);
+    });
+  }
+}
+
+// reduce_cast_kernel followed by the conjugate rotation of the cast value, rounded again to the destination dtype:
+// dst = T(rope*(T(sum_i srcs[i]))) with T = bf16 (kToBf16) or fp32, the sum in source order. dst may be a source
+// (in place: every element is read by the thread that writes it, before it writes it), hence no __restrict__ on it.
+template <bool kToBf16>
+__global__ void __launch_bounds__(256) reduce_cast_rope_kernel(const ReduceSrcs srcs, int n_src, void* dst,
+                                                               const int* __restrict__ pos,
+                                                               const float* __restrict__ inv_freq, long long n_tok,
+                                                               int H) {
+  __shared__ float2 cs[kRopePos][kRopePairs];
+  const int vt = H * (kRopeDim / 8);
+  for (long long tok0 = (long long)blockIdx.x * kRopePos; tok0 < n_tok; tok0 += (long long)gridDim.x * kRopePos) {
+    __syncthreads();
+    rope_fill_table(cs, pos, inv_freq, tok0, n_tok, -1.0f);
+    __syncthreads();
+    const long long left = n_tok - tok0;
+    const int total = (left < kRopePos ? int(left) : kRopePos) * vt;
+    const long long q0 = tok0 * H * (kRopeDim / 4);     // in float4
+    for (int v = threadIdx.x; v < total; v += blockDim.x) {
+      const long long i = q0 + 2LL * v;
+      float4 a = srcs.p[0][i], c = srcs.p[0][i + 1];
+      for (int s = 1; s < n_src; ++s) {
+        const float4 b = srcs.p[s][i], d = srcs.p[s][i + 1];
+        a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
+        c.x += d.x; c.y += d.y; c.z += d.z; c.w += d.w;
+      }
+      float xv[8] = {a.x, a.y, a.z, a.w, c.x, c.y, c.z, c.w}, y[8];
+      const int p = v / vt, r = v - p * vt;
+      if (kToBf16) {
+        round8<__nv_bfloat16>(xv);
+        rope_rotate8(xv, y, &cs[0][0], p * kRopePairs + (r & 15) * 4);
+        store8<__nv_bfloat16>(reinterpret_cast<__nv_bfloat16*>(dst) + 4 * i, y);
+      } else {
+        rope_rotate8(xv, y, &cs[0][0], p * kRopePairs + (r & 15) * 4);
+        store8<float>(reinterpret_cast<float*>(dst) + 4 * i, y);
+      }
+    }
+  }
+}
+
 }  // namespace lwm
 
 using namespace lwm;
@@ -379,4 +508,90 @@ extern "C" int lwm_reduce_cast_f32(const float* const* host_srcs, int n_src, voi
   if (dst_dtype == 1) reduce_cast_kernel<true><<<grid_for(n / 4, 256, 16), 256, 0, st>>>(rs, n_src, dst, n / 4);
   else reduce_cast_kernel<false><<<grid_for(n / 4, 256, 16), 256, 0, st>>>(rs, n_src, dst, n / 4);
   return lwm_check_launch("reduce_cast_kernel");
+}
+
+// ---- entry points of the rotating passes: x [B,S,H,128] (dtype 0 fp32, 1 bf16), position_ids int32 [B,S], inv_freq [64]
+
+// LWM_ERR_ARG with the message "<fn>: <reason>"
+static int rope_fail(const char* fn, const char* reason) {
+  char msg[128];
+  snprintf(msg, sizeof(msg), "%s: %s", fn, reason);
+  return lwm_fail(LWM_ERR_ARG, msg);
+}
+
+// LWM_OK, or the failure status of the rotation arguments every rotating pass takes: positions, inv_freq, B, S, H
+static int rope_table_args(const char* fn, const int* pos, const float* inv_freq, int B, int S, int H) {
+  if (!pos || !inv_freq) return rope_fail(fn, "null pointer");
+  if (B <= 0 || S <= 0 || H <= 0) return rope_fail(fn, "bad sizes");
+  return LWM_OK;
+}
+
+// LWM_OK, or the failure status of an input x [B,S,H,128] of dtype code 0 (fp32) or 1 (bf16) and its rotation
+static int rope_input_args(const char* fn, const void* x, int dtype, const int* pos, const float* inv_freq, int B, int S,
+                           int H) {
+  if (!x) return rope_fail(fn, "null pointer");
+  if (dtype != 0 && dtype != 1) return rope_fail(fn, "dtype codes are 0 (fp32) or 1 (bf16)");
+  return rope_table_args(fn, pos, inv_freq, B, S, H);
+}
+
+static unsigned rope_grid(long long n_tok) { return grid_for((n_tok + kRopePos - 1) / kRopePos, 1, 8); }
+
+extern "C" int lwm_attn_absmax_rope(const void* x, int dtype, const int* position_ids, const float* inv_freq, int B,
+                                    int S, int H, unsigned* out_bits, void* stream) {
+  if (int e = rope_input_args("attn_absmax_rope", x, dtype, position_ids, inv_freq, B, S, H)) return e;
+  if (!out_bits) return lwm_fail(LWM_ERR_ARG, "attn_absmax_rope: null pointer");
+  if (!lwm_check_device()) return LWM_ERR_DEVICE;
+  const long long n_tok = (long long)B * S;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (dtype == 1)
+    absmax_rope_kernel<__nv_bfloat16><<<rope_grid(n_tok), 256, 0, st>>>(
+        reinterpret_cast<const __nv_bfloat16*>(x), position_ids, inv_freq, n_tok, H, out_bits);
+  else
+    absmax_rope_kernel<float><<<rope_grid(n_tok), 256, 0, st>>>(reinterpret_cast<const float*>(x), position_ids,
+                                                                inv_freq, n_tok, H, out_bits);
+  return lwm_check_launch("absmax_rope_kernel");
+}
+
+extern "C" int lwm_attn_stage_rope(const void* x, int dtype, void* dst, int dst_dtype, const float* scale,
+                                   const int* position_ids, const float* inv_freq, int B, int S, int H, void* stream) {
+  if (int e = rope_input_args("attn_stage_rope", x, dtype, position_ids, inv_freq, B, S, H)) return e;
+  if (!dst) return lwm_fail(LWM_ERR_ARG, "attn_stage_rope: null pointer");
+  if (dst_dtype != 1 && dst_dtype != 2)
+    return lwm_fail(LWM_ERR_ARG, "attn_stage_rope: dst dtype codes are 1 (bf16) or 2 (scaled fp16)");
+  if (dst_dtype == 2 && !scale) return lwm_fail(LWM_ERR_ARG, "attn_stage_rope: scaled fp16 needs a scale");
+  if (!lwm_check_device()) return LWM_ERR_DEVICE;
+  const long long n_tok = (long long)B * S;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  uint4* y = reinterpret_cast<uint4*>(dst);
+  const unsigned g = rope_grid(n_tok);
+  if (dtype == 1) {
+    const __nv_bfloat16* xb = reinterpret_cast<const __nv_bfloat16*>(x);
+    if (dst_dtype == 2) stage_rope_kernel<__nv_bfloat16, true><<<g, 256, 0, st>>>(xb, y, scale, position_ids, inv_freq, n_tok, H);
+    else stage_rope_kernel<__nv_bfloat16, false><<<g, 256, 0, st>>>(xb, y, scale, position_ids, inv_freq, n_tok, H);
+  } else {
+    const float* xf = reinterpret_cast<const float*>(x);
+    if (dst_dtype == 2) stage_rope_kernel<float, true><<<g, 256, 0, st>>>(xf, y, scale, position_ids, inv_freq, n_tok, H);
+    else stage_rope_kernel<float, false><<<g, 256, 0, st>>>(xf, y, scale, position_ids, inv_freq, n_tok, H);
+  }
+  return lwm_check_launch("stage_rope_kernel");
+}
+
+extern "C" int lwm_reduce_cast_rope_f32(const float* const* host_srcs, int n_src, void* dst, int dst_dtype,
+                                        const int* position_ids, const float* inv_freq, int B, int S, int H,
+                                        void* stream) {
+  if (!host_srcs || !dst || n_src < 1 || n_src > LWM_REDUCE_MAX_SRCS || (dst_dtype != 0 && dst_dtype != 1))
+    return lwm_fail(LWM_ERR_ARG, "reduce_cast_rope_f32: bad arguments (1..16 sources, dst dtype 0 or 1)");
+  if (int e = rope_table_args("reduce_cast_rope_f32", position_ids, inv_freq, B, S, H)) return e;
+  for (int i = 0; i < n_src; ++i)
+    if (!host_srcs[i]) return lwm_fail(LWM_ERR_ARG, "reduce_cast_rope_f32: null source");
+  if (!lwm_check_device()) return LWM_ERR_DEVICE;
+  ReduceSrcs rs;
+  for (int i = 0; i < LWM_REDUCE_MAX_SRCS; ++i) rs.p[i] = reinterpret_cast<const float4*>(host_srcs[i < n_src ? i : 0]);
+  const long long n_tok = (long long)B * S;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (dst_dtype == 1)
+    reduce_cast_rope_kernel<true><<<rope_grid(n_tok), 256, 0, st>>>(rs, n_src, dst, position_ids, inv_freq, n_tok, H);
+  else
+    reduce_cast_rope_kernel<false><<<rope_grid(n_tok), 256, 0, st>>>(rs, n_src, dst, position_ids, inv_freq, n_tok, H);
+  return lwm_check_launch("reduce_cast_rope_kernel");
 }

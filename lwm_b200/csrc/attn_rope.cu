@@ -10,63 +10,10 @@
 // thread rotates 8-element vectors of all heads of Q and K for those positions, so the transcendental cost is
 // amortised over H heads and the kernel is a pure HBM stream: each element is read once and written once.
 // The [B,S,H*D] projection output and the op's [B,S,H,D] input are the same memory: the head split is free.
-#include <cuda_bf16.h>
-
 #include "capi_internal.h"
+#include "rope_common.cuh"
 
 namespace lwm {
-
-constexpr int kRopeDim = 128;
-constexpr int kRopePairs = kRopeDim / 2;
-constexpr int kRopePos = 4;
-
-// 8 consecutive elements as loaded (kept raw until use, so that a batch of loads costs few registers)
-template <typename T>
-struct Raw8;
-template <>
-struct Raw8<float> {
-  float4 a, b;
-  static constexpr int kBatch = 4;
-  __device__ __forceinline__ void load(const float* p) {
-    a = reinterpret_cast<const float4*>(p)[0];
-    b = reinterpret_cast<const float4*>(p)[1];
-  }
-  __device__ __forceinline__ void unpack(float (&x)[8]) const {
-    x[0] = a.x; x[1] = a.y; x[2] = a.z; x[3] = a.w; x[4] = b.x; x[5] = b.y; x[6] = b.z; x[7] = b.w;
-  }
-};
-template <>
-struct Raw8<__nv_bfloat16> {
-  uint4 a;
-  static constexpr int kBatch = 8;
-  __device__ __forceinline__ void load(const __nv_bfloat16* p) { a = reinterpret_cast<const uint4*>(p)[0]; }
-  __device__ __forceinline__ void unpack(float (&x)[8]) const {
-    const unsigned w[4] = {a.x, a.y, a.z, a.w};
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      x[2 * i] = __uint_as_float(w[i] << 16);
-      x[2 * i + 1] = __uint_as_float(w[i] & 0xffff0000u);
-    }
-  }
-};
-template <typename T>
-__device__ __forceinline__ void store8(T* p, const float (&y)[8]);
-template <>
-__device__ __forceinline__ void store8<float>(float* p, const float (&y)[8]) {
-  reinterpret_cast<float4*>(p)[0] = make_float4(y[0], y[1], y[2], y[3]);
-  reinterpret_cast<float4*>(p)[1] = make_float4(y[4], y[5], y[6], y[7]);
-}
-template <>
-__device__ __forceinline__ void store8<__nv_bfloat16>(__nv_bfloat16* p, const float (&y)[8]) {
-  uint4 o;
-  unsigned* w = reinterpret_cast<unsigned*>(&o);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const __nv_bfloat162 v = __floats2bfloat162_rn(y[2 * i], y[2 * i + 1]);
-    w[i] = *reinterpret_cast<const unsigned*>(&v);
-  }
-  reinterpret_cast<uint4*>(p)[0] = o;
-}
 
 template <typename TIn, typename TOut>
 __global__ void __launch_bounds__(256, 3) rope_kernel(const TIn* __restrict__ xq, const TIn* __restrict__ xk,
@@ -76,16 +23,7 @@ __global__ void __launch_bounds__(256, 3) rope_kernel(const TIn* __restrict__ xq
                                                    int Hk, float sin_sign) {
   __shared__ float2 cs[kRopePos][kRopePairs];
   const long long tok0 = (long long)blockIdx.x * kRopePos;
-  {
-    const int p = threadIdx.x >> 6, j = threadIdx.x & 63;
-    const long long tok = tok0 + p;
-    if (tok < n_tok) {
-      const float angle = (float)((double)position_ids[tok] * (double)inv_freq[j]);
-      double s, c;
-      sincos((double)angle, &s, &c);
-      cs[p][j] = make_float2((float)c, sin_sign * (float)s);
-    }
-  }
+  rope_fill_table(cs, position_ids, inv_freq, tok0, n_tok, sin_sign);
   __syncthreads();
   const int vq = Hq * (kRopeDim / 8), vk = Hk * (kRopeDim / 8), vt = vq + vk;
   // batches of independent 16/32-byte loads per thread (8 / 4) before the first use: ~100 KB in flight per SM
@@ -113,13 +51,7 @@ __global__ void __launch_bounds__(256, 3) rope_kernel(const TIn* __restrict__ xq
       if (!live[u]) continue;
       float x[8], y[8];
       raw[u].unpack(x);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float2 f = (&cs[0][0])[cs_idx[u] + i];
-        // (a + ib)(c + is) = (ac - bs) + i(as + bc), separately rounded products as in a plain complex64 multiply
-        y[2 * i] = __fsub_rn(__fmul_rn(x[2 * i], f.x), __fmul_rn(x[2 * i + 1], f.y));
-        y[2 * i + 1] = __fadd_rn(__fmul_rn(x[2 * i], f.y), __fmul_rn(x[2 * i + 1], f.x));
-      }
+      rope_rotate8(x, y, &cs[0][0], cs_idx[u]);
       store8<TOut>((is_q[u] ? oq + tok0 * Hq * kRopeDim : ok + tok0 * Hk * kRopeDim) + off[u], y);
     }
   }

@@ -5,6 +5,10 @@ kernel launches with their first/last carry flags.
 The step functions are injected (`ops`), so the very same sequencing code is exercised on CPU
 with the gloo backend and an oracle-backed `ops` in tests/test_ring_gloo.py, and on H100s with
 the CUDA C-ABI calls of lwm_b200.ringattention.
+
+The rotary embedding of `ringattention(..., freqs_cis=, position_ids=)` is not folded into this executor's staging:
+on this path the op runs the composition, `apply_rotary_emb` on q and k and then this executor on the rotated tensors,
+which is bit-identical to the fused passes of the one-GPU and peer-memory paths by construction.
 """
 import os
 from typing import List

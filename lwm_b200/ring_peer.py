@@ -291,33 +291,45 @@ def _layout_for(plan, q_shape, Sk, ops):
     return Layout(B, Sq, Sk, H, D, plan.world, plan.chunks_per_rank, ops.op_itemsize)
 
 
-def _stage_and_announce(tr, lay, which, pid, ops, k, v, x, cols, known=None):
+def _stage_and_announce(tr, lay, which, pid, ops, k, v, x, cols, known=None, rope=None, rope_x=False):
     """Scales of the local shards -> my row of the scale table (in the heap: peers pull it with the data); K/V -> own
     rows of the position-ordered arrays, x (Q or dO) -> the stage; then STAGED[rank] = pid on every peer.
     cols = (column of k, of v, of x) in the table row [sq, sk, sv, sdo]; known = {column: scale tensor} to reuse (the
     backward re-stages K/V with the forward's scales). Every operand has its OWNER's scale: no cross-rank agreement and
-    therefore no exchange is needed — a launch only ever combines one Q-side owner with one K/V owner."""
+    therefore no exchange is needed — a launch only ever combines one Q-side owner with one K/V owner.
+    rope: None, or (positions int32 [B,Sk], inv_freq): k (and x when rope_x) are un-rotated, and their scales and staged
+    copies are those of the rotated rows. Every rank stages its own rows, so only local positions are needed."""
     P, r = tr.world, tr.rank
     B, Sk = k.shape[0], k.shape[1]
     table = tr.heap_view(lay.base(which) + lay.abs, (P, 4), torch.float32)
     KG = tr.heap_view(lay.base(which) + lay.kg, (B, P * Sk) + tuple(k.shape[2:]), ops.op_dtype)
     VG = tr.heap_view(lay.base(which) + lay.vg, (B, P * Sk) + tuple(k.shape[2:]), ops.op_dtype)
     QS = tr.heap_view(lay.base(which) + lay.qs, tuple(x.shape), ops.op_dtype)
+    rot = (rope is not None, False, rope is not None and rope_x)
     sc = []
-    for t, c in zip((k, v, x), cols):
+    for t, c, rt in zip((k, v, x), cols, rot):
         dst = table[r, c:c + 1]
         if not ops.scaled:
             sc.append(None)
         elif known is not None and c in known:
             dst.copy_(known[c])
             sc.append(dst)
+        elif rt:
+            ops.scale_of_rope(t, dst, *rope)
+            sc.append(dst)
         else:
             ops.scale_of(t, dst)
             sc.append(dst)
     for b in range(B):
-        ops.stage(k[b], KG[b, r * Sk:(r + 1) * Sk], sc[0])
+        if rot[0]:
+            ops.stage_rope(k[b], KG[b, r * Sk:(r + 1) * Sk], sc[0], rope[0][b], rope[1])
+        else:
+            ops.stage(k[b], KG[b, r * Sk:(r + 1) * Sk], sc[0])
         ops.stage(v[b], VG[b, r * Sk:(r + 1) * Sk], sc[1])
-    ops.stage(x, QS, sc[2])
+    if rot[2]:
+        ops.stage_rope(x, QS, sc[2], *rope)
+    else:
+        ops.stage(x, QS, sc[2])
     for p in range(P):
         if p != r:
             tr.signal(p, FLAG_STAGED + r, pid, "main")
@@ -381,16 +393,26 @@ def _pull_group(tr, lay, which, group, KG, VG, gate):
     return tr.record("pull")
 
 
-def _return_rows(tr, lay, which, pid, plan, chunks, out, region, itemsize):
+def _return_rows(tr, lay, which, pid, plan, chunks, out, region, itemsize, ops=None, rope=None):
     """Exit permutation: rows computed here for other ranks go to the owner's landing area, mine come back the same way.
-    chunks[i] belongs to plan.q_chunks[i]; `out` [B, Sq, H, D] is this rank's contiguous result."""
+    chunks[i] belongs to plan.q_chunks[i]; `out` [B, Sq, H, D] is this rank's contiguous result. rope: None, or
+    (positions int32 [B,Sq], inv_freq): the rows are gradients w.r.t. rotated rows, and the owner's copies into `out`
+    are the conjugate rotations (ops.rope_conj) that make them gradients w.r.t. the un-rotated ones."""
     B, r = out.shape[0], tr.rank
+
+    def place(s, l, src):
+        if rope is None:
+            out[:, s:s + l].copy_(src)
+            return
+        for b in range(B):
+            ops.rope_conj(src[b], out[b, s:s + l], rope[0][b, s:s + l], rope[1])
+
     ev = tr.record("main")
     tr.wait_event("push", ev)
     dests = {}
     for qc, c in zip(plan.q_chunks, chunks):
         if qc.owner == r:
-            out[:, qc.start:qc.start + qc.length].copy_(c)
+            place(qc.start, qc.length, c)
         else:
             st = dests.setdefault(qc.owner, _pick(tr, "push"))     # a destination's payloads and its flag: one stream
             for b in range(B):
@@ -401,7 +423,7 @@ def _return_rows(tr, lay, which, pid, plan, chunks, out, region, itemsize):
     for peer in sorted({peer for (_, _, peer) in plan.q_sends}):
         tr.wait(FLAG_RES + peer, pid, "main")
     for (s, l, peer) in plan.q_sends:
-        out[:, s:s + l].copy_(land[:, s:s + l])
+        place(s, l, land[:, s:s + l])
     return out
 
 
@@ -426,8 +448,9 @@ def _sc(table, owner, col):
     return None if table is None else table[owner, col:col + 1]
 
 
-def run_forward(plan, q, k, v, bias, seg, causal, ops, tr, want_f32=False):
-    """-> (out [B,Sq,H,D] in bf16 or fp32, residuals). q/k/v: bf16 or fp32 shards (contiguous sharding)."""
+def run_forward(plan, q, k, v, bias, seg, causal, ops, tr, want_f32=False, rope=None):
+    """-> (out [B,Sq,H,D] in bf16 or fp32, residuals). q/k/v: bf16 or fp32 shards (contiguous sharding).
+    rope: None, or (positions int32 [B,S], inv_freq): q and k are un-rotated and are rotated while staged."""
     B, Sq, H, D = q.shape
     Sk = k.shape[1]
     dev = q.device
@@ -451,7 +474,7 @@ def run_forward(plan, q, k, v, bias, seg, causal, ops, tr, want_f32=False):
                       torch.empty((B, H, lens[i]), dtype=torch.float32, device=dev),
                       torch.empty((B, H, lens[i]), dtype=torch.float32, device=dev))
     with _span(tr, "fwd stage q,k,v", "main"):
-        KG, VG, QS, table = _stage_and_announce(tr, lay, which, pid, ops, k, v, q, (1, 2, 0))
+        KG, VG, QS, table = _stage_and_announce(tr, lay, which, pid, ops, k, v, q, (1, 2, 0), rope=rope, rope_x=True)
     # scale rows [sq, sk, sv, sdo] of every owner, local copy (mine straight from the heap row I just wrote)
     scales = None
     if ops.scaled:
@@ -510,9 +533,10 @@ def run_forward(plan, q, k, v, bias, seg, causal, ops, tr, want_f32=False):
     return out, res
 
 
-def run_backward(plan, res, k, v, dout, bias, seg, causal, ops, tr, want_f32=False):
+def run_backward(plan, res, k, v, dout, bias, seg, causal, ops, tr, want_f32=False, rope=None):
     """-> dq, dk, dv (contiguous shards; bf16, or fp32 when want_f32). `res`: residuals of run_forward
-    (scales = one Q scale per compute chunk, then this rank's own K and V scales)."""
+    (scales = one Q scale per compute chunk, then this rank's own K and V scales). rope: as run_forward's; K is
+    re-staged rotated, and dq / dk are the gradients w.r.t. the un-rotated q and k."""
     B, Sk, H, D = k.shape
     Sq = dout.shape[1]
     dev = k.device
@@ -526,7 +550,7 @@ def run_backward(plan, res, k, v, dout, bias, seg, causal, ops, tr, want_f32=Fal
     q_scales, (sk_own, sv_own) = res["scales"][:n_q], res["scales"][n_q:n_q + 2]
     with _span(tr, "bwd stage k,v,dO", "main"):
         KG, VG, DS, table = _stage_and_announce(tr, lay, which, pid, ops, k, v, dout, (1, 2, 3),
-                                                known={1: sk_own, 2: sv_own} if ops.scaled else None)
+                                                known={1: sk_own, 2: sv_own} if ops.scaled else None, rope=rope)
     scales = None
     if ops.scaled:
         scales = torch.empty((P, 4), dtype=torch.float32, device=dev)
@@ -587,7 +611,7 @@ def run_backward(plan, res, k, v, dout, bias, seg, causal, ops, tr, want_f32=Fal
             dq_chunks.append(c)
     with _span(tr, "bwd return dQ rows", "main"):
         dq = _return_rows(tr, lay, which, pid, plan, dq_chunks, torch.empty((B, Sq, H, D), dtype=res_dtype, device=dev),
-                          "lq4" if want_f32 else "lq2", 4 if want_f32 else 2)
+                          "lq4" if want_f32 else "lq2", 4 if want_f32 else 2, ops, rope)
     # dK/dV: own partial + landed partials -> one fused sum + cast per chunk
     dk = torch.empty((B, Sk, H, D), dtype=res_dtype, device=dev)
     dv = torch.empty((B, Sk, H, D), dtype=res_dtype, device=dev)
@@ -606,7 +630,9 @@ def run_backward(plan, res, k, v, dout, bias, seg, causal, ops, tr, want_f32=Fal
                         if cj == ci:
                             off = lay.slot_off(which, plan.slot(ci, peer), t) + b * L * lay.row * 4
                             srcs.append(tr.heap_view(off, (L, H, D), torch.float32))
-                    if srcs:
+                    if srcs and rope is not None and t == 0:
+                        ops.reduce_cast_rope(srcs, dst[b, ci * L:(ci + 1) * L], rope[0][b, ci * L:(ci + 1) * L], rope[1])
+                    elif srcs:
                         ops.reduce_cast(srcs, dst[b, ci * L:(ci + 1) * L])
                     else:
                         dst[b, ci * L:(ci + 1) * L].zero_()

@@ -23,6 +23,7 @@ import torch.distributed as dist
 
 from . import _lib
 from . import ring_exec as rx
+from . import rope as _rope
 from . import ring_peer as rp
 from . import ring_schedule as rs
 
@@ -117,31 +118,37 @@ def _prep_bias(attn_bias, B):
 
 class _RingAttnFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, q, k, v, bias, seg, causal, axis_name, layout, precision):
+    def forward(ctx, q, k, v, bias, seg, causal, axis_name, layout, precision, rope_pos=None, inv_freq=None):
+        """rope_pos / inv_freq: None, or q and k are un-rotated and the rotary embedding at these positions (int32
+        [B,S]) is applied inside the operand staging; k and the positions are saved instead of a rotated k"""
         group, rank, world = _resolve_group(axis_name)
-        out, res = ring_forward(q, k, v, bias, seg, causal, group, rank, world, layout, precision)
+        rope = None if rope_pos is None else (rope_pos, inv_freq)
+        out, res = ring_forward(q, k, v, bias, seg, causal, group, rank, world, layout, precision, rope)
         # residuals stay in the schedule's compute layout (zigzag chunks, operand dtype), so the backward only has
         # to permute dout on entry and dq on exit
         ctx.n_chunks = len(res["q_chunks"])
         sc = [t for t in res.get("scales", ()) if t is not None]
         ctx.n_scales = len(sc)
-        ctx.save_for_backward(k, v, bias, seg, *res["q_chunks"], *res["out_chunks"], *res["lse_chunks"], *sc)
+        ctx.save_for_backward(k, v, bias, seg, rope_pos, *res["q_chunks"], *res["out_chunks"], *res["lse_chunks"],
+                              *sc)
         ctx.causal, ctx.axis_name, ctx.layout, ctx.precision = causal, axis_name, layout, precision
+        ctx.inv_freq = inv_freq
         return out
 
     @staticmethod
     def backward(ctx, dout):
         saved = ctx.saved_tensors
-        k, v, bias, seg = saved[:4]
+        k, v, bias, seg, rope_pos = saved[:5]
         n = ctx.n_chunks
-        res = dict(q_chunks=list(saved[4:4 + n]), out_chunks=list(saved[4 + n:4 + 2 * n]),
-                   lse_chunks=list(saved[4 + 2 * n:4 + 3 * n]))
-        sc = list(saved[4 + 3 * n:4 + 3 * n + ctx.n_scales])
+        res = dict(q_chunks=list(saved[5:5 + n]), out_chunks=list(saved[5 + n:5 + 2 * n]),
+                   lse_chunks=list(saved[5 + 2 * n:5 + 3 * n]))
+        sc = list(saved[5 + 3 * n:5 + 3 * n + ctx.n_scales])
         res["scales"] = tuple(sc) if sc else (None,) * (n + 2)
         group, rank, world = _resolve_group(ctx.axis_name)
+        rope = None if rope_pos is None else (rope_pos, ctx.inv_freq)
         dq, dk, dv = ring_backward(res, k, v, dout.contiguous(), bias, seg, ctx.causal, group, rank, world,
-                                   ctx.layout, ctx.precision)
-        return dq, dk, dv, None, None, None, None, None, None
+                                   ctx.layout, ctx.precision, rope)
+        return dq, dk, dv, None, None, None, None, None, None, None, None
 
 
 def _check_mask_extent(bias, seg, rank, world, Sq, Sk):
@@ -155,8 +162,39 @@ def _check_mask_extent(bias, seg, rank, world, Sq, Sk):
                          "(lwm/llama.py:564)" % (seg.shape[-1], max(world * Sq, world * Sk)))
 
 
+def _check_rope(freqs_cis, position_ids, q, k):
+    """the rotary-embedding keywords of ringattention -> None or (position_ids int32 [B,S_loc] on q's device, inv_freq)"""
+    if freqs_cis is None and position_ids is None:
+        return None
+    if freqs_cis is None or position_ids is None:
+        raise ValueError("ringattention: freqs_cis and position_ids go together (the rotary embedding needs both)")
+    if not isinstance(freqs_cis, _rope.RotaryTable):
+        raise ValueError("ringattention: freqs_cis must come from lwm_b200.rope.precompute_freqs_cis")
+    if q.shape[1] != k.shape[1]:
+        raise ValueError("ringattention: the rotary embedding is applied to q and k at the same positions, which needs "
+                         "Sq == Sk (got %d and %d); with a rotated KV cache call apply_rotary_emb on q yourself"
+                         % (q.shape[1], k.shape[1]))
+    if tuple(position_ids.shape) != (q.shape[0], q.shape[1]):
+        raise ValueError("ringattention: position_ids must be [B, S_loc] = %s, got %s"
+                         % ((q.shape[0], q.shape[1]), tuple(position_ids.shape)))
+    if int(position_ids.max()) >= freqs_cis.max_position or int(position_ids.min()) < 0:
+        raise ValueError("ringattention: position_ids outside [0, max_position_embedding)")
+    return position_ids.to(device=q.device, dtype=torch.int32).contiguous(), freqs_cis.inv_freq
+
+
+def _peer_ready(q, k, causal, group, rank, world, layout, precision):
+    """world > 1: whether this call runs on the peer-memory executor (sets up its heap, as ring_forward would)"""
+    if _transport(group) != "peer":
+        return False
+    lay = rs.choose_layout(world, q.shape[1], k.shape[1], causal, layout)
+    plan = rs.make_peer_plan(world, rank, q.shape[1], k.shape[1], causal, lay)
+    tr = _peer_transport(group, q.device, rp._layout_for(plan, q.shape, k.shape[1], _peer_ops(precision)).total)
+    return tr is not None
+
+
 def ringattention(q, k, v, attn_bias=None, segment_ids=None, *, axis_name="sp", float32_logits=True,
-                  cache_idx=None, blockwise_kwargs=None, layout="auto", precision=None):
+                  cache_idx=None, blockwise_kwargs=None, layout="auto", precision=None, freqs_cis=None,
+                  position_ids=None):
     """Drop-in for the reference op. q [B,Sq_loc,H,D], k/v [B,Sk_loc,H,D] CUDA shards of the contiguously
     sequence-sharded tensors (in_specs lwm/llama.py:559-565), all bfloat16 or all float32 (the dtype the reference's
     scripts run with); attn_bias [B,1,1,S_global] additive (0 / finfo.min), segment_ids [B,S_global] or None, both
@@ -168,12 +206,21 @@ def ringattention(q, k, v, attn_bias=None, segment_ids=None, *, axis_name="sp", 
     float32_logits: logits/softmax/carries are always fp32 here (the reference default, True).
     layout: 'contiguous' = the reference's schedule; 'zigzag' = internally rebalance the causal
     work across ranks (same inputs/outputs); 'auto' picks zigzag when it applies.
-    precision: None -> module default (set_default_precision / $LWM_ATTN_PRECISION): 'fp16' | 'bf16'."""
+    precision: None -> module default (set_default_precision / $LWM_ATTN_PRECISION): 'fp16' | 'bf16'.
+
+    freqs_cis, position_ids: both None (the reference call), or q and k are the UN-rotated head-split projections and
+    the op applies the rotary embedding of lwm/llama.py:517-519 itself: freqs_cis is the RotaryTable of
+    lwm_b200.rope.precompute_freqs_cis, position_ids [B,S_loc] the positions of this rank's rows (sharded like q; Sq ==
+    Sk). Bit-identical to ringattention(*apply_rotary_emb(q, k, freqs_cis, q.dtype, position_ids=position_ids), v, ...)
+    under autograd (dQ up to the order of its fp32 reductions), but on one GPU and on the peer-memory ring the rotation
+    happens inside the passes that stage q and k (and the conjugate rotation inside the final casts of dQ and dK), so the
+    rotated q and k are never written to memory. position_ids gets no gradient."""
     precision = precision or _DEFAULT_PRECISION
     if precision not in ("bf16", "fp16"):
         raise ValueError("precision must be 'bf16' or 'fp16'")
     if cache_idx is not None:
         raise NotImplementedError("cache_idx is always None at the reference call site (lwm/llama.py:544)")
+    rope = _check_rope(freqs_cis, position_ids, q, k)
     if not q.is_cuda:
         raise _lib.LwmError("ringattention: tensors must live on an sm_90 GPU (no CPU fallback)")
     in_dtype = q.dtype
@@ -182,18 +229,26 @@ def ringattention(q, k, v, attn_bias=None, segment_ids=None, *, axis_name="sp", 
                         "are internal)")
     group, rank, world = _resolve_group(axis_name)
     native_f32 = in_dtype == torch.float32 and precision == "fp16" and (world == 1 or _transport(group) == "peer")
+    B, Sq, H, D = q.shape
+    causal = _check_blockwise_kwargs(blockwise_kwargs, Sq, k.shape[1])
+    if rope is not None:
+        to_bf16 = in_dtype == torch.float32 and not native_f32
+        if to_bf16 or not (world == 1 or _peer_ready(q, k, causal, group, rank, world, layout, precision)):
+            # bf16 operands from fp32 inputs (rotated straight into bf16: the same bits as rotating in fp32 and then
+            # rounding), or the two-sided NCCL executor: the rotation is a pass of its own, then the plain op
+            q, k = _rope.apply_rotary_emb(q, k, freqs_cis, torch.bfloat16 if to_bf16 else in_dtype,
+                                          position_ids=position_ids)
+            rope = None
     if in_dtype == torch.float32 and not native_f32:
         # bf16 operand mode / NCCL transport: fp32 callers go through one rounding of q/k/v to bf16 (2^-9 relative)
         q, k, v = q.to(torch.bfloat16), k.to(torch.bfloat16), v.to(torch.bfloat16)
-    B, Sq, H, D = q.shape
-    causal = _check_blockwise_kwargs(blockwise_kwargs, Sq, k.shape[1])
     bias = _prep_bias(attn_bias, B)
     seg = None
     if segment_ids is not None:
         seg = segment_ids.to(torch.int32).contiguous()
     _check_mask_extent(bias, seg, rank, world, Sq, k.shape[1])
     out = _RingAttnFn.apply(q.contiguous(), k.contiguous(), v.contiguous(), bias, seg, causal, axis_name, layout,
-                            precision)
+                            precision, *(rope or (None, None)))
     return out if out.dtype == in_dtype else out.to(in_dtype)
 
 
@@ -470,10 +525,47 @@ class PeerOpsF16:
 
     cast = staticmethod(cast_f32_to_bf16)
 
+    # -- the same passes over un-rotated q / k with the rotary embedding applied on the fly: x [..., H, 128]
+    # (contiguous) with pos int32 [...] (contiguous, one position per row), inv_freq [64] of the RotaryTable
+    _STAGE_DST = 2          # lwm_attn_stage_rope: scaled fp16
+
+    @staticmethod
+    def absmax_rope(x, bits, pos, inv_freq):
+        _lib.call("lwm_attn_absmax_rope", _lib.ptr(x), _dt(x), _lib.ptr(pos), _lib.ptr(inv_freq), 1, pos.numel(),
+                  x.shape[-2], _lib.ptr(bits), _lib.stream_ptr())
+
+    @classmethod
+    def scale_of_rope(cls, x, out, pos, inv_freq):
+        """scale_of of rope(x)"""
+        bits = torch.zeros(1, dtype=torch.int32, device=x.device)
+        cls.absmax_rope(x, bits, pos, inv_freq)
+        _lib.call("lwm_attn_scale_from_absmax", _lib.ptr(bits), 1, 1, _lib.ptr(out), _lib.stream_ptr())
+
+    @classmethod
+    def stage_rope(cls, x, dst, scale, pos, inv_freq):
+        """stage of rope(x)"""
+        _lib.call("lwm_attn_stage_rope", _lib.ptr(x), _dt(x), _lib.ptr(dst), cls._STAGE_DST, _lib.ptr(scale),
+                  _lib.ptr(pos), _lib.ptr(inv_freq), 1, pos.numel(), x.shape[-2], _lib.stream_ptr())
+
+    @staticmethod
+    def reduce_cast_rope(srcs, dst, pos, inv_freq):
+        """reduce_cast, then the conjugate rotation of the cast value, rounded again to dst's dtype"""
+        import ctypes
+        arr = (ctypes.c_void_p * len(srcs))(*[t.data_ptr() for t in srcs])
+        _lib.call("lwm_reduce_cast_rope_f32", arr, len(srcs), _lib.ptr(dst), _dt(dst), _lib.ptr(pos),
+                  _lib.ptr(inv_freq), 1, pos.numel(), dst.shape[-2], _lib.stream_ptr())
+
+    @staticmethod
+    def rope_conj(src, dst, pos, inv_freq):
+        """dst = the conjugate rotation of src (a gradient w.r.t. rotated rows -> w.r.t. the un-rotated ones)"""
+        _lib.call("lwm_attn_rope", _lib.ptr(src), None, _dt(src), _lib.ptr(dst), None, _dt(dst), _lib.ptr(pos),
+                  _lib.ptr(inv_freq), 1, pos.numel(), src.shape[-2], 0, src.shape[-1], 1, _lib.stream_ptr())
+
 
 class PeerOpsBf16(PeerOpsF16):
     """bf16 operand mode: staging is a plain copy (fp32 inputs are rounded to bf16 there), no scales."""
     op_dtype, op_itemsize, scaled = torch.bfloat16, 2, False
+    _STAGE_DST = 1          # lwm_attn_stage_rope: bf16, the copy's rounding
 
     @staticmethod
     def stage(x, dst, scale):
@@ -536,19 +628,28 @@ def _peer_ops(precision):
     return PeerOpsF16 if precision == "fp16" else PeerOpsBf16
 
 
-def _local_scales(ops, tensors):
-    """single GPU: per-tensor scales from the local |max| (same kernels as the sharded exchange, world = 1)"""
+def _local_scales(ops, tensors, rope=None):
+    """single GPU: per-tensor scales from the local |max| (same kernels as the sharded exchange, world = 1).
+    rope: None, or (positions, inv_freq): the first two tensors (q, k) are scaled as rotated"""
     if not ops.scaled:
         return [None] * len(tensors)
     table = torch.zeros((1, 4), dtype=torch.int32, device=tensors[0].device)
     out = []
     for c, t in enumerate(tensors):
-        ops.absmax(t, table[0, c:c + 1])
+        if rope is not None and c < 2:
+            ops.absmax_rope(t, table[0, c:c + 1], *rope)
+        else:
+            ops.absmax(t, table[0, c:c + 1])
         out.append(ops.make_scale(table, c))
     return out
 
 
-def _stage_local(ops, x, scale):
+def _stage_local(ops, x, scale, rope=None):
+    """x's operand copy; rope: None, or (positions, inv_freq) to stage the rotation of x"""
+    if rope is not None:
+        y = torch.empty(x.shape, dtype=ops.op_dtype, device=x.device)
+        ops.stage_rope(x, y, scale, *rope)
+        return y
     if not ops.scaled and x.dtype == ops.op_dtype:
         return x
     y = torch.empty(x.shape, dtype=ops.op_dtype, device=x.device)
@@ -556,15 +657,16 @@ def _stage_local(ops, x, scale):
     return y
 
 
-def ring_forward(q, k, v, bias, seg, causal, group, rank, world, layout="auto", precision="bf16"):
+def ring_forward(q, k, v, bias, seg, causal, group, rank, world, layout="auto", precision="bf16", rope=None):
     """-> (out, residuals). out is fp32 (un-rounded) for fp32 inputs, bf16 otherwise. world == 1 is the
-    single-launch path (no carry buffers)."""
+    single-launch path (no carry buffers). rope: None, or (positions int32 [B,S], inv_freq): q and k are un-rotated and
+    are rotated while they are staged (one GPU and the peer-memory executor only)."""
     B, Sq, H, D = q.shape
     want_f32 = q.dtype == torch.float32
     if world == 1:
         ops = _peer_ops(precision)
-        sq, sk, sv = _local_scales(ops, (q, k, v))
-        q16, k16, v16 = _stage_local(ops, q, sq), _stage_local(ops, k, sk), _stage_local(ops, v, sv)
+        sq, sk, sv = _local_scales(ops, (q, k, v), rope)
+        q16, k16, v16 = _stage_local(ops, q, sq, rope), _stage_local(ops, k, sk, rope), _stage_local(ops, v, sv)
         out = torch.empty((B, Sq, H, D), dtype=torch.bfloat16, device=q.device)
         out32 = torch.empty((B, Sq, H, D), dtype=torch.float32, device=q.device) if (ops.scaled or want_f32) else None
         lse = torch.empty((B, H, Sq), dtype=torch.float32, device=q.device)
@@ -577,18 +679,21 @@ def ring_forward(q, k, v, bias, seg, causal, group, rank, world, layout="auto", 
         pops = _peer_ops(precision)
         tr = _peer_transport(group, q.device, rp._layout_for(plan, q.shape, k.shape[1], pops).total)
         if tr is not None:
-            return rp.run_forward(plan, q, k, v, bias, seg, causal, pops, tr, want_f32)
+            return rp.run_forward(plan, q, k, v, bias, seg, causal, pops, tr, want_f32, rope)
         if want_f32:        # the NCCL executor takes bf16 operands (documented in ringattention())
             out, res = ring_forward(q.to(torch.bfloat16), k.to(torch.bfloat16), v.to(torch.bfloat16), bias, seg, causal,
-                                    group, rank, world, layout, precision)
+                                    group, rank, world, layout, precision, rope)
             return out.float(), res
+    if rope is not None:
+        raise _lib.LwmError("ring_forward: the rotary embedding is folded into the one-GPU and peer-memory paths only")
     ops = _ops_for(precision)
     plan = rs.make_plan(world, rank, Sq, k.shape[1], causal, lay, n_sub_first=rs.auto_sub(world, k.shape[1], lay))
     out, res = rx.run_forward(plan, q, k, v, bias, seg, causal, group, ops)
     return out, _f32_residuals(ops, res)
 
 
-def ring_backward(res, k, v, dout, bias, seg, causal, group, rank, world, layout="auto", precision="bf16"):
+def ring_backward(res, k, v, dout, bias, seg, causal, group, rank, world, layout="auto", precision="bf16", rope=None):
+    """rope: as ring_forward's; dq and dk are then the gradients w.r.t. the un-rotated q and k"""
     B, Sk, H, D = k.shape
     dev = k.device
     want_f32 = k.dtype == torch.float32
@@ -598,7 +703,7 @@ def ring_backward(res, k, v, dout, bias, seg, causal, group, rank, world, layout
         sq, sk, sv = res["scales"]
         Sq = q16.shape[1]
         sdo = _local_scales(ops, (dout,))[0]
-        k16, v16, d16 = _stage_local(ops, k, sk), _stage_local(ops, v, sv), _stage_local(ops, dout, sdo)
+        k16, v16, d16 = _stage_local(ops, k, sk, rope), _stage_local(ops, v, sv), _stage_local(ops, dout, sdo)
         delta = torch.empty((B, H, Sq), dtype=torch.float32, device=dev)
         ops.bwd_prep(out, d16, sdo, delta)
         nlse = ops.lse_for_bwd(lse)
@@ -607,6 +712,17 @@ def ring_backward(res, k, v, dout, bias, seg, causal, group, rank, world, layout
         dv_acc = torch.empty((B, Sk, H, D), dtype=torch.float32, device=dev)
         ops.bwd_step(q16, k16, v16, d16, nlse, delta, dq_acc, dk_acc, dv_acc, 0, 0, causal, bias, seg,
                      (sq, sk, sv, sdo), True)
+        if rope is not None:
+            # the final casts of dQ and dK carry the conjugate rotation (a single source: no sum; fp32 results are
+            # rotated in place, so the rotation allocates nothing)
+            if want_f32:
+                dq, dk, dv = dq_acc, dk_acc, dv_acc
+            else:
+                dq, dk, dv = [torch.empty(t.shape, dtype=torch.bfloat16, device=dev) for t in (dq_acc, dk_acc, dv_acc)]
+                cast_f32_to_bf16(dv_acc, dv)
+            ops.reduce_cast_rope([dq_acc], dq, *rope)
+            ops.reduce_cast_rope([dk_acc], dk, *rope)
+            return dq, dk, dv
         if want_f32:
             return dq_acc, dk_acc, dv_acc
         dq, dk, dv = [torch.empty(t.shape, dtype=torch.bfloat16, device=dev) for t in (dq_acc, dk_acc, dv_acc)]
@@ -618,7 +734,9 @@ def ring_backward(res, k, v, dout, bias, seg, causal, group, rank, world, layout
     if _transport(group) == "peer":
         plan = rs.make_peer_plan(world, rank, dout.shape[1], Sk, causal, lay)
         return rp.run_backward(plan, res, k, v, dout, bias, seg, causal, _peer_ops(precision),
-                               rp.CudaPeerTransport.get(group, dev), want_f32)
+                               rp.CudaPeerTransport.get(group, dev), want_f32, rope)
+    if rope is not None:
+        raise _lib.LwmError("ring_backward: the rotary embedding is folded into the one-GPU and peer-memory paths only")
     if want_f32:            # forward fell back to the NCCL executor: bf16 operands in, fp32 gradients out
         dq, dk, dv = ring_backward(res, k.to(torch.bfloat16), v.to(torch.bfloat16), dout.to(torch.bfloat16), bias, seg,
                                    causal, group, rank, world, layout, precision)

@@ -289,10 +289,12 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         l_run[hh] = __fmul_rn(l_run[hh], alpha[hh]);
       }
       const float neg_m[2] = {-m_run[0], -m_run[1]};
+      // masked tiles hold s * scale already: fmaf(s, 1, -m) rounds exactly as s - m does
+      const float mul = need_mask ? 1.0f : scale;
 #pragma unroll
       for (int i = 0; i < 64; ++i) {
         const int hh = (i >> 1) & 1;
-        s[i] = need_mask ? ex2f(s[i] + neg_m[hh]) : ex2f(fmaf(s[i], scale, neg_m[hh]));
+        s[i] = ex2f(fmaf(s[i], mul, neg_m[hh]));
         l_run[hh] += s[i];
       }
     };
@@ -333,11 +335,20 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       reg_fence(s);
       release(2 * j);
       softmax(j);
-      wgmma_wait<0>();
-      reg_fence(o);
-      release(2 * j - 1);
+      // No rescale when no row of the warp raised its max (alpha == 1, and x * 1 is exact). The branch also ends the
+      // basic block of the exponentials, which is why the PV wait sits in both arms: in one block with them, ptxas
+      // hoists the wait above them, and they would run after PV_{j-1} instead of under it
+      // (tests/test_attn_fwd_schedule_cpu.py checks the SASS).
+      if (__any_sync(0xffffffffu, alpha[0] != 1.f || alpha[1] != 1.f)) {
+        wgmma_wait<0>();
+        reg_fence(o);
 #pragma unroll
-      for (int i = 0; i < 64; ++i) o[i] *= alpha[(i >> 1) & 1];
+        for (int i = 0; i < 64; ++i) o[i] *= alpha[(i >> 1) & 1];
+      } else {
+        wgmma_wait<0>();
+        reg_fence(o);
+      }
+      release(2 * j - 1);
       pack_p();
     }
     // ---- epilogue: the last O += P V

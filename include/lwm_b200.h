@@ -189,6 +189,18 @@ int lwm_attn_decode_partial_f32(const float* q, const float* k, const float* v, 
                                 float* o_part, float* ml_part, void* workspace, int B, int H, int Q, int Sk, int D,
                                 long long k_pos0, long long mask_stride_b, long long mask_stride_q, int splits,
                                 float softmax_scale, void* stream);
+/* The same two partials with UN-rotated q [B,Q,H,128] (bf16, resp. fp32): position_ids int32 [B,Q] and inv_freq [64]
+ * as for lwm_attn_rope. q is rotated as it is loaded, rounded to its dtype: bit for bit lwm_attn_rope (out_dtype = the
+ * input dtype) followed by lwm_attn_decode_partial(_f32), without the rotated q in memory. */
+int lwm_attn_decode_partial_rope(const void* q, const void* k, const void* v, const unsigned char* mask, float* o_part,
+                                 float* ml_part, void* workspace, int B, int H, int Q, int Sk, int D, long long k_pos0,
+                                 long long mask_stride_b, long long mask_stride_q, int splits, float softmax_scale,
+                                 const int* position_ids, const float* inv_freq, void* stream);
+int lwm_attn_decode_partial_rope_f32(const float* q, const float* k, const float* v, const unsigned char* mask,
+                                     float* o_part, float* ml_part, void* workspace, int B, int H, int Q, int Sk,
+                                     int D, long long k_pos0, long long mask_stride_b, long long mask_stride_q,
+                                     int splits, float softmax_scale, const int* position_ids, const float* inv_freq,
+                                     void* stream);
 int lwm_attn_decode_merge_f32(const float* o_parts, const float* ml_parts, int n_part, float* out, float* lse,
                               long long rows, void* stream);
 
@@ -244,6 +256,15 @@ int lwm_attn_infer_bwd(const void* q16, const void* k16, const void* v16, const 
 int lwm_attn_rope(const void* xq, const void* xk, int in_dtype, void* out_q, void* out_k, int out_dtype,
                   const int* position_ids, const float* inv_freq, int B, int S, int Hq, int Hk, int D, int conj,
                   void* stream);
+
+/* The KV-cache write of the generation path with the rotary embedding on the keys (`ShardedKVCache.concatenate(...,
+ * freqs_cis, position_ids)`): rows [src0, src0+n) of the UN-rotated k_new and of v_new [B,n_src,H,128] go to rows
+ * [dst0, dst0+n) of this rank's cache shards cache_k / cache_v [B,L,H,128], all of one dtype (0 = fp32, 1 = bf16).
+ * k is rotated at position_ids [B,n_src] int32 (the positions of the source rows) and rounded to the cache dtype, v
+ * is copied: bit for bit lwm_attn_rope (out_dtype = in_dtype) followed by two row copies, in one launch. */
+int lwm_kv_cache_write_rope(const void* k_new, const void* v_new, int dtype, void* cache_k, void* cache_v,
+                            const int* position_ids, const float* inv_freq, int B, int n_src, long long src0, int n,
+                            int L, long long dst0, int H, int D, void* stream);
 
 /* The operand passes of the attention op with the rotary embedding folded in (`ringattention(..., freqs_cis,
  * position_ids)`): x [B,S,H,128] fp32 (0) or bf16 (1) holds UN-rotated q or k, position_ids int32 [B,S], inv_freq [64]

@@ -55,6 +55,12 @@ _SIGNATURES = {
     "lwm_attn_decode_merge": [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_ll, c_void_p],
     "lwm_attn_decode_partial_f32": [c_void_p] * 7 + [c_int] * 5 + [c_ll, c_ll, c_ll, c_int, c_float, c_void_p],
     "lwm_attn_decode_merge_f32": [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_ll, c_void_p],
+    "lwm_attn_decode_partial_rope": [c_void_p] * 7 + [c_int] * 5 + [c_ll, c_ll, c_ll, c_int, c_float]
+                                    + [c_void_p] * 3,
+    "lwm_attn_decode_partial_rope_f32": [c_void_p] * 7 + [c_int] * 5 + [c_ll, c_ll, c_ll, c_int, c_float]
+                                        + [c_void_p] * 3,
+    "lwm_kv_cache_write_rope": [c_void_p, c_void_p, c_int] + [c_void_p] * 4 + [c_int, c_int, c_ll, c_int, c_int, c_ll,
+                                                                               c_int, c_int, c_void_p],
     "lwm_attn_mask_pack": [c_void_p, c_ll, c_ll, c_ll, c_int, c_int, c_ll, c_int, c_int, c_void_p, c_void_p, c_void_p],
     "lwm_attn_infer_tilemap": [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p],
     "lwm_attn_infer_partial": [c_void_p] * 12 + [c_int] * 6 + [c_float, c_void_p],

@@ -10,10 +10,13 @@
 //                          lane l owns dims [4l, 4l+4) of q, k, v rows (one coalesced 256 B row per load)
 //                          bf16 or fp32 rows (one uint2 / float4 per lane and row). Below INFER_MIN_Q query
 //                          rows only; longer queries go to the tensor-core inference mode of attn_fwd_kernel.
+//                          kRope: q is un-rotated and is rotated at its position as it is loaded (lane l's dims are
+//                          the whole pairs 2l, 2l+1), rounded to q's dtype first: the value lwm_attn_rope would write.
 //   decode_merge_kernel    merges `n_part` partials per (b, q, h): used for the key splits (of both kernels) and,
 //                          after the exchange, for the ranks; writes bf16 or fp32.
 #include "attn_common.cuh"
 #include "capi_internal.h"
+#include "rope_common.cuh"
 
 #include <type_traits>
 
@@ -21,13 +24,14 @@ namespace lwm {
 
 constexpr int kDecWarps = 4;
 
-template <typename T>
+template <typename T, bool kRope = false>
 __global__ void __launch_bounds__(kDecWarps * 32)
 decode_partial_kernel(const T* __restrict__ q, const T* __restrict__ k,
                       const T* __restrict__ v, const unsigned char* __restrict__ mask,
                       float* __restrict__ o_part, float* __restrict__ ml_part, int B, int H, int Q, int Sk,
                       long long k_pos0, long long mask_stride_b, long long mask_stride_q, int splits,
-                      float scale_log2) {
+                      float scale_log2, const int* __restrict__ position_ids = nullptr,
+                      const float* __restrict__ inv_freq = nullptr) {
   constexpr bool kF32 = std::is_same<T, float>::value;   // fp32 rows: one float4 per lane, bf16 rows: one uint2
   using Raw = typename std::conditional<kF32, float4, uint2>::type;
   const int split = blockIdx.x, h = blockIdx.y;
@@ -39,14 +43,30 @@ decode_partial_kernel(const T* __restrict__ q, const T* __restrict__ k,
   float q0, q1, q2, q3;
   if constexpr (kF32) {
     const float4 qf = reinterpret_cast<const float4*>(q + (((size_t)b * Q + qi) * H + h) * kHeadDim)[lane];
-    q0 = qf.x * scale_log2; q1 = qf.y * scale_log2; q2 = qf.z * scale_log2; q3 = qf.w * scale_log2;
+    q0 = qf.x; q1 = qf.y; q2 = qf.z; q3 = qf.w;
   } else {
     const uint2 qraw = reinterpret_cast<const uint2*>(q + (((size_t)b * Q + qi) * H + h) * kHeadDim)[lane];
     const __nv_bfloat162 q01 = *reinterpret_cast<const __nv_bfloat162*>(&qraw.x);
     const __nv_bfloat162 q23 = *reinterpret_cast<const __nv_bfloat162*>(&qraw.y);
-    q0 = __low2float(q01) * scale_log2; q1 = __high2float(q01) * scale_log2;
-    q2 = __low2float(q23) * scale_log2; q3 = __high2float(q23) * scale_log2;
+    q0 = __low2float(q01); q1 = __high2float(q01);
+    q2 = __low2float(q23); q3 = __high2float(q23);
   }
+  if constexpr (kRope) {
+    // pairs (2*lane, 2*lane+1) at this row's position, with rope_rotate8's separately rounded products
+    const long long tok = (long long)b * Q + qi;
+    const float2 f0 = rope_cos_sin(position_ids, inv_freq, tok, 2 * lane, 1.0f);
+    const float2 f1 = rope_cos_sin(position_ids, inv_freq, tok, 2 * lane + 1, 1.0f);
+    float y0 = __fsub_rn(__fmul_rn(q0, f0.x), __fmul_rn(q1, f0.y));
+    float y1 = __fadd_rn(__fmul_rn(q0, f0.y), __fmul_rn(q1, f0.x));
+    float y2 = __fsub_rn(__fmul_rn(q2, f1.x), __fmul_rn(q3, f1.y));
+    float y3 = __fadd_rn(__fmul_rn(q2, f1.y), __fmul_rn(q3, f1.x));
+    if constexpr (!kF32) {
+      y0 = __bfloat162float(__float2bfloat16_rn(y0)); y1 = __bfloat162float(__float2bfloat16_rn(y1));
+      y2 = __bfloat162float(__float2bfloat16_rn(y2)); y3 = __bfloat162float(__float2bfloat16_rn(y3));
+    }
+    q0 = y0; q1 = y1; q2 = y2; q3 = y3;
+  }
+  q0 *= scale_log2; q1 *= scale_log2; q2 *= scale_log2; q3 *= scale_log2;
   const unsigned char* mrow = mask ? mask + (size_t)b * mask_stride_b + (size_t)qi * mask_stride_q + k_pos0 : nullptr;
 
   float m = -INFINITY, l = 0.f, a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
@@ -184,13 +204,16 @@ void lwm_decode_merge_partials(const float* o_parts, const float* ml_parts, int 
                                                                        o_merged, ml_merged, rows);
 }
 
-template <typename T>
+template <typename T, bool kRope = false>
 static int decode_partial_launch(const void* q, const void* k, const void* v, const unsigned char* mask,
                                  float* o_part, float* ml_part, void* workspace, int B, int H, int Q, int Sk, int D,
                                  long long k_pos0, long long mask_stride_b, long long mask_stride_q, int splits,
-                                 float softmax_scale, void* stream) {
+                                 float softmax_scale, void* stream, const int* position_ids = nullptr,
+                                 const float* inv_freq = nullptr) {
   if (D != kHeadDim) return lwm_fail(LWM_ERR_SHAPE, "attn_decode: head_dim must be 128");
   if (!q || !k || !v || !o_part || !ml_part || !workspace) return lwm_fail(LWM_ERR_ARG, "attn_decode: null pointer");
+  if (kRope && (!position_ids || !inv_freq))
+    return lwm_fail(LWM_ERR_ARG, "attn_decode_rope: null position_ids / inv_freq");
   if (B <= 0 || H <= 0 || Q <= 0 || Sk <= 0 || splits <= 0 || (long long)B * Q > 65535)
     return lwm_fail(LWM_ERR_SHAPE, "attn_decode: bad shape");
   if (!lwm_check_device()) return LWM_ERR_DEVICE;
@@ -199,9 +222,9 @@ static int decode_partial_launch(const void* q, const void* k, const void* v, co
   float* ws_o = reinterpret_cast<float*>(workspace);
   float* ws_ml = ws_o + rows * splits * kHeadDim;
   dim3 grid(splits, H, B * Q);
-  decode_partial_kernel<T><<<grid, kDecWarps * 32, 0, st>>>(
+  decode_partial_kernel<T, kRope><<<grid, kDecWarps * 32, 0, st>>>(
       reinterpret_cast<const T*>(q), reinterpret_cast<const T*>(k), reinterpret_cast<const T*>(v), mask, ws_o, ws_ml,
-      B, H, Q, Sk, k_pos0, mask_stride_b, mask_stride_q, splits, softmax_scale * kLog2e);
+      B, H, Q, Sk, k_pos0, mask_stride_b, mask_stride_q, splits, softmax_scale * kLog2e, position_ids, inv_freq);
   lwm_decode_merge_partials(ws_o, ws_ml, splits, o_part, ml_part, rows, st);
   return lwm_check_launch("attn_decode kernels");
 }
@@ -225,6 +248,29 @@ extern "C" int lwm_attn_decode_partial_f32(const float* q, const float* k, const
                                            int splits, float softmax_scale, void* stream) {
   return decode_partial_launch<float>(q, k, v, mask, o_part, ml_part, workspace, B, H, Q, Sk, D, k_pos0,
                                       mask_stride_b, mask_stride_q, splits, softmax_scale, stream);
+}
+
+// the same with un-rotated q: position_ids int32 [B,Q], inv_freq [64] (as for lwm_attn_rope); q is rotated as it is
+// loaded, so the result equals lwm_attn_rope (out_dtype = q's) followed by lwm_attn_decode_partial bit for bit
+extern "C" int lwm_attn_decode_partial_rope(const void* q, const void* k, const void* v, const unsigned char* mask,
+                                            float* o_part, float* ml_part, void* workspace, int B, int H, int Q,
+                                            int Sk, int D, long long k_pos0, long long mask_stride_b,
+                                            long long mask_stride_q, int splits, float softmax_scale,
+                                            const int* position_ids, const float* inv_freq, void* stream) {
+  return decode_partial_launch<__nv_bfloat16, true>(q, k, v, mask, o_part, ml_part, workspace, B, H, Q, Sk, D, k_pos0,
+                                                    mask_stride_b, mask_stride_q, splits, softmax_scale, stream,
+                                                    position_ids, inv_freq);
+}
+
+extern "C" int lwm_attn_decode_partial_rope_f32(const float* q, const float* k, const float* v,
+                                                const unsigned char* mask, float* o_part, float* ml_part,
+                                                void* workspace, int B, int H, int Q, int Sk, int D,
+                                                long long k_pos0, long long mask_stride_b, long long mask_stride_q,
+                                                int splits, float softmax_scale, const int* position_ids,
+                                                const float* inv_freq, void* stream) {
+  return decode_partial_launch<float, true>(q, k, v, mask, o_part, ml_part, workspace, B, H, Q, Sk, D, k_pos0,
+                                            mask_stride_b, mask_stride_q, splits, softmax_scale, stream, position_ids,
+                                            inv_freq);
 }
 
 // merge n_part partials per row (e.g. the all-gathered per-rank partials) into out (bf16) and lse.

@@ -55,6 +55,10 @@ struct Raw8<float> {
     a = reinterpret_cast<const float4*>(p)[0];
     b = reinterpret_cast<const float4*>(p)[1];
   }
+  __device__ __forceinline__ void store(float* p) const {
+    reinterpret_cast<float4*>(p)[0] = a;
+    reinterpret_cast<float4*>(p)[1] = b;
+  }
   __device__ __forceinline__ void unpack(float (&x)[8]) const {
     x[0] = a.x; x[1] = a.y; x[2] = a.z; x[3] = a.w; x[4] = b.x; x[5] = b.y; x[6] = b.z; x[7] = b.w;
   }
@@ -64,6 +68,7 @@ struct Raw8<__nv_bfloat16> {
   uint4 a;
   static constexpr int kBatch = 8;
   __device__ __forceinline__ void load(const __nv_bfloat16* p) { a = reinterpret_cast<const uint4*>(p)[0]; }
+  __device__ __forceinline__ void store(__nv_bfloat16* p) const { reinterpret_cast<uint4*>(p)[0] = a; }
   __device__ __forceinline__ void unpack(float (&x)[8]) const {
     const unsigned w[4] = {a.x, a.y, a.z, a.w};
 #pragma unroll

@@ -7,18 +7,43 @@ process-per-GPU model: every rank of the 'sp' group holds the rows [rank*L, (ran
   * prefill (query length > 1, llama.py:485-487: `dynamic_update_slice` at `cache_index`): the new rows are sharded like
     the queries (rank r holds rows [r*q_loc, (r+1)*q_loc) of them), their destination slots generally belong to other
     ranks, so the shards are all-gathered once and every rank copies the slice that falls into its own cache rows.
-Pure data movement (copies and one all-gather): no arithmetic, no kernels of its own. The cache shards are exactly the
-k / v arguments `ringattention` (prefill: "K/V = whole cache") and `ringattention_inference` (decode) take."""
+Without the rotary keywords this is pure data movement (copies and one all-gather). With them (freqs_cis, position_ids)
+the new keys arrive un-rotated and are rotated as they are written (lwm_kv_cache_write_rope: one launch for k and v), so
+the cache holds what apply_rotary_emb followed by the plain update would leave in it, bit for bit. The cache shards are
+exactly the k / v arguments `ringattention` (prefill: "K/V = whole cache") and `ringattention_inference` (decode) take
+(with rotate_k=False when q is rotated inside the op)."""
 import torch
 import torch.distributed as dist
 
+from . import _lib
+from . import rope as _rope
+from .ringattention import TorchComm, _dt
+
+
+def kv_cache_write_rope(k_src, v_src, src0, n, cache_k, cache_v, dst0, pos, inv_freq):
+    """rows [src0, src0+n) of k_src / v_src [B,n_src,H,128] -> rows [dst0, dst0+n) of cache_k / cache_v [B,L,H,128]
+    (one dtype), k rotated at pos int32 [B,n_src] and rounded to the cache dtype, v copied (lwm_kv_cache_write_rope)"""
+    B, n_src, H, D = k_src.shape
+    _lib.call("lwm_kv_cache_write_rope", _lib.ptr(k_src), _lib.ptr(v_src), _dt(cache_k), _lib.ptr(cache_k),
+              _lib.ptr(cache_v), _lib.ptr(pos), _lib.ptr(inv_freq), B, n_src, int(src0), int(n), cache_k.shape[1],
+              int(dst0), H, D, _lib.stream_ptr())
+
 
 class ShardedKVCache:
-    def __init__(self, batch, max_length, num_heads, head_dim, dtype=torch.bfloat16, device="cuda", group=None):
+    """comm: None (torch.distributed over `group`, or a ring of one), or an object with TorchComm's all_gather and
+    `world` / `rank` attributes (e.g. an in-process stand-in that runs the real kernels on emulated ranks)."""
+    write_rope = staticmethod(kv_cache_write_rope)
+
+    def __init__(self, batch, max_length, num_heads, head_dim, dtype=torch.bfloat16, device="cuda", group=None,
+                 comm=None):
         self.group = group
         self.world, self.rank = 1, 0
-        if dist.is_available() and dist.is_initialized():
+        if comm is not None:
+            self.world, self.rank = comm.world, comm.rank
+        elif dist.is_available() and dist.is_initialized():
             self.world, self.rank = dist.get_world_size(group), dist.get_rank(group)
+            comm = TorchComm(group, self.world)
+        self.comm = comm
         if max_length % self.world:
             raise ValueError("max_length %d must be divisible by the ring size %d" % (max_length, self.world))
         self.max_length = max_length
@@ -28,25 +53,46 @@ class ShardedKVCache:
         self.cached_value = torch.zeros(shape, dtype=dtype, device=device)
         self.cache_index = 0
 
-    def concatenate(self, key, value):
+    def concatenate(self, key, value, *, freqs_cis=None, position_ids=None):
         """key/value: the new rows. Decode: [B,1,H,D], replicated along the ring. Prefill: this rank's shard
         [B,q_loc,H,D] of the q_loc*world new rows. Returns (cached_key, cached_value) shards after the update and
-        advances cache_index by the number of new rows (llama.py:488-491)."""
+        advances cache_index by the number of new rows (llama.py:488-491).
+        freqs_cis, position_ids: both None (key is already rotated), or key is the un-rotated head-split projection and
+        position_ids [B,1] (decode, replicated) or [B,q_loc] (prefill, this rank's rows) are the positions of the new
+        rows (checked as ringattention checks them); key and value must then have the cache's dtype. Decode: the owner
+        of the slot makes one write launch. Prefill: the positions travel with the rows through the all-gather and
+        every rank rotates only the slice it keeps, straight into its shard."""
+        rope = _rope.check_position_ids("ShardedKVCache.concatenate", freqs_cis, position_ids,
+                                        (key.shape[0], key.shape[1]), key.device)
+        if rope is not None and not (key.dtype == value.dtype == self.cached_key.dtype):
+            raise ValueError("ShardedKVCache.concatenate: with the rotary keywords key and value must have the cache "
+                             "dtype %s, got %s and %s" % (self.cached_key.dtype, key.dtype, value.dtype))
         lo = self.rank * self.shard_len
         if key.shape[1] == 1 and value.shape[1] == 1 and self._is_decode(key):
             cur = self.cache_index - lo
             if 0 <= cur < self.shard_len:
-                self.cached_key[:, cur].copy_(key[:, -1])
-                self.cached_value[:, cur].copy_(value[:, -1])
+                if rope is None:
+                    self.cached_key[:, cur].copy_(key[:, -1])
+                    self.cached_value[:, cur].copy_(value[:, -1])
+                else:
+                    self.write_rope(key.contiguous(), value.contiguous(), 0, 1, self.cached_key, self.cached_value, cur,
+                                    *rope)
             n_new = 1
         else:
             n_new = key.shape[1] * self.world
             if self.cache_index + n_new > self.max_length:
                 raise ValueError("cache overflow: %d + %d > %d" % (self.cache_index, n_new, self.max_length))
+            # global slots [cache_index, cache_index + n_new) intersected with my rows [lo, lo + shard_len)
+            a, b = max(self.cache_index, lo), min(self.cache_index + n_new, lo + self.shard_len)
+            if rope is not None:
+                k_all, v_all, p_all = (self._gather_rows(t.contiguous()) for t in (key, value, rope[0]))
+                if b > a:
+                    self.write_rope(k_all.contiguous(), v_all.contiguous(), a - self.cache_index, b - a,
+                                    self.cached_key, self.cached_value, a - lo, p_all.contiguous(), rope[1])
+                self.cache_index += n_new
+                return self.cached_key, self.cached_value
             for new, cache in ((key, self.cached_key), (value, self.cached_value)):
                 full = self._gather_rows(new.contiguous())
-                # global slots [cache_index, cache_index + n_new) intersected with my rows [lo, lo + shard_len)
-                a, b = max(self.cache_index, lo), min(self.cache_index + n_new, lo + self.shard_len)
                 if b > a:
                     cache[:, a - lo:b - lo].copy_(full[:, a - self.cache_index:b - self.cache_index])
         self.cache_index += n_new
@@ -61,6 +107,5 @@ class ShardedKVCache:
         if self.world == 1:
             return x
         B, n = x.shape[0], x.shape[1]
-        g = torch.empty((self.world * B, n) + tuple(x.shape[2:]), dtype=x.dtype, device=x.device)
-        dist.all_gather_into_tensor(g, x, group=self.group)        # rank-major along dim 0
-        return g.view((self.world, B, n) + tuple(x.shape[2:])).transpose(0, 1).reshape((B, self.world * n) + tuple(x.shape[2:]))
+        g = self.comm.all_gather(x)                                 # [world, B, n, ...], rank-major
+        return g.transpose(0, 1).reshape((B, self.world * n) + tuple(x.shape[2:]))

@@ -291,21 +291,22 @@ def _layout_for(plan, q_shape, Sk, ops):
     return Layout(B, Sq, Sk, H, D, plan.world, plan.chunks_per_rank, ops.op_itemsize)
 
 
-def _stage_and_announce(tr, lay, which, pid, ops, k, v, x, cols, known=None, rope=None, rope_x=False):
+def _stage_and_announce(tr, lay, which, pid, ops, k, v, x, cols, known=None, rope=None, rope_x=False, rope_k=True):
     """Scales of the local shards -> my row of the scale table (in the heap: peers pull it with the data); K/V -> own
     rows of the position-ordered arrays, x (Q or dO) -> the stage; then STAGED[rank] = pid on every peer.
     cols = (column of k, of v, of x) in the table row [sq, sk, sv, sdo]; known = {column: scale tensor} to reuse (the
     backward re-stages K/V with the forward's scales). Every operand has its OWNER's scale: no cross-rank agreement and
     therefore no exchange is needed — a launch only ever combines one Q-side owner with one K/V owner.
-    rope: None, or (positions int32 [B,Sk], inv_freq): k (and x when rope_x) are un-rotated, and their scales and staged
-    copies are those of the rotated rows. Every rank stages its own rows, so only local positions are needed."""
+    rope: None, or (positions int32 [B,Sk], inv_freq): k (unless not rope_k) and x (when rope_x) are un-rotated, and their
+    scales and staged copies are those of the rotated rows. Every rank stages its own rows, so only local positions are
+    needed (rope_k=False: x's positions [B,Sq])."""
     P, r = tr.world, tr.rank
     B, Sk = k.shape[0], k.shape[1]
     table = tr.heap_view(lay.base(which) + lay.abs, (P, 4), torch.float32)
     KG = tr.heap_view(lay.base(which) + lay.kg, (B, P * Sk) + tuple(k.shape[2:]), ops.op_dtype)
     VG = tr.heap_view(lay.base(which) + lay.vg, (B, P * Sk) + tuple(k.shape[2:]), ops.op_dtype)
     QS = tr.heap_view(lay.base(which) + lay.qs, tuple(x.shape), ops.op_dtype)
-    rot = (rope is not None, False, rope is not None and rope_x)
+    rot = (rope is not None and rope_k, False, rope is not None and rope_x)
     sc = []
     for t, c, rt in zip((k, v, x), cols, rot):
         dst = table[r, c:c + 1]
@@ -448,9 +449,10 @@ def _sc(table, owner, col):
     return None if table is None else table[owner, col:col + 1]
 
 
-def run_forward(plan, q, k, v, bias, seg, causal, ops, tr, want_f32=False, rope=None):
+def run_forward(plan, q, k, v, bias, seg, causal, ops, tr, want_f32=False, rope=None, rope_k=True):
     """-> (out [B,Sq,H,D] in bf16 or fp32, residuals). q/k/v: bf16 or fp32 shards (contiguous sharding).
-    rope: None, or (positions int32 [B,S], inv_freq): q and k are un-rotated and are rotated while staged."""
+    rope: None, or (positions int32 [B,Sq], inv_freq): q (and k when rope_k, Sq == Sk) are un-rotated and are rotated
+    while staged."""
     B, Sq, H, D = q.shape
     Sk = k.shape[1]
     dev = q.device
@@ -474,7 +476,8 @@ def run_forward(plan, q, k, v, bias, seg, causal, ops, tr, want_f32=False, rope=
                       torch.empty((B, H, lens[i]), dtype=torch.float32, device=dev),
                       torch.empty((B, H, lens[i]), dtype=torch.float32, device=dev))
     with _span(tr, "fwd stage q,k,v", "main"):
-        KG, VG, QS, table = _stage_and_announce(tr, lay, which, pid, ops, k, v, q, (1, 2, 0), rope=rope, rope_x=True)
+        KG, VG, QS, table = _stage_and_announce(tr, lay, which, pid, ops, k, v, q, (1, 2, 0), rope=rope, rope_x=True,
+                                                rope_k=rope_k)
     # scale rows [sq, sk, sv, sdo] of every owner, local copy (mine straight from the heap row I just wrote)
     scales = None
     if ops.scaled:
@@ -533,10 +536,10 @@ def run_forward(plan, q, k, v, bias, seg, causal, ops, tr, want_f32=False, rope=
     return out, res
 
 
-def run_backward(plan, res, k, v, dout, bias, seg, causal, ops, tr, want_f32=False, rope=None):
+def run_backward(plan, res, k, v, dout, bias, seg, causal, ops, tr, want_f32=False, rope=None, rope_k=True):
     """-> dq, dk, dv (contiguous shards; bf16, or fp32 when want_f32). `res`: residuals of run_forward
-    (scales = one Q scale per compute chunk, then this rank's own K and V scales). rope: as run_forward's; K is
-    re-staged rotated, and dq / dk are the gradients w.r.t. the un-rotated q and k."""
+    (scales = one Q scale per compute chunk, then this rank's own K and V scales). rope, rope_k: as run_forward's; K is
+    re-staged rotated when rope_k, and dq (and dk when rope_k) are the gradients w.r.t. the un-rotated q (and k)."""
     B, Sk, H, D = k.shape
     Sq = dout.shape[1]
     dev = k.device
@@ -550,7 +553,8 @@ def run_backward(plan, res, k, v, dout, bias, seg, causal, ops, tr, want_f32=Fal
     q_scales, (sk_own, sv_own) = res["scales"][:n_q], res["scales"][n_q:n_q + 2]
     with _span(tr, "bwd stage k,v,dO", "main"):
         KG, VG, DS, table = _stage_and_announce(tr, lay, which, pid, ops, k, v, dout, (1, 2, 3),
-                                                known={1: sk_own, 2: sv_own} if ops.scaled else None, rope=rope)
+                                                known={1: sk_own, 2: sv_own} if ops.scaled else None,
+                                                rope=rope if rope_k else None)
     scales = None
     if ops.scaled:
         scales = torch.empty((P, 4), dtype=torch.float32, device=dev)
@@ -630,7 +634,7 @@ def run_backward(plan, res, k, v, dout, bias, seg, causal, ops, tr, want_f32=Fal
                         if cj == ci:
                             off = lay.slot_off(which, plan.slot(ci, peer), t) + b * L * lay.row * 4
                             srcs.append(tr.heap_view(off, (L, H, D), torch.float32))
-                    if srcs and rope is not None and t == 0:
+                    if srcs and rope is not None and rope_k and t == 0:
                         ops.reduce_cast_rope(srcs, dst[b, ci * L:(ci + 1) * L], rope[0][b, ci * L:(ci + 1) * L], rope[1])
                     elif srcs:
                         ops.reduce_cast(srcs, dst[b, ci * L:(ci + 1) * L])

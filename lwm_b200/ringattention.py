@@ -118,12 +118,13 @@ def _prep_bias(attn_bias, B):
 
 class _RingAttnFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, q, k, v, bias, seg, causal, axis_name, layout, precision, rope_pos=None, inv_freq=None):
-        """rope_pos / inv_freq: None, or q and k are un-rotated and the rotary embedding at these positions (int32
-        [B,S]) is applied inside the operand staging; k and the positions are saved instead of a rotated k"""
+    def forward(ctx, q, k, v, bias, seg, causal, axis_name, layout, precision, rope_pos=None, inv_freq=None,
+                rope_k=True):
+        """rope_pos / inv_freq: None, or q (and k when rope_k) are un-rotated and the rotary embedding at these positions
+        (int32 [B,Sq]) is applied inside the operand staging; k and the positions are saved instead of a rotated k"""
         group, rank, world = _resolve_group(axis_name)
         rope = None if rope_pos is None else (rope_pos, inv_freq)
-        out, res = ring_forward(q, k, v, bias, seg, causal, group, rank, world, layout, precision, rope)
+        out, res = ring_forward(q, k, v, bias, seg, causal, group, rank, world, layout, precision, rope, rope_k)
         # residuals stay in the schedule's compute layout (zigzag chunks, operand dtype), so the backward only has
         # to permute dout on entry and dq on exit
         ctx.n_chunks = len(res["q_chunks"])
@@ -132,7 +133,7 @@ class _RingAttnFn(torch.autograd.Function):
         ctx.save_for_backward(k, v, bias, seg, rope_pos, *res["q_chunks"], *res["out_chunks"], *res["lse_chunks"],
                               *sc)
         ctx.causal, ctx.axis_name, ctx.layout, ctx.precision = causal, axis_name, layout, precision
-        ctx.inv_freq = inv_freq
+        ctx.inv_freq, ctx.rope_k = inv_freq, rope_k
         return out
 
     @staticmethod
@@ -147,8 +148,8 @@ class _RingAttnFn(torch.autograd.Function):
         group, rank, world = _resolve_group(ctx.axis_name)
         rope = None if rope_pos is None else (rope_pos, ctx.inv_freq)
         dq, dk, dv = ring_backward(res, k, v, dout.contiguous(), bias, seg, ctx.causal, group, rank, world,
-                                   ctx.layout, ctx.precision, rope)
-        return dq, dk, dv, None, None, None, None, None, None, None, None
+                                   ctx.layout, ctx.precision, rope, ctx.rope_k)
+        return dq, dk, dv, None, None, None, None, None, None, None, None, None
 
 
 def _check_mask_extent(bias, seg, rank, world, Sq, Sk):
@@ -162,24 +163,14 @@ def _check_mask_extent(bias, seg, rank, world, Sq, Sk):
                          "(lwm/llama.py:564)" % (seg.shape[-1], max(world * Sq, world * Sk)))
 
 
-def _check_rope(freqs_cis, position_ids, q, k):
-    """the rotary-embedding keywords of ringattention -> None or (position_ids int32 [B,S_loc] on q's device, inv_freq)"""
-    if freqs_cis is None and position_ids is None:
-        return None
-    if freqs_cis is None or position_ids is None:
-        raise ValueError("ringattention: freqs_cis and position_ids go together (the rotary embedding needs both)")
-    if not isinstance(freqs_cis, _rope.RotaryTable):
-        raise ValueError("ringattention: freqs_cis must come from lwm_b200.rope.precompute_freqs_cis")
-    if q.shape[1] != k.shape[1]:
+def _check_rope(freqs_cis, position_ids, q, k, rotate_k=True):
+    """the rotary-embedding keywords of ringattention -> None or (position_ids int32 [B,Sq_loc] on q's device, inv_freq)"""
+    if (rotate_k and freqs_cis is not None and position_ids is not None and isinstance(freqs_cis, _rope.RotaryTable)
+            and q.shape[1] != k.shape[1]):
         raise ValueError("ringattention: the rotary embedding is applied to q and k at the same positions, which needs "
                          "Sq == Sk (got %d and %d); with a rotated KV cache call apply_rotary_emb on q yourself"
                          % (q.shape[1], k.shape[1]))
-    if tuple(position_ids.shape) != (q.shape[0], q.shape[1]):
-        raise ValueError("ringattention: position_ids must be [B, S_loc] = %s, got %s"
-                         % ((q.shape[0], q.shape[1]), tuple(position_ids.shape)))
-    if int(position_ids.max()) >= freqs_cis.max_position or int(position_ids.min()) < 0:
-        raise ValueError("ringattention: position_ids outside [0, max_position_embedding)")
-    return position_ids.to(device=q.device, dtype=torch.int32).contiguous(), freqs_cis.inv_freq
+    return _rope.check_position_ids("ringattention", freqs_cis, position_ids, (q.shape[0], q.shape[1]), q.device)
 
 
 def _peer_ready(q, k, causal, group, rank, world, layout, precision):
@@ -194,7 +185,7 @@ def _peer_ready(q, k, causal, group, rank, world, layout, precision):
 
 def ringattention(q, k, v, attn_bias=None, segment_ids=None, *, axis_name="sp", float32_logits=True,
                   cache_idx=None, blockwise_kwargs=None, layout="auto", precision=None, freqs_cis=None,
-                  position_ids=None):
+                  position_ids=None, rotate_k=True):
     """Drop-in for the reference op. q [B,Sq_loc,H,D], k/v [B,Sk_loc,H,D] CUDA shards of the contiguously
     sequence-sharded tensors (in_specs lwm/llama.py:559-565), all bfloat16 or all float32 (the dtype the reference's
     scripts run with); attn_bias [B,1,1,S_global] additive (0 / finfo.min), segment_ids [B,S_global] or None, both
@@ -214,13 +205,19 @@ def ringattention(q, k, v, attn_bias=None, segment_ids=None, *, axis_name="sp", 
     Sk). Bit-identical to ringattention(*apply_rotary_emb(q, k, freqs_cis, q.dtype, position_ids=position_ids), v, ...)
     under autograd (dQ up to the order of its fp32 reductions), but on one GPU and on the peer-memory ring the rotation
     happens inside the passes that stage q and k (and the conjugate rotation inside the final casts of dQ and dK), so the
-    rotated q and k are never written to memory. position_ids gets no gradient."""
+    rotated q and k are never written to memory. position_ids gets no gradient.
+
+    rotate_k=False: k is already rotated (the KV cache of the generation path, written by ShardedKVCache.concatenate
+    with the same keywords) and only q is rotated, at position_ids [B,Sq_loc]; Sq != Sk is allowed (the cached prefill:
+    q against the whole cache). Bit-identical to ringattention(apply_rotary_emb(q, ...)[0], k, v, ...) in the same sense;
+    dK is the gradient w.r.t. k as passed, and only dQ gets the conjugate rotation."""
     precision = precision or _DEFAULT_PRECISION
     if precision not in ("bf16", "fp16"):
         raise ValueError("precision must be 'bf16' or 'fp16'")
     if cache_idx is not None:
         raise NotImplementedError("cache_idx is always None at the reference call site (lwm/llama.py:544)")
-    rope = _check_rope(freqs_cis, position_ids, q, k)
+    rope = _check_rope(freqs_cis, position_ids, q, k, rotate_k)
+    rotate_k = bool(rotate_k)
     if not q.is_cuda:
         raise _lib.LwmError("ringattention: tensors must live on an sm_90 GPU (no CPU fallback)")
     in_dtype = q.dtype
@@ -236,8 +233,11 @@ def ringattention(q, k, v, attn_bias=None, segment_ids=None, *, axis_name="sp", 
         if to_bf16 or not (world == 1 or _peer_ready(q, k, causal, group, rank, world, layout, precision)):
             # bf16 operands from fp32 inputs (rotated straight into bf16: the same bits as rotating in fp32 and then
             # rounding), or the two-sided NCCL executor: the rotation is a pass of its own, then the plain op
-            q, k = _rope.apply_rotary_emb(q, k, freqs_cis, torch.bfloat16 if to_bf16 else in_dtype,
-                                          position_ids=position_ids)
+            if rotate_k:
+                q, k = _rope.apply_rotary_emb(q, k, freqs_cis, torch.bfloat16 if to_bf16 else in_dtype,
+                                              position_ids=position_ids)
+            else:
+                q = _rope.rotate(q, freqs_cis, torch.bfloat16 if to_bf16 else in_dtype, position_ids=rope[0])
             rope = None
     if in_dtype == torch.float32 and not native_f32:
         # bf16 operand mode / NCCL transport: fp32 callers go through one rounding of q/k/v to bf16 (2^-9 relative)
@@ -248,7 +248,7 @@ def ringattention(q, k, v, attn_bias=None, segment_ids=None, *, axis_name="sp", 
         seg = segment_ids.to(torch.int32).contiguous()
     _check_mask_extent(bias, seg, rank, world, Sq, k.shape[1])
     out = _RingAttnFn.apply(q.contiguous(), k.contiguous(), v.contiguous(), bias, seg, causal, axis_name, layout,
-                            precision, *(rope or (None, None)))
+                            precision, *(rope or (None, None)), rotate_k)
     return out if out.dtype == in_dtype else out.to(in_dtype)
 
 
@@ -628,15 +628,15 @@ def _peer_ops(precision):
     return PeerOpsF16 if precision == "fp16" else PeerOpsBf16
 
 
-def _local_scales(ops, tensors, rope=None):
+def _local_scales(ops, tensors, rope=None, n_rot=2):
     """single GPU: per-tensor scales from the local |max| (same kernels as the sharded exchange, world = 1).
-    rope: None, or (positions, inv_freq): the first two tensors (q, k) are scaled as rotated"""
+    rope: None, or (positions, inv_freq): the first n_rot tensors (q, k) are scaled as rotated"""
     if not ops.scaled:
         return [None] * len(tensors)
     table = torch.zeros((1, 4), dtype=torch.int32, device=tensors[0].device)
     out = []
     for c, t in enumerate(tensors):
-        if rope is not None and c < 2:
+        if rope is not None and c < n_rot:
             ops.absmax_rope(t, table[0, c:c + 1], *rope)
         else:
             ops.absmax(t, table[0, c:c + 1])
@@ -657,16 +657,18 @@ def _stage_local(ops, x, scale, rope=None):
     return y
 
 
-def ring_forward(q, k, v, bias, seg, causal, group, rank, world, layout="auto", precision="bf16", rope=None):
+def ring_forward(q, k, v, bias, seg, causal, group, rank, world, layout="auto", precision="bf16", rope=None,
+                 rope_k=True):
     """-> (out, residuals). out is fp32 (un-rounded) for fp32 inputs, bf16 otherwise. world == 1 is the
-    single-launch path (no carry buffers). rope: None, or (positions int32 [B,S], inv_freq): q and k are un-rotated and
-    are rotated while they are staged (one GPU and the peer-memory executor only)."""
+    single-launch path (no carry buffers). rope: None, or (positions int32 [B,Sq], inv_freq): q (and k when rope_k) are
+    un-rotated and are rotated while they are staged (one GPU and the peer-memory executor only)."""
     B, Sq, H, D = q.shape
     want_f32 = q.dtype == torch.float32
     if world == 1:
         ops = _peer_ops(precision)
-        sq, sk, sv = _local_scales(ops, (q, k, v), rope)
-        q16, k16, v16 = _stage_local(ops, q, sq, rope), _stage_local(ops, k, sk, rope), _stage_local(ops, v, sv)
+        sq, sk, sv = _local_scales(ops, (q, k, v), rope, 2 if rope_k else 1)
+        q16, k16, v16 = (_stage_local(ops, q, sq, rope), _stage_local(ops, k, sk, rope if rope_k else None),
+                         _stage_local(ops, v, sv))
         out = torch.empty((B, Sq, H, D), dtype=torch.bfloat16, device=q.device)
         out32 = torch.empty((B, Sq, H, D), dtype=torch.float32, device=q.device) if (ops.scaled or want_f32) else None
         lse = torch.empty((B, H, Sq), dtype=torch.float32, device=q.device)
@@ -679,7 +681,7 @@ def ring_forward(q, k, v, bias, seg, causal, group, rank, world, layout="auto", 
         pops = _peer_ops(precision)
         tr = _peer_transport(group, q.device, rp._layout_for(plan, q.shape, k.shape[1], pops).total)
         if tr is not None:
-            return rp.run_forward(plan, q, k, v, bias, seg, causal, pops, tr, want_f32, rope)
+            return rp.run_forward(plan, q, k, v, bias, seg, causal, pops, tr, want_f32, rope, rope_k)
         if want_f32:        # the NCCL executor takes bf16 operands (documented in ringattention())
             out, res = ring_forward(q.to(torch.bfloat16), k.to(torch.bfloat16), v.to(torch.bfloat16), bias, seg, causal,
                                     group, rank, world, layout, precision, rope)
@@ -692,8 +694,9 @@ def ring_forward(q, k, v, bias, seg, causal, group, rank, world, layout="auto", 
     return out, _f32_residuals(ops, res)
 
 
-def ring_backward(res, k, v, dout, bias, seg, causal, group, rank, world, layout="auto", precision="bf16", rope=None):
-    """rope: as ring_forward's; dq and dk are then the gradients w.r.t. the un-rotated q and k"""
+def ring_backward(res, k, v, dout, bias, seg, causal, group, rank, world, layout="auto", precision="bf16", rope=None,
+                  rope_k=True):
+    """rope, rope_k: as ring_forward's; dq (and dk when rope_k) are then the gradients w.r.t. the un-rotated q (and k)"""
     B, Sk, H, D = k.shape
     dev = k.device
     want_f32 = k.dtype == torch.float32
@@ -703,7 +706,8 @@ def ring_backward(res, k, v, dout, bias, seg, causal, group, rank, world, layout
         sq, sk, sv = res["scales"]
         Sq = q16.shape[1]
         sdo = _local_scales(ops, (dout,))[0]
-        k16, v16, d16 = _stage_local(ops, k, sk, rope), _stage_local(ops, v, sv), _stage_local(ops, dout, sdo)
+        k16, v16 = _stage_local(ops, k, sk, rope if rope_k else None), _stage_local(ops, v, sv)
+        d16 = _stage_local(ops, dout, sdo)
         delta = torch.empty((B, H, Sq), dtype=torch.float32, device=dev)
         ops.bwd_prep(out, d16, sdo, delta)
         nlse = ops.lse_for_bwd(lse)
@@ -720,8 +724,11 @@ def ring_backward(res, k, v, dout, bias, seg, causal, group, rank, world, layout
             else:
                 dq, dk, dv = [torch.empty(t.shape, dtype=torch.bfloat16, device=dev) for t in (dq_acc, dk_acc, dv_acc)]
                 cast_f32_to_bf16(dv_acc, dv)
+                if not rope_k:
+                    cast_f32_to_bf16(dk_acc, dk)
             ops.reduce_cast_rope([dq_acc], dq, *rope)
-            ops.reduce_cast_rope([dk_acc], dk, *rope)
+            if rope_k:
+                ops.reduce_cast_rope([dk_acc], dk, *rope)
             return dq, dk, dv
         if want_f32:
             return dq_acc, dk_acc, dv_acc
@@ -734,7 +741,7 @@ def ring_backward(res, k, v, dout, bias, seg, causal, group, rank, world, layout
     if _transport(group) == "peer":
         plan = rs.make_peer_plan(world, rank, dout.shape[1], Sk, causal, lay)
         return rp.run_backward(plan, res, k, v, dout, bias, seg, causal, _peer_ops(precision),
-                               rp.CudaPeerTransport.get(group, dev), want_f32, rope)
+                               rp.CudaPeerTransport.get(group, dev), want_f32, rope, rope_k)
     if rope is not None:
         raise _lib.LwmError("ring_backward: the rotary embedding is folded into the one-GPU and peer-memory paths only")
     if want_f32:            # forward fell back to the NCCL executor: bf16 operands in, fp32 gradients out
@@ -762,9 +769,10 @@ def _check_infer_dtypes(q, k, v):
         raise TypeError("ringattention_inference: q, k, v must all be bfloat16 or all float32")
 
 
-def decode_partial(q, k, v, mask_u8, k_pos0, stream=None):
+def decode_partial(q, k, v, mask_u8, k_pos0, stream=None, rope=None):
     """This rank's partial over its KV shard with the GEMV kernel (bf16 or fp32 q/k/v, read as they are)
-    -> (o_part [B*Q*H,128] fp32, ml_part [B*Q*H,2] fp32)."""
+    -> (o_part [B*Q*H,128] fp32, ml_part [B*Q*H,2] fp32). rope: None, or (positions int32 [B,Q], inv_freq): q is
+    un-rotated and the kernel rotates it as it loads it."""
     B, Q, H, D = q.shape
     Sk = k.shape[1]
     rows = B * Q * H
@@ -776,9 +784,13 @@ def decode_partial(q, k, v, mask_u8, k_pos0, stream=None):
     if mask_u8 is not None:
         sb, sq = mask_u8.stride(0), mask_u8.stride(-2)
     fn = "lwm_attn_decode_partial_f32" if q.dtype == torch.float32 else "lwm_attn_decode_partial"
-    _lib.call(fn, _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(mask_u8), _lib.ptr(o_part),
-              _lib.ptr(ml_part), _lib.ptr(ws), B, H, Q, Sk, D, int(k_pos0), int(sb), int(sq), splits,
-              1.0 / math.sqrt(D), _lib.stream_ptr(stream))
+    args = (_lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(mask_u8), _lib.ptr(o_part), _lib.ptr(ml_part), _lib.ptr(ws),
+            B, H, Q, Sk, D, int(k_pos0), int(sb), int(sq), splits, 1.0 / math.sqrt(D))
+    if rope is None:
+        _lib.call(fn, *args, _lib.stream_ptr(stream))
+    else:
+        _lib.call(fn.replace("partial", "partial_rope"), *args, _lib.ptr(rope[0]), _lib.ptr(rope[1]),
+                  _lib.stream_ptr(stream))
     return o_part, ml_part
 
 
@@ -814,6 +826,22 @@ def _scaled_f16(x):
     scale = torch.empty(1, dtype=torch.float32, device=x.device)
     PeerOpsF16.scale_of(x, scale)
     return _stage_local(PeerOpsF16, x, scale), scale
+
+
+def _scaled_f16_rope(x, pos, inv_freq):
+    """_scaled_f16 of x rotated at pos [B,S] (rounded to x's dtype), without the rotated x in memory"""
+    scale = torch.empty(1, dtype=torch.float32, device=x.device)
+    PeerOpsF16.scale_of_rope(x, scale, pos, inv_freq)
+    return _stage_local(PeerOpsF16, x, scale, (pos, inv_freq)), scale
+
+
+def rope_rows(x, pos, inv_freq):
+    """x [B,S,H,128] rotated at pos int32 [B,S], in x's dtype (lwm_attn_rope)"""
+    B, S, H, D = x.shape
+    y = torch.empty(x.shape, dtype=x.dtype, device=x.device)
+    _lib.call("lwm_attn_rope", _lib.ptr(x), None, _dt(x), _lib.ptr(y), None, _dt(x), _lib.ptr(pos), _lib.ptr(inv_freq),
+              B, S, H, 0, D, 0, _lib.stream_ptr())
+    return y
 
 
 def infer_partial(q, k, v, bits, row_any, staged=None):
@@ -881,6 +909,15 @@ class InferOps:
     stage = staticmethod(_scaled_f16)
     backward = staticmethod(infer_backward)
     reduce_cast = staticmethod(PeerOpsF16.reduce_cast)
+    # with the rotary embedding: (pos, inv_freq) follow the tensor they rotate
+    stage_rope = staticmethod(_scaled_f16_rope)
+    rope = staticmethod(rope_rows)
+    reduce_cast_rope = staticmethod(PeerOpsF16.reduce_cast_rope)
+
+    @staticmethod
+    def partial_rope(q, k, v, mask, pos, inv_freq):
+        """the GEMV partial of partial() with un-rotated q, rotated inside the kernel at pos [B,Q]"""
+        return decode_partial(q, k, v, mask, 0, rope=(pos, inv_freq))
 
     @staticmethod
     def partial(q, k, v, mask, row_any, tensor_cores, staged=None):
@@ -959,12 +996,29 @@ def _return_partials(o, ml, comm, B, Ql, H, D):
     return o.contiguous(), ml.contiguous()
 
 
-def _infer_sharded(q, k, v, mask, comm, ops=InferOps, saved=None):
+def _stage(ops, x, pos, inv_freq):
+    """ops.stage of x, or of x rotated at pos when pos is given"""
+    return ops.stage(x) if pos is None else ops.stage_rope(x, pos, inv_freq)
+
+
+def _gemv_partial(ops, q, k, v, mask, pos_q, pos_k, inv_freq):
+    """the GEMV partial; pos_q / pos_k: None, or the positions q / k are rotated at (k by a pass of its own first: a
+    per-key rotation inside the kernel's loop would cost more than the pass)"""
+    if pos_k is not None:
+        k = ops.rope(k, pos_k, inv_freq)
+    if pos_q is None:
+        return ops.partial(q, k, v, mask, None, False)
+    return ops.partial_rope(q, k, v, mask, pos_q, inv_freq)
+
+
+def _infer_sharded(q, k, v, mask, comm, ops=InferOps, saved=None, rope=None):
     """q-sharded protocol (query length > 1 on a ring of comm.world ranks): q [B,Q_loc,H,D] and mask [Bm,1,Q_loc,K]
     are this rank's query rows, k/v [B,S_loc,H,D] its KV shard (K = world*S_loc). Each rank computes the partials of
     ALL world*Q_loc rows over its own keys, so K/V never move; per rank the traffic is world*Q_loc*H*D words of q and
     of partials plus Q_loc*K/8 bytes of mask. Returns this rank's [B,Q_loc,H,D] output.
-    saved: None, or a dict that receives what _infer_sharded_bwd needs (the output is the same either way)."""
+    saved: None, or a dict that receives what _infer_sharded_bwd needs (the output is the same either way).
+    rope: None, or (pos [B,Q_loc] of my query rows, pos_k [B,S_loc] of my keys or None, inv_freq): q (and k when pos_k
+    is given) are un-rotated; the positions are all-gathered with q and every pass works on the rotated rows."""
     B, Ql, H, D = q.shape
     Sk = k.shape[1]
     W = comm.world
@@ -975,6 +1029,12 @@ def _infer_sharded(q, k, v, mask, comm, ops=InferOps, saved=None):
     Qg = W * Ql
     # 1. every rank gets all query rows (it stages them with one scale, from the same data)
     q_all = comm.all_gather(q).transpose(0, 1).reshape(B, Qg, H, D)
+    pq = pk = inv = None
+    if rope is not None:
+        pos, pk, inv = rope
+        pq = comm.all_gather(pos).transpose(0, 1).reshape(B, Qg)
+        if saved is not None:
+            saved.update(pos_all=pq, pos_own=pos, **({} if pk is None else {"pos_k": pk}))
     tc = Qg >= INFER_MIN_Q
     m = row_any = None
     if mask is not None:
@@ -988,16 +1048,18 @@ def _infer_sharded(q, k, v, mask, comm, ops=InferOps, saved=None):
             slabs = m8[:, 0, :, :W * Sk].expand(B, Ql, W * Sk).reshape(B, Ql, W, Sk).permute(2, 0, 1, 3)
             m = comm.all_to_all(slabs).transpose(0, 1).reshape(B, Qg, Sk)
     # 4. partials of all rows over my keys (key splits merged locally)
-    if saved is None:
+    if saved is None and rope is None:
         o, ml = ops.partial(q_all, k, v, m, row_any, tc)
     elif tc:
-        staged = ops.stage(q_all), ops.stage(k), ops.stage(v)
+        staged = _stage(ops, q_all, pq, inv), _stage(ops, k, pk, inv), ops.stage(v)
         o, ml = ops.partial(q_all, k, v, m, row_any, tc, staged=staged)
-        saved.update(staged=staged, bits=m, row_any=row_any)
+        if saved is not None:
+            saved.update(staged=staged, bits=m, row_any=row_any)
     else:
         # the backward recomputes the row statistics on tensor cores (_infer_sharded_bwd)
-        o, ml = ops.partial(q_all, k, v, m, row_any, tc)
-        saved.update(q_all=q_all, k=k, v=v, slabs=m)
+        o, ml = _gemv_partial(ops, q_all, k, v, m, pq, pk, inv)
+        if saved is not None:
+            saved.update(q_all=q_all, k=k, v=v, slabs=m)
     # 5. each owner gets its rows' partials back
     o, ml = _return_partials(o, ml, comm, B, Ql, H, D)
     # 6. merge the world partials
@@ -1008,26 +1070,28 @@ def _infer_sharded(q, k, v, mask, comm, ops=InferOps, saved=None):
     return out
 
 
-def _infer_replicated(q, k, v, mask, rank, comm, ops=InferOps):
+def _infer_replicated(q, k, v, mask, rank, comm, ops=InferOps, rope=None):
     """Replicated protocol (one query row, the generation call, on a ring of comm.world ranks): q [B,1,H,D] and mask
     [Bm,1,1,K] are the same on every rank, k/v [B,S_loc,H,D] are this rank's KV shard (keys [rank*S_loc,
     (rank+1)*S_loc) of K). Each rank reduces its shard to an (o, max, sum) partial with the GEMV kernel, the partials
-    (a few KB) are all-gathered rank-major and merged. Returns the [B,1,H,D] output, the same on every rank."""
+    (a few KB) are all-gathered rank-major and merged. Returns the [B,1,H,D] output, the same on every rank.
+    rope: as _infer_sharded's; every rank rotates the same q at the same positions inside its GEMV."""
     B, Q, H, D = q.shape
     Sk = k.shape[1]
     m = None
     if mask is not None:
         m = mask[:, 0, :, rank * Sk:(rank + 1) * Sk].to(torch.uint8).expand(B, Q, Sk).contiguous()
-    o, ml = ops.partial(q, k, v, m, None, False)
+    o, ml = _gemv_partial(ops, q, k, v, m, *(rope or (None, None, None)))
     o = comm.all_gather(o).transpose(0, 1).contiguous()           # [row][rank][D]
     ml = comm.all_gather(ml).transpose(0, 1).contiguous()
     return ops.merge(o, ml, comm.world, (B, Q, H, D), q.dtype)
 
 
-def _row_stats_tc(q_all, k, v, slabs, comm, ops):
+def _row_stats_tc(q_all, k, v, slabs, comm, ops, pos_all=None, pos_k=None, inv_freq=None):
     """A forward that ran the GEMV kernel (world*Q_loc < INFER_MIN_Q): its uint8 mask slabs [B,Qg,S_loc] (or None)
     become bits, row_any is made global, and the fp32 output and lse of my rows are recomputed with one tensor-core
-    partial and merge on the staged operands, so that the backward's P sums to one over each row.
+    partial and merge on the staged operands, so that the backward's P sums to one over each row. pos_all / pos_k: None,
+    or the positions q_all / k are staged rotated at.
     -> (staged, bits, row_any, o32, lse)"""
     B, Qg, H, D = q_all.shape
     W = comm.world
@@ -1036,14 +1100,14 @@ def _row_stats_tc(q_all, k, v, slabs, comm, ops):
         bits, any_loc = ops.mask_pack(slabs[:, None], B, 1, k.shape[1])
         bits = bits[0]
         row_any = comm.all_gather(any_loc).amax(0)
-    staged = ops.stage(q_all), ops.stage(k), ops.stage(v)
+    staged = _stage(ops, q_all, pos_all, inv_freq), _stage(ops, k, pos_k, inv_freq), ops.stage(v)
     o, ml = ops.partial(q_all, k, v, bits, row_any, True, staged=staged)
     o, ml = _return_partials(o, ml, comm, B, Qg // W, H, D)
     o32, lse = ops.merge_lse(o, ml, W, (B, Qg // W, H, D))
     return staged, bits, row_any, o32, lse
 
 
-def _infer_sharded_bwd(saved, dout, comm, ops=InferOps):
+def _infer_sharded_bwd(saved, dout, comm, ops=InferOps, inv_freq=None):
     """Backward of _infer_sharded (and, with world = 1, of the single-GPU op), mirroring its protocol: K and V never
     move. dout [B,Q_loc,H,D] is the gradient of this rank's rows; saved is what the forward recorded.
       1. all-gather dO; every rank stages all world*Q_loc rows with one shared scale;
@@ -1052,15 +1116,18 @@ def _infer_sharded_bwd(saved, dout, comm, ops=InferOps):
       4. one backward launch of all rows against the local K/V: dK and dV come out complete on their owner;
       5. the fp32 dQ partials go back to the row owners (all_to_all), which sum them in rank order.
     Per rank the traffic is world*Q_loc*H*D words of dO and of fp32 dQ partials, plus world*Q_loc*H*2 floats of lse
-    and delta. -> (dq, dk, dv) in dout's dtype."""
+    and delta. -> (dq, dk, dv) in dout's dtype.
+    With the rotary embedding (saved "pos_own" / "pos_all", and "pos_k" when k was rotated too; inv_freq): the final
+    casts of dQ (and dK) carry the conjugate rotation, so they are the gradients w.r.t. the un-rotated rows."""
     B, Ql, H, D = dout.shape
     W = comm.world
     Qg = W * Ql
+    pos_own, pos_k = saved.get("pos_own"), saved.get("pos_k")
     if "o32" in saved:
         staged, bits, row_any, o32, lse = (saved[n] for n in ("staged", "bits", "row_any", "o32", "lse"))
     else:
         staged, bits, row_any, o32, lse = _row_stats_tc(saved["q_all"], saved["k"], saved["v"], saved["slabs"],
-                                                        comm, ops)
+                                                        comm, ops, saved.get("pos_all"), pos_k, inv_freq)
     (q16, sq), (k16, sk), (v16, sv) = staged
     # 1.
     do_all = comm.all_gather(dout).transpose(0, 1).reshape(B, Qg, H, D)
@@ -1083,11 +1150,18 @@ def _infer_sharded_bwd(saved, dout, comm, ops=InferOps):
         acc = torch.empty(srcs[0].shape, dtype=srcs[0].dtype, device=srcs[0].device)
         ops.reduce_cast(srcs[:LWM_REDUCE_MAX_SRCS], acc)
         srcs = [acc] + srcs[LWM_REDUCE_MAX_SRCS:]
-    ops.reduce_cast([s.contiguous() for s in srcs], dq)
+    if pos_own is None:
+        ops.reduce_cast([s.contiguous() for s in srcs], dq)
+    else:
+        ops.reduce_cast_rope([s.contiguous() for s in srcs], dq, pos_own, inv_freq)
+    if pos_k is not None:       # (fp32: rotated in place)
+        dk_out = dk if dout.dtype == torch.float32 else torch.empty(dk.shape, dtype=dout.dtype, device=dk.device)
+        ops.reduce_cast_rope([dk], dk_out, pos_k, inv_freq)
+        return dq, dk_out, ops.cast(dv, dout.dtype)
     return dq, ops.cast(dk, dout.dtype), ops.cast(dv, dout.dtype)
 
 
-def ringattention_inference(q, k, v, attn_mask, axis_name="sp"):
+def ringattention_inference(q, k, v, attn_mask, axis_name="sp", *, freqs_cis=None, position_ids=None, rotate_k=True):
     """Drop-in for the reference's inference-time op (bound at lwm/llama.py:601-614 inside shard_map).
     q, k, v all bfloat16 or all float32; the output has their dtype (fp32: the un-rounded fp32 result).
     k/v [B,S_loc,H,D] = this rank's contiguous shard of the KV cache.
@@ -1098,43 +1172,68 @@ def ringattention_inference(q, k, v, attn_mask, axis_name="sp"):
     Below INFER_MIN_Q query rows the GEMV kernel runs; from there on the tensor-core kernel over scaled fp16 copies
     of q, k, v with fp32 logits, softmax and accumulation, visiting only the KV tiles the mask leaves visible.
     attn_mask: bool/uint8 [B or 1,1,Q,K_global] (nonzero = attend) or None (every key visible). A row with no true
-    entry in all of K_global averages V over all keys (the reference's finfo.min semantics)."""
-    if not q.is_cuda:
-        raise _lib.LwmError("ringattention_inference: tensors must live on an sm_90 GPU (no CPU fallback)")
-    _check_infer_dtypes(q, k, v)
+    entry in all of K_global averages V over all keys (the reference's finfo.min semantics).
+
+    freqs_cis, position_ids, rotate_k: as on ringattention. Both None: q and k are already rotated (the reference call).
+    Given: q is un-rotated and position_ids [B,Q_loc] are its rows' positions ([B,1], replicated, while generating);
+      * rotate_k=False (decode and cached prefill): k is the rotated KV cache; only q is rotated, inside the GEMV kernel
+        as it loads q, or inside the passes that stage q for the tensor cores (after the all-gather of q and its
+        positions on a q-sharded ring);
+      * rotate_k=True (no KV cache: q and k are the same rows, Q_loc == S_loc): k is rotated at the same positions, by a
+        pass of its own before the GEMV kernel, or inside its staging for the tensor cores.
+    Bit-identical to the call on apply_rotary_emb's rotated q (and k) under autograd (dQ up to the order of its fp32
+    sums); dQ (and dK with rotate_k) are the gradients w.r.t. the un-rotated rows, and position_ids gets none."""
     group, rank, world = _resolve_group(axis_name)
     B, Q, H, D = q.shape
     Sk = k.shape[1]
+    rope = _rope.check_position_ids("ringattention_inference", freqs_cis, position_ids, (B, Q), q.device)
+    if rope is not None and rotate_k and Q != Sk:
+        raise ValueError("ringattention_inference: rotate_k=True rotates q and k at the same positions, which needs "
+                         "Q_loc == S_loc (got %d and %d); with a rotated KV cache pass rotate_k=False" % (Q, Sk))
+    if not q.is_cuda:
+        raise _lib.LwmError("ringattention_inference: tensors must live on an sm_90 GPU (no CPU fallback)")
+    _check_infer_dtypes(q, k, v)
     if attn_mask is not None:
         if attn_mask.dim() != 4 or attn_mask.shape[1] != 1 or attn_mask.shape[2] != Q or attn_mask.shape[0] not in (1, B):
             raise ValueError("attn_mask must be [B,1,Q,K_global] (lwm/llama.py:585-590)")
         if attn_mask.shape[-1] < (world if Q > 1 else rank + 1) * Sk:
             raise ValueError("attn_mask covers %d keys but the ring holds %d" % (attn_mask.shape[-1], world * Sk))
     q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
+    rope_args = (None, None, True) if rope is None else (rope[0], rope[1], bool(rotate_k))
     if torch.is_grad_enabled() and (q.requires_grad or k.requires_grad or v.requires_grad):
-        return _InferAttnFn.apply(q, k, v, attn_mask, axis_name)
-    return _infer_forward(q, k, v, attn_mask, group, rank, world)
+        return _InferAttnFn.apply(q, k, v, attn_mask, axis_name, *rope_args)
+    return _infer_forward(q, k, v, attn_mask, group, rank, world, rope=_infer_rope(*rope_args))
 
 
-def _infer_forward(q, k, v, attn_mask, group, rank, world, saved=None):
+def _infer_rope(pos, inv_freq, rope_k):
+    """-> None, or the (pos_q, pos_k or None, inv_freq) of _infer_sharded"""
+    return None if pos is None else (pos, pos if rope_k else None, inv_freq)
+
+
+def _infer_forward(q, k, v, attn_mask, group, rank, world, saved=None, rope=None):
     """the forward of ringattention_inference; saved: None, or a dict that receives what the backward needs (the
-    output is bit-identical either way)"""
+    output is bit-identical either way); rope: as _infer_sharded's"""
     B, Q, H, D = q.shape
     Sk = k.shape[1]
     if world > 1:
         if Q > 1:
-            return _infer_sharded(q, k, v, attn_mask, TorchComm(group, world), saved=saved)
-        return _infer_replicated(q, k, v, attn_mask, rank, TorchComm(group, world))
+            return _infer_sharded(q, k, v, attn_mask, TorchComm(group, world), saved=saved, rope=rope)
+        return _infer_replicated(q, k, v, attn_mask, rank, TorchComm(group, world), rope=rope)
+    pq, pk, inv = rope or (None, None, None)
+    if saved is not None and rope is not None:
+        saved.update(pos_all=pq, pos_own=pq, **({} if pk is None else {"pos_k": pk}))
     if Q >= INFER_MIN_Q:
         bits = row_any = None
         if attn_mask is not None:
             bits, row_any = mask_pack(attn_mask, B, 1, Sk)
             bits = bits[0]
-        if saved is None:
+        if saved is None and rope is None:
             o_part, ml_part = infer_partial(q, k, v, bits, row_any)
             return decode_merge(o_part, ml_part, 1, (B, Q, H, D), q.dtype)
-        staged = _scaled_f16(q), _scaled_f16(k), _scaled_f16(v)
+        staged = _stage(InferOps, q, pq, inv), _stage(InferOps, k, pk, inv), _scaled_f16(v)
         o_part, ml_part = infer_partial(q, k, v, bits, row_any, staged)
+        if saved is None:
+            return decode_merge(o_part, ml_part, 1, (B, Q, H, D), q.dtype)
         out = decode_merge(o_part, ml_part, 1, (B, Q, H, D), q.dtype)
         o32, lse = decode_merge(o_part, ml_part, 1, (B, Q, H, D), torch.float32, with_lse=True)
         saved.update(staged=staged, bits=bits, row_any=row_any, o32=o32, lse=lse)
@@ -1142,27 +1241,29 @@ def _infer_forward(q, k, v, attn_mask, group, rank, world, saved=None):
     mask = None
     if attn_mask is not None:
         mask = attn_mask.to(torch.uint8).expand(B, 1, Q, attn_mask.shape[-1]).contiguous()
-    o_part, ml_part = decode_partial(q, k, v, mask, 0)
+    o_part, ml_part = _gemv_partial(InferOps, q, k, v, mask, pq, pk, inv)
     if saved is not None:
         # GEMV forward: the backward recomputes the row statistics on tensor cores (_row_stats_tc)
         saved.update(q_all=q, k=k, v=v, slabs=None if attn_mask is None else attn_mask[:, 0])
     return decode_merge(o_part, ml_part, 1, (B, Q, H, D), q.dtype)
 
 
-_INFER_SAVED = ("bits", "row_any", "o32", "lse", "q_all", "k", "v", "slabs")
+_INFER_SAVED = ("bits", "row_any", "o32", "lse", "q_all", "k", "v", "slabs", "pos_all", "pos_own", "pos_k")
 
 
 class _InferAttnFn(torch.autograd.Function):
     """ringattention_inference with a backward w.r.t. q, k, v (the mask gets none). Saves the staged fp16 operands
     with their scales, the fp32 output and lse of this rank's rows and the mask bits with row_any (tensor-core
-    forward), or the operands and mask slabs (GEMV forward: the backward recomputes the row statistics)."""
+    forward), or the operands and mask slabs (GEMV forward: the backward recomputes the row statistics); with the rotary
+    embedding also the positions (the operands are the un-rotated ones)."""
 
     @staticmethod
-    def forward(ctx, q, k, v, attn_mask, axis_name):
+    def forward(ctx, q, k, v, attn_mask, axis_name, rope_pos=None, inv_freq=None, rope_k=True):
         group, rank, world = _resolve_group(axis_name)
         saved = {}
-        out = _infer_forward(q, k, v, attn_mask, group, rank, world, saved)
+        out = _infer_forward(q, k, v, attn_mask, group, rank, world, saved, _infer_rope(rope_pos, inv_freq, rope_k))
         ctx.axis_name, ctx.replicated = axis_name, world > 1 and q.shape[1] == 1
+        ctx.inv_freq = inv_freq
         # a ring whose world*Q_loc rows run the GEMV kernel: not validated on real kernels yet (see DESIGN §3.6)
         ctx.small_ring = world > 1 and 1 < q.shape[1] and world * q.shape[1] < INFER_MIN_Q
         staged = saved.pop("staged", None)
@@ -1188,5 +1289,5 @@ class _InferAttnFn(torch.autograd.Function):
         saved.update(zip(ctx.keys, t))
         group, rank, world = _resolve_group(ctx.axis_name)
         comm = TorchComm(group, world) if world > 1 else _LocalComm()
-        dq, dk, dv = _infer_sharded_bwd(saved, dout.contiguous(), comm)
-        return dq, dk, dv, None, None
+        dq, dk, dv = _infer_sharded_bwd(saved, dout.contiguous(), comm, inv_freq=ctx.inv_freq)
+        return dq, dk, dv, None, None, None, None, None

@@ -78,6 +78,33 @@ def apply_rotary_emb(xq, xk, freqs_cis, dtype=torch.float32, *, position_ids):
     return _Rope.apply(xq, xk, position_ids, freqs_cis, dtype)
 
 
+def rotate(x, freqs_cis, dtype, *, position_ids):
+    """apply_rotary_emb on one tensor: x [B,S,H,128] rotated at position_ids int32 [B,S] (same device, already checked
+    by check_position_ids), in `dtype`; differentiable like apply_rotary_emb."""
+    return _Rope.apply(x, x[:, :, :0], position_ids, freqs_cis, dtype)[0]
+
+
+def check_position_ids(who, freqs_cis, position_ids, shape, device):
+    """The rotary-embedding keywords of the ops that rotate inside their own passes -> None (both None) or
+    (position_ids int32 [shape] contiguous on `device`, inv_freq). Raises ValueError unless they come together, freqs_cis
+    is a RotaryTable, position_ids has `shape` and every position is in [0, max_position). Device positions cost one
+    device->host synchronisation (the range check); host positions none (the copy to the device is asynchronous)."""
+    if freqs_cis is None and position_ids is None:
+        return None
+    if freqs_cis is None or position_ids is None:
+        raise ValueError("%s: freqs_cis and position_ids go together (the rotary embedding needs both)" % who)
+    if not isinstance(freqs_cis, RotaryTable):
+        raise ValueError("%s: freqs_cis must come from lwm_b200.rope.precompute_freqs_cis" % who)
+    if tuple(position_ids.shape) != tuple(shape):
+        raise ValueError("%s: position_ids must be [B, S_loc] = %s, got %s" % (who, tuple(shape), tuple(position_ids.shape)))
+    if position_ids.numel():
+        lo, hi = torch.stack(torch.aminmax(position_ids)).tolist()
+        if lo < 0 or hi >= freqs_cis.max_position:
+            raise ValueError("%s: position_ids outside [0, max_position_embedding)" % who)
+    pos = position_ids.to(dtype=torch.int32)
+    return pos.to(device=device, non_blocking=True).contiguous(), freqs_cis.inv_freq
+
+
 def split_heads(x, num_heads, head_dim=128):
     """_split_heads (llama.py:376-377): [B,S,H*D] -> [B,S,H,D] — a view, never a copy."""
     return x.view(x.shape[0], x.shape[1], num_heads, head_dim)

@@ -92,7 +92,8 @@ int lwm_attn_bwd_step(const void* q, const void* k, const void* v, const void* d
 
 /* fp16-internal precision mode (optional): the tensor cores take bf16 x bf16 or fp16 x fp16 only, so the
  * higher-precision mode converts every operand once to an exact, power-of-two-scaled fp16 copy
- * (lwm_attn_to_f16: x16 = x / scale, scale = 2^(e-12) with e the exponent of the tensor's |max|) and keeps the
+ * (lwm_attn_to_f16: x16 = x / scale, scale = 2^(e-12) with e the exponent of the tensor's largest FINITE |x|,
+ * clamped at -114; 1 when no element is finite and nonzero; NaN and +-inf stay what they are) and keeps the
  * probabilities P and dS at fp16's 11 significant bits instead of bf16's 8. scale_* are DEVICE scalars written
  * by lwm_attn_to_f16; all scale factors are undone in fp32 inside the kernels. Same semantics otherwise.
  * out_f32_or_null: un-rounded copy of `out` written on the last step, so that delta = rowsum(dO o O) of the
@@ -151,8 +152,9 @@ int lwm_attn_bwd_step_map_f16(const void* q16, const void* k16, const void* v16,
                               const float* bias, long long bias_stride, const int* segment_ids, long long seg_stride,
                               float softmax_scale, int dkv_init, const int* tiles, const int* tile_count, void* stream);
 
-/* Sharded-tensor variant of the fp16 operand conversion (ring executor): every rank publishes the |max| bit pattern of
- * its shard (lwm_attn_absmax: atomicMax into *out_bits, caller zeroes it; dtype 0 = fp32, 1 = bf16), all ranks derive
+/* Sharded-tensor variant of the fp16 operand conversion (ring executor): every rank publishes the bit pattern of the
+ * largest finite |x| of its shard (lwm_attn_absmax: atomicMax into *out_bits, caller zeroes it; NaN and +-inf are
+ * skipped; dtype 0 = fp32, 1 = bf16), all ranks derive
  * the SAME power-of-two scale from the gathered patterns (lwm_attn_scale_from_absmax over bits[i*stride], i < n), and
  * convert with it (lwm_attn_to_f16_scaled: dst = fp16(x / *scale); an fp32 source — the dtype the reference's scripts
  * run with — is rounded ONCE to fp16's 11 significant bits instead of going through bf16's 8).
@@ -162,7 +164,7 @@ int lwm_attn_bwd_step_map_f16(const void* q16, const void* k16, const void* v16,
  * HOST array of device pointers. */
 #define LWM_REDUCE_MAX_SRCS 16
 int lwm_attn_absmax(const void* x, int dtype, long long n, unsigned* out_bits, void* stream);
-/* |x|max -> *scale_out = 2^(e-12) in one call (workspace: 4 bytes, zeroed here) */
+/* largest finite |x| -> *scale_out = 2^(e-12) in one call (workspace: 4 bytes, zeroed here) */
 int lwm_attn_absmax_scale(const void* x, int dtype, long long n, unsigned* workspace, float* scale_out, void* stream);
 int lwm_attn_scale_from_absmax(const unsigned* bits, int n, int stride, float* scale_out, void* stream);
 int lwm_attn_to_f16_scaled(const void* x, int dtype, void* dst_f16, const float* scale, long long n, void* stream);
@@ -270,7 +272,7 @@ int lwm_kv_cache_write_rope(const void* k_new, const void* v_new, int dtype, voi
  * position_ids)`): x [B,S,H,128] fp32 (0) or bf16 (1) holds UN-rotated q or k, position_ids int32 [B,S], inv_freq [64]
  * as for lwm_attn_rope. Every pass works on rope(x) rounded to x's dtype — bit for bit what lwm_attn_rope writes — so
  * each equals lwm_attn_rope followed by the plain pass, without the rotated tensor in memory.
- * lwm_attn_absmax_rope      atomicMax of the |rope(x)| bit patterns into *out_bits (caller zeroes it), as lwm_attn_absmax.
+ * lwm_attn_absmax_rope      atomicMax of the finite |rope(x)| bit patterns into *out_bits (caller zeroes it), as lwm_attn_absmax.
  * lwm_attn_stage_rope       dst_dtype 2: dst = fp16(rope(x) / *scale), as lwm_attn_to_f16_scaled; dst_dtype 1: dst =
  *                           bf16(rope(x)), the bf16 operand mode's copy (scale unused, may be null).
  * lwm_reduce_cast_rope_f32  dst [B,S,H,128] = T(rope*(T(sum of n_src <= 16 fp32 arrays, fixed order))), T = fp32 (0) or
@@ -393,8 +395,8 @@ int lwm_vq_conv_cin3(const float* x, const float* w_hwio, const float* bias, flo
 /* "fp16x2" precision mode of the conv stack (the default: <= 1e-3 vs the fp32 reference at 2x instead of 3x the
  * algorithmic tensor work and half the operand bytes):
  * lwm_vq_prep_f16    like lwm_vq_prep, but ONE fp16 operand plane [N,H',W',C_pad] holding y / s, with a power of two s
- *                    written to the device float *scale_out. Without GroupNorm s = 2^(e-12), e the exponent of |x|max:
- *                    x_absmax (required then) holds |x|max's bit pattern when x_absmax_given (lwm_vq_conv2d_f16's
+ *                    written to the device float *scale_out. Without GroupNorm s = 2^(e-12), e the exponent of the
+ *                    largest finite |x|: x_absmax (required then) holds its bit pattern when x_absmax_given (lwm_vq_conv2d_f16's
  *                    absmax_out of the conv that produced x), else it is computed into it; with GroupNorm s brings a bound on
  *                    |y| derived from gn_stats, gamma and beta into [1, 2^13) (s = 1 for ordinary layers). The plane is
  *                    then never inf nor fp16-subnormal because of the activation's magnitude.
@@ -407,7 +409,7 @@ int lwm_vq_conv_cin3(const float* x, const float* w_hwio, const float* bias, flo
  *                    also accumulates (sum, sum of squares) of the OUTPUT per (sample, group) — the statistics of the
  *                    GroupNorm that consumes this tensor (vqgan.py:251,254,161,181), so lwm_vq_gn_stats' extra pass
  *                    over the activation disappears. absmax_out (optional; zeroed by the caller): atomicMax of the
- *                    output's |value| bit patterns, the x_absmax of an lwm_vq_prep_f16 that reads this tensor. */
+ *                    output's finite |value| bit patterns, the x_absmax of an lwm_vq_prep_f16 that reads this tensor. */
 int lwm_vq_prep_f16(const float* x, const double* gn_stats, const float* gamma, const float* beta, void* out,
                     float* scale_out, unsigned* x_absmax, int x_absmax_given, int N, int H, int W, int C, int C_pad,
                     int groups, int upsample2x, float eps, void* stream);

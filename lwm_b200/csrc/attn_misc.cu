@@ -87,7 +87,7 @@ __global__ void add_f32_kernel(float4* __restrict__ dst, const float4* __restric
   }
 }
 
-// |x| max over a bf16 tensor as raw bits (non-negative floats order like unsigned ints)
+// largest finite |x| over a bf16 tensor as raw fp32 bits (NaN and +-inf are skipped: finite_abs_bits)
 __global__ void absmax_bf16_kernel(const uint4* __restrict__ x, long long n8, unsigned* __restrict__ out_bits) {
   unsigned m = 0;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n8;
@@ -96,8 +96,8 @@ __global__ void absmax_bf16_kernel(const uint4* __restrict__ x, long long n8, un
     const unsigned w[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      m = max(m, (w[k] & 0x7fffu) << 16);          // low bf16, sign cleared, as fp32 bits
-      m = max(m, w[k] & 0x7fff0000u);              // high bf16
+      m = max(m, finite_abs_bits(w[k] << 16));           // low bf16, as fp32 bits
+      m = max(m, finite_abs_bits(w[k] & 0xffff0000u));   // high bf16
     }
   }
 #pragma unroll
@@ -105,13 +105,14 @@ __global__ void absmax_bf16_kernel(const uint4* __restrict__ x, long long n8, un
   if ((threadIdx.x & 31) == 0 && m) atomicMax(out_bits, m);
 }
 
-// x16 = fp16(x / scale) with scale = 2^(e-12), e = exponent of the tensor's |max| (scale 1 for an all-zero
-// tensor): the largest magnitude lands in [2^12, 2^13), so anything down to 2^-26 of it stays a normal fp16
-// and the conversion of every such bf16 value (8 significant bits) is exact.
+// x16 = fp16(x / scale) with scale = 2^(e-12), e = exponent of the tensor's largest finite |x| (scale 1 when no
+// element is finite and nonzero): that magnitude lands in [2^12, 2^13), so anything down to 2^-26 of it stays a
+// normal fp16 and the conversion of every such bf16 value (8 significant bits) is exact. NaN and +-inf stay what
+// they are. e is clamped at -114 as in scale_from_absmax_kernel, so that 2^(e-12) and 2^(12-e) are normal floats.
 __global__ void bf16_to_scaled_f16_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, long long n8,
                                           const unsigned* __restrict__ absmax_bits, float* __restrict__ scale_out) {
   const unsigned bits = *absmax_bits;
-  const int e = int(bits >> 23) - 127;
+  const int e = max(int(bits >> 23) - 127, -114);
   const float inv = bits ? __uint_as_float(unsigned(127 - (e - 12)) << 23) : 1.0f;   // 2^(12-e)
   if (blockIdx.x == 0 && threadIdx.x == 0) *scale_out = bits ? __uint_as_float(unsigned(127 + (e - 12)) << 23) : 1.0f;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n8;
@@ -129,13 +130,14 @@ __global__ void bf16_to_scaled_f16_kernel(const uint4* __restrict__ x, uint4* __
 }
 
 
-// |x| max over an fp32 tensor as raw bits
+// largest finite |x| over an fp32 tensor as raw bits
 __global__ void absmax_f32_kernel(const uint4* __restrict__ x, long long n4, unsigned* __restrict__ out_bits) {
   unsigned m = 0;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4;
        i += (long long)gridDim.x * blockDim.x) {
     const uint4 v = x[i];
-    m = max(max(m, v.x & 0x7fffffffu), max(v.y & 0x7fffffffu, max(v.z & 0x7fffffffu, v.w & 0x7fffffffu)));
+    m = max(max(m, finite_abs_bits(v.x)),
+            max(finite_abs_bits(v.y), max(finite_abs_bits(v.z), finite_abs_bits(v.w))));
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
@@ -276,7 +278,7 @@ __device__ __forceinline__ void rope_group_apply(const TIn* __restrict__ x, cons
   }
 }
 
-// absmax_*_kernel of rope(x): atomicMax of the |value| bit patterns into *out_bits
+// absmax_*_kernel of rope(x): atomicMax of the finite |value| bit patterns into *out_bits
 template <typename TIn>
 __global__ void __launch_bounds__(256) absmax_rope_kernel(const TIn* __restrict__ x, const int* __restrict__ pos,
                                                           const float* __restrict__ inv_freq, long long n_tok, int H,
@@ -286,7 +288,7 @@ __global__ void __launch_bounds__(256) absmax_rope_kernel(const TIn* __restrict_
   for (long long tok0 = (long long)blockIdx.x * kRopePos; tok0 < n_tok; tok0 += (long long)gridDim.x * kRopePos) {
     rope_group_apply<TIn>(x, pos, inv_freq, tok0, n_tok, H, cs, [&](long long, const float (&y)[8]) {
 #pragma unroll
-      for (int i = 0; i < 8; ++i) m = max(m, __float_as_uint(y[i]) & 0x7fffffffu);
+      for (int i = 0; i < 8; ++i) m = max(m, finite_abs_bits(__float_as_uint(y[i])));
     });
   }
 #pragma unroll

@@ -163,6 +163,14 @@ LWM_DEVICE uint32_t pack_f16x2(float lo, float hi) {
   asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
   return r;
 }
+// The power-of-two operand scales are taken from the largest FINITE |x|: a NaN or an infinity would otherwise set the
+// scale to 2^116 and flush every finite element of the tensor to zero. Both helpers map a non-finite value to 0.
+// finite_abs_bits: |x| as fp32 bits (non-negative floats order like unsigned ints); finite_absf: |x| as a float.
+LWM_DEVICE uint32_t finite_abs_bits(uint32_t fp32_bits) {
+  const uint32_t a = fp32_bits & 0x7fffffffu;
+  return a < 0x7f800000u ? a : 0u;
+}
+LWM_DEVICE float finite_absf(float x) { return fabsf(x) < INFINITY ? fabsf(x) : 0.f; }
 LWM_DEVICE float ex2f(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));

@@ -148,7 +148,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_consta
   const int cpg = p.stats ? p.Cout / p.groups : 1;
   // fp16x2: accumulator units -> output units, w_scale_inv * a_scale (a product of powers of two: exact)
   const float out_scale = (kF16 && p.a_scale) ? p.w_scale_inv * *p.a_scale : p.w_scale_inv;
-  float amax = 0.f;     // |output| max (fmaxf skips a NaN output, which the next plane keeps as NaN anyway)
+  float amax = 0.f;     // largest finite |output|: a NaN or inf output stays one in the next plane, whatever its scale
   auto flush_stats = [&]() {
     if (st_n < 0) return;
 #pragma unroll
@@ -242,7 +242,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_consta
             o2.y = fminf(fmaxf(o2.y, -1.f), 1.f);
           }
           *reinterpret_cast<float2*>(dst + c) = o2;
-          if (kF16 && p.absmax) amax = fmaxf(amax, fmaxf(fabsf(o2.x), fabsf(o2.y)));
+          if (kF16 && p.absmax) amax = fmaxf(amax, fmaxf(finite_absf(o2.x), finite_absf(o2.y)));
           if (kF16 && p.stats) {   // stats need Cout % 16 == 0 (checked on the host): always this path
             st1[g < kStatG ? g : 0] += o2.x + o2.y;
             st2[g < kStatG ? g : 0] += o2.x * o2.x + o2.y * o2.y;
@@ -256,7 +256,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_consta
               if (res) o += res[c + e];
               if (p.clip) o = fminf(fmaxf(o, -1.f), 1.f);
               dst[c + e] = o;
-              if (kF16 && p.absmax) amax = fmaxf(amax, fabsf(o));
+              if (kF16 && p.absmax) amax = fmaxf(amax, finite_absf(o));
             }
         }
       }

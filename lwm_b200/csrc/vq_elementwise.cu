@@ -57,7 +57,7 @@ __global__ void gn_stats_kernel(const float* __restrict__ x, double* __restrict_
 // kF16: ONE fp16 plane (the fp16x2 conv mode: 11 significant bits, half the bytes of the hi+lo pair) instead, written
 // as y / s with a power-of-two scale s (block 0 stores s to *scale_out; the conv multiplies it back in fp32), so that
 // the plane is neither inf nor fp16-subnormal whatever the activation's magnitude:
-//   no GroupNorm  s = 2^(e-12), e the exponent of |x|max (*absmax_bits: from the producing conv's epilogue, or from
+//   no GroupNorm  s = 2^(e-12), e the exponent of the largest finite |x| (*absmax_bits: from the producing conv's epilogue, or from
 //                 an absmax pass over x): the largest element lands in [2^12, 2^13), as for the attention operands.
 //                 Scaling x by 2^k gives the same plane.
 //   GroupNorm     |silu(t)| <= |t| <= max|gamma| * (sqrt(n_g * E[x^2]) + |mean|) * rstd + max|beta| over every
@@ -93,15 +93,17 @@ __global__ void prep_kernel(const float* __restrict__ x, const double* __restric
       var = fmaxf(var, 0.f);
       s_mr[2 * i] = mean;
       s_mr[2 * i + 1] = rsqrtf(var + eps);
-      if (kF16) dev_max = fmaxf(dev_max, (sqrtf(n_g * msq) + fabsf(mean)) * s_mr[2 * i + 1]);
+      // finite terms only: a (sample, group) with non-finite statistics has a non-finite plane at any scale, and must
+      // not flush the planes of the other samples to zero
+      if (kF16) dev_max = fmaxf(dev_max, finite_absf((sqrtf(n_g * msq) + fabsf(mean)) * s_mr[2 * i + 1]));
     }
     if (kF16) {
       float g_max = 0.f, b_max = 0.f;
       for (int c = threadIdx.x; c < C; c += blockDim.x) {
-        g_max = fmaxf(g_max, fabsf(gamma[c]));
-        b_max = fmaxf(b_max, fabsf(beta[c]));
+        g_max = fmaxf(g_max, finite_absf(gamma[c]));
+        b_max = fmaxf(b_max, finite_absf(beta[c]));
       }
-      // non-negative floats order like their bit patterns (a NaN sorts above +inf)
+      // non-negative floats order like their bit patterns
       const unsigned m0 = __reduce_max_sync(0xffffffffu, __float_as_uint(dev_max));
       const unsigned m1 = __reduce_max_sync(0xffffffffu, __float_as_uint(g_max));
       const unsigned m2 = __reduce_max_sync(0xffffffffu, __float_as_uint(b_max));

@@ -93,6 +93,57 @@ def attention_dense_grads(q, k, v, dout, **kw):
     return dq, dk, dv
 
 
+def visible_pairs(B, Sq, Sk, q_pos0=0, k_pos0=0, attn_bias=None, segment_ids=None, causal=True, mask_value=None):
+    """[B,1,Sq,Sk] bool: the (q, k) pairs that dense_bias leaves unmasked"""
+    mv = finfo_min("bf16") if mask_value is None else mask_value
+    return dense_bias(B, Sq, Sk, q_pos0, k_pos0, attn_bias, segment_ids, causal, mask_value) > mv * 0.5
+
+
+def _contract(w, x, vis, over_keys):
+    """sum_j w[b,h,i,j] x[b,j,h,:] (over_keys) or sum_i w[b,h,i,j] x[b,i,h,:], w zero outside vis [B,1,Sq,Sk]: a
+    non-finite entry of x enters only the products of the pairs in vis (0 * inf would make every pair NaN)"""
+    fin = np.isfinite(x)
+    r = np.einsum("bhqk,bkhd->bqhd" if over_keys else "bhqk,bqhd->bkhd", w, np.where(fin, x, 0.0))
+    for b, n, h, d in zip(*np.nonzero(~fin)):
+        col, vc = (w[b, h, :, n], vis[b, 0, :, n]) if over_keys else (w[b, h, n, :], vis[b, 0, n, :])
+        r[b, :, h, d] += np.where(vc, col * x[b, n, h, d], 0.0)
+    return r
+
+
+def attention_visible(q, k, v, visible, dout=None, mask_value=None):
+    """float64 attention over the pairs where visible [B or 1,1,Sq,Sk] holds, with the masked pairs kept out of every
+    sum by np.where instead of an additive finfo.min, so that a NaN or inf operand reaches only the pairs that see it
+    (NaN + finfo.min would be NaN). A row with no visible pair averages every key uniformly, as attention_dense's fully
+    masked rows do; on finite inputs the results equal attention_dense / attention_dense_grads (and
+    attention_inference_dense). -> (out [B,Sq,H,D], lse [B,H,Sq]), with dout also (dq, dk, dv)."""
+    q, k, v = (np.asarray(t, dtype=np.float64) for t in (q, k, v))
+    B, Sq, H, D = q.shape
+    Sk = k.shape[1]
+    mv = finfo_min("bf16") if mask_value is None else mask_value
+    vis = np.broadcast_to(np.asarray(visible, dtype=bool), (B, 1, Sq, Sk))
+    live = vis.any(-1, keepdims=True)                      # [B,1,Sq,1]
+    vis = vis | ~live
+    with np.errstate(invalid="ignore", over="ignore", divide="ignore"):
+        s = np.einsum("bqhd,bkhd->bhqk", q, k) / np.sqrt(D)
+        s = np.where(live, np.where(vis, s, -np.inf), 0.0)    # dead rows: equal logits, a uniform average
+        m = s.max(axis=-1, keepdims=True)
+        p = np.where(vis, np.exp(s - m), 0.0)
+        den = p.sum(axis=-1, keepdims=True)
+        p = p / den
+        out = _contract(p, v, vis, True)
+        lse = np.where(live[..., 0], (m + np.log(den))[..., 0], mv + np.log(Sk))
+        if dout is None:
+            return out, lse
+        g = np.asarray(dout, dtype=np.float64)
+        dv = _contract(p, g, vis, False)
+        dp = np.einsum("bqhd,bkhd->bhqk", g, v)
+        delta = np.einsum("bqhd,bqhd->bhq", g, out)
+        ds = np.where(vis, p * (dp - delta[..., None]), 0.0)
+        dq = _contract(ds, k, vis, True) / np.sqrt(D)
+        dk = _contract(ds, q, vis, False) / np.sqrt(D)
+    return out, lse, dq, dk, dv
+
+
 def attention_inference_dense(q, k, v, attn_mask, mask_value=None):
     """`ringattention_inference` semantics (SURVEY.md Appendix A; call site lwm/llama.py:601-614):
     q [B,Q,H,D], k/v [B,K,H,D] (the whole, un-sharded cache), attn_mask bool [B,1,Q,K]:

@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define LWM_B200_ABI_VERSION 3
+#define LWM_B200_ABI_VERSION 4
 
 #define LWM_OK 0
 #define LWM_ERR_DEVICE 1
@@ -42,6 +42,10 @@ const char* lwm_last_error(void);
  *
  *   q            [B, Sq, H, D] bf16      local query shard (contiguous)
  *   k, v         [B, Sk, H, D] bf16      the K/V block currently held by this rank
+ *   scale_q/k/v  all NULL (bf16 operands), or all given: fp16 operand mode (below), q/k/v are the scaled fp16 copies
+ *                and these their device scales
+ *   out_f32      fp16 operand mode only, else NULL: the un-rounded fp32 copy of `out`, written when `last`, so that
+ *                delta = rowsum(dO o O) of the backward is not limited by the bf16 rounding of `out`
  *   out          [B, Sq, H, D] bf16      final output, written when `last`
  *   lse          [B, H, Sq]    fp32      log-sum-exp (natural log) of the scaled+biased logits,
  *                                        written when `last` (residual for the backward)
@@ -57,21 +61,26 @@ const char* lwm_last_error(void);
  *                (the [B,1,1,S_global] attn_bias of lwm/llama.py:533-537 squeezed), or NULL
  *   segment_ids  [B, seg_stride] int32 indexed by global position, or NULL
  *   softmax_scale 1/sqrt(D)
- * Constraints: D == 128; Sq, Sk multiples of 128.
+ *   tiles, tile_count  both NULL, or the forward block map of lwm_attn_step_tilemap built from the same arguments (bias
+ *                or segment_ids required then): the kernel visits only the KV tiles in it. Results are bit-identical.
+ * Constraints: D == 128; Sq, Sk multiples of 128. A partial set of scales, out_f32 without scales, or only one of
+ * tiles / tile_count is LWM_ERR_ARG.
  */
-int lwm_attn_fwd_step(const void* q, const void* k, const void* v, void* out, float* lse, float* acc_o,
-                      float* acc_m, float* acc_l, int B, int H, int Sq, int Sk, int D, long long q_pos0,
-                      long long k_pos0, int causal, const float* bias, long long bias_stride,
-                      const int* segment_ids, long long seg_stride, float softmax_scale, int first, int last,
-                      void* stream);
+int lwm_attn_fwd_step(const void* q, const void* k, const void* v, const float* scale_q, const float* scale_k,
+                      const float* scale_v, float* out_f32, void* out, float* lse, float* acc_o, float* acc_m,
+                      float* acc_l, int B, int H, int Sq, int Sk, int D, long long q_pos0, long long k_pos0, int causal,
+                      const float* bias, long long bias_stride, const int* segment_ids, long long seg_stride,
+                      float softmax_scale, int first, int last, const int* tiles, const int* tile_count, void* stream);
 
 /* Ring attention, backward.
- * lwm_attn_bwd_prep: delta[b,h,s] = sum_d dout[b,s,h,d] * out[b,s,h,d]  (fp32), once per backward.
+ * lwm_attn_bwd_prep: delta[b,h,s] = sum_d dout[b,s,h,d] * out[b,s,h,d]  (fp32), once per backward. out fp32
+ *                    (out_dtype 0) or bf16 (1); dout bf16 when scale_do is NULL, else its scaled fp16 copy with its
+ *                    device scale.
  * lwm_attn_bwd_lse:  nlse2[i] = -lse[i]*log2(e) + offset_log2 (-inf for rows whose lse is at the masked level), once per
  *                    backward; lwm_attn_bwd_step takes THIS array as its `lse` argument (the per-tile kernel is
- *                    exp-bound). offset_log2 = 0 for lwm_attn_bwd_step (bf16 operands) and
- *                    LWM_ATTN_F16_P_BOOST_LOG2 for lwm_attn_bwd_step_f16: the fp16 kernel keeps P^T * 2^14 so that the
- *                    normalised probabilities of a 128K .. 1M-key row stay normal fp16 numbers.
+ *                    exp-bound). offset_log2 = 0 for bf16 operands and LWM_ATTN_F16_P_BOOST_LOG2 for the fp16 operand
+ *                    mode: the fp16 kernel keeps P^T * 2^14 so that the normalised probabilities of a 128K .. 1M-key
+ *                    row stay normal fp16 numbers.
  * lwm_attn_bwd_step: one ring step of the reference's custom_vjp bwd (SURVEY.md Appendix A `bwd`):
  *   recomputes P from (q, k, lse), accumulates
  *     dq_acc [B,Sq,H,D] fp32 += dS K / sqrt(D)        (atomic fp32 tile reductions; zero it first)
@@ -80,37 +89,29 @@ int lwm_attn_fwd_step(const void* q, const void* k, const void* v, void* out, fl
  *   dk_acc/dv_acc travel with the K/V block around the ring exactly like the reference's dk, dv.
  *   dkv_init != 0: the dk_acc/dv_acc rows of the key tiles this launch visits are WRITTEN instead of accumulated
  *   (first visit of a block: saves zero-filling the accumulators); key tiles no query row can see are zero-filled.
+ *   scale_q/k/v/do: all NULL (bf16 operands) or all given (fp16 operand mode, dout its scaled fp16 copy too);
+ *   tiles, tile_count: both NULL, or the backward block map of lwm_attn_step_tilemap (bias or segment_ids required):
+ *   dK and dV are bit-identical to the call without it, dQ differs only by the order of its fp32 reductions, which
+ *   already varies from run to run. Other arguments as for lwm_attn_fwd_step.
  */
 #define LWM_ATTN_F16_P_BOOST_LOG2 14.0f
-int lwm_attn_bwd_prep(const void* out, const void* dout, float* delta, int B, int H, int Sq, int D, void* stream);
+int lwm_attn_bwd_prep(const void* out, int out_dtype, const void* dout, const float* scale_do, float* delta, int B,
+                      int H, int Sq, int D, void* stream);
 int lwm_attn_bwd_lse(const float* lse, float* nlse2, long long n, float offset_log2, void* stream);
-int lwm_attn_bwd_step(const void* q, const void* k, const void* v, const void* dout, const float* lse,
-                      const float* delta, float* dq_acc, float* dk_acc, float* dv_acc, int B, int H, int Sq,
-                      int Sk, int D, long long q_pos0, long long k_pos0, int causal, const float* bias,
-                      long long bias_stride, const int* segment_ids, long long seg_stride, float softmax_scale,
-                      int dkv_init, void* stream);
+int lwm_attn_bwd_step(const void* q, const void* k, const void* v, const void* dout, const float* scale_q,
+                      const float* scale_k, const float* scale_v, const float* scale_do, const float* lse,
+                      const float* delta, float* dq_acc, float* dk_acc, float* dv_acc, int B, int H, int Sq, int Sk,
+                      int D, long long q_pos0, long long k_pos0, int causal, const float* bias, long long bias_stride,
+                      const int* segment_ids, long long seg_stride, float softmax_scale, int dkv_init,
+                      const int* tiles, const int* tile_count, void* stream);
 
 /* fp16-internal precision mode (optional): the tensor cores take bf16 x bf16 or fp16 x fp16 only, so the
  * higher-precision mode converts every operand once to an exact, power-of-two-scaled fp16 copy
  * (lwm_attn_to_f16: x16 = x / scale, scale = 2^(e-12) with e the exponent of the tensor's largest FINITE |x|,
  * clamped at -114; 1 when no element is finite and nonzero; NaN and +-inf stay what they are) and keeps the
- * probabilities P and dS at fp16's 11 significant bits instead of bf16's 8. scale_* are DEVICE scalars written
- * by lwm_attn_to_f16; all scale factors are undone in fp32 inside the kernels. Same semantics otherwise.
- * out_f32_or_null: un-rounded copy of `out` written on the last step, so that delta = rowsum(dO o O) of the
- * backward (lwm_attn_bwd_prep_f32) is not limited by the bf16 rounding of `out`. */
-int lwm_attn_bwd_prep_f32(const float* out_f32, const void* dout, float* delta, int B, int H, int Sq, int D, void* stream);
+ * probabilities P and dS at fp16's 11 significant bits instead of bf16's 8. The scales are DEVICE scalars written
+ * by lwm_attn_to_f16; all scale factors are undone in fp32 inside the kernels. Same semantics otherwise. */
 int lwm_attn_to_f16(const void* src_bf16, void* dst_f16, float* scale_out, void* workspace4, long long n, void* stream);
-int lwm_attn_fwd_step_f16(const void* q16, const void* k16, const void* v16, const float* scale_q, const float* scale_k,
-                          const float* scale_v, float* out_f32_or_null, void* out, float* lse, float* acc_o, float* acc_m, float* acc_l, int B,
-                          int H, int Sq, int Sk, int D, long long q_pos0, long long k_pos0, int causal,
-                          const float* bias, long long bias_stride, const int* segment_ids, long long seg_stride,
-                          float softmax_scale, int first, int last, void* stream);
-int lwm_attn_bwd_step_f16(const void* q16, const void* k16, const void* v16, const void* dout16, const float* scale_q,
-                          const float* scale_k, const float* scale_v, const float* scale_do, const float* lse,
-                          const float* delta, float* dq_acc, float* dk_acc, float* dv_acc, int B, int H, int Sq, int Sk,
-                          int D, long long q_pos0, long long k_pos0, int causal, const float* bias,
-                          long long bias_stride, const int* segment_ids, long long seg_stride, float softmax_scale,
-                          int dkv_init, void* stream);
 
 /* Block map of a training step with a padding bias and/or segment ids (packed or padded sequences): the tile kernels
  * then visit only the (Q tile, KV tile) pairs that hold a visible entry, and read the mask only where it varies.
@@ -121,36 +122,10 @@ int lwm_attn_bwd_step_f16(const void* q16, const void* k16, const void* v16, con
  *                        [B][Sk/128]. Either map may be omitted (both of its pointers null). workspace >=
  *                        B * (Sq/64 + Sk/128) * 16 bytes. A pair is left out when every entry is masked (bias below the
  *                        masked level, or disjoint segment ids); in the forward only for Q tiles whose every row sees its
- *                        own key in this step. mixed = the pair reads bias / segment ids per element.
- * lwm_attn_{fwd,bwd}_step_map[_f16]  lwm_attn_{fwd,bwd}_step[_f16] with the matching map of lwm_attn_step_tilemap
- *                        (built from the same arguments) appended; bias or segment_ids required. out, lse, the carries,
- *                        dK and dV are bit-identical to the calls without a map; dQ differs only by the order of its
- *                        fp32 reductions, which already varies from run to run. */
+ *                        own key in this step. mixed = the pair reads bias / segment ids per element. */
 int lwm_attn_step_tilemap(const float* bias, long long bias_stride, const int* segment_ids, long long seg_stride, int B,
                           int Sq, int Sk, long long q_pos0, long long k_pos0, int causal, int* fwd_tiles, int* fwd_count,
                           int* bwd_tiles, int* bwd_count, void* workspace, void* stream);
-int lwm_attn_fwd_step_map(const void* q, const void* k, const void* v, void* out, float* lse, float* acc_o,
-                          float* acc_m, float* acc_l, int B, int H, int Sq, int Sk, int D, long long q_pos0,
-                          long long k_pos0, int causal, const float* bias, long long bias_stride,
-                          const int* segment_ids, long long seg_stride, float softmax_scale, int first, int last,
-                          const int* tiles, const int* tile_count, void* stream);
-int lwm_attn_fwd_step_map_f16(const void* q16, const void* k16, const void* v16, const float* scale_q,
-                              const float* scale_k, const float* scale_v, float* out_f32_or_null, void* out, float* lse,
-                              float* acc_o, float* acc_m, float* acc_l, int B, int H, int Sq, int Sk, int D,
-                              long long q_pos0, long long k_pos0, int causal, const float* bias, long long bias_stride,
-                              const int* segment_ids, long long seg_stride, float softmax_scale, int first, int last,
-                              const int* tiles, const int* tile_count, void* stream);
-int lwm_attn_bwd_step_map(const void* q, const void* k, const void* v, const void* dout, const float* lse,
-                          const float* delta, float* dq_acc, float* dk_acc, float* dv_acc, int B, int H, int Sq,
-                          int Sk, int D, long long q_pos0, long long k_pos0, int causal, const float* bias,
-                          long long bias_stride, const int* segment_ids, long long seg_stride, float softmax_scale,
-                          int dkv_init, const int* tiles, const int* tile_count, void* stream);
-int lwm_attn_bwd_step_map_f16(const void* q16, const void* k16, const void* v16, const void* dout16,
-                              const float* scale_q, const float* scale_k, const float* scale_v, const float* scale_do,
-                              const float* lse, const float* delta, float* dq_acc, float* dk_acc, float* dv_acc, int B,
-                              int H, int Sq, int Sk, int D, long long q_pos0, long long k_pos0, int causal,
-                              const float* bias, long long bias_stride, const int* segment_ids, long long seg_stride,
-                              float softmax_scale, int dkv_init, const int* tiles, const int* tile_count, void* stream);
 
 /* Sharded-tensor variant of the fp16 operand conversion (ring executor): every rank publishes the bit pattern of the
  * largest finite |x| of its shard (lwm_attn_absmax: atomicMax into *out_bits, caller zeroes it; NaN and +-inf are
@@ -158,7 +133,6 @@ int lwm_attn_bwd_step_map_f16(const void* q16, const void* k16, const void* v16,
  * the SAME power-of-two scale from the gathered patterns (lwm_attn_scale_from_absmax over bits[i*stride], i < n), and
  * convert with it (lwm_attn_to_f16_scaled: dst = fp16(x / *scale); an fp32 source — the dtype the reference's scripts
  * run with — is rounded ONCE to fp16's 11 significant bits instead of going through bf16's 8).
- * lwm_attn_bwd_prep_f16: delta = rowsum(out o dout) with dout given as its scaled fp16 copy; out fp32 (0) or bf16 (1).
  * lwm_reduce_cast_f32: dst = cast(sum of n_src <= 16 fp32 arrays, fixed order) — folds the dK/dV partials that
  * landed in the owner's heap and writes the gradient in its final dtype (0 fp32, 1 bf16) in one pass. host_srcs is a
  * HOST array of device pointers. */
@@ -168,43 +142,25 @@ int lwm_attn_absmax(const void* x, int dtype, long long n, unsigned* out_bits, v
 int lwm_attn_absmax_scale(const void* x, int dtype, long long n, unsigned* workspace, float* scale_out, void* stream);
 int lwm_attn_scale_from_absmax(const unsigned* bits, int n, int stride, float* scale_out, void* stream);
 int lwm_attn_to_f16_scaled(const void* x, int dtype, void* dst_f16, const float* scale, long long n, void* stream);
-int lwm_attn_bwd_prep_f16(const void* out, int out_dtype, const void* dout16, const float* scale_do, float* delta, int B,
-                          int H, int Sq, int D, void* stream);
 int lwm_reduce_cast_f32(const float* const* host_srcs, int n_src, void* dst, int dst_dtype, long long n, void* stream);
 
 /* Decode-time attention — the reference's `ringattention_inference(q, k, v, attn_mask, axis_name)` (call site
  * lwm/llama.py:601-614; SURVEY.md §8f next-row 1): a few query rows against this rank's KV-cache shard with an
  * explicit boolean mask [B,1,Q,K_global] (nonzero = attend; masked logits take finfo.min semantics).
  * lwm_attn_decode_partial reduces the local shard to one partial per (b, q, h): numerator o_part [B*Q*H,128] fp32 and
- * ml_part [B*Q*H,2] = (max in the log2 domain, denominator); lwm_attn_decode_merge folds n_part partials (the
- * all-gathered per-rank partials, laid out [row][n_part]) into out (bf16 [B,Q,H,128]) and lse [B*Q*H].
- * workspace >= splits * B*Q*H * 130 floats. HBM-bound: K and V are streamed exactly once. */
-int lwm_attn_decode_partial(const void* q, const void* k, const void* v, const unsigned char* mask, float* o_part,
-                            float* ml_part, void* workspace, int B, int H, int Q, int Sk, int D, long long k_pos0,
-                            long long mask_stride_b, long long mask_stride_q, int splits, float softmax_scale,
-                            void* stream);
-int lwm_attn_decode_merge(const float* o_parts, const float* ml_parts, int n_part, void* out, float* lse,
+ * ml_part [B*Q*H,2] = (max in the log2 domain, denominator). q, k, v are all fp32 (dtype 0, read directly) or all bf16
+ * (1). position_ids int32 [B,Q] and inv_freq [64] as for lwm_attn_rope, or both NULL: q is UN-rotated and is rotated as
+ * it is loaded, rounded to its dtype — bit for bit lwm_attn_rope (out_dtype = dtype) followed by the call without
+ * them, without the rotated q in memory. workspace >= splits * B*Q*H * 130 floats. HBM-bound: K and V are streamed
+ * exactly once.
+ * lwm_attn_decode_merge folds n_part partials (the all-gathered per-rank partials, laid out [row][n_part]) into out
+ * [B,Q,H,128], bf16 (out_dtype 1) or the un-rounded fp32 (0), and lse [B*Q*H]. */
+int lwm_attn_decode_partial(const void* q, const void* k, const void* v, int dtype, const unsigned char* mask,
+                            float* o_part, float* ml_part, void* workspace, int B, int H, int Q, int Sk, int D,
+                            long long k_pos0, long long mask_stride_b, long long mask_stride_q, int splits,
+                            float softmax_scale, const int* position_ids, const float* inv_freq, void* stream);
+int lwm_attn_decode_merge(const float* o_parts, const float* ml_parts, int n_part, void* out, int out_dtype, float* lse,
                           long long rows, void* stream);
-/* fp32 inputs / fp32 output: lwm_attn_decode_partial_f32 reads fp32 q, k, v directly (same arguments, same partial
- * layout); lwm_attn_decode_merge_f32 writes the un-rounded fp32 output. */
-int lwm_attn_decode_partial_f32(const float* q, const float* k, const float* v, const unsigned char* mask,
-                                float* o_part, float* ml_part, void* workspace, int B, int H, int Q, int Sk, int D,
-                                long long k_pos0, long long mask_stride_b, long long mask_stride_q, int splits,
-                                float softmax_scale, void* stream);
-/* The same two partials with UN-rotated q [B,Q,H,128] (bf16, resp. fp32): position_ids int32 [B,Q] and inv_freq [64]
- * as for lwm_attn_rope. q is rotated as it is loaded, rounded to its dtype: bit for bit lwm_attn_rope (out_dtype = the
- * input dtype) followed by lwm_attn_decode_partial(_f32), without the rotated q in memory. */
-int lwm_attn_decode_partial_rope(const void* q, const void* k, const void* v, const unsigned char* mask, float* o_part,
-                                 float* ml_part, void* workspace, int B, int H, int Q, int Sk, int D, long long k_pos0,
-                                 long long mask_stride_b, long long mask_stride_q, int splits, float softmax_scale,
-                                 const int* position_ids, const float* inv_freq, void* stream);
-int lwm_attn_decode_partial_rope_f32(const float* q, const float* k, const float* v, const unsigned char* mask,
-                                     float* o_part, float* ml_part, void* workspace, int B, int H, int Q, int Sk,
-                                     int D, long long k_pos0, long long mask_stride_b, long long mask_stride_q,
-                                     int splits, float softmax_scale, const int* position_ids, const float* inv_freq,
-                                     void* stream);
-int lwm_attn_decode_merge_f32(const float* o_parts, const float* ml_parts, int n_part, float* out, float* lse,
-                              long long rows, void* stream);
 
 /* Tensor-core inference path (multi-row queries). The mask becomes bits and a per-(b, 128-row Q tile) list of KV tiles:
  * lwm_attn_mask_pack      mask element (b, q, k) at mask[b*stride_b + q*stride_q + k*stride_k] (uint8/bool, nonzero =

@@ -14,33 +14,19 @@ c_void_p, c_int, c_ll, c_float = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlon
 # name -> argtypes ; every function returns int status except where noted
 _SIGNATURES = {
     "lwm_abi_version": [],
-    "lwm_attn_fwd_step": [c_void_p] * 8 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll,
-                                                       c_float, c_int, c_int, c_void_p],
-    "lwm_attn_bwd_prep": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
+    "lwm_attn_fwd_step": [c_void_p] * 12 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll, c_float,
+                                                         c_int, c_int, c_void_p, c_void_p, c_void_p],
+    "lwm_attn_bwd_prep": [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
     "lwm_attn_bwd_lse": [c_void_p, c_void_p, c_ll, c_float, c_void_p],
-    "lwm_attn_bwd_step": [c_void_p] * 9 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll,
-                                                       c_float, c_int, c_void_p],
+    "lwm_attn_bwd_step": [c_void_p] * 13 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll, c_float,
+                                                         c_int, c_void_p, c_void_p, c_void_p],
     "lwm_attn_to_f16": [c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_void_p],
-    "lwm_attn_bwd_prep_f32": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
-    "lwm_attn_fwd_step_f16": [c_void_p] * 12 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll,
-                                                             c_float, c_int, c_int, c_void_p],
-    "lwm_attn_bwd_step_f16": [c_void_p] * 13 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll,
-                                                             c_float, c_int, c_void_p],
     "lwm_attn_step_tilemap": [c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_ll, c_ll, c_int]
                              + [c_void_p] * 6,
-    "lwm_attn_fwd_step_map": [c_void_p] * 8 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll,
-                                                           c_float, c_int, c_int, c_void_p, c_void_p, c_void_p],
-    "lwm_attn_fwd_step_map_f16": [c_void_p] * 12 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll,
-                                                                 c_float, c_int, c_int, c_void_p, c_void_p, c_void_p],
-    "lwm_attn_bwd_step_map": [c_void_p] * 9 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll,
-                                                           c_float, c_int, c_void_p, c_void_p, c_void_p],
-    "lwm_attn_bwd_step_map_f16": [c_void_p] * 13 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll,
-                                                                 c_float, c_int, c_void_p, c_void_p, c_void_p],
     "lwm_attn_absmax": [c_void_p, c_int, c_ll, c_void_p, c_void_p],
     "lwm_attn_absmax_scale": [c_void_p, c_int, c_ll, c_void_p, c_void_p, c_void_p],
     "lwm_attn_scale_from_absmax": [c_void_p, c_int, c_int, c_void_p, c_void_p],
     "lwm_attn_to_f16_scaled": [c_void_p, c_int, c_void_p, c_void_p, c_ll, c_void_p],
-    "lwm_attn_bwd_prep_f16": [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
     "lwm_reduce_cast_f32": [c_void_p, c_int, c_void_p, c_int, c_ll, c_void_p],
     "lwm_ring_ctx_create": [c_int, c_int, c_ll, c_int, c_void_p],
     "lwm_ring_ctx_get_handle": [c_void_p, c_void_p],
@@ -51,14 +37,9 @@ _SIGNATURES = {
     "lwm_ring_ctx_destroy": [c_void_p],
     "lwm_ring_plan": [c_int, c_int, c_ll, c_ll, c_int, c_int, c_int, c_void_p],
     "lwm_ring_layout": [c_int, c_ll, c_ll, c_int, c_int, c_int, c_int, c_int, c_void_p],
-    "lwm_attn_decode_partial": [c_void_p] * 7 + [c_int] * 5 + [c_ll, c_ll, c_ll, c_int, c_float, c_void_p],
-    "lwm_attn_decode_merge": [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_ll, c_void_p],
-    "lwm_attn_decode_partial_f32": [c_void_p] * 7 + [c_int] * 5 + [c_ll, c_ll, c_ll, c_int, c_float, c_void_p],
-    "lwm_attn_decode_merge_f32": [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_ll, c_void_p],
-    "lwm_attn_decode_partial_rope": [c_void_p] * 7 + [c_int] * 5 + [c_ll, c_ll, c_ll, c_int, c_float]
-                                    + [c_void_p] * 3,
-    "lwm_attn_decode_partial_rope_f32": [c_void_p] * 7 + [c_int] * 5 + [c_ll, c_ll, c_ll, c_int, c_float]
-                                        + [c_void_p] * 3,
+    "lwm_attn_decode_partial": [c_void_p] * 3 + [c_int] + [c_void_p] * 4 + [c_int] * 5 + [c_ll, c_ll, c_ll, c_int, c_float]
+                               + [c_void_p] * 3,
+    "lwm_attn_decode_merge": [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_ll, c_void_p],
     "lwm_kv_cache_write_rope": [c_void_p, c_void_p, c_int] + [c_void_p] * 4 + [c_int, c_int, c_ll, c_int, c_int, c_ll,
                                                                                c_int, c_int, c_void_p],
     "lwm_attn_mask_pack": [c_void_p, c_ll, c_ll, c_ll, c_int, c_int, c_ll, c_int, c_int, c_void_p, c_void_p, c_void_p],

@@ -452,12 +452,18 @@ static bool make_f32_tmap(CUtensorMap* tm, const void* ptr, int B, int S, int H,
 
 using namespace lwm;
 
-static int attn_bwd_launch(const void* q, const void* k, const void* v, const void* dout, const float* lse,
-                           const float* delta, float* dq_acc, float* dk_acc, float* dv_acc, int B, int H, int Sq,
-                           int Sk, int D, long long q_pos0, long long k_pos0, int causal, const float* bias,
-                           long long bias_stride, const int* segment_ids, long long seg_stride, float softmax_scale,
-                           const float* scale_q, const float* scale_k, const float* scale_v, const float* scale_do,
-                           int dkv_init, const int* tiles, const int* tile_count, void* stream) {
+// One ring step (include/lwm_b200.h): the scales select the fp16-operand kernel, tiles / tile_count the block map.
+extern "C" int lwm_attn_bwd_step(const void* q, const void* k, const void* v, const void* dout, const float* scale_q,
+                                 const float* scale_k, const float* scale_v, const float* scale_do, const float* lse,
+                                 const float* delta, float* dq_acc, float* dk_acc, float* dv_acc, int B, int H,
+                                 int Sq, int Sk, int D, long long q_pos0, long long k_pos0, int causal,
+                                 const float* bias, long long bias_stride, const int* segment_ids,
+                                 long long seg_stride, float softmax_scale, int dkv_init, const int* tiles,
+                                 const int* tile_count, void* stream) {
+  if (!scale_k != !scale_q || !scale_v != !scale_q || !scale_do != !scale_q)
+    return lwm_fail(LWM_ERR_ARG, "attn_bwd: scales are all given (fp16 operands) or all null (bf16)");
+  if (!tiles != !tile_count) return lwm_fail(LWM_ERR_ARG, "attn_bwd: tiles and tile_count are both given or both null");
+  if (tiles && !bias && !segment_ids) return lwm_fail(LWM_ERR_ARG, "attn_bwd: a block map needs bias or segment_ids");
   if (D != kHeadDim) return lwm_fail(LWM_ERR_SHAPE, "attn_bwd: head_dim must be 128");
   if (B <= 0 || H <= 0 || Sq <= 0 || Sk <= 0 || Sq % kTile || Sk % kTile)
     return lwm_fail(LWM_ERR_SHAPE, "attn_bwd: Sq and Sk must be positive multiples of 128");
@@ -470,7 +476,7 @@ static int attn_bwd_launch(const void* q, const void* k, const void* v, const vo
   if (segment_ids && (seg_stride < q_pos0 + Sq || seg_stride < k_pos0 + Sk))
     return lwm_fail(LWM_ERR_SHAPE, "attn_bwd: segment_ids is indexed by GLOBAL position: seg_stride < max(q_pos0 + Sq, k_pos0 + Sk)");
   if (tiles && (long long)B * (Sk / kTile) * (Sq / kBQ) > 0x7fffffffLL)
-    return lwm_fail(LWM_ERR_SHAPE, "attn_bwd_map: B * Sk/128 * Sq/64 must fit in int32");
+    return lwm_fail(LWM_ERR_SHAPE, "attn_bwd: B * Sk/128 * Sq/64 must fit in int32 with a block map");
   if (!lwm_check_device()) return LWM_ERR_DEVICE;
   CUtensorMap tq, tk, tv, tdo, tdq;
   if (!make_bf16_tmap(&tq, q, B, Sq, H, kBQ) || !make_bf16_tmap(&tk, k, B, Sk, H, kTile) ||
@@ -514,66 +520,6 @@ static int attn_bwd_launch(const void* q, const void* k, const void* v, const vo
   if (scale_q) attn_bwd_kernel<true><<<grid, kBwdThreads, kBwdSmemBytes, st>>>(tq, tk, tv, tdo, tdq, p);
   else attn_bwd_kernel<false><<<grid, kBwdThreads, kBwdSmemBytes, st>>>(tq, tk, tv, tdo, tdq, p);
   return lwm_check_launch("attn_bwd_kernel");
-}
-
-extern "C" int lwm_attn_bwd_step(const void* q, const void* k, const void* v, const void* dout, const float* lse,
-                                 const float* delta, float* dq_acc, float* dk_acc, float* dv_acc, int B, int H,
-                                 int Sq, int Sk, int D, long long q_pos0, long long k_pos0, int causal,
-                                 const float* bias, long long bias_stride, const int* segment_ids,
-                                 long long seg_stride, float softmax_scale, int dkv_init, void* stream) {
-  return attn_bwd_launch(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, B, H, Sq, Sk, D, q_pos0, k_pos0, causal,
-                         bias, bias_stride, segment_ids, seg_stride, softmax_scale, nullptr, nullptr, nullptr, nullptr,
-                         dkv_init, nullptr, nullptr, stream);
-}
-
-// fp16-operand variant: scale_* = device scalars of the four fp16 operand copies (lwm_attn_to_f16).
-extern "C" int lwm_attn_bwd_step_f16(const void* q16, const void* k16, const void* v16, const void* dout16,
-                                     const float* scale_q, const float* scale_k, const float* scale_v,
-                                     const float* scale_do, const float* lse, const float* delta, float* dq_acc,
-                                     float* dk_acc, float* dv_acc, int B, int H, int Sq, int Sk, int D,
-                                     long long q_pos0, long long k_pos0, int causal, const float* bias,
-                                     long long bias_stride, const int* segment_ids, long long seg_stride,
-                                     float softmax_scale, int dkv_init, void* stream) {
-  if (!scale_q || !scale_k || !scale_v || !scale_do) return lwm_fail(LWM_ERR_ARG, "attn_bwd_f16: scales required");
-  return attn_bwd_launch(q16, k16, v16, dout16, lse, delta, dq_acc, dk_acc, dv_acc, B, H, Sq, Sk, D, q_pos0, k_pos0,
-                         causal, bias, bias_stride, segment_ids, seg_stride, softmax_scale, scale_q, scale_k, scale_v,
-                         scale_do, dkv_init, nullptr, nullptr, stream);
-}
-
-// Block-map variants (a bias or segment ids given): tiles / tile_count are the backward map of lwm_attn_step_tilemap,
-// built with the same (bias, segment_ids, B, Sq, Sk, q_pos0, k_pos0, causal). dK and dV are bit-identical to
-// lwm_attn_bwd_step / lwm_attn_bwd_step_f16; dQ differs only by the order of its reductions.
-static int bwd_map_args(const float* bias, const int* segment_ids, const int* tiles, const int* tile_count) {
-  if (!bias && !segment_ids) return lwm_fail(LWM_ERR_ARG, "attn_bwd_map: bias or segment_ids required");
-  if (!tiles || !tile_count) return lwm_fail(LWM_ERR_ARG, "attn_bwd_map: null tiles / tile_count");
-  return LWM_OK;
-}
-
-extern "C" int lwm_attn_bwd_step_map(const void* q, const void* k, const void* v, const void* dout, const float* lse,
-                                     const float* delta, float* dq_acc, float* dk_acc, float* dv_acc, int B, int H,
-                                     int Sq, int Sk, int D, long long q_pos0, long long k_pos0, int causal,
-                                     const float* bias, long long bias_stride, const int* segment_ids,
-                                     long long seg_stride, float softmax_scale, int dkv_init, const int* tiles,
-                                     const int* tile_count, void* stream) {
-  if (int e = bwd_map_args(bias, segment_ids, tiles, tile_count)) return e;
-  return attn_bwd_launch(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, B, H, Sq, Sk, D, q_pos0, k_pos0, causal,
-                         bias, bias_stride, segment_ids, seg_stride, softmax_scale, nullptr, nullptr, nullptr, nullptr,
-                         dkv_init, tiles, tile_count, stream);
-}
-
-extern "C" int lwm_attn_bwd_step_map_f16(const void* q16, const void* k16, const void* v16, const void* dout16,
-                                         const float* scale_q, const float* scale_k, const float* scale_v,
-                                         const float* scale_do, const float* lse, const float* delta, float* dq_acc,
-                                         float* dk_acc, float* dv_acc, int B, int H, int Sq, int Sk, int D,
-                                         long long q_pos0, long long k_pos0, int causal, const float* bias,
-                                         long long bias_stride, const int* segment_ids, long long seg_stride,
-                                         float softmax_scale, int dkv_init, const int* tiles, const int* tile_count,
-                                         void* stream) {
-  if (!scale_q || !scale_k || !scale_v || !scale_do) return lwm_fail(LWM_ERR_ARG, "attn_bwd_map_f16: scales required");
-  if (int e = bwd_map_args(bias, segment_ids, tiles, tile_count)) return e;
-  return attn_bwd_launch(q16, k16, v16, dout16, lse, delta, dq_acc, dk_acc, dv_acc, B, H, Sq, Sk, D, q_pos0, k_pos0,
-                         causal, bias, bias_stride, segment_ids, seg_stride, softmax_scale, scale_q, scale_k, scale_v,
-                         scale_do, dkv_init, tiles, tile_count, stream);
 }
 
 // Backward of ringattention_inference (attn_bwd_kernel<true, true, true>): any Q and Sk. q16 / dout16 [B,Q,H,128],

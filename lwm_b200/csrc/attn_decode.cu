@@ -204,16 +204,13 @@ void lwm_decode_merge_partials(const float* o_parts, const float* ml_parts, int 
                                                                        o_merged, ml_merged, rows);
 }
 
-template <typename T, bool kRope = false>
+template <typename T, bool kRope>
 static int decode_partial_launch(const void* q, const void* k, const void* v, const unsigned char* mask,
                                  float* o_part, float* ml_part, void* workspace, int B, int H, int Q, int Sk, int D,
                                  long long k_pos0, long long mask_stride_b, long long mask_stride_q, int splits,
-                                 float softmax_scale, void* stream, const int* position_ids = nullptr,
-                                 const float* inv_freq = nullptr) {
+                                 float softmax_scale, const int* position_ids, const float* inv_freq, void* stream) {
   if (D != kHeadDim) return lwm_fail(LWM_ERR_SHAPE, "attn_decode: head_dim must be 128");
   if (!q || !k || !v || !o_part || !ml_part || !workspace) return lwm_fail(LWM_ERR_ARG, "attn_decode: null pointer");
-  if (kRope && (!position_ids || !inv_freq))
-    return lwm_fail(LWM_ERR_ARG, "attn_decode_rope: null position_ids / inv_freq");
   if (B <= 0 || H <= 0 || Q <= 0 || Sk <= 0 || splits <= 0 || (long long)B * Q > 65535)
     return lwm_fail(LWM_ERR_SHAPE, "attn_decode: bad shape");
   if (!lwm_check_device()) return LWM_ERR_DEVICE;
@@ -229,67 +226,37 @@ static int decode_partial_launch(const void* q, const void* k, const void* v, co
   return lwm_check_launch("attn_decode kernels");
 }
 
-// q [B,Q,H,128] bf16 ; k,v [B,Sk,H,128] bf16 (this rank's KV shard) ; mask uint8 [B, ., Q, .] addressed as
-// mask[b*mask_stride_b + q*mask_stride_q + k_pos0 + j] (nonzero = attend) or NULL ;
-// o_part [B*Q*H, 128] fp32 + ml_part [B*Q*H, 2] fp32 : this rank's partial (numerator, (max_log2, denominator));
-// workspace: splits * B*Q*H * (128 + 2) floats.
-extern "C" int lwm_attn_decode_partial(const void* q, const void* k, const void* v, const unsigned char* mask,
+// q [B,Q,H,128], k,v [B,Sk,H,128] (this rank's KV shard), all fp32 (dtype 0: read directly, one float4 per lane and
+// row) or all bf16 (1); mask uint8 [B, ., Q, .] addressed as mask[b*mask_stride_b + q*mask_stride_q + k_pos0 + j]
+// (nonzero = attend) or NULL; o_part [B*Q*H, 128] fp32 + ml_part [B*Q*H, 2] fp32 : this rank's partial (numerator,
+// (max_log2, denominator)); workspace: splits * B*Q*H * (128 + 2) floats. position_ids int32 [B,Q] and inv_freq [64]
+// (as for lwm_attn_rope), or both null: q is un-rotated and is rotated as it is loaded, so the result equals
+// lwm_attn_rope (out_dtype = q's) followed by the call without them, bit for bit.
+extern "C" int lwm_attn_decode_partial(const void* q, const void* k, const void* v, int dtype, const unsigned char* mask,
                                        float* o_part, float* ml_part, void* workspace, int B, int H, int Q, int Sk,
                                        int D, long long k_pos0, long long mask_stride_b, long long mask_stride_q,
-                                       int splits, float softmax_scale, void* stream) {
-  return decode_partial_launch<__nv_bfloat16>(q, k, v, mask, o_part, ml_part, workspace, B, H, Q, Sk, D, k_pos0,
-                                              mask_stride_b, mask_stride_q, splits, softmax_scale, stream);
+                                       int splits, float softmax_scale, const int* position_ids, const float* inv_freq,
+                                       void* stream) {
+  if (dtype != 0 && dtype != 1) return lwm_fail(LWM_ERR_ARG, "attn_decode: dtype codes are 0 (fp32) or 1 (bf16)");
+  if (!position_ids != !inv_freq) return lwm_fail(LWM_ERR_ARG, "attn_decode: null position_ids / inv_freq");
+  const bool rope = position_ids != nullptr;
+  auto* launch = dtype == 1 ? (rope ? decode_partial_launch<__nv_bfloat16, true>
+                                   : decode_partial_launch<__nv_bfloat16, false>)
+                            : (rope ? decode_partial_launch<float, true> : decode_partial_launch<float, false>);
+  return launch(q, k, v, mask, o_part, ml_part, workspace, B, H, Q, Sk, D, k_pos0, mask_stride_b, mask_stride_q, splits,
+                softmax_scale, position_ids, inv_freq, stream);
 }
 
-// the same with fp32 q, k, v (read directly: one float4 per lane and row)
-extern "C" int lwm_attn_decode_partial_f32(const float* q, const float* k, const float* v, const unsigned char* mask,
-                                           float* o_part, float* ml_part, void* workspace, int B, int H, int Q, int Sk,
-                                           int D, long long k_pos0, long long mask_stride_b, long long mask_stride_q,
-                                           int splits, float softmax_scale, void* stream) {
-  return decode_partial_launch<float>(q, k, v, mask, o_part, ml_part, workspace, B, H, Q, Sk, D, k_pos0,
-                                      mask_stride_b, mask_stride_q, splits, softmax_scale, stream);
-}
-
-// the same with un-rotated q: position_ids int32 [B,Q], inv_freq [64] (as for lwm_attn_rope); q is rotated as it is
-// loaded, so the result equals lwm_attn_rope (out_dtype = q's) followed by lwm_attn_decode_partial bit for bit
-extern "C" int lwm_attn_decode_partial_rope(const void* q, const void* k, const void* v, const unsigned char* mask,
-                                            float* o_part, float* ml_part, void* workspace, int B, int H, int Q,
-                                            int Sk, int D, long long k_pos0, long long mask_stride_b,
-                                            long long mask_stride_q, int splits, float softmax_scale,
-                                            const int* position_ids, const float* inv_freq, void* stream) {
-  return decode_partial_launch<__nv_bfloat16, true>(q, k, v, mask, o_part, ml_part, workspace, B, H, Q, Sk, D, k_pos0,
-                                                    mask_stride_b, mask_stride_q, splits, softmax_scale, stream,
-                                                    position_ids, inv_freq);
-}
-
-extern "C" int lwm_attn_decode_partial_rope_f32(const float* q, const float* k, const float* v,
-                                                const unsigned char* mask, float* o_part, float* ml_part,
-                                                void* workspace, int B, int H, int Q, int Sk, int D,
-                                                long long k_pos0, long long mask_stride_b, long long mask_stride_q,
-                                                int splits, float softmax_scale, const int* position_ids,
-                                                const float* inv_freq, void* stream) {
-  return decode_partial_launch<float, true>(q, k, v, mask, o_part, ml_part, workspace, B, H, Q, Sk, D, k_pos0,
-                                            mask_stride_b, mask_stride_q, splits, softmax_scale, stream, position_ids,
-                                            inv_freq);
-}
-
-// merge n_part partials per row (e.g. the all-gathered per-rank partials) into out (bf16) and lse.
-extern "C" int lwm_attn_decode_merge(const float* o_parts, const float* ml_parts, int n_part, void* out, float* lse,
-                                     long long rows, void* stream) {
+// merge n_part partials per row (e.g. the all-gathered per-rank partials) into out, bf16 (out_dtype 1) or the
+// un-rounded fp32 (0), and lse.
+extern "C" int lwm_attn_decode_merge(const float* o_parts, const float* ml_parts, int n_part, void* out, int out_dtype,
+                                     float* lse, long long rows, void* stream) {
   if (!o_parts || !ml_parts || !out || n_part <= 0 || rows <= 0) return lwm_fail(LWM_ERR_ARG, "attn_decode_merge: bad args");
+  if (out_dtype != 0 && out_dtype != 1)
+    return lwm_fail(LWM_ERR_ARG, "attn_decode_merge: out dtype codes are 0 (fp32) or 1 (bf16)");
   if (!lwm_check_device()) return LWM_ERR_DEVICE;
-  decode_merge_kernel<false><<<unsigned((rows + 3) / 4), 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      o_parts, ml_parts, n_part, out, lse, nullptr, nullptr, rows);
-  return lwm_check_launch("decode_merge_kernel");
-}
-
-// the same, writing the un-rounded fp32 output
-extern "C" int lwm_attn_decode_merge_f32(const float* o_parts, const float* ml_parts, int n_part, float* out,
-                                         float* lse, long long rows, void* stream) {
-  if (!o_parts || !ml_parts || !out || n_part <= 0 || rows <= 0)
-    return lwm_fail(LWM_ERR_ARG, "attn_decode_merge_f32: bad args");
-  if (!lwm_check_device()) return LWM_ERR_DEVICE;
-  decode_merge_kernel<true><<<unsigned((rows + 3) / 4), 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      o_parts, ml_parts, n_part, out, lse, nullptr, nullptr, rows);
+  auto* kernel = out_dtype == 0 ? decode_merge_kernel<true> : decode_merge_kernel<false>;
+  kernel<<<unsigned((rows + 3) / 4), 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(o_parts, ml_parts, n_part, out,
+                                                                                       lse, nullptr, nullptr, rows);
   return lwm_check_launch("decode_merge_kernel");
 }

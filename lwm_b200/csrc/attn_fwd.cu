@@ -448,12 +448,19 @@ static bool make_qkv_tmap(CUtensorMap* tm, const void* ptr, int B, int S, int H)
 
 using namespace lwm;
 
-static int attn_fwd_launch(const void* q, const void* k, const void* v, void* out, float* lse, float* acc_o,
-                           float* acc_m, float* acc_l, int B, int H, int Sq, int Sk, int D, long long q_pos0,
-                           long long k_pos0, int causal, const float* bias, long long bias_stride,
-                           const int* segment_ids, long long seg_stride, float softmax_scale, int first, int last,
-                           const float* scale_q, const float* scale_k, const float* scale_v, float* out_f32,
-                           const int* tiles, const int* tile_count, void* stream) {
+// One ring step (include/lwm_b200.h): the scales select the fp16-operand kernel, tiles / tile_count the block map.
+extern "C" int lwm_attn_fwd_step(const void* q, const void* k, const void* v, const float* scale_q,
+                                 const float* scale_k, const float* scale_v, float* out_f32, void* out, float* lse,
+                                 float* acc_o, float* acc_m, float* acc_l, int B, int H, int Sq, int Sk, int D,
+                                 long long q_pos0, long long k_pos0, int causal, const float* bias,
+                                 long long bias_stride, const int* segment_ids, long long seg_stride,
+                                 float softmax_scale, int first, int last, const int* tiles, const int* tile_count,
+                                 void* stream) {
+  if (!scale_k != !scale_q || !scale_v != !scale_q)
+    return lwm_fail(LWM_ERR_ARG, "attn_fwd: scales are all given (fp16 operands) or all null (bf16)");
+  if (out_f32 && !scale_q) return lwm_fail(LWM_ERR_ARG, "attn_fwd: out_f32 needs the fp16 operand scales");
+  if (!tiles != !tile_count) return lwm_fail(LWM_ERR_ARG, "attn_fwd: tiles and tile_count are both given or both null");
+  if (tiles && !bias && !segment_ids) return lwm_fail(LWM_ERR_ARG, "attn_fwd: a block map needs bias or segment_ids");
   if (D != kHeadDim) return lwm_fail(LWM_ERR_SHAPE, "attn_fwd: head_dim must be 128");
   if (B <= 0 || H <= 0 || Sq <= 0 || Sk <= 0 || Sq % kTile || Sk % kTile)
     return lwm_fail(LWM_ERR_SHAPE, "attn_fwd: Sq and Sk must be positive multiples of 128");
@@ -510,64 +517,6 @@ static int attn_fwd_launch(const void* q, const void* k, const void* v, void* ou
   if (scale_q) attn_fwd_kernel<true><<<grid, kFwdThreads, kFwdSmemBytes, st>>>(tq, tk, tv, p);
   else attn_fwd_kernel<false><<<grid, kFwdThreads, kFwdSmemBytes, st>>>(tq, tk, tv, p);
   return lwm_check_launch("attn_fwd_kernel");
-}
-
-extern "C" int lwm_attn_fwd_step(const void* q, const void* k, const void* v, void* out, float* lse, float* acc_o,
-                                 float* acc_m, float* acc_l, int B, int H, int Sq, int Sk, int D,
-                                 long long q_pos0, long long k_pos0, int causal, const float* bias,
-                                 long long bias_stride, const int* segment_ids, long long seg_stride,
-                                 float softmax_scale, int first, int last, void* stream) {
-  return attn_fwd_launch(q, k, v, out, lse, acc_o, acc_m, acc_l, B, H, Sq, Sk, D, q_pos0, k_pos0, causal, bias,
-                         bias_stride, segment_ids, seg_stride, softmax_scale, first, last, nullptr, nullptr, nullptr, nullptr,
-                         nullptr, nullptr, stream);
-}
-
-// fp16-operand variant: q/k/v are the fp16 copies made by lwm_attn_to_f16, scale_* their device scalars.
-extern "C" int lwm_attn_fwd_step_f16(const void* q16, const void* k16, const void* v16, const float* scale_q,
-                                     const float* scale_k, const float* scale_v, float* out_f32,
-                                     void* out, float* lse, float* acc_o, float* acc_m, float* acc_l, int B, int H,
-                                     int Sq, int Sk, int D, long long q_pos0, long long k_pos0, int causal,
-                                     const float* bias, long long bias_stride, const int* segment_ids,
-                                     long long seg_stride, float softmax_scale, int first, int last, void* stream) {
-  if (!scale_q || !scale_k || !scale_v) return lwm_fail(LWM_ERR_ARG, "attn_fwd_f16: scales required");
-  return attn_fwd_launch(q16, k16, v16, out, lse, acc_o, acc_m, acc_l, B, H, Sq, Sk, D, q_pos0, k_pos0, causal, bias,
-                         bias_stride, segment_ids, seg_stride, softmax_scale, first, last, scale_q, scale_k, scale_v,
-                         out_f32, nullptr, nullptr, stream);
-}
-
-// Block-map variants (a bias or segment ids given): tiles / tile_count are the forward map of lwm_attn_step_tilemap,
-// built with the same (bias, segment_ids, B, Sq, Sk, q_pos0, k_pos0, causal). Results are bit-identical to
-// lwm_attn_fwd_step / lwm_attn_fwd_step_f16.
-static int fwd_map_args(const float* bias, const int* segment_ids, const int* tiles, const int* tile_count) {
-  if (!bias && !segment_ids) return lwm_fail(LWM_ERR_ARG, "attn_fwd_map: bias or segment_ids required");
-  if (!tiles || !tile_count) return lwm_fail(LWM_ERR_ARG, "attn_fwd_map: null tiles / tile_count");
-  return LWM_OK;
-}
-
-extern "C" int lwm_attn_fwd_step_map(const void* q, const void* k, const void* v, void* out, float* lse, float* acc_o,
-                                     float* acc_m, float* acc_l, int B, int H, int Sq, int Sk, int D,
-                                     long long q_pos0, long long k_pos0, int causal, const float* bias,
-                                     long long bias_stride, const int* segment_ids, long long seg_stride,
-                                     float softmax_scale, int first, int last, const int* tiles,
-                                     const int* tile_count, void* stream) {
-  if (int e = fwd_map_args(bias, segment_ids, tiles, tile_count)) return e;
-  return attn_fwd_launch(q, k, v, out, lse, acc_o, acc_m, acc_l, B, H, Sq, Sk, D, q_pos0, k_pos0, causal, bias,
-                         bias_stride, segment_ids, seg_stride, softmax_scale, first, last, nullptr, nullptr, nullptr, nullptr,
-                         tiles, tile_count, stream);
-}
-
-extern "C" int lwm_attn_fwd_step_map_f16(const void* q16, const void* k16, const void* v16, const float* scale_q,
-                                         const float* scale_k, const float* scale_v, float* out_f32,
-                                         void* out, float* lse, float* acc_o, float* acc_m, float* acc_l, int B, int H,
-                                         int Sq, int Sk, int D, long long q_pos0, long long k_pos0, int causal,
-                                         const float* bias, long long bias_stride, const int* segment_ids,
-                                         long long seg_stride, float softmax_scale, int first, int last,
-                                         const int* tiles, const int* tile_count, void* stream) {
-  if (!scale_q || !scale_k || !scale_v) return lwm_fail(LWM_ERR_ARG, "attn_fwd_map_f16: scales required");
-  if (int e = fwd_map_args(bias, segment_ids, tiles, tile_count)) return e;
-  return attn_fwd_launch(q16, k16, v16, out, lse, acc_o, acc_m, acc_l, B, H, Sq, Sk, D, q_pos0, k_pos0, causal, bias,
-                         bias_stride, segment_ids, seg_stride, softmax_scale, first, last, scale_q, scale_k, scale_v,
-                         out_f32, tiles, tile_count, stream);
 }
 
 // Inference mode (ringattention_inference with Q >= kInferMinQ rows): q16 [B,Q,H,128], k16/v16 [B,Sk,H,128] scaled fp16

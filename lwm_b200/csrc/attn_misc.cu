@@ -357,30 +357,6 @@ __global__ void __launch_bounds__(256) reduce_cast_rope_kernel(const ReduceSrcs 
 
 using namespace lwm;
 
-extern "C" int lwm_attn_bwd_prep(const void* out, const void* dout, float* delta, int B, int H, int Sq, int D,
-                                 void* stream) {
-  if (D != kHeadDim) return lwm_fail(LWM_ERR_SHAPE, "attn_bwd_prep: head_dim must be 128");
-  if (!out || !dout || !delta) return lwm_fail(LWM_ERR_ARG, "attn_bwd_prep: null pointer");
-  if (!lwm_check_device()) return LWM_ERR_DEVICE;
-  const long long rows = (long long)B * Sq * H;
-  const int warps = 8;
-  bwd_prep_kernel<<<unsigned((rows + warps - 1) / warps), warps * 32, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      reinterpret_cast<const __nv_bfloat16*>(out), reinterpret_cast<const __nv_bfloat16*>(dout), delta, B, H, Sq);
-  return lwm_check_launch("bwd_prep_kernel");
-}
-
-extern "C" int lwm_attn_bwd_prep_f32(const float* out_f32, const void* dout, float* delta, int B, int H, int Sq, int D,
-                                     void* stream) {
-  if (D != kHeadDim) return lwm_fail(LWM_ERR_SHAPE, "attn_bwd_prep_f32: head_dim must be 128");
-  if (!out_f32 || !dout || !delta) return lwm_fail(LWM_ERR_ARG, "attn_bwd_prep_f32: null pointer");
-  if (!lwm_check_device()) return LWM_ERR_DEVICE;
-  const long long rows = (long long)B * Sq * H;
-  const int warps = 8;
-  bwd_prep_f32_kernel<<<unsigned((rows + warps - 1) / warps), warps * 32, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      out_f32, reinterpret_cast<const __nv_bfloat16*>(dout), delta, B, H, Sq);
-  return lwm_check_launch("bwd_prep_f32_kernel");
-}
-
 extern "C" int lwm_attn_bwd_lse(const float* lse, float* nlse2, long long n, float offset_log2, void* stream) {
   if (!lse || !nlse2 || n <= 0) return lwm_fail(LWM_ERR_ARG, "attn_bwd_lse: bad args");
   if (!lwm_check_device()) return LWM_ERR_DEVICE;
@@ -483,18 +459,25 @@ extern "C" int lwm_attn_to_f16_scaled(const void* x, int dtype, void* dst_f16, c
   return lwm_check_launch("to_f16_by_scale kernel");
 }
 
-extern "C" int lwm_attn_bwd_prep_f16(const void* out, int out_dtype, const void* dout16, const float* scale_do, float* delta,
-                                     int B, int H, int Sq, int D, void* stream) {
-  if (D != kHeadDim) return lwm_fail(LWM_ERR_SHAPE, "attn_bwd_prep_f16: head_dim must be 128");
-  if (!out || !dout16 || !scale_do || !delta || (out_dtype != 0 && out_dtype != 1)) return lwm_fail(LWM_ERR_ARG, "attn_bwd_prep_f16: bad arguments");
+// delta = rowsum(out o dout); out fp32 (out_dtype 0) or bf16 (1); dout bf16, or its scaled fp16 copy when scale_do is
+// given (the ring executor only ever holds the fp16 copy of a remote dO chunk).
+extern "C" int lwm_attn_bwd_prep(const void* out, int out_dtype, const void* dout, const float* scale_do, float* delta,
+                                 int B, int H, int Sq, int D, void* stream) {
+  if (D != kHeadDim) return lwm_fail(LWM_ERR_SHAPE, "attn_bwd_prep: head_dim must be 128");
+  if (!out || !dout || !delta) return lwm_fail(LWM_ERR_ARG, "attn_bwd_prep: null pointer");
+  if (out_dtype != 0 && out_dtype != 1) return lwm_fail(LWM_ERR_ARG, "attn_bwd_prep: out dtype codes are 0 (fp32) or 1 (bf16)");
   if (!lwm_check_device()) return LWM_ERR_DEVICE;
   const long long rows = (long long)B * Sq * H;
   const int warps = 8;
   const unsigned blocks = unsigned((rows + warps - 1) / warps);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (out_dtype == 0) bwd_prep_f16_kernel<true><<<blocks, warps * 32, 0, st>>>(out, reinterpret_cast<const __half*>(dout16), scale_do, delta, B, H, Sq);
-  else bwd_prep_f16_kernel<false><<<blocks, warps * 32, 0, st>>>(out, reinterpret_cast<const __half*>(dout16), scale_do, delta, B, H, Sq);
-  return lwm_check_launch("bwd_prep_f16_kernel");
+  const __nv_bfloat16* dout_bf16 = reinterpret_cast<const __nv_bfloat16*>(dout);
+  const __half* dout16 = reinterpret_cast<const __half*>(dout);
+  if (scale_do && out_dtype == 0) bwd_prep_f16_kernel<true><<<blocks, warps * 32, 0, st>>>(out, dout16, scale_do, delta, B, H, Sq);
+  else if (scale_do) bwd_prep_f16_kernel<false><<<blocks, warps * 32, 0, st>>>(out, dout16, scale_do, delta, B, H, Sq);
+  else if (out_dtype == 0) bwd_prep_f32_kernel<<<blocks, warps * 32, 0, st>>>(reinterpret_cast<const float*>(out), dout_bf16, delta, B, H, Sq);
+  else bwd_prep_kernel<<<blocks, warps * 32, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(out), dout_bf16, delta, B, H, Sq);
+  return lwm_check_launch("bwd_prep kernel");
 }
 
 // host_srcs: HOST array of n_src device pointers (fp32, n elements each); dst_dtype 0 = fp32, 1 = bf16.

@@ -282,48 +282,25 @@ def step_tilemap(B, Sq, Sk, q_pos0, k_pos0, causal, bias, seg, fwd=True, bwd=Tru
 
 def fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last,
              stream=None, scales=None, out_f32=None, tilemap=None):
-    """tilemap: None, or the forward map (tiles, counts) of step_tilemap for these arguments: the tile kernel then
-    visits only the KV tiles in it (same results, bit for bit)."""
+    """scales: None (bf16 operands), or the device scales (sq, sk, sv) of fp16 operand copies q/k/v; out_f32 (fp16
+    operands only): the un-rounded output, written on the last step. tilemap: None, or the forward map (tiles, counts)
+    of step_tilemap for these arguments: the tile kernel then visits only the KV tiles in it (same results, bit for
+    bit)."""
     B, Sq, H, D = q.shape
-    Sk = k.shape[1]
-    if tilemap is not None:
-        tail = (_lib.ptr(tilemap[0]), _lib.ptr(tilemap[1]), _lib.stream_ptr(stream))
-        if scales is not None:
-            _lib.call("lwm_attn_fwd_step_map_f16", _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(scales[0]),
-                      _lib.ptr(scales[1]), _lib.ptr(scales[2]), _lib.ptr(out_f32), _lib.ptr(out), _lib.ptr(lse),
-                      _lib.ptr(acc_o), _lib.ptr(acc_m), _lib.ptr(acc_l), B, H, Sq, Sk, D, int(q_pos0), int(k_pos0),
-                      int(bool(causal)), _lib.ptr(bias), 0 if bias is None else bias.shape[1], _lib.ptr(seg),
-                      0 if seg is None else seg.shape[1], 1.0 / math.sqrt(D), int(first), int(last), *tail)
-        else:
-            _lib.call("lwm_attn_fwd_step_map", _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(out), _lib.ptr(lse),
-                      _lib.ptr(acc_o), _lib.ptr(acc_m), _lib.ptr(acc_l), B, H, Sq, Sk, D, int(q_pos0), int(k_pos0),
-                      int(bool(causal)), _lib.ptr(bias), 0 if bias is None else bias.shape[1], _lib.ptr(seg),
-                      0 if seg is None else seg.shape[1], 1.0 / math.sqrt(D), int(first), int(last), *tail)
-        return
-    if scales is not None:   # fp16-operand kernels: q/k/v are fp16 copies, scales = (sq, sk, sv) device scalars
-        _lib.call("lwm_attn_fwd_step_f16", _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(scales[0]),
-                  _lib.ptr(scales[1]), _lib.ptr(scales[2]), _lib.ptr(out_f32), _lib.ptr(out), _lib.ptr(lse),
-                  _lib.ptr(acc_o),
-                  _lib.ptr(acc_m), _lib.ptr(acc_l), B, H, Sq, Sk, D, int(q_pos0), int(k_pos0), int(bool(causal)),
-                  _lib.ptr(bias), 0 if bias is None else bias.shape[1], _lib.ptr(seg),
-                  0 if seg is None else seg.shape[1], 1.0 / math.sqrt(D), int(first), int(last),
-                  _lib.stream_ptr(stream))
-        return
-    _lib.call("lwm_attn_fwd_step", _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(out), _lib.ptr(lse),
-              _lib.ptr(acc_o), _lib.ptr(acc_m), _lib.ptr(acc_l), B, H, Sq, Sk, D, int(q_pos0), int(k_pos0),
-              int(bool(causal)), _lib.ptr(bias), 0 if bias is None else bias.shape[1], _lib.ptr(seg),
-              0 if seg is None else seg.shape[1], 1.0 / math.sqrt(D), int(first), int(last),
-              _lib.stream_ptr(stream))
+    sq, sk, sv = scales if scales is not None else (None, None, None)
+    tiles, counts = tilemap if tilemap is not None else (None, None)
+    _lib.call("lwm_attn_fwd_step", _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(sq), _lib.ptr(sk), _lib.ptr(sv),
+              _lib.ptr(out_f32), _lib.ptr(out), _lib.ptr(lse), _lib.ptr(acc_o), _lib.ptr(acc_m), _lib.ptr(acc_l), B, H,
+              Sq, k.shape[1], D, int(q_pos0), int(k_pos0), int(bool(causal)), _lib.ptr(bias),
+              0 if bias is None else bias.shape[1], _lib.ptr(seg), 0 if seg is None else seg.shape[1],
+              1.0 / math.sqrt(D), int(first), int(last), _lib.ptr(tiles), _lib.ptr(counts), _lib.stream_ptr(stream))
 
 
-def bwd_prep(out, dout, delta, stream=None):
+def bwd_prep(out, dout, delta, stream=None, scale_do=None):
+    """delta = rowsum(out o dout): out fp32 or bf16; dout bf16, or its scaled fp16 copy with its device scale scale_do"""
     B, Sq, H, D = out.shape
-    if out.dtype == torch.float32:
-        _lib.call("lwm_attn_bwd_prep_f32", _lib.ptr(out), _lib.ptr(dout), _lib.ptr(delta), B, H, Sq, D,
-                  _lib.stream_ptr(stream))
-        return
-    _lib.call("lwm_attn_bwd_prep", _lib.ptr(out), _lib.ptr(dout), _lib.ptr(delta), B, H, Sq, D,
-              _lib.stream_ptr(stream))
+    _lib.call("lwm_attn_bwd_prep", _lib.ptr(out), _dt(out), _lib.ptr(dout), _lib.ptr(scale_do), _lib.ptr(delta), B, H,
+              Sq, D, _lib.stream_ptr(stream))
 
 
 F16_P_BOOST_LOG2 = 14.0      # include/lwm_b200.h: LWM_ATTN_F16_P_BOOST_LOG2
@@ -341,37 +318,18 @@ def lse_for_bwd(lse, stream=None, f16=False):
 
 def bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg, stream=None,
              scales=None, init=False, tilemap=None):
-    """`lse` is the PRE-SCALED array returned by lse_for_bwd. init=True: dk_acc/dv_acc rows are written, not accumulated.
+    """`lse` is the PRE-SCALED array returned by lse_for_bwd. scales: None (bf16 operands), or (sq, sk, sv, sdo) of
+    fp16 operand copies q/k/v/dout. init=True: dk_acc/dv_acc rows are written, not accumulated.
     tilemap: None, or the backward map (tiles, counts) of step_tilemap for these arguments (dK, dV bit-identical; dQ
     up to the order of its reductions)."""
     B, Sq, H, D = q.shape
-    Sk = k.shape[1]
-    if tilemap is not None:
-        tail = (_lib.ptr(tilemap[0]), _lib.ptr(tilemap[1]), _lib.stream_ptr(stream))
-        if scales is not None:
-            _lib.call("lwm_attn_bwd_step_map_f16", _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(dout),
-                      _lib.ptr(scales[0]), _lib.ptr(scales[1]), _lib.ptr(scales[2]), _lib.ptr(scales[3]), _lib.ptr(lse),
-                      _lib.ptr(delta), _lib.ptr(dq_acc), _lib.ptr(dk_acc), _lib.ptr(dv_acc), B, H, Sq, Sk, D,
-                      int(q_pos0), int(k_pos0), int(bool(causal)), _lib.ptr(bias), 0 if bias is None else bias.shape[1],
-                      _lib.ptr(seg), 0 if seg is None else seg.shape[1], 1.0 / math.sqrt(D), int(bool(init)), *tail)
-        else:
-            _lib.call("lwm_attn_bwd_step_map", _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(dout), _lib.ptr(lse),
-                      _lib.ptr(delta), _lib.ptr(dq_acc), _lib.ptr(dk_acc), _lib.ptr(dv_acc), B, H, Sq, Sk, D,
-                      int(q_pos0), int(k_pos0), int(bool(causal)), _lib.ptr(bias), 0 if bias is None else bias.shape[1],
-                      _lib.ptr(seg), 0 if seg is None else seg.shape[1], 1.0 / math.sqrt(D), int(bool(init)), *tail)
-        return
-    if scales is not None:   # (sq, sk, sv, sdo)
-        _lib.call("lwm_attn_bwd_step_f16", _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(dout), _lib.ptr(scales[0]),
-                  _lib.ptr(scales[1]), _lib.ptr(scales[2]), _lib.ptr(scales[3]), _lib.ptr(lse), _lib.ptr(delta),
-                  _lib.ptr(dq_acc), _lib.ptr(dk_acc), _lib.ptr(dv_acc), B, H, Sq, Sk, D, int(q_pos0), int(k_pos0),
-                  int(bool(causal)), _lib.ptr(bias), 0 if bias is None else bias.shape[1], _lib.ptr(seg),
-                  0 if seg is None else seg.shape[1], 1.0 / math.sqrt(D), int(bool(init)), _lib.stream_ptr(stream))
-        return
-    _lib.call("lwm_attn_bwd_step", _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(dout), _lib.ptr(lse),
-              _lib.ptr(delta), _lib.ptr(dq_acc), _lib.ptr(dk_acc), _lib.ptr(dv_acc), B, H, Sq, Sk, D,
-              int(q_pos0), int(k_pos0), int(bool(causal)), _lib.ptr(bias),
+    sq, sk, sv, sdo = scales if scales is not None else (None, None, None, None)
+    tiles, counts = tilemap if tilemap is not None else (None, None)
+    _lib.call("lwm_attn_bwd_step", _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(dout), _lib.ptr(sq), _lib.ptr(sk),
+              _lib.ptr(sv), _lib.ptr(sdo), _lib.ptr(lse), _lib.ptr(delta), _lib.ptr(dq_acc), _lib.ptr(dk_acc),
+              _lib.ptr(dv_acc), B, H, Sq, k.shape[1], D, int(q_pos0), int(k_pos0), int(bool(causal)), _lib.ptr(bias),
               0 if bias is None else bias.shape[1], _lib.ptr(seg), 0 if seg is None else seg.shape[1],
-              1.0 / math.sqrt(D), int(bool(init)), _lib.stream_ptr(stream))
+              1.0 / math.sqrt(D), int(bool(init)), _lib.ptr(tiles), _lib.ptr(counts), _lib.stream_ptr(stream))
 
 
 def _map_kw(q, k, q_pos0, k_pos0, causal, bias, seg, fwd):
@@ -503,10 +461,8 @@ class PeerOpsF16:
                         scales=scales, out_f32=out_f32)
 
     @staticmethod
-    def bwd_prep(out, dout16, sdo, delta):
-        B, Sq, H, D = out.shape
-        _lib.call("lwm_attn_bwd_prep_f16", _lib.ptr(out), _dt(out), _lib.ptr(dout16), _lib.ptr(sdo), _lib.ptr(delta),
-                  B, H, Sq, D, _lib.stream_ptr())
+    def bwd_prep(out, dout, sdo, delta):
+        bwd_prep(out, dout, delta, scale_do=sdo)
 
     @staticmethod
     def lse_for_bwd(lse):
@@ -576,10 +532,6 @@ class PeerOpsBf16(PeerOpsF16):
         mapped_fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last)
         if last and out_f32 is not None:
             out_f32.copy_(out)
-
-    @staticmethod
-    def bwd_prep(out, dout, sdo, delta):
-        bwd_prep(out, dout, delta)
 
     @staticmethod
     def lse_for_bwd(lse):
@@ -783,14 +735,10 @@ def decode_partial(q, k, v, mask_u8, k_pos0, stream=None, rope=None):
     sb = sq = 0
     if mask_u8 is not None:
         sb, sq = mask_u8.stride(0), mask_u8.stride(-2)
-    fn = "lwm_attn_decode_partial_f32" if q.dtype == torch.float32 else "lwm_attn_decode_partial"
-    args = (_lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(mask_u8), _lib.ptr(o_part), _lib.ptr(ml_part), _lib.ptr(ws),
-            B, H, Q, Sk, D, int(k_pos0), int(sb), int(sq), splits, 1.0 / math.sqrt(D))
-    if rope is None:
-        _lib.call(fn, *args, _lib.stream_ptr(stream))
-    else:
-        _lib.call(fn.replace("partial", "partial_rope"), *args, _lib.ptr(rope[0]), _lib.ptr(rope[1]),
-                  _lib.stream_ptr(stream))
+    pos, inv_freq = rope if rope is not None else (None, None)
+    _lib.call("lwm_attn_decode_partial", _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _dt(q), _lib.ptr(mask_u8),
+              _lib.ptr(o_part), _lib.ptr(ml_part), _lib.ptr(ws), B, H, Q, Sk, D, int(k_pos0), int(sb), int(sq), splits,
+              1.0 / math.sqrt(D), _lib.ptr(pos), _lib.ptr(inv_freq), _lib.stream_ptr(stream))
     return o_part, ml_part
 
 
@@ -800,9 +748,8 @@ def decode_merge(o_parts, ml_parts, n_part, out_shape, dtype, with_lse=False):
     out = torch.empty(out_shape, dtype=dtype, device=o_parts.device)
     rows = o_parts.shape[0]
     lse = torch.empty(rows, dtype=torch.float32, device=o_parts.device)
-    fn = "lwm_attn_decode_merge_f32" if dtype == torch.float32 else "lwm_attn_decode_merge"
-    _lib.call(fn, _lib.ptr(o_parts), _lib.ptr(ml_parts), n_part, _lib.ptr(out), _lib.ptr(lse), rows,
-              _lib.stream_ptr())
+    _lib.call("lwm_attn_decode_merge", _lib.ptr(o_parts), _lib.ptr(ml_parts), n_part, _lib.ptr(out), _dt(out),
+              _lib.ptr(lse), rows, _lib.stream_ptr())
     return (out, lse) if with_lse else out
 
 

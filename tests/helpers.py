@@ -22,3 +22,22 @@ def make_qkv(B, Sq, Sk, H, D=128, seed=1234, device="cuda", n_extra=0):
 
 def to_np(t):
     return t.detach().float().cpu().numpy()
+
+
+def abi_row_id(name, args):
+    """Test id of a C-ABI call row: the entry point without `lwm_`, and for the attention passes whose options are
+    nullable arguments, the operand mode the row selects (bf16 / f16 / f32, map: a block map, rope: the rotary
+    embedding of q; for lwm_attn_bwd_prep the dtype is out's and f16 marks the scaled fp16 dout), so that every mode of
+    one entry point has an id of its own."""
+    given = [a is not None for a in args]
+    dtype = {0: "f32", 1: "bf16"}
+    if name in ("lwm_attn_fwd_step", "lwm_attn_bwd_step"):
+        scales = given[3:6] if name == "lwm_attn_fwd_step" else given[4:8]
+        return name[4:] + ("-f16" if any(scales) else "-bf16") + ("-map" if any(given[-3:-1]) else "")
+    if name == "lwm_attn_bwd_prep":          # (out, out_dtype, dout, scale_do, ...)
+        return name[4:] + "-" + dtype.get(args[1], "bad_dtype") + ("-f16" if given[3] else "")
+    if name == "lwm_attn_decode_partial":    # (q, k, v, dtype, ..., position_ids, inv_freq, stream)
+        return name[4:] + "-" + dtype.get(args[3], "bad_dtype") + ("-rope" if any(given[-3:-1]) else "")
+    if name == "lwm_attn_decode_merge":      # (o_parts, ml_parts, n_part, out, out_dtype, ...)
+        return name[4:] + "-" + dtype.get(args[4], "bad_dtype")
+    return name[4:]

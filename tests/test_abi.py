@@ -21,17 +21,50 @@ def test_library_exports_every_declared_symbol_and_its_abi_version(lib):
     assert len(names) >= 13
     for n in names:
         assert hasattr(lib, n), "liblwm_b200.so does not export %s" % n
-    # version 3: lwm_vq_prep_f16 writes a scaled fp16 plane (scale_out, x_absmax) and lwm_vq_conv2d_f16 reads its scale
-    # (a_scale) and can return the output's |max| (absmax_out)
+    # version 4: the attention passes take their options as nullable arguments of one entry point each
+    # (lwm_attn_fwd_step / lwm_attn_bwd_step: scales, block map; lwm_attn_bwd_prep: out dtype, scale_do;
+    # lwm_attn_decode_partial: dtype, position_ids / inv_freq; lwm_attn_decode_merge: out dtype), and the per-option
+    # variants of them are no longer exported
     src = open(os.path.join(ROOT, "include", "lwm_b200.h")).read()
-    assert re.search(r"#define LWM_B200_ABI_VERSION 3\b", src)
-    assert lib.lwm_abi_version() == 3
+    assert re.search(r"#define LWM_B200_ABI_VERSION 4\b", src)
+    assert lib.lwm_abi_version() == 4
 
 
 def test_python_binding_covers_header():
     from lwm_b200 import _lib
     bound = set(_lib._SIGNATURES) | {"lwm_last_error", "lwm_ring_ctx_heap", "lwm_ring_ctx_heap_bytes"}
     assert set(_declared()) <= bound
+
+
+def _prototypes():
+    """name -> parameter type list of every function the header declares (comments removed)"""
+    src = open(os.path.join(ROOT, "include", "lwm_b200.h")).read()
+    src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
+    protos = {}
+    for m in re.finditer(r"\b(lwm_[a-z0-9_]+)\s*\(([^()]*)\)\s*;", src):
+        params = " ".join(m.group(2).split())
+        protos[m.group(1)] = [] if params in ("", "void") else [p.strip() for p in params.split(",")]
+    return protos
+
+
+def _ctype_of(param):
+    """the ctypes type that binds a C parameter declaration: any pointer is c_void_p, else its scalar type"""
+    if "*" in param:
+        return ctypes.c_void_p
+    words = re.sub(r"\bconst\b", "", param).split()[:-1]       # drop the parameter name
+    return {"int": ctypes.c_int, "long long": ctypes.c_longlong, "float": ctypes.c_float,
+            "unsigned": ctypes.c_uint}[" ".join(words)]
+
+
+def test_python_binding_matches_header_prototypes():
+    """every bound entry point has argtypes of the same count and kind as the header's prototype, slot by slot: ctypes
+    does not check a slip (an int passed where a pointer goes) and the call would only fail on the device"""
+    from lwm_b200 import _lib
+    protos = _prototypes()
+    assert len(protos) >= len(_declared())
+    for name, argtypes in _lib._SIGNATURES.items():
+        assert name in protos, name
+        assert argtypes == [_ctype_of(p) for p in protos[name]], name
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="checks the no-GPU failure mode")

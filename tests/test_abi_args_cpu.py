@@ -7,6 +7,8 @@ import ctypes
 import pytest
 import torch
 
+from helpers import abi_row_id
+
 P = ctypes.c_void_p(0x1000)      # fake non-null pointer
 N = None
 SHAPE, ARG, DEVICE = 2, 3, 1
@@ -20,26 +22,37 @@ def _status(lib, name, *args):
 
 BAD_CALLS = [
     # (entry, args, expected status, message fragment)
-    ("lwm_attn_fwd_step", (P, P, P, P, P, N, N, N, 1, 2, 128, 128, 64, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N), SHAPE, "head_dim"),
-    ("lwm_attn_fwd_step", (P, P, P, P, P, N, N, N, 1, 2, 100, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N), SHAPE, "multiples of 128"),
-    ("lwm_attn_fwd_step", (N, P, P, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N), ARG, "null"),
-    ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N), ARG, "last step"),
-    ("lwm_attn_fwd_step", (P, P, P, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 0, N), ARG, "carry"),
-    ("lwm_attn_fwd_step", (P, P, P, P, P, N, N, N, 1, 2, 128, 128, 128, 1 << 31, 0, 1, N, 0, N, 0, 0.1, 1, 1, N), SHAPE, "int32"),
-    ("lwm_attn_bwd_step", (P, P, P, P, P, P, P, P, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 0, N), ARG, "null"),
-    ("lwm_attn_bwd_step", (P, P, P, P, P, P, P, P, P, 1, 2, 128, 192, 128, 0, 0, 1, N, 0, N, 0, 0.1, 0, N), SHAPE, "multiples of 128"),
+    # lwm_attn_fwd_step(q, k, v, scale_q, scale_k, scale_v, out_f32, out, lse, acc_o, acc_m, acc_l, B, H, Sq, Sk, D,
+    #                   q_pos0, k_pos0, causal, bias, bias_stride, segment_ids, seg_stride, softmax_scale, first, last,
+    #                   tiles, tile_count, stream)
+    ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 128, 128, 64, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, N), SHAPE, "head_dim"),
+    ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 100, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, N), SHAPE, "multiples of 128"),
+    ("lwm_attn_fwd_step", (N, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, N), ARG, "null"),
+    ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, N, N, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, N), ARG, "last step"),
+    ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 0, N, N, N), ARG, "carry"),
+    ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 128, 128, 128, 1 << 31, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, N), SHAPE, "int32"),
+    ("lwm_attn_fwd_step", (P, P, P, P, N, P, P, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, N), ARG, "scales"),
+    ("lwm_attn_fwd_step", (P, P, P, N, N, N, P, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, N), ARG, "out_f32"),
+    # lwm_attn_bwd_step(q, k, v, dout, scale_q, scale_k, scale_v, scale_do, lse, delta, dq_acc, dk_acc, dv_acc, B, H, Sq,
+    #                   Sk, D, q_pos0, k_pos0, causal, bias, bias_stride, segment_ids, seg_stride, softmax_scale,
+    #                   dkv_init, tiles, tile_count, stream)
+    ("lwm_attn_bwd_step", (P, P, P, P, N, N, N, N, P, P, P, P, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 0, N, N, N), ARG, "null"),
+    ("lwm_attn_bwd_step", (P, P, P, P, N, N, N, N, P, P, P, P, P, 1, 2, 128, 192, 128, 0, 0, 1, N, 0, N, 0, 0.1, 0, N, N, N), SHAPE, "multiples of 128"),
     ("lwm_attn_absmax", (P, 2, 64, P, N), ARG, "bad arguments"),
     ("lwm_attn_to_f16_scaled", (P, 1, P, P, 12, N), ARG, "n % 8"),
-    ("lwm_attn_bwd_prep_f16", (P, 0, P, P, P, 1, 2, 128, 64, N), SHAPE, "head_dim"),
+    ("lwm_attn_bwd_prep", (P, 0, P, P, P, 1, 2, 128, 64, N), SHAPE, "head_dim"),
     ("lwm_reduce_cast_f32", (P, 17, P, 1, 64, N), ARG, "1..16 sources"),
     ("lwm_ring_ctx_create", (3, 2, 1024, 0, P), ARG, "bad rank/world"),
     ("lwm_ring_copy", (N, P, 16, N), ARG, "bad arguments"),
     ("lwm_ring_signal", (N, 0, 0, 1, N), ARG, "null context"),
-    ("lwm_attn_bwd_prep", (P, P, P, 1, 2, 128, 96, N), SHAPE, "head_dim"),
+    ("lwm_attn_bwd_prep", (P, 1, P, N, P, 1, 2, 128, 96, N), SHAPE, "head_dim"),
+    ("lwm_attn_bwd_prep", (P, 2, P, N, P, 1, 2, 128, 128, N), ARG, "out dtype"),
     ("lwm_attn_bwd_lse", (P, P, 0, 0.0, N), ARG, "bad args"),
     ("lwm_attn_to_f16", (P, P, P, P, 12, N), SHAPE, "multiple of 8"),
-    ("lwm_attn_decode_partial", (P, P, P, N, P, P, N, 1, 2, 1, 128, 128, 0, 0, 0, 4, 0.1, N), ARG, "null"),
-    ("lwm_attn_decode_merge", (P, P, 0, P, P, 8, N), ARG, "bad args"),
+    ("lwm_attn_decode_partial", (P, P, P, 1, N, P, P, N, 1, 2, 1, 128, 128, 0, 0, 0, 4, 0.1, N, N, N), ARG, "null"),
+    ("lwm_attn_decode_partial", (P, P, P, 2, N, P, P, P, 1, 2, 1, 128, 128, 0, 0, 0, 4, 0.1, N, N, N), ARG, "dtype"),
+    ("lwm_attn_decode_merge", (P, P, 0, P, 1, P, 8, N), ARG, "bad args"),
+    ("lwm_attn_decode_merge", (P, P, 2, P, 2, P, 8, N), ARG, "dtype"),
     ("lwm_attn_rope", (P, P, 0, P, P, 2, P, P, 1, 8, 2, 2, 128, 0, N), ARG, "dtype"),
     ("lwm_attn_rope", (P, P, 0, P, P, 1, P, P, 1, 8, 2, 2, 64, 0, N), SHAPE, "head_dim"),
     ("lwm_cast_f32_to_bf16", (P, P, 6, N), SHAPE, "multiple of 4"),
@@ -65,7 +78,8 @@ BAD_CALLS = [
 ]
 
 
-@pytest.mark.parametrize("name,args,code,frag", BAD_CALLS, ids=["%s-%s" % (c[0][4:], c[3].replace(" ", "_")) for c in BAD_CALLS])
+@pytest.mark.parametrize("name,args,code,frag", BAD_CALLS,
+                         ids=["%s-%s" % (abi_row_id(*c[:2]), c[3].replace(" ", "_")) for c in BAD_CALLS])
 def test_bad_arguments_are_rejected_with_a_message(lib, name, args, code, frag):
     status, msg = _status(lib, name, *args)
     assert status == code, (status, msg)
@@ -73,10 +87,14 @@ def test_bad_arguments_are_rejected_with_a_message(lib, name, args, code, frag):
 
 
 GOOD_CALLS = [
-    ("lwm_attn_fwd_step", (P, P, P, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N)),
-    ("lwm_attn_bwd_step", (P, P, P, P, P, P, P, P, P, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, N)),
+    ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, N)),
+    ("lwm_attn_fwd_step", (P, P, P, P, P, P, P, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, N)),
+    ("lwm_attn_bwd_step", (P, P, P, P, N, N, N, N, P, P, P, P, P, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, N, N, N)),
+    ("lwm_attn_bwd_step", (P, P, P, P, P, P, P, P, P, P, P, P, P, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, N, N, N)),
     ("lwm_attn_absmax", (P, 1, 64, P, N)),
-    ("lwm_attn_bwd_prep_f16", (P, 0, P, P, P, 1, 2, 128, 128, N)),
+    ("lwm_attn_bwd_prep", (P, 0, P, P, P, 1, 2, 128, 128, N)),
+    ("lwm_attn_bwd_prep", (P, 0, P, N, P, 1, 2, 128, 128, N)),
+    ("lwm_attn_bwd_prep", (P, 1, P, N, P, 1, 2, 128, 128, N)),
     ("lwm_attn_rope", (P, P, 1, P, P, 1, P, P, 1, 8, 2, 2, 128, 0, N)),
     ("lwm_vq_conv2d", (P, P, P, P, P, N, P, 1, 16, 16, 64, 16, 16, 64, 64, 3, 1, 1, 3, 0, N)),
     ("lwm_vq_argmin", (P, P, P, N, P, 16, 8192, 64, N)),
@@ -91,7 +109,7 @@ GOOD_CALLS = [
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="fake pointers: only meaningful where the device check fails")
-@pytest.mark.parametrize("name,args", GOOD_CALLS, ids=[c[0][4:] for c in GOOD_CALLS])
+@pytest.mark.parametrize("name,args", GOOD_CALLS, ids=[abi_row_id(*c) for c in GOOD_CALLS])
 def test_well_formed_calls_fail_with_device_error_without_gpu(lib, name, args):
     status, msg = _status(lib, name, *args)
     assert status == DEVICE, (status, msg)

@@ -51,7 +51,7 @@ def test_decode_shard_merge_equals_whole():
     ml = torch.stack([p[1] for p in parts], 1).contiguous()
     out = torch.empty(B, Q, H, 128, dtype=torch.bfloat16, device="cuda")
     lse = torch.empty(B * Q * H, dtype=torch.float32, device="cuda")
-    _lib.call("lwm_attn_decode_merge", _lib.ptr(o), _lib.ptr(ml), 2, _lib.ptr(out), _lib.ptr(lse), B * Q * H,
+    _lib.call("lwm_attn_decode_merge", _lib.ptr(o), _lib.ptr(ml), 2, _lib.ptr(out), 1, _lib.ptr(lse), B * Q * H,
               _lib.stream_ptr())
     torch.cuda.synchronize()
     ref = attention_inference_dense(to_np(q), to_np(k), to_np(v), mask.bool().cpu().numpy())

@@ -1,7 +1,7 @@
 """The training block map (lwm_attn_step_tilemap), restated in numpy (tests/tilemap_model.py), against a brute-force
 per-element mask: a pair left out of a list has every entry masked, a clean pair has no mask beyond the causal one, and
 a forward Q tile with a row that does not see its own key visits its whole causal range as mixed. Also the argument
-checks of the new C entry points, which run before any device is looked for."""
+checks of the map and of the step entry points given one, which run before any device is looked for."""
 import ctypes
 
 import numpy as np
@@ -9,6 +9,7 @@ import pytest
 import torch
 
 import tilemap_model as tm
+from helpers import abi_row_id
 
 CASES = tm.sweep_cases()
 
@@ -94,26 +95,34 @@ BAD_CALLS = [
     ("lwm_attn_step_tilemap", (P, 256, N, 0, 1, 256, 256, 0, 1 << 31, 1, P, P, P, P, P, N), SHAPE, "positions"),
     ("lwm_attn_step_tilemap", (P, 256, N, 0, 1, 256, 256, 0, 128, 1, P, P, P, P, P, N), SHAPE, "bias_stride"),
     ("lwm_attn_step_tilemap", (N, 0, P, 256, 1, 256, 256, 128, 0, 1, P, P, P, P, P, N), SHAPE, "seg_stride"),
-    ("lwm_attn_fwd_step_map", (P, P, P, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, P, P, N),
-     ARG, "bias or segment_ids"),
-    ("lwm_attn_fwd_step_map", (P, P, P, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, P, 128, N, 0, 0.1, 1, 1, N, P, N),
-     ARG, "tiles"),
-    ("lwm_attn_fwd_step_map", (P, P, P, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, P, 64, N, 0, 0.1, 1, 1, P, P, N),
-     SHAPE, "bias_stride"),
-    ("lwm_attn_fwd_step_map", (P, P, P, P, P, N, N, N, 1, 2, 100, 128, 128, 0, 0, 1, P, 128, N, 0, 0.1, 1, 1, P, P, N),
-     SHAPE, "multiples of 128"),
-    ("lwm_attn_fwd_step_map_f16", (P, P, P, N, P, P, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, P, 128, N, 0, 0.1,
-                                   1, 1, P, P, N), ARG, "scales"),
-    ("lwm_attn_fwd_step_map_f16", (P, P, P, P, P, P, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, P, 128, 0.1,
-                                   1, 1, P, N, N), ARG, "tiles"),
-    ("lwm_attn_bwd_step_map", (P, P, P, P, P, P, P, P, P, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, P, P, N),
-     ARG, "bias or segment_ids"),
-    ("lwm_attn_bwd_step_map", (P, P, P, P, P, P, P, P, P, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, P, 128, 0.1, 1, P, N, N),
-     ARG, "tiles"),
-    ("lwm_attn_bwd_step_map", (P, P, P, P, P, P, P, P, P, 1, 2, 128, 128, 128, 128, 0, 1, N, 0, P, 128, 0.1, 1, P, P, N),
-     SHAPE, "seg_stride"),
-    ("lwm_attn_bwd_step_map_f16", (P, P, P, P, P, P, P, N, P, P, P, P, P, 1, 2, 128, 128, 128, 0, 0, 1, P, 128, N, 0,
-                                   0.1, 1, P, P, N), ARG, "scales"),
+    # lwm_attn_fwd_step(q, k, v, scale_q, scale_k, scale_v, out_f32, out, lse, acc_o, acc_m, acc_l, B, H, Sq, Sk, D,
+    #                   q_pos0, k_pos0, causal, bias, bias_stride, segment_ids, seg_stride, softmax_scale, first, last,
+    #                   tiles, tile_count, stream)
+    ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1,
+                           P, P, N), ARG, "bias or segment_ids"),
+    ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, P, 128, N, 0, 0.1, 1, 1,
+                           N, P, N), ARG, "tiles"),
+    ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, P, 64, N, 0, 0.1, 1, 1,
+                           P, P, N), SHAPE, "bias_stride"),
+    ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 100, 128, 128, 0, 0, 1, P, 128, N, 0, 0.1, 1, 1,
+                           P, P, N), SHAPE, "multiples of 128"),
+    ("lwm_attn_fwd_step", (P, P, P, N, P, P, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, P, 128, N, 0, 0.1, 1, 1,
+                           P, P, N), ARG, "scales"),
+    ("lwm_attn_fwd_step", (P, P, P, P, P, P, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, P, 128, 0.1, 1, 1,
+                           P, N, N), ARG, "tiles"),
+    # lwm_attn_bwd_step(q, k, v, dout, scale_q, scale_k, scale_v, scale_do, lse, delta, dq_acc, dk_acc, dv_acc, B, H, Sq,
+    #                   Sk, D, q_pos0, k_pos0, causal, bias, bias_stride, segment_ids, seg_stride, softmax_scale,
+    #                   dkv_init, tiles, tile_count, stream)
+    ("lwm_attn_bwd_step", (P, P, P, P, N, N, N, N, P, P, P, P, P, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1,
+                           P, P, N), ARG, "bias or segment_ids"),
+    ("lwm_attn_bwd_step", (P, P, P, P, N, N, N, N, P, P, P, P, P, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, P, 128, 0.1, 1,
+                           P, N, N), ARG, "tiles"),
+    ("lwm_attn_bwd_step", (P, P, P, P, N, N, N, N, P, P, P, P, P, 1, 2, 128, 128, 128, 128, 0, 1, N, 0, P, 128, 0.1, 1,
+                           P, P, N), SHAPE, "seg_stride"),
+    ("lwm_attn_bwd_step", (P, P, P, P, P, P, P, N, P, P, P, P, P, 1, 2, 128, 128, 128, 0, 0, 1, P, 128, N, 0, 0.1, 1,
+                           P, P, N), ARG, "scales"),
+    ("lwm_attn_bwd_step", (P, P, P, P, P, P, P, P, P, P, P, P, P, 1, 2, 128, 128, 128, 0, 0, 1, P, 128, N, 0, 0.1, 1,
+                           N, P, N), ARG, "tiles"),
 ]
 
 
@@ -124,7 +133,7 @@ def _status(lib, name, *args):
 
 
 @pytest.mark.parametrize("name,args,code,frag", BAD_CALLS,
-                         ids=["%s-%d-%s" % (c[0][4:], i, c[3].replace(" ", "_")) for i, c in enumerate(BAD_CALLS)])
+                         ids=["%s-%d-%s" % (abi_row_id(*c[:2]), i, c[3].replace(" ", "_")) for i, c in enumerate(BAD_CALLS)])
 def test_map_entry_points_reject_bad_arguments(lib, name, args, code, frag):
     status, msg = _status(lib, name, *args)
     assert status == code, (status, msg)
@@ -134,17 +143,19 @@ def test_map_entry_points_reject_bad_arguments(lib, name, args, code, frag):
 GOOD_CALLS = [
     ("lwm_attn_step_tilemap", (P, 256, N, 0, 1, 256, 256, 0, 0, 1, P, P, P, P, P, N)),
     ("lwm_attn_step_tilemap", (N, 0, P, 512, 2, 256, 256, 256, 0, 1, N, N, P, P, P, N)),
-    ("lwm_attn_fwd_step_map", (P, P, P, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, P, 128, N, 0, 0.1, 1, 1, P, P, N)),
-    ("lwm_attn_fwd_step_map_f16", (P, P, P, P, P, P, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, P, 128, 0.1,
-                                   1, 1, P, P, N)),
-    ("lwm_attn_bwd_step_map", (P, P, P, P, P, P, P, P, P, 1, 2, 128, 128, 128, 0, 0, 1, P, 128, N, 0, 0.1, 1, P, P, N)),
-    ("lwm_attn_bwd_step_map_f16", (P, P, P, P, P, P, P, P, P, P, P, P, P, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, P, 128,
-                                   0.1, 0, P, P, N)),
+    ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, P, 128, N, 0, 0.1, 1, 1,
+                           P, P, N)),
+    ("lwm_attn_fwd_step", (P, P, P, P, P, P, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, P, 128, 0.1, 1, 1,
+                           P, P, N)),
+    ("lwm_attn_bwd_step", (P, P, P, P, N, N, N, N, P, P, P, P, P, 1, 2, 128, 128, 128, 0, 0, 1, P, 128, N, 0, 0.1, 1,
+                           P, P, N)),
+    ("lwm_attn_bwd_step", (P, P, P, P, P, P, P, P, P, P, P, P, P, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, P, 128, 0.1, 0,
+                           P, P, N)),
 ]
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="fake pointers: only meaningful where the device check fails")
-@pytest.mark.parametrize("name,args", GOOD_CALLS, ids=["%s-%d" % (c[0][4:], i) for i, c in enumerate(GOOD_CALLS)])
+@pytest.mark.parametrize("name,args", GOOD_CALLS, ids=["%s-%d" % (abi_row_id(*c), i) for i, c in enumerate(GOOD_CALLS)])
 def test_well_formed_map_calls_fail_with_device_error_without_gpu(lib, name, args):
     status, msg = _status(lib, name, *args)
     assert status == DEVICE, (status, msg)

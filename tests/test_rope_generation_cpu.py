@@ -1,6 +1,6 @@
 """The rotary embedding of the generation path without a GPU: the keyword checks of `ringattention(rotate_k=False)`,
 `ringattention_inference(freqs_cis=, position_ids=, rotate_k=)` and `ShardedKVCache.concatenate(freqs_cis=,
-position_ids=)`; the argument validation of the new C entries (lwm_attn_decode_partial_rope(_f32),
+position_ids=)`; the argument validation of the C entries that rotate (lwm_attn_decode_partial given position_ids,
 lwm_kv_cache_write_rope), which reject bad arguments before they look for a device; and, under gloo, the rotating
 prefill write of the sequence-sharded cache with a CPU stand-in for the kernel: every rank keeps the same rows the
 un-sharded update would hold."""
@@ -12,13 +12,15 @@ import numpy as np
 import pytest
 import torch
 
+from helpers import abi_row_id
+
 P = ctypes.c_void_p(0x1000)      # fake non-null pointer
 N = None
 SHAPE, ARG, DEVICE = 2, 3, 1
 
-# lwm_attn_decode_partial_rope(q, k, v, mask, o_part, ml_part, ws, B, H, Q, Sk, D, k_pos0, sb, sq, splits, scale,
-#                              position_ids, inv_freq, stream)
-DEC = (P, P, P, N, P, P, P, 1, 2, 1, 128, 128, 0, 0, 0, 4, 0.1, P, P, N)
+# lwm_attn_decode_partial(q, k, v, dtype, mask, o_part, ml_part, ws, B, H, Q, Sk, D, k_pos0, sb, sq, splits, scale,
+#                         position_ids, inv_freq, stream), bf16 (dtype 1) and fp32 (0)
+DEC = (P, P, P, 1, N, P, P, P, 1, 2, 1, 128, 128, 0, 0, 0, 4, 0.1, P, P, N)
 # lwm_kv_cache_write_rope(k_new, v_new, dtype, cache_k, cache_v, position_ids, inv_freq, B, n_src, src0, n, L, dst0,
 #                         H, D, stream)
 KVW = (P, P, 1, P, P, P, P, 2, 8, 0, 8, 64, 8, 2, 128, N)
@@ -31,13 +33,15 @@ def _with(args, **at):
     return tuple(a)
 
 
+DEC32 = _with(DEC, a3=0)
+
 BAD_CALLS = [
-    ("lwm_attn_decode_partial_rope", _with(DEC, a17=N), ARG, "null position_ids"),
-    ("lwm_attn_decode_partial_rope", _with(DEC, a18=N), ARG, "null position_ids"),
-    ("lwm_attn_decode_partial_rope", _with(DEC, a0=N), ARG, "null pointer"),
-    ("lwm_attn_decode_partial_rope", _with(DEC, a11=64), SHAPE, "head_dim"),
-    ("lwm_attn_decode_partial_rope_f32", _with(DEC, a17=N), ARG, "null position_ids"),
-    ("lwm_attn_decode_partial_rope_f32", _with(DEC, a9=0), SHAPE, "bad shape"),
+    ("lwm_attn_decode_partial", _with(DEC, a18=N), ARG, "null position_ids"),
+    ("lwm_attn_decode_partial", _with(DEC, a19=N), ARG, "null position_ids"),
+    ("lwm_attn_decode_partial", _with(DEC, a0=N), ARG, "null pointer"),
+    ("lwm_attn_decode_partial", _with(DEC, a12=64), SHAPE, "head_dim"),
+    ("lwm_attn_decode_partial", _with(DEC32, a18=N), ARG, "null position_ids"),
+    ("lwm_attn_decode_partial", _with(DEC32, a10=0), SHAPE, "bad shape"),
     ("lwm_kv_cache_write_rope", _with(KVW, a14=64), SHAPE, "head_dim"),
     ("lwm_kv_cache_write_rope", _with(KVW, a10=0), SHAPE, "bad sizes"),
     ("lwm_kv_cache_write_rope", _with(KVW, a9=1), SHAPE, "out of range"),       # src0 + n > n_src
@@ -56,19 +60,20 @@ def _status(lib, name, *args):
     return getattr(lib, name)(*args), lib.lwm_last_error().decode()
 
 
-@pytest.mark.parametrize("name,args,code,frag", BAD_CALLS, ids=["%s-%d" % (c[0][4:], i) for i, c in enumerate(BAD_CALLS)])
+@pytest.mark.parametrize("name,args,code,frag", BAD_CALLS,
+                         ids=["%s-%d" % (abi_row_id(*c[:2]), i) for i, c in enumerate(BAD_CALLS)])
 def test_new_entries_reject_bad_arguments(lib, name, args, code, frag):
     status, msg = _status(lib, name, *args)
     assert status == code, (status, msg)
     assert frag in msg, msg
 
 
-GOOD_CALLS = [("lwm_attn_decode_partial_rope", DEC), ("lwm_attn_decode_partial_rope_f32", DEC),
+GOOD_CALLS = [("lwm_attn_decode_partial", DEC), ("lwm_attn_decode_partial", DEC32),
               ("lwm_kv_cache_write_rope", KVW), ("lwm_kv_cache_write_rope", _with(KVW, a2=0, a9=3, a10=5, a12=59))]
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="fake pointers: only meaningful where the device check fails")
-@pytest.mark.parametrize("name,args", GOOD_CALLS, ids=["%s-%d" % (c[0][4:], i) for i, c in enumerate(GOOD_CALLS)])
+@pytest.mark.parametrize("name,args", GOOD_CALLS, ids=["%s-%d" % (abi_row_id(*c), i) for i, c in enumerate(GOOD_CALLS)])
 def test_new_entries_fail_with_device_error_without_gpu(lib, name, args):
     status, msg = _status(lib, name, *args)
     assert status == DEVICE, (status, msg)

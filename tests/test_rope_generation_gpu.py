@@ -6,8 +6,8 @@ Contract: each fused call is bit-identical to the composition on the same inputs
 cache update, then the plain op): outputs, dK and dV are torch.equal; dQ may differ by the order of the backward
 kernels' fp32 dQ sums, so it is held to the larger of a small bound and twice the composition's own run-to-run spread.
 
-  * kernels: lwm_attn_decode_partial_rope(_f32) against lwm_attn_rope + lwm_attn_decode_partial(_f32) at the split and
-    warp edges of the GEMV kernel; lwm_kv_cache_write_rope against lwm_attn_rope + copy_ at decode slots and at prefill
+  * kernels: lwm_attn_decode_partial with position_ids against lwm_attn_rope + lwm_attn_decode_partial without, in bf16
+    and fp32, at the split and warp edges of the GEMV kernel; lwm_kv_cache_write_rope against lwm_attn_rope + copy_ at decode slots and at prefill
     slices that straddle shard boundaries;
   * the ops on one GPU; the replicated and q-sharded protocols on threads (tests/thread_comm.py); the cached prefill on
     the peer-memory executor (tests/peer_emulation.py); a left-padded prefill + 16 decode steps end to end."""

@@ -33,6 +33,13 @@ def test_ring_on_all_visible_gpus_dense_oracle():
 
 
 @pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2, reason="needs >= 2 GPUs")
+def test_ring_on_all_visible_gpus_nccl_transport_dense_oracle():
+    """the two-sided executor (ring_exec.py) on real NCCL side streams: fp32 inputs reach it as bf16 operands, and the
+    worker then holds their results to the bf16-result bound"""
+    _launch({"LWM_RING_TRANSPORT": "nccl"}, 29573)
+
+
+@pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2, reason="needs >= 2 GPUs")
 def test_ring_on_all_visible_gpus_baseline_length_sampled_oracle():
     n = _n_gpus()
     _launch({"RING_TEST_MODE": "sampled", "RING_TEST_S": str(32768 if n == 2 else 65536 if n == 4 else 131072)}, 29572)

@@ -10,48 +10,16 @@ carry a magnitude of their own, so every owner has its own power-of-two scales i
 with zigzag chunk offsets, per-batch launches (B = 2), and the heap regions of both pass parities reused by the passes
 that follow. Results are compared on the global tensors with the float64 dense oracle (oracle/attn_dense.py).
 
-Tolerances (those of tests/ring_multi_gpu_worker.py): 1e-3 for fp32 results of the default mode, 3e-3 for bf16
-results (their own rounding), 5e-3 in the legacy bf16 operand mode. Padded query rows are excluded from out / dq."""
+Inputs and tolerances: tests/ring_emulated_inputs.py."""
 import threading
 
 import numpy as np
 import pytest
 import torch
 
+from ring_emulated_inputs import NPAD, TOL_BF16_MODE, TOL_BF16_RESULT, TOL_F32_READOUT, _passes
+
 pytestmark = pytest.mark.gpu
-
-TOL_F32_READOUT, TOL_BF16_RESULT, TOL_BF16_MODE = 1e-3, 3e-3, 5e-3
-B, H, D, NPAD = 2, 2, 128, 37
-
-
-def _inputs(world, Sl, seed, masks):
-    """global q, k, v, dO (float32 holding bf16 values) with per-rank magnitudes, and the masks"""
-    from oracle.attn_dense import finfo_min
-    S = world * Sl
-    g = torch.Generator().manual_seed(seed)
-    q, k, v, do = [torch.randn(B, S, H, D, generator=g) for _ in range(4)]
-    for r in range(world):
-        sl = slice(r * Sl, (r + 1) * Sl)
-        q[:, sl] *= 2.0 ** -r * 1.3
-        k[:, sl] *= 2.0 ** r * 0.7
-        v[:, sl] *= 2.0 ** -r
-        do[:, sl] *= 2.0 ** (r - 8)
-    q, k, v, do = [t.to(torch.bfloat16).float() for t in (q, k, v, do)]
-    bias = seg = None
-    if masks:
-        bias = torch.zeros(B, S)
-        bias[0, :NPAD] = finfo_min("bf16")
-        seg = torch.zeros(B, S, dtype=torch.int32)
-        seg[B - 1, S // 2 + 5:] = 1
-        do[0, :NPAD] = 0
-    return q, k, v, do, bias, seg
-
-
-def _passes(world, Sl):
-    """every (precision mode, input dtype) pair, each once without and once with masks: consecutive passes never see
-    the same inputs, so a read of a heap region left over from an earlier pass cannot go unnoticed"""
-    sets = [_inputs(world, Sl, 500 + world, False), _inputs(world, Sl, 600 + world, True)]
-    return [(prec, dt, m, sets[m]) for prec in ("fp16", "bf16") for dt in (torch.float32, torch.bfloat16) for m in (0, 1)]
 
 
 @pytest.mark.parametrize("world,layout,causal,Sl", [(2, "zigzag", True, 512), (4, "zigzag", True, 512),

@@ -105,6 +105,22 @@ int lwm_attn_bwd_step(const void* q, const void* k, const void* v, const void* d
                       const int* segment_ids, long long seg_stride, float softmax_scale, int dkv_init,
                       const int* tiles, const int* tile_count, void* stream);
 
+/* Reproducible dQ (what torch.use_deterministic_algorithms(True) asks for): lwm_attn_bwd_step_ordered and
+ * lwm_attn_infer_bwd_ordered (below) compute the same as lwm_attn_bwd_step / lwm_attn_infer_bwd, but every dQ element
+ * receives its key tiles' fp32 contributions in ascending key-tile order, so dQ is the same bits on every run (dK and dV
+ * already are). order_ws is a caller-owned int32 workspace of
+ *     2 + B * H * ceil(Sq/64)                    words without a block map,
+ *     2 + B * H * ceil(Sq/64) + B * n_kt * ceil(Sq/64)   with one (n_kt = ceil(Sk/128); Sq = Q for the inference op),
+ * used on the call's stream and zeroed there by the call; it must not be shared by calls that may run concurrently.
+ * Word 1 is an error flag: nonzero after the call if a dQ tile waited more than 4 s for its turn (a bug, never expected;
+ * the reduction then went on unordered). A null order_ws is LWM_ERR_ARG. */
+int lwm_attn_bwd_step_ordered(const void* q, const void* k, const void* v, const void* dout, const float* scale_q,
+                              const float* scale_k, const float* scale_v, const float* scale_do, const float* lse,
+                              const float* delta, float* dq_acc, float* dk_acc, float* dv_acc, int B, int H, int Sq,
+                              int Sk, int D, long long q_pos0, long long k_pos0, int causal, const float* bias,
+                              long long bias_stride, const int* segment_ids, long long seg_stride, float softmax_scale,
+                              int dkv_init, const int* tiles, const int* tile_count, int* order_ws, void* stream);
+
 /* fp16-internal precision mode (optional): the tensor cores take bf16 x bf16 or fp16 x fp16 only, so the
  * higher-precision mode converts every operand once to an exact, power-of-two-scaled fp16 copy
  * (lwm_attn_to_f16: x16 = x / scale, scale = 2^(e-12) with e the exponent of the tensor's largest FINITE |x|,
@@ -202,6 +218,12 @@ int lwm_attn_infer_bwd(const void* q16, const void* k16, const void* v16, const 
                        const float* delta, const unsigned* bits, const int* tiles, const int* tile_count,
                        float* dq_acc, float* dk_acc, float* dv_acc, int B, int H, int Q, int Sk, int D,
                        float softmax_scale, void* stream);
+/* lwm_attn_infer_bwd with dQ reduced in a fixed order: order_ws as for lwm_attn_bwd_step_ordered, with its block map */
+int lwm_attn_infer_bwd_ordered(const void* q16, const void* k16, const void* v16, const void* dout16,
+                               const float* scale_q, const float* scale_k, const float* scale_v, const float* scale_do,
+                               const float* lse, const float* delta, const unsigned* bits, const int* tiles,
+                               const int* tile_count, float* dq_acc, float* dk_acc, float* dv_acc, int B, int H, int Q,
+                               int Sk, int D, float softmax_scale, int* order_ws, void* stream);
 
 /* Attention prologue: rotary position embedding (lwm/llama.py:344-375 precompute_freqs_cis / apply_rotary_emb, applied
  * at llama.py:517-519 on the head-split projections right before the ring-attention call; SURVEY.md §8f next-row 2).

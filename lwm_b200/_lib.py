@@ -20,6 +20,8 @@ _SIGNATURES = {
     "lwm_attn_bwd_lse": [c_void_p, c_void_p, c_ll, c_float, c_void_p],
     "lwm_attn_bwd_step": [c_void_p] * 13 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll, c_float,
                                                          c_int, c_void_p, c_void_p, c_void_p],
+    "lwm_attn_bwd_step_ordered": [c_void_p] * 13 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll,
+                                                                 c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p],
     "lwm_attn_to_f16": [c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_void_p],
     "lwm_attn_step_tilemap": [c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_ll, c_ll, c_int]
                              + [c_void_p] * 6,
@@ -47,6 +49,7 @@ _SIGNATURES = {
     "lwm_attn_infer_partial": [c_void_p] * 12 + [c_int] * 6 + [c_float, c_void_p],
     "lwm_attn_infer_bwd_tilemap": [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p],
     "lwm_attn_infer_bwd": [c_void_p] * 16 + [c_int] * 5 + [c_float, c_void_p],
+    "lwm_attn_infer_bwd_ordered": [c_void_p] * 16 + [c_int] * 5 + [c_float, c_void_p, c_void_p],
     "lwm_cast_f32_to_bf16": [c_void_p, c_void_p, c_ll, c_void_p],
     "lwm_add_f32": [c_void_p, c_void_p, c_ll, c_void_p],
     "lwm_vq_gn_stats": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],

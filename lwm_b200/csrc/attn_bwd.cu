@@ -52,6 +52,10 @@ struct BwdParams {
   // forward's mask, [B, q_rows, gridDim.x * 4] words (bit j of word w <=> key 32 w + j; 1 = attend), or null.
   const uint32_t* bits;
   int q_rows;
+  // kOrdered: order_ws = [ticket, error flag, dQ semaphores [B][H][Sq/64]] (zeroed by the entry point); with kMap,
+  // turns [B, Sk/128, Sq/64] holds each list entry's turn (dq_turns_kernel)
+  int* order_ws;
+  const int* turns;
 };
 
 constexpr int kBQ = 64;                         // query rows per inner iteration
@@ -78,7 +82,63 @@ struct BwdBarriers {
 // kMap: the list entry of the Q tile in stage st, written by the producer before it arms q_full[st] (the consumers read
 // it there instead of holding a pointer into the list across their loop)
 constexpr int kOffEntry = kOffBars + 96;
-static_assert(sizeof(BwdBarriers) <= 96 && 96 + 2 * 4 <= 128, "attn_bwd: barrier block layout");
+// kOrdered: the (n, h, b) of the CTA's ticket, written by thread 0
+constexpr int kOffTicket = kOffEntry + 2 * 4;
+static_assert(sizeof(BwdBarriers) <= 96 && 96 + 5 * 4 <= 128, "attn_bwd: barrier block layout");
+
+// ---- kOrdered: dQ reduced in a fixed key-tile order (lwm_attn_bwd_step_ordered, lwm_attn_infer_bwd_ordered)
+// Every element of dQ tile (b, h, 64-row Q tile i) receives the contributions of its key tiles in ascending key-tile
+// order, so dQ is the same bits on every run. Each (b, h, i) has a semaphore, the number of key tiles that have added
+// into the tile. Warp 9 of key tile n waits until it equals n's turn, the number of key tiles below n that reduce into
+// tile i (without a map they are a prefix, as i_start is monotone in n: the turn is n), issues its four reductions,
+// waits for them to complete, and increments the semaphore.
+// Forward progress does not rest on the order in which CTAs are dispatched: each CTA takes a ticket with one atomicAdd
+// when it starts and works on the (n, h, b) the ticket names, h fastest, then b, then n. A CTA only waits on key tiles
+// below its own, whose tickets are smaller; their CTAs have started, so they are resident or finished, and by induction
+// on the ticket every wait ends. (With n fastest, neighbouring key tiles of one head would run together and each would
+// stall behind the one before it.)
+// Memory ordering (PTX memory consistency model): the reductions are async-proxy writes of global memory. The
+// signaller waits for their completion (cp.async.bulk.wait_group 0: the writes are performed, not only the smem source
+// read), orders them before its generic-proxy accesses with fence.proxy.async.global, and publishes with a release
+// increment at gpu scope. The waiter's ld.acquire.gpu that reads the new count synchronises with that release, and its
+// fence.proxy.async.global orders the acquire before its own async-proxy reductions. So the previous key tile's adds
+// happen before the next one's, element for element.
+constexpr int kOrderHeader = 2;                          // order_ws[0] ticket, order_ws[1] error flag
+constexpr unsigned long long kTurnTimeoutNs = 4000000000ull;
+
+LWM_DEVICE void take_ticket(int* counter, int H, int B, volatile int* s_nhb) {
+  if (threadIdx.x == 0) {
+    const int t = atomicAdd(counter, 1);
+    s_nhb[0] = t / (H * B);
+    s_nhb[1] = t % H;
+    s_nhb[2] = t / H % B;
+  }
+  __syncthreads();
+}
+
+// Spin until *sem == turn. A wait longer than kTurnTimeoutNs is a bug (a turn that never comes): it sets the error flag
+// and carries on with the reduction, so it shows up as a flag the caller reads and never as a hang.
+LWM_DEVICE void dq_wait_turn(const int* sem, int turn, int* err) {
+  if (ld_acquire_gpu(sem) != turn) {
+    const uint64_t t0 = globaltimer_ns();
+    uint32_t ns = 32;
+    while (ld_acquire_gpu(sem) != turn) {
+      __nanosleep(ns);
+      ns = min(ns * 2, 1024u);
+      if (globaltimer_ns() - t0 > kTurnTimeoutNs) {
+        atomicOr(err, 1);
+        break;
+      }
+    }
+  }
+  fence_proxy_async_global();
+}
+
+LWM_DEVICE void dq_pass_turn(int* sem) {
+  tma_wait_group<0>();
+  fence_proxy_async_global();
+  red_release_gpu_add(sem, 1);
+}
 
 LWM_DEVICE void load_tile_nb(uint8_t* dst, const CUtensorMap* tm, uint64_t* bar, int h, int row0, int b, int half_bytes) {
   tma_load_4d(dst, tm, bar, 0, h, row0, b);
@@ -105,7 +165,8 @@ constexpr float kPBoostInv = 1.0f / 16384.0f;
 // the unmasked path, mixed tiles read one mask word per query column and give masked entries and keys >= Sk P = 0.
 // Rows >= q_rows and rows without any visible key carry lse = -inf (P = 0, dS = 0). Q / dO rows past q_rows and K / V
 // rows past Sk are zero-filled by TMA, the dQ reduction clips rows >= q_rows, and dK / dV rows >= Sk are not written.
-template <bool kF16, bool kMap = false, bool kBits = false>
+// kOrdered: dQ is reduced in ascending key-tile order (above); the grid's shape is the same, blockIdx is not used.
+template <bool kF16, bool kMap = false, bool kBits = false, bool kOrdered = false>
 __global__ void __launch_bounds__(kBwdThreads, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
@@ -119,15 +180,23 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int n = blockIdx.x;  // kv tile (ascending = heaviest first under causal masking)
-  const int h = blockIdx.y, b = blockIdx.z;
+  // (n, h, b): blockIdx, or with kOrdered the ticket's, kept in shared memory. The consumer warpgroups re-read them
+  // where they use them (as the other instances re-read blockIdx) rather than hold them in registers across their loop.
+  volatile int* s_nhb = reinterpret_cast<volatile int*>(smem + kOffTicket);
+  if constexpr (kOrdered) take_ticket(p.order_ws, p.H, p.B, s_nhb);
+  auto cta_n = [&]() -> int { return kOrdered ? s_nhb[0] : int(blockIdx.x); };
+  auto cta_h = [&]() -> int { return kOrdered ? s_nhb[1] : int(blockIdx.y); };
+  auto cta_b = [&]() -> int { return kOrdered ? s_nhb[2] : int(blockIdx.z); };
+  const int n = cta_n();  // kv tile (ascending = heaviest first under causal masking)
+  const int h = cta_h(), b = cta_b();
   const int n_q_tiles = p.Sq / kBQ;
-  // first Q tile with a row that can see key 0 of this tile
-  int i_start = 0;
-  if (p.mask.causal) {
-    const long long diff = (long long)p.mask.k_pos0 + (long long)n * kTile - p.mask.q_pos0;
-    i_start = diff <= 0 ? 0 : int(min(diff / kBQ, (long long)n_q_tiles));
-  }
+  // first Q tile with a row that can see key 0 of key tile kt
+  auto first_q_tile = [&](int kt) {
+    if (!p.mask.causal) return 0;
+    const long long diff = (long long)p.mask.k_pos0 + (long long)kt * kTile - p.mask.q_pos0;
+    return diff <= 0 ? 0 : int(min(diff / kBQ, (long long)n_q_tiles));
+  };
+  const int i_start = first_q_tile(n);
   int nq = n_q_tiles - i_start;
   int list0 = 0;   // kMap: offset of this K tile's list in p.tiles (B * Sk/128 * Sq/64 < 2^31: checked on the host)
   if constexpr (kMap) {
@@ -176,12 +245,18 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         const int st = it & 1;
         const int row0 = q_tile(it) * kBQ;
         mbar_wait(&bars.dq_full[st], (it >> 1) & 1);
+        int* sem = nullptr;
+        if constexpr (kOrdered) {
+          sem = p.order_ws + kOrderHeader + (b * p.H + h) * n_q_tiles + row0 / kBQ;
+          dq_wait_turn(sem, kMap ? p.turns[list0 + it] : n, p.order_ws + 1);
+        }
 #pragma unroll
         for (int j = 0; j < kHeadDim / 32; ++j)
           tma_reduce_add_4d(&tmDQ, smem + kOffDQ + st * kDQB + j * kDQBox, 32 * j, h, row0, b);
         tma_commit_group();
         tma_wait_group_read<0>();
-        mbar_arrive(&bars.dq_empty[st]);
+        mbar_arrive(&bars.dq_empty[st]);   // the staging tile is free once read, before the reductions complete
+        if constexpr (kOrdered) dq_pass_turn(sem);
       }
       tma_wait_group<0>();
     }
@@ -222,8 +297,10 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const float scale_log2 = p.scale_log2 * (kF16 ? (*p.scale_q) * (*p.scale_k) : 1.0f);
   const float delta_mul = kF16 ? 1.0f / ((*p.scale_do) * (*p.scale_v)) : 1.0f;   // exact: a power of two
   const float ds_mul = p.scale * (kF16 ? kDsNorm * kPBoostInv : 1.0f);    // P holds P * 2^14 in fp16 mode
-  // positions fit in int32 (checked on the host); int keeps the loop under the register budget
+  // positions fit in int32 (checked on the host); int keeps the loop under the register budget. kOrdered recomputes it
+  // (and i_start) from cta_n() where it is used.
   const int wg_k_last = p.mask.k_pos0 + n * kTile + wg * 64 + 63;
+  auto k_last = [&]() { return kOrdered ? p.mask.k_pos0 + cta_n() * kTile + wg * 64 + 63 : wg_k_last; };
 
   const uint32_t aK = smem_u32(smem + kOffK), aV = smem_u32(smem + kOffV), aDS = smem_u32(smem + kOffDS);
   const uint64_t dK_k = desc_kmajor_sw128(aK + wg * 64 * 128), dV_k = desc_kmajor_sw128(aV + wg * 64 * 128);
@@ -265,10 +342,10 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     reg_fence(sacc);
 
     // ---- P^T = exp2(S^T * scale_log2 (+bias) - lse2)
-    const int q_tile_pos = p.mask.q_pos0 + (kMap ? entry >> 1 : i_start + it) * kBQ;
+    const int q_tile_pos = p.mask.q_pos0 + (kMap ? entry >> 1 : (kOrdered ? first_q_tile(cta_n()) : i_start) + it) * kBQ;
     // kMap: clean tiles keep the masked path's rounding (fmaf(s, scale, 0)): bit-identical to the step without a map
     const bool need_mask =
-        kBits ? bool(entry & 1) : (kMap || has_bias || has_seg || (p.mask.causal && q_tile_pos < wg_k_last));
+        kBits ? bool(entry & 1) : (kMap || has_bias || has_seg || (p.mask.causal && q_tile_pos < k_last()));
     const bool mixed = kMap ? (entry & 1) : true;   // the tile reads bias and segment ids
     uint32_t pk[4][4], dsk[4][4];   // P^T and dS^T as A fragments, one 16-query slice per entry
     float pr[4][8];
@@ -282,10 +359,10 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     } else if constexpr (kBits) {
       // keys kr0 and kr0 + 8 sit in one 32-bit word of every query row's bits (bits sh and sh + 8). Rows past q_rows
       // read the last row instead: their lse is -inf, whatever the bits say. Masked entries and keys >= Sk get P = 0.
-      const int key0 = n * kTile + kr0;
+      const int key0 = cta_n() * kTile + kr0;
       const int sh = key0 & 31;
       const int kw = gridDim.x * 4;
-      const uint32_t* wcol = p.bits ? p.bits + (long long)b * p.q_rows * kw + (key0 >> 5) : nullptr;
+      const uint32_t* wcol = p.bits ? p.bits + (long long)cta_b() * p.q_rows * kw + (key0 >> 5) : nullptr;
       const bool key_in[2] = {key0 < p.Sk, key0 + 8 < p.Sk};
 #pragma unroll
       for (int g = 0; g < 8; ++g)
@@ -303,8 +380,9 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     } else {
       // per-key mask inputs, reloaded per masked tile (L1 hits) rather than held in registers across the loop
       const bool use_bias = has_bias && mixed, use_seg = has_seg && mixed;
-      const int* seg_row = use_seg ? p.mask.seg + (long long)b * p.mask.seg_stride : nullptr;
-      const int k_pos = p.mask.k_pos0 + n * kTile + kr0;   // this thread's keys: k_pos, k_pos + 8
+      const int bt = cta_b();
+      const int* seg_row = use_seg ? p.mask.seg + (long long)bt * p.mask.seg_stride : nullptr;
+      const int k_pos = p.mask.k_pos0 + cta_n() * kTile + kr0;   // this thread's keys: k_pos, k_pos + 8
       int my_seg[2];
       float bias_t[2] = {0.f, 0.f};
       bool key_masked[2] = {false, false};
@@ -312,7 +390,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       for (int hh = 0; hh < 2; ++hh) {
         my_seg[hh] = use_seg ? seg_row[k_pos + 8 * hh] : 0;
         if (use_bias) {
-          bias_t[hh] = p.mask.bias[(long long)b * p.mask.bias_stride + k_pos + 8 * hh] * kLog2e;
+          bias_t[hh] = p.mask.bias[(long long)bt * p.mask.bias_stride + k_pos + 8 * hh] * kLog2e;
           key_masked[hh] = bias_t[hh] < kMaskedLogit;
         }
       }
@@ -414,8 +492,9 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const float dv_mul = kF16 ? (*p.scale_do) * kPBoostInv : 1.0f;
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
-    if (kBits && n * kTile + kr0 + 8 * hh >= p.Sk) continue;   // key rows past the cache are not written
-    const long long row = ((((long long)b * p.Sk + (long long)n * kTile + kr0 + 8 * hh) * p.H + h) * kHeadDim);
+    if (kBits && cta_n() * kTile + kr0 + 8 * hh >= p.Sk) continue;   // key rows past the cache are not written
+    const long long row =
+        ((((long long)cta_b() * p.Sk + (long long)cta_n() * kTile + kr0 + 8 * hh) * p.H + cta_h()) * kHeadDim);
 #pragma unroll
     for (int g = 0; g < kHeadDim / 8; ++g) {
       const int c = g * 8 + quad * 2;
@@ -448,18 +527,90 @@ static bool make_f32_tmap(CUtensorMap* tm, const void* ptr, int B, int S, int H,
   return encode_tmap(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, ptr, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
+// turns[b][n][pos] = #{n' < n : the list of K tile n' holds Q tile tiles[b][n][pos] >> 1}, over the backward lists of
+// lwm_attn_step_tilemap and lwm_attn_infer_bwd_tilemap (the same format): the turn of each list entry in the ordered dQ
+// reduction. One warp per (b, Q tile) walks the K tiles 32 at a time, finds the Q tile in each ascending list by
+// binary search and numbers the lists that hold it in key-tile order. Entries past a list's count are not written.
+constexpr int kTurnThreads = 128;
+__global__ void __launch_bounds__(kTurnThreads)
+dq_turns_kernel(const int* __restrict__ tiles, const int* __restrict__ counts, int n_kt, int n_q64,
+                int* __restrict__ turns) {
+  const int qt = int((blockIdx.x * kTurnThreads + threadIdx.x) >> 5), lane = threadIdx.x & 31, b = blockIdx.y;
+  if (qt >= n_q64) return;   // whole warps
+  int turn = 0;
+  for (int base = 0; base < n_kt; base += 32) {
+    const int kt = base + lane;
+    int pos = -1;
+    if (kt < n_kt) {
+      const long long lt = (long long)b * n_kt + kt;
+      const int* list = tiles + lt * n_q64;
+      const int cnt = counts[lt];
+      int lo = 0, hi = cnt;   // first entry whose Q tile is >= qt
+      while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if ((list[mid] >> 1) < qt) lo = mid + 1;
+        else hi = mid;
+      }
+      if (lo < cnt && (list[lo] >> 1) == qt) pos = lo;
+    }
+    const unsigned hit = __ballot_sync(0xffffffffu, pos >= 0);
+    if (pos >= 0) turns[((long long)b * n_kt + kt) * n_q64 + pos] = turn + __popc(hit & ((1u << lane) - 1u));
+    turn += __popc(hit);
+  }
+}
+
+template <bool kF16, bool kMap, bool kBits, bool kOrdered>
+static int launch_bwd(dim3 grid, cudaStream_t st, const CUtensorMap (&tm)[5], const BwdParams& p, const char* what) {
+  static bool attr_set_dev[64] = {};
+  int cur_dev = 0;
+  cudaGetDevice(&cur_dev);
+  bool& attr_set = attr_set_dev[cur_dev & 63];      // function attributes are per device
+  if (!attr_set) {
+    if (cudaFuncSetAttribute(attn_bwd_kernel<kF16, kMap, kBits, kOrdered>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             kBwdSmemBytes) != cudaSuccess)
+      return lwm_fail(LWM_ERR_CUDA, "attn_bwd: cannot raise dynamic shared memory limit");
+    attr_set = true;
+  }
+  attn_bwd_kernel<kF16, kMap, kBits, kOrdered><<<grid, kBwdThreads, kBwdSmemBytes, st>>>(tm[0], tm[1], tm[2], tm[3],
+                                                                                        tm[4], p);
+  return lwm_check_launch(what);
+}
+
+// The ordered launches' set-up on the call's stream: the ticket, the error flag and n_sem dQ semaphores are zeroed, and
+// with a block map its turns are written after the semaphores.
+static int order_prologue(int* order_ws, long long n_sem, const int* tiles, const int* tile_count, int B, int n_kt,
+                          int n_q64, cudaStream_t st, BwdParams& p) {
+  if (cudaMemsetAsync(order_ws, 0, (kOrderHeader + n_sem) * sizeof(int), st) != cudaSuccess)
+    return lwm_fail(LWM_ERR_CUDA, "attn_bwd (ordered): cudaMemsetAsync of order_ws failed");
+  p.order_ws = order_ws;
+  p.turns = nullptr;
+  if (!tiles) return LWM_OK;
+  int* turns = order_ws + kOrderHeader + n_sem;
+  constexpr int kWarps = kTurnThreads / 32;
+  dq_turns_kernel<<<dim3((n_q64 + kWarps - 1) / kWarps, B), kTurnThreads, 0, st>>>(tiles, tile_count, n_kt, n_q64,
+                                                                                    turns);
+  p.turns = turns;
+  return lwm_check_launch("dq_turns_kernel");
+}
+
+// Size checks of the ordered launches: semaphore indices, tickets and turn indices are int32.
+static bool order_fits(int B, int H, int n_kt, int n_q64, bool map) {
+  const long long sem = (long long)B * H * n_q64, tickets = (long long)B * H * n_kt;
+  const long long turns = map ? (long long)B * n_kt * n_q64 : 0;
+  return B <= 65535 && H <= 65535 && kOrderHeader + sem + turns <= 0x7fffffffLL && tickets <= 0x7fffffffLL;
+}
+
 }  // namespace lwm
 
 using namespace lwm;
 
-// One ring step (include/lwm_b200.h): the scales select the fp16-operand kernel, tiles / tile_count the block map.
-extern "C" int lwm_attn_bwd_step(const void* q, const void* k, const void* v, const void* dout, const float* scale_q,
-                                 const float* scale_k, const float* scale_v, const float* scale_do, const float* lse,
-                                 const float* delta, float* dq_acc, float* dk_acc, float* dv_acc, int B, int H,
-                                 int Sq, int Sk, int D, long long q_pos0, long long k_pos0, int causal,
-                                 const float* bias, long long bias_stride, const int* segment_ids,
-                                 long long seg_stride, float softmax_scale, int dkv_init, const int* tiles,
-                                 const int* tile_count, void* stream) {
+// One ring step; order_ws null: the unordered reduction of lwm_attn_bwd_step, else lwm_attn_bwd_step_ordered's.
+static int bwd_step(const void* q, const void* k, const void* v, const void* dout, const float* scale_q,
+                    const float* scale_k, const float* scale_v, const float* scale_do, const float* lse,
+                    const float* delta, float* dq_acc, float* dk_acc, float* dv_acc, int B, int H, int Sq, int Sk,
+                    int D, long long q_pos0, long long k_pos0, int causal, const float* bias, long long bias_stride,
+                    const int* segment_ids, long long seg_stride, float softmax_scale, int dkv_init, const int* tiles,
+                    const int* tile_count, int* order_ws, void* stream) {
   if (!scale_k != !scale_q || !scale_v != !scale_q || !scale_do != !scale_q)
     return lwm_fail(LWM_ERR_ARG, "attn_bwd: scales are all given (fp16 operands) or all null (bf16)");
   if (!tiles != !tile_count) return lwm_fail(LWM_ERR_ARG, "attn_bwd: tiles and tile_count are both given or both null");
@@ -477,11 +628,13 @@ extern "C" int lwm_attn_bwd_step(const void* q, const void* k, const void* v, co
     return lwm_fail(LWM_ERR_SHAPE, "attn_bwd: segment_ids is indexed by GLOBAL position: seg_stride < max(q_pos0 + Sq, k_pos0 + Sk)");
   if (tiles && (long long)B * (Sk / kTile) * (Sq / kBQ) > 0x7fffffffLL)
     return lwm_fail(LWM_ERR_SHAPE, "attn_bwd: B * Sk/128 * Sq/64 must fit in int32 with a block map");
+  if (order_ws && !order_fits(B, H, Sk / kTile, Sq / kBQ, tiles != nullptr))
+    return lwm_fail(LWM_ERR_SHAPE, "attn_bwd_ordered: B, H <= 65535 and the order_ws words, B * H * Sk/128 must fit in int32");
   if (!lwm_check_device()) return LWM_ERR_DEVICE;
-  CUtensorMap tq, tk, tv, tdo, tdq;
-  if (!make_bf16_tmap(&tq, q, B, Sq, H, kBQ) || !make_bf16_tmap(&tk, k, B, Sk, H, kTile) ||
-      !make_bf16_tmap(&tv, v, B, Sk, H, kTile) || !make_bf16_tmap(&tdo, dout, B, Sq, H, kBQ) ||
-      !make_f32_tmap(&tdq, dq_acc, B, Sq, H, kBQ))
+  CUtensorMap tm[5];   // q, k, v, dout, dq_acc
+  if (!make_bf16_tmap(&tm[0], q, B, Sq, H, kBQ) || !make_bf16_tmap(&tm[1], k, B, Sk, H, kTile) ||
+      !make_bf16_tmap(&tm[2], v, B, Sk, H, kTile) || !make_bf16_tmap(&tm[3], dout, B, Sq, H, kBQ) ||
+      !make_f32_tmap(&tm[4], dq_acc, B, Sq, H, kBQ))
     return lwm_fail(LWM_ERR_CUDA, "attn_bwd: cuTensorMapEncodeTiled failed (pointers must be 16B aligned)");
   BwdParams p;
   p.B = B; p.H = H; p.Sq = Sq; p.Sk = Sk;
@@ -494,44 +647,64 @@ extern "C" int lwm_attn_bwd_step(const void* q, const void* k, const void* v, co
   p.scale_q = scale_q; p.scale_k = scale_k; p.scale_v = scale_v; p.scale_do = scale_do;
   p.dkv_init = dkv_init ? 1 : 0;
   p.tiles = tiles; p.tile_count = tile_count;
-  static bool attr_set_dev[64] = {};
-  int cur_dev = 0;
-  cudaGetDevice(&cur_dev);
-  bool& attr_set = attr_set_dev[cur_dev & 63];      // function attributes are per device
-  if (!attr_set) {
-    if (cudaFuncSetAttribute(attn_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBwdSmemBytes) !=
-            cudaSuccess ||
-        cudaFuncSetAttribute(attn_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBwdSmemBytes) !=
-            cudaSuccess ||
-        cudaFuncSetAttribute(attn_bwd_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             kBwdSmemBytes) != cudaSuccess ||
-        cudaFuncSetAttribute(attn_bwd_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             kBwdSmemBytes) != cudaSuccess)
-      return lwm_fail(LWM_ERR_CUDA, "attn_bwd: cannot raise dynamic shared memory limit");
-    attr_set = true;
-  }
+  p.order_ws = nullptr; p.turns = nullptr;
   dim3 grid(Sk / kTile, H, B);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (tiles) {
-    if (scale_q) attn_bwd_kernel<true, true><<<grid, kBwdThreads, kBwdSmemBytes, st>>>(tq, tk, tv, tdo, tdq, p);
-    else attn_bwd_kernel<false, true><<<grid, kBwdThreads, kBwdSmemBytes, st>>>(tq, tk, tv, tdo, tdq, p);
-    return lwm_check_launch("attn_bwd_kernel (block map)");
+  if (order_ws) {
+    const int s = order_prologue(order_ws, (long long)B * H * (Sq / kBQ), tiles, tile_count, B, Sk / kTile, Sq / kBQ,
+                                 st, p);
+    if (s) return s;
+    if (tiles)
+      return scale_q ? launch_bwd<true, true, false, true>(grid, st, tm, p, "attn_bwd_kernel (ordered, block map)")
+                     : launch_bwd<false, true, false, true>(grid, st, tm, p, "attn_bwd_kernel (ordered, block map)");
+    return scale_q ? launch_bwd<true, false, false, true>(grid, st, tm, p, "attn_bwd_kernel (ordered)")
+                   : launch_bwd<false, false, false, true>(grid, st, tm, p, "attn_bwd_kernel (ordered)");
   }
-  if (scale_q) attn_bwd_kernel<true><<<grid, kBwdThreads, kBwdSmemBytes, st>>>(tq, tk, tv, tdo, tdq, p);
-  else attn_bwd_kernel<false><<<grid, kBwdThreads, kBwdSmemBytes, st>>>(tq, tk, tv, tdo, tdq, p);
-  return lwm_check_launch("attn_bwd_kernel");
+  if (tiles)
+    return scale_q ? launch_bwd<true, true, false, false>(grid, st, tm, p, "attn_bwd_kernel (block map)")
+                   : launch_bwd<false, true, false, false>(grid, st, tm, p, "attn_bwd_kernel (block map)");
+  return scale_q ? launch_bwd<true, false, false, false>(grid, st, tm, p, "attn_bwd_kernel")
+                 : launch_bwd<false, false, false, false>(grid, st, tm, p, "attn_bwd_kernel");
+}
+
+// One ring step (include/lwm_b200.h): the scales select the fp16-operand kernel, tiles / tile_count the block map.
+extern "C" int lwm_attn_bwd_step(const void* q, const void* k, const void* v, const void* dout, const float* scale_q,
+                                 const float* scale_k, const float* scale_v, const float* scale_do, const float* lse,
+                                 const float* delta, float* dq_acc, float* dk_acc, float* dv_acc, int B, int H,
+                                 int Sq, int Sk, int D, long long q_pos0, long long k_pos0, int causal,
+                                 const float* bias, long long bias_stride, const int* segment_ids,
+                                 long long seg_stride, float softmax_scale, int dkv_init, const int* tiles,
+                                 const int* tile_count, void* stream) {
+  return bwd_step(q, k, v, dout, scale_q, scale_k, scale_v, scale_do, lse, delta, dq_acc, dk_acc, dv_acc, B, H, Sq, Sk,
+                  D, q_pos0, k_pos0, causal, bias, bias_stride, segment_ids, seg_stride, softmax_scale, dkv_init, tiles,
+                  tile_count, nullptr, stream);
+}
+
+// lwm_attn_bwd_step with dQ reduced in ascending key-tile order (include/lwm_b200.h)
+extern "C" int lwm_attn_bwd_step_ordered(const void* q, const void* k, const void* v, const void* dout,
+                                         const float* scale_q, const float* scale_k, const float* scale_v,
+                                         const float* scale_do, const float* lse, const float* delta, float* dq_acc,
+                                         float* dk_acc, float* dv_acc, int B, int H, int Sq, int Sk, int D,
+                                         long long q_pos0, long long k_pos0, int causal, const float* bias,
+                                         long long bias_stride, const int* segment_ids, long long seg_stride,
+                                         float softmax_scale, int dkv_init, const int* tiles, const int* tile_count,
+                                         int* order_ws, void* stream) {
+  if (!order_ws) return lwm_fail(LWM_ERR_ARG, "attn_bwd_ordered: null order_ws");
+  return bwd_step(q, k, v, dout, scale_q, scale_k, scale_v, scale_do, lse, delta, dq_acc, dk_acc, dv_acc, B, H, Sq, Sk,
+                  D, q_pos0, k_pos0, causal, bias, bias_stride, segment_ids, seg_stride, softmax_scale, dkv_init, tiles,
+                  tile_count, order_ws, stream);
 }
 
 // Backward of ringattention_inference (attn_bwd_kernel<true, true, true>): any Q and Sk. q16 / dout16 [B,Q,H,128],
 // k16 / v16 [B,Sk,H,128] scaled fp16 copies with their device scales; lse (pre-scaled by lwm_attn_bwd_lse with the fp16
 // offset, -inf for rows without a visible key) and delta [B,H,Qp], Qp = Q rounded up to 64, rows >= Q: lse = -inf;
 // bits [B,Q,ceil(Sk/128)*4] or null; tiles / tile_count from lwm_attn_infer_bwd_tilemap. dq_acc [B,Q,H,128] fp32 is
-// accumulated into (zero it first); dk_acc / dv_acc [B,Sk,H,128] fp32 are written.
-extern "C" int lwm_attn_infer_bwd(const void* q16, const void* k16, const void* v16, const void* dout16,
-                                  const float* scale_q, const float* scale_k, const float* scale_v,
-                                  const float* scale_do, const float* lse, const float* delta, const unsigned* bits,
-                                  const int* tiles, const int* tile_count, float* dq_acc, float* dk_acc, float* dv_acc,
-                                  int B, int H, int Q, int Sk, int D, float softmax_scale, void* stream) {
+// accumulated into (zero it first); dk_acc / dv_acc [B,Sk,H,128] fp32 are written. order_ws: as in bwd_step.
+static int infer_bwd(const void* q16, const void* k16, const void* v16, const void* dout16, const float* scale_q,
+                     const float* scale_k, const float* scale_v, const float* scale_do, const float* lse,
+                     const float* delta, const unsigned* bits, const int* tiles, const int* tile_count, float* dq_acc,
+                     float* dk_acc, float* dv_acc, int B, int H, int Q, int Sk, int D, float softmax_scale,
+                     int* order_ws, void* stream) {
   if (D != kHeadDim) return lwm_fail(LWM_ERR_SHAPE, "attn_infer_bwd: head_dim must be 128");
   if (!q16 || !k16 || !v16 || !dout16 || !scale_q || !scale_k || !scale_v || !scale_do || !lse || !delta || !tiles ||
       !tile_count || !dq_acc || !dk_acc || !dv_acc)
@@ -541,11 +714,13 @@ extern "C" int lwm_attn_infer_bwd(const void* q16, const void* k16, const void* 
   const int n_kt = (Sk + kTile - 1) / kTile, qp = (Q + kBQ - 1) / kBQ * kBQ;
   if ((long long)B * n_kt * (qp / kBQ) > 0x7fffffffLL || (long long)Q + kBQ > 0x7fffffffLL)
     return lwm_fail(LWM_ERR_SHAPE, "attn_infer_bwd: B * ceil(Sk/128) * ceil(Q/64) must fit in int32");
+  if (order_ws && !order_fits(B, H, n_kt, qp / kBQ, true))
+    return lwm_fail(LWM_ERR_SHAPE, "attn_infer_bwd_ordered: the order_ws words and B * H * ceil(Sk/128) must fit in int32");
   if (!lwm_check_device()) return LWM_ERR_DEVICE;
-  CUtensorMap tq, tk, tv, tdo, tdq;
-  if (!make_bf16_tmap(&tq, q16, B, Q, H, kBQ) || !make_bf16_tmap(&tk, k16, B, Sk, H, kTile) ||
-      !make_bf16_tmap(&tv, v16, B, Sk, H, kTile) || !make_bf16_tmap(&tdo, dout16, B, Q, H, kBQ) ||
-      !make_f32_tmap(&tdq, dq_acc, B, Q, H, kBQ))
+  CUtensorMap tm[5];
+  if (!make_bf16_tmap(&tm[0], q16, B, Q, H, kBQ) || !make_bf16_tmap(&tm[1], k16, B, Sk, H, kTile) ||
+      !make_bf16_tmap(&tm[2], v16, B, Sk, H, kTile) || !make_bf16_tmap(&tm[3], dout16, B, Q, H, kBQ) ||
+      !make_f32_tmap(&tm[4], dq_acc, B, Q, H, kBQ))
     return lwm_fail(LWM_ERR_CUDA, "attn_infer_bwd: cuTensorMapEncodeTiled failed (pointers must be 16B aligned)");
   BwdParams p{};
   p.B = B; p.H = H; p.Sq = qp; p.Sk = Sk;
@@ -556,17 +731,33 @@ extern "C" int lwm_attn_infer_bwd(const void* q16, const void* k16, const void* 
   p.dkv_init = 1;
   p.tiles = tiles; p.tile_count = tile_count;
   p.bits = bits; p.q_rows = Q;
-  static bool attr_set_dev[64] = {};
-  int cur_dev = 0;
-  cudaGetDevice(&cur_dev);
-  bool& attr_set = attr_set_dev[cur_dev & 63];
-  if (!attr_set) {
-    if (cudaFuncSetAttribute(attn_bwd_kernel<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             kBwdSmemBytes) != cudaSuccess)
-      return lwm_fail(LWM_ERR_CUDA, "attn_infer_bwd: cannot raise dynamic shared memory limit");
-    attr_set = true;
+  const dim3 grid(n_kt, H, B);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (order_ws) {
+    const int s = order_prologue(order_ws, (long long)B * H * (qp / kBQ), tiles, tile_count, B, n_kt, qp / kBQ, st, p);
+    if (s) return s;
+    return launch_bwd<true, true, true, true>(grid, st, tm, p, "attn_bwd_kernel (inference, ordered)");
   }
-  attn_bwd_kernel<true, true, true><<<dim3(n_kt, H, B), kBwdThreads, kBwdSmemBytes,
-                                      reinterpret_cast<cudaStream_t>(stream)>>>(tq, tk, tv, tdo, tdq, p);
-  return lwm_check_launch("attn_bwd_kernel (inference)");
+  return launch_bwd<true, true, true, false>(grid, st, tm, p, "attn_bwd_kernel (inference)");
+}
+
+extern "C" int lwm_attn_infer_bwd(const void* q16, const void* k16, const void* v16, const void* dout16,
+                                  const float* scale_q, const float* scale_k, const float* scale_v,
+                                  const float* scale_do, const float* lse, const float* delta, const unsigned* bits,
+                                  const int* tiles, const int* tile_count, float* dq_acc, float* dk_acc, float* dv_acc,
+                                  int B, int H, int Q, int Sk, int D, float softmax_scale, void* stream) {
+  return infer_bwd(q16, k16, v16, dout16, scale_q, scale_k, scale_v, scale_do, lse, delta, bits, tiles, tile_count,
+                   dq_acc, dk_acc, dv_acc, B, H, Q, Sk, D, softmax_scale, nullptr, stream);
+}
+
+// lwm_attn_infer_bwd with dQ reduced in ascending key-tile order (include/lwm_b200.h)
+extern "C" int lwm_attn_infer_bwd_ordered(const void* q16, const void* k16, const void* v16, const void* dout16,
+                                          const float* scale_q, const float* scale_k, const float* scale_v,
+                                          const float* scale_do, const float* lse, const float* delta,
+                                          const unsigned* bits, const int* tiles, const int* tile_count,
+                                          float* dq_acc, float* dk_acc, float* dv_acc, int B, int H, int Q, int Sk,
+                                          int D, float softmax_scale, int* order_ws, void* stream) {
+  if (!order_ws) return lwm_fail(LWM_ERR_ARG, "attn_infer_bwd_ordered: null order_ws");
+  return infer_bwd(q16, k16, v16, dout16, scale_q, scale_k, scale_v, scale_do, lse, delta, bits, tiles, tile_count,
+                   dq_acc, dk_acc, dv_acc, B, H, Q, Sk, D, softmax_scale, order_ws, stream);
 }

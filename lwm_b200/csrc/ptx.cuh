@@ -103,6 +103,23 @@ template <int N>
 LWM_DEVICE void tma_wait_group() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
+// orders this thread's generic-proxy accesses of global memory with its async-proxy (bulk copy / reduce) accesses
+LWM_DEVICE void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
+
+// ---------------------------------------------------------------- device-scope flags
+LWM_DEVICE int ld_acquire_gpu(const int* p) {
+  int v;
+  asm volatile("ld.acquire.gpu.global.b32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+LWM_DEVICE void red_release_gpu_add(int* p, int v) {
+  asm volatile("red.release.gpu.global.add.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+LWM_DEVICE uint64_t globaltimer_ns() {
+  uint64_t t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
 
 // ---------------------------------------------------------------- wgmma: descriptors and ordering
 // Shared-memory matrix descriptor (64 bit). Fields (PTX ISA "Matrix Descriptor Format", sm_90):

@@ -316,20 +316,33 @@ def lse_for_bwd(lse, stream=None, f16=False):
     return out
 
 
+def order_workspace(words, device):
+    """the int32 workspace of an ordered dQ reduction (include/lwm_b200.h: lwm_attn_bwd_step_ordered); the call zeroes
+    it on its stream. Word 1 is the call's error flag."""
+    return torch.empty(words, dtype=torch.int32, device=device)
+
+
 def bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg, stream=None,
              scales=None, init=False, tilemap=None):
     """`lse` is the PRE-SCALED array returned by lse_for_bwd. scales: None (bf16 operands), or (sq, sk, sv, sdo) of
     fp16 operand copies q/k/v/dout. init=True: dk_acc/dv_acc rows are written, not accumulated.
     tilemap: None, or the backward map (tiles, counts) of step_tilemap for these arguments (dK, dV bit-identical; dQ
-    up to the order of its reductions)."""
+    up to the order of its reductions).
+    Under torch.use_deterministic_algorithms(True) dQ is reduced in ascending key-tile order
+    (lwm_attn_bwd_step_ordered): the same bits on every run."""
     B, Sq, H, D = q.shape
     sq, sk, sv, sdo = scales if scales is not None else (None, None, None, None)
     tiles, counts = tilemap if tilemap is not None else (None, None)
-    _lib.call("lwm_attn_bwd_step", _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(dout), _lib.ptr(sq), _lib.ptr(sk),
-              _lib.ptr(sv), _lib.ptr(sdo), _lib.ptr(lse), _lib.ptr(delta), _lib.ptr(dq_acc), _lib.ptr(dk_acc),
-              _lib.ptr(dv_acc), B, H, Sq, k.shape[1], D, int(q_pos0), int(k_pos0), int(bool(causal)), _lib.ptr(bias),
-              0 if bias is None else bias.shape[1], _lib.ptr(seg), 0 if seg is None else seg.shape[1],
-              1.0 / math.sqrt(D), int(bool(init)), _lib.ptr(tiles), _lib.ptr(counts), _lib.stream_ptr(stream))
+    args = (_lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(dout), _lib.ptr(sq), _lib.ptr(sk), _lib.ptr(sv),
+            _lib.ptr(sdo), _lib.ptr(lse), _lib.ptr(delta), _lib.ptr(dq_acc), _lib.ptr(dk_acc), _lib.ptr(dv_acc), B, H,
+            Sq, k.shape[1], D, int(q_pos0), int(k_pos0), int(bool(causal)), _lib.ptr(bias),
+            0 if bias is None else bias.shape[1], _lib.ptr(seg), 0 if seg is None else seg.shape[1], 1.0 / math.sqrt(D),
+            int(bool(init)), _lib.ptr(tiles), _lib.ptr(counts))
+    if torch.are_deterministic_algorithms_enabled():
+        ws = order_workspace(2 + B * H * (Sq // 64) + (0 if tiles is None else tiles.numel()), q.device)
+        _lib.call("lwm_attn_bwd_step_ordered", *args, _lib.ptr(ws), _lib.stream_ptr(stream))
+    else:
+        _lib.call("lwm_attn_bwd_step", *args, _lib.stream_ptr(stream))
 
 
 def _map_kw(q, k, q_pos0, k_pos0, causal, bias, seg, fwd):
@@ -823,7 +836,8 @@ def infer_backward(q16, k16, v16, do16, scales, lse, delta, bits, row_any):
     """One backward launch of the inference op over this rank's keys: q16 / do16 [B,Q,H,128], k16 / v16 [B,Sk,H,128]
     scaled fp16 copies, scales = (sq, sk, sv, sdo); lse [B,H,Q] (natural log, -inf for rows with no visible key),
     delta [B,H,Q] = rowsum(dO o O); bits [B,Q,kw] / row_any [B,Q] (over the whole ring) or None
-    -> fp32 (dq [B,Q,H,128], dk, dv [B,Sk,H,128])."""
+    -> fp32 (dq [B,Q,H,128], dk, dv [B,Sk,H,128]). Under torch.use_deterministic_algorithms(True) dQ is reduced in
+    ascending key-tile order (lwm_attn_infer_bwd_ordered), as in bwd_step."""
     B, Q, H, D = q16.shape
     Sk = k16.shape[1]
     dev = q16.device
@@ -842,10 +856,14 @@ def infer_backward(q16, k16, v16, do16, scales, lse, delta, bits, row_any):
     dk = torch.empty((B, Sk, H, D), dtype=torch.float32, device=dev)
     dv = torch.empty((B, Sk, H, D), dtype=torch.float32, device=dev)
     sq, sk, sv, sdo = scales
-    _lib.call("lwm_attn_infer_bwd", _lib.ptr(q16), _lib.ptr(k16), _lib.ptr(v16), _lib.ptr(do16), _lib.ptr(sq),
-              _lib.ptr(sk), _lib.ptr(sv), _lib.ptr(sdo), _lib.ptr(nlse), _lib.ptr(delta_p), _lib.ptr(bits),
-              _lib.ptr(tiles), _lib.ptr(counts), _lib.ptr(dq), _lib.ptr(dk), _lib.ptr(dv), B, H, Q, Sk, D,
-              1.0 / math.sqrt(D), _lib.stream_ptr())
+    args = (_lib.ptr(q16), _lib.ptr(k16), _lib.ptr(v16), _lib.ptr(do16), _lib.ptr(sq), _lib.ptr(sk), _lib.ptr(sv),
+            _lib.ptr(sdo), _lib.ptr(nlse), _lib.ptr(delta_p), _lib.ptr(bits), _lib.ptr(tiles), _lib.ptr(counts),
+            _lib.ptr(dq), _lib.ptr(dk), _lib.ptr(dv), B, H, Q, Sk, D, 1.0 / math.sqrt(D))
+    if torch.are_deterministic_algorithms_enabled():
+        ws = order_workspace(2 + B * H * (Qp // 64) + tiles.numel(), dev)
+        _lib.call("lwm_attn_infer_bwd_ordered", *args, _lib.ptr(ws), _lib.stream_ptr())
+    else:
+        _lib.call("lwm_attn_infer_bwd", *args, _lib.stream_ptr())
     return dq, dk, dv
 
 

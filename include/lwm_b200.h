@@ -395,6 +395,30 @@ int lwm_vq_conv2d_f16(const void* a, const float* a_scale, const void* w_stacked
                       const float* residual, float* out, double* gn_stats_out, unsigned* absmax_out, int N, int Hin,
                       int Win, int Cpad, int Ho, int Wo, int Cout, int Cout_pad, int ksize, int stride, int pad,
                       float w_scale_inv, int groups, int clip, void* stream);
+/* Reproducible, batch-invariant tokenizer (what torch.use_deterministic_algorithms(True) asks for): with these in
+ * place of lwm_vq_gn_stats, lwm_vq_prep_f16 and lwm_vq_conv2d_f16, every sample's result is the same bits on every run
+ * and whatever else shares its batch. No atomics feed a sum, and no scale spans the batch:
+ * lwm_vq_gn_stats_ordered    the statistics of lwm_vq_gn_stats (same [N, groups, 2] float64 layout), from per-block
+ *                            partials over fixed 128-pixel ranges of each image, summed in a fixed order in float64.
+ *                            workspace: caller-owned, >= N * ceil(H*W/128) * groups * 2 floats (workspace_bytes).
+ * lwm_vq_prep_f16_ordered    lwm_vq_prep_f16 with one power-of-two scale per sample: scale_out [N], x_absmax [N]
+ *                            (uint32 bit patterns; computed into it per sample unless x_absmax_given), the GroupNorm
+ *                            bound taken over the sample's own groups.
+ * lwm_vq_conv2d_f16_ordered  lwm_vq_conv2d_f16 reading a_scale [N] (NULL = 1) and writing absmax_out [N] (zeroed by
+ *                            the call). gn_stats_out (optional) is written, not accumulated: every (8x16-pixel tile,
+ *                            warp) stores its per-group partials to workspace (>= N * Ho/8 * Wo/16 * 8 * groups * 2
+ *                            floats), which are summed in a fixed order in float64. It needs Cout/groups == 4, or a
+ *                            multiple of 8 that divides the N tile (every LWM layer that has a GroupNorm qualifies). */
+int lwm_vq_gn_stats_ordered(const float* x, double* stats, float* workspace, long long workspace_bytes, int N, int H,
+                            int W, int C, int groups, void* stream);
+int lwm_vq_prep_f16_ordered(const float* x, const double* gn_stats, const float* gamma, const float* beta, void* out,
+                            float* scale_out, unsigned* x_absmax, int x_absmax_given, int N, int H, int W, int C,
+                            int C_pad, int groups, int upsample2x, float eps, void* stream);
+int lwm_vq_conv2d_f16_ordered(const void* a, const float* a_scale, const void* w_stacked, const float* bias,
+                              const float* residual, float* out, double* gn_stats_out, float* workspace,
+                              long long workspace_bytes, unsigned* absmax_out, int N, int Hin, int Win, int Cpad,
+                              int Ho, int Wo, int Cout, int Cout_pad, int ksize, int stride, int pad,
+                              float w_scale_inv, int groups, int clip, void* stream);
 int lwm_vq_argmin(const float* z, const float* codebook, int* idx, float* zq_st, void* workspace, int N, int n_e,
                   int e_dim, void* stream);
 int lwm_vq_gather(const int* idx, const float* codebook, float* out, long long N, int n_e, int e_dim, void* stream);

@@ -58,6 +58,9 @@ _SIGNATURES = {
     "lwm_vq_conv_cin3": [c_void_p] * 4 + [c_int] * 4 + [c_void_p],
     "lwm_vq_prep_f16": [c_void_p] * 7 + [c_int] * 8 + [c_float, c_void_p],
     "lwm_vq_conv2d_f16": [c_void_p] * 8 + [c_int] * 11 + [c_float, c_int, c_int, c_void_p],
+    "lwm_vq_gn_stats_ordered": [c_void_p, c_void_p, c_void_p, c_ll, c_int, c_int, c_int, c_int, c_int, c_void_p],
+    "lwm_vq_prep_f16_ordered": [c_void_p] * 7 + [c_int] * 8 + [c_float, c_void_p],
+    "lwm_vq_conv2d_f16_ordered": [c_void_p] * 8 + [c_ll, c_void_p] + [c_int] * 11 + [c_float, c_int, c_int, c_void_p],
     "lwm_vq_argmin": [c_void_p] * 5 + [c_int] * 3 + [c_void_p],
     "lwm_vq_gather": [c_void_p] * 3 + [c_ll, c_int, c_int, c_void_p],
     "lwm_attn_rope": [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p] + [c_int] * 6 + [c_void_p],

@@ -21,6 +21,11 @@
 //   GN stats   optional epilogue: per-(sample, group) sum / sum of squares of the conv OUTPUT (bias and residual
 //              included) — the statistics the next GroupNorm needs — so no separate pass re-reads the activation;
 //              likewise |output|max, the scale of a raw fp16 plane of the output (Downsample, 1x1 shortcut).
+//   ordered    kOrdered instances (torch.use_deterministic_algorithms): no atomics and no sums carried across tiles. Each
+//              (tile, consumer warp) writes its per-group (sum, sumsq) to its own slot of a workspace indexed by (image,
+//              M tile within the image, warp), so the reduction order depends on the image's own pixels only, never on N,
+//              the grid or the SM count; gn_finalize_kernel adds the slots in a fixed order. The fp16 plane has one scale
+//              per image (a_scale[n]) and the |output|max goes to absmax[n].
 //   pipeline   warp 8: TMA producer through a ring of `stages` slots; warpgroups 0 / 1: pixels [0,64) / [64,128)
 //              of the 8x16 tile, fp32 accumulators in registers, epilogue (+ bias (+ residual) -> fp32 NHWC)
 //              straight from the accumulator fragment. Grid = #SMs, tiles strided.
@@ -51,10 +56,12 @@ struct ConvParams {
   const float* bias;              // [Cout]
   const float* residual;          // [N,Ho,Wo,Cout] or null
   float* out;                     // [N,Ho,Wo,Cout]
+  float* part;                    // kOrdered, optional: [N][Ho/8 * Wo/16][8 warps][groups][2] (sum, sumsq) per (tile, warp)
 };
 
-// NI: the wgmma N (BN, or 2*BN for the stacked fp16x2 weights); kF16: fp16 operands (n_pass 2), else bf16.
-template <int NI, bool kF16>
+// NI: the wgmma N (BN, or 2*BN for the stacked fp16x2 weights); kF16: fp16 operands (n_pass 2), else bf16;
+// kOrdered (kF16 only): per-image a_scale / absmax, and the statistics as per-(tile, warp) partials in p.part.
+template <int NI, bool kF16, bool kOrdered>
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant__ CUtensorMap tmAlo,
                   const __grid_constant__ CUtensorMap tmBhi, const __grid_constant__ CUtensorMap tmBlo,
@@ -145,7 +152,8 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_consta
 #pragma unroll
   for (int i = 0; i < kStatG; ++i) st1[i] = st2[i] = 0.f;
   int st_n = -1, st_nt = -1;
-  const int cpg = p.stats ? p.Cout / p.groups : 1;
+  const bool want_stats = kOrdered ? p.part != nullptr : p.stats != nullptr;
+  const int cpg = want_stats ? p.Cout / p.groups : 1;
   // fp16x2: accumulator units -> output units, w_scale_inv * a_scale (a product of powers of two: exact)
   const float out_scale = (kF16 && p.a_scale) ? p.w_scale_inv * *p.a_scale : p.w_scale_inv;
   float amax = 0.f;     // largest finite |output|: a NaN or inf output stays one in the next plane, whatever its scale
@@ -179,7 +187,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_consta
   for (int tile = tile_begin; tile < tile_end; ++tile) {
     int n, oh0, ow0, nt;
     decode_tile(tile, n, oh0, ow0, nt);
-    if (p.stats && (n != st_n || nt != st_nt)) {
+    if (!kOrdered && p.stats && (n != st_n || nt != st_nt)) {
       flush_stats();
       st_n = n;
       st_nt = nt;
@@ -214,6 +222,8 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_consta
 
     // ---- epilogue: this thread's pixels are rows r and r + 8 of its warp's 16 (one image row of the 8x16 tile)
     const int c_base = nt * p.BN;
+    float tile_scale = out_scale;
+    if constexpr (kOrdered) tile_scale = p.a_scale ? p.w_scale_inv * p.a_scale[n] : p.w_scale_inv;
     const bool vec = (p.Cout & 1) == 0;
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
@@ -226,8 +236,8 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_consta
         const int c = c_base + g * 8 + quad * 2;
         float v0 = acc[4 * g + 2 * hh], v1 = acc[4 * g + 2 * hh + 1];
         if (kF16) {
-          v0 = (v0 + acc[4 * g + 2 * hh + NI / 4]) * out_scale;
-          v1 = (v1 + acc[4 * g + 2 * hh + 1 + NI / 4]) * out_scale;
+          v0 = (v0 + acc[4 * g + 2 * hh + NI / 4]) * tile_scale;
+          v1 = (v1 + acc[4 * g + 2 * hh + 1 + NI / 4]) * tile_scale;
         }
         if (vec && c + 1 < p.Cout) {
           const float2 b2 = *reinterpret_cast<const float2*>(p.bias + c);
@@ -243,7 +253,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_consta
           }
           *reinterpret_cast<float2*>(dst + c) = o2;
           if (kF16 && p.absmax) amax = fmaxf(amax, fmaxf(finite_absf(o2.x), finite_absf(o2.y)));
-          if (kF16 && p.stats) {   // stats need Cout % 16 == 0 (checked on the host): always this path
+          if (kF16 && want_stats) {   // stats need Cout % 16 == 0 (checked on the host): always this path
             st1[g < kStatG ? g : 0] += o2.x + o2.y;
             st2[g < kStatG ? g : 0] += o2.x * o2.x + o2.y * o2.y;
           }
@@ -261,9 +271,48 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_consta
         }
       }
     }
+    if constexpr (kOrdered) {
+      if (want_stats) {
+        // this warp's 16 pixels: add the 8 row lanes of each channel pair, then the pairs of a group, then (cpg > 8) the
+        // 8-channel chunks of a group in ascending order — a fixed shuffle tree, no atomics
+        float* slot = p.part + (((size_t)n * tiles_h * tiles_w + (oh0 / 8) * tiles_w + ow0 / 16) * 8 + warp) * p.groups * 2;
+        float g1 = 0.f, g2 = 0.f;
+#pragma unroll
+        for (int g = 0; g < kStatG; ++g) {
+          float s1 = st1[g], s2 = st2[g];
+          st1[g] = st2[g] = 0.f;
+#pragma unroll
+          for (int sh = 4; sh < 32; sh <<= 1) {
+            s1 += __shfl_xor_sync(0xffffffffu, s1, sh);
+            s2 += __shfl_xor_sync(0xffffffffu, s2, sh);
+          }
+          s1 += __shfl_xor_sync(0xffffffffu, s1, 1);
+          s2 += __shfl_xor_sync(0xffffffffu, s2, 1);
+          if (cpg >= 8) {
+            s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
+            s2 += __shfl_xor_sync(0xffffffffu, s2, 2);
+          }
+          const int c = c_base + g * 8;   // first channel of the chunk (warp-uniform)
+          if (g * 8 >= ncols || c >= p.Cout) continue;
+          if (cpg <= 8) {       // lanes 0 (and 2 when cpg == 4) hold the chunk's whole groups
+            if (lane == 0 || (cpg == 4 && lane == 2))
+              *reinterpret_cast<float2*>(slot + 2 * ((c + 2 * lane) / cpg)) = make_float2(s1, s2);
+          } else {
+            g1 = c % cpg ? g1 + s1 : s1;
+            g2 = c % cpg ? g2 + s2 : s2;
+            if ((c + 8) % cpg == 0 && lane == 0) *reinterpret_cast<float2*>(slot + 2 * (c / cpg)) = make_float2(g1, g2);
+          }
+        }
+      }
+      if (p.absmax) {   // atomicMax: the result does not depend on the order
+        const unsigned m = __reduce_max_sync(0xffffffffu, __float_as_uint(amax));
+        if (lane == 0 && m) atomicMax(p.absmax + n, m);
+        amax = 0.f;
+      }
+    }
   }
-  if (p.stats) flush_stats();
-  if (kF16 && p.absmax) {
+  if (!kOrdered && p.stats) flush_stats();
+  if (!kOrdered && kF16 && p.absmax) {
     // non-negative floats order like their bit patterns
     const unsigned m = __reduce_max_sync(0xffffffffu, __float_as_uint(amax));
     if (lane == 0 && m) atomicMax(p.absmax, m);
@@ -273,29 +322,45 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_consta
 typedef void (*ConvKernel)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const ConvParams);
 
 // the instantiated wgmma widths: bf16 (n_pass 1 / 3) BN in {16, 32, 64, 128, 256}; fp16x2 2*BN in {32, 64, ..., 256}
-static ConvKernel conv_kernel_for(int NI, bool f16, int* variant) {
-#define LWM_CONV_CASE(n, f, idx) \
-  if (NI == n && f16 == f) {     \
-    *variant = idx;              \
-    return conv_wgmma_kernel<n, f>; \
+// the ordered instances: fp16x2 only
+static ConvKernel conv_kernel_for(int NI, bool f16, bool ordered, int* variant) {
+#define LWM_CONV_CASE(n, f, o, idx)             \
+  if (NI == n && f16 == f && ordered == o) {    \
+    *variant = idx;                             \
+    return conv_wgmma_kernel<n, f, o>;          \
   }
-  LWM_CONV_CASE(16, false, 0) LWM_CONV_CASE(32, false, 1) LWM_CONV_CASE(64, false, 2) LWM_CONV_CASE(128, false, 3)
-  LWM_CONV_CASE(256, false, 4)
-  LWM_CONV_CASE(32, true, 5) LWM_CONV_CASE(64, true, 6) LWM_CONV_CASE(96, true, 7) LWM_CONV_CASE(128, true, 8)
-  LWM_CONV_CASE(160, true, 9) LWM_CONV_CASE(192, true, 10) LWM_CONV_CASE(224, true, 11) LWM_CONV_CASE(256, true, 12)
+  LWM_CONV_CASE(16, false, false, 0) LWM_CONV_CASE(32, false, false, 1) LWM_CONV_CASE(64, false, false, 2)
+  LWM_CONV_CASE(128, false, false, 3) LWM_CONV_CASE(256, false, false, 4)
+  LWM_CONV_CASE(32, true, false, 5) LWM_CONV_CASE(64, true, false, 6) LWM_CONV_CASE(96, true, false, 7)
+  LWM_CONV_CASE(128, true, false, 8) LWM_CONV_CASE(160, true, false, 9) LWM_CONV_CASE(192, true, false, 10)
+  LWM_CONV_CASE(224, true, false, 11) LWM_CONV_CASE(256, true, false, 12)
+  LWM_CONV_CASE(32, true, true, 13) LWM_CONV_CASE(64, true, true, 14) LWM_CONV_CASE(96, true, true, 15)
+  LWM_CONV_CASE(128, true, true, 16) LWM_CONV_CASE(160, true, true, 17) LWM_CONV_CASE(192, true, true, 18)
+  LWM_CONV_CASE(224, true, true, 19) LWM_CONV_CASE(256, true, true, 20)
 #undef LWM_CONV_CASE
   return nullptr;
 }
-constexpr int kConvVariants = 13;
+constexpr int kConvVariants = 21;
 
 }  // namespace lwm
 
 using namespace lwm;
 
+int lwm_vq_gn_finalize(const float* part, double* stats, int N, int P, int cols, cudaStream_t st);   // vq_elementwise.cu
+
+// fp16x2 stacks hi|lo: the wgmma is 2*BN wide -> BN = largest multiple of 16 <= 128 dividing Cout_pad
+static int f16_tile_n(int Cout_pad) {
+  int BN;
+  for (BN = 128; BN >= 16; BN -= 16)
+    if (Cout_pad % BN == 0) break;
+  return BN;
+}
+
 static int conv_launch(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo, const float* bias,
                        const float* residual, float* out, int N, int Hin, int Win, int Cpad, int Ho, int Wo, int Cout,
                        int Cout_pad, int ksize, int stride, int pad, int n_pass, int clip, float w_scale_inv,
-                       const float* a_scale, double* stats, unsigned* absmax, int groups, void* stream) {
+                       const float* a_scale, double* stats, unsigned* absmax, int groups, void* stream,
+                       bool ordered = false, float* part = nullptr, long long part_bytes = 0) {
   if (!a_hi || !w_hi || !bias || !out) return lwm_fail(LWM_ERR_ARG, "vq_conv2d: null pointer");
   if (n_pass < 1 || n_pass > 3) return lwm_fail(LWM_ERR_ARG, "vq_conv2d: n_pass must be 1 (bf16), 2 (fp16x2) or 3 (bf16x3)");
   if (n_pass == 3 && (!a_lo || !w_lo)) return lwm_fail(LWM_ERR_ARG, "vq_conv2d: n_pass=3 needs the lo planes");
@@ -306,11 +371,21 @@ static int conv_launch(const void* a_hi, const void* a_lo, const void* w_hi, con
     return lwm_fail(LWM_ERR_SHAPE, "vq_conv2d: output statistics need Cout % 16 == 0 and (Cout/groups) % 4 == 0, groups <= 64");
   if (stats && n_pass != 2)
     return lwm_fail(LWM_ERR_ARG, "vq_conv2d: output statistics are an epilogue of the fp16x2 scheme (N tile <= 128)");
+  const long long m_tiles = (long long)N * (Ho / 8) * (Wo / 16);
+  if (ordered && stats) {
+    // a group's channels lie in one 8-channel chunk (cpg 4) or in whole chunks of one N tile
+    const int cpg = Cout / groups, bn = f16_tile_n(Cout_pad);
+    if (cpg != 4 && (cpg % 8 || bn % cpg))
+      return lwm_fail(LWM_ERR_SHAPE, "vq_conv2d_f16_ordered: ordered statistics need Cout/groups == 4, or a multiple of 8 "
+                                     "that divides the N tile");
+    if (!part) return lwm_fail(LWM_ERR_ARG, "vq_conv2d_f16_ordered: output statistics need the workspace");
+    if (part_bytes < m_tiles * 8 * groups * 2 * (long long)sizeof(float))
+      return lwm_fail(LWM_ERR_SHAPE, "vq_conv2d_f16_ordered: workspace too small (N * Ho/8 * Wo/16 * 8 * groups * 2 floats)");
+  }
   if (!lwm_check_device()) return LWM_ERR_DEVICE;
   int BN = Cout_pad;
-  if (n_pass == 2) {      // fp16x2 stacks hi|lo: the wgmma is 2*BN wide -> BN = largest multiple of 16 <= 128 dividing Cout_pad
-    for (BN = 128; BN >= 16; BN -= 16)
-      if (Cout_pad % BN == 0) break;
+  if (n_pass == 2) {
+    BN = f16_tile_n(Cout_pad);
   } else {
     if (Cout_pad > 256 && Cout_pad % 128)
       return lwm_fail(LWM_ERR_SHAPE, "vq_conv2d: Cout_pad > 256 must be a multiple of 128");
@@ -318,7 +393,7 @@ static int conv_launch(const void* a_hi, const void* a_lo, const void* w_hi, con
       if (Cout_pad % BN == 0) break;
   }
   int variant = 0;
-  const ConvKernel kern = conv_kernel_for(n_pass == 2 ? 2 * BN : BN, n_pass == 2, &variant);
+  const ConvKernel kern = conv_kernel_for(n_pass == 2 ? 2 * BN : BN, n_pass == 2, ordered, &variant);
   if (!kern) return lwm_fail(LWM_ERR_SHAPE, "vq_conv2d: no kernel for this N tile");
   const int taps = ksize * ksize;
   const CUtensorMapDataType dt = n_pass == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
@@ -351,7 +426,8 @@ static int conv_launch(const void* a_hi, const void* a_lo, const void* w_hi, con
   p.taps_w = ksize; p.taps = taps; p.stride = stride; p.pad = pad;
   p.BN = BN; p.n_tiles = Cout_pad / BN; p.n_pass = n_pass;
   p.bias = bias; p.residual = residual; p.out = out; p.clip = clip;
-  p.w_scale_inv = w_scale_inv; p.a_scale = a_scale; p.stats = stats; p.absmax = absmax; p.groups = groups;
+  p.w_scale_inv = w_scale_inv; p.a_scale = a_scale; p.stats = ordered ? nullptr : stats; p.absmax = absmax;
+  p.groups = groups; p.part = ordered && stats ? part : nullptr;
   const int stage_bytes = (n_pass == 3 ? 2 : 1) * (kATile + wrows * BN * 128);
   int stages = (227 * 1024 - 2048) / stage_bytes;
   if (stages > 6) stages = 6;
@@ -369,8 +445,13 @@ static int conv_launch(const void* a_hi, const void* a_lo, const void* w_hi, con
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int total_tiles = N * (Ho / 8) * (Wo / 16) * p.n_tiles;
   const int grid = total_tiles < sms ? total_tiles : sms;
-  kern<<<grid, kConvThreads, smem_bytes, reinterpret_cast<cudaStream_t>(stream)>>>(tAh, tAl, tBh, tBl, p);
-  return lwm_check_launch("conv_wgmma_kernel");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (ordered && absmax && cudaMemsetAsync(absmax, 0, sizeof(unsigned) * N, st) != cudaSuccess)
+    return lwm_fail(LWM_ERR_CUDA, "vq_conv2d_f16_ordered: memset failed");
+  kern<<<grid, kConvThreads, smem_bytes, st>>>(tAh, tAl, tBh, tBl, p);
+  const int status = lwm_check_launch("conv_wgmma_kernel");
+  if (status != LWM_OK || !p.part) return status;
+  return lwm_vq_gn_finalize(p.part, stats, N, int(m_tiles / N) * 8, groups * 2, st);
 }
 
 // a_hi/a_lo: [N,Hin,Win,Cpad] bf16 planes; w_hi/w_lo: [taps][Cout_pad][Cpad] bf16; out/residual fp32 NHWC.
@@ -395,4 +476,20 @@ extern "C" int lwm_vq_conv2d_f16(const void* a, const float* a_scale, const void
   if (!(w_scale_inv > 0.f)) return lwm_fail(LWM_ERR_ARG, "vq_conv2d_f16: w_scale_inv must be positive");
   return conv_launch(a, nullptr, w_stacked, nullptr, bias, residual, out, N, Hin, Win, Cpad, Ho, Wo, Cout, Cout_pad,
                      ksize, stride, pad, 2, clip, w_scale_inv, a_scale, gn_stats_out, absmax_out, groups, stream);
+}
+
+// lwm_vq_conv2d_f16 whose result does not depend on the batch or the run: a_scale [N] (one scale per image, NULL = 1),
+// absmax_out [N] (zeroed here), and gn_stats_out [N, groups, 2] double summed in a fixed order from per-(tile, warp)
+// partials in `workspace` (N * Ho/8 * Wo/16 * 8 * groups * 2 floats).
+extern "C" int lwm_vq_conv2d_f16_ordered(const void* a, const float* a_scale, const void* w_stacked, const float* bias,
+                                         const float* residual, float* out, double* gn_stats_out, float* workspace,
+                                         long long workspace_bytes, unsigned* absmax_out, int N, int Hin, int Win,
+                                         int Cpad, int Ho, int Wo, int Cout, int Cout_pad, int ksize, int stride,
+                                         int pad, float w_scale_inv, int groups, int clip, void* stream) {
+  if (!(w_scale_inv > 0.f)) return lwm_fail(LWM_ERR_ARG, "vq_conv2d_f16_ordered: w_scale_inv must be positive");
+  if (N <= 0 || Hin <= 0 || Win <= 0 || Ho <= 0 || Wo <= 0 || Cout <= 0)
+    return lwm_fail(LWM_ERR_SHAPE, "vq_conv2d_f16_ordered: empty tensor");
+  return conv_launch(a, nullptr, w_stacked, nullptr, bias, residual, out, N, Hin, Win, Cpad, Ho, Wo, Cout, Cout_pad,
+                     ksize, stride, pad, 2, clip, w_scale_inv, a_scale, gn_stats_out, absmax_out, groups, stream, true,
+                     workspace, workspace_bytes);
 }

@@ -1,6 +1,7 @@
 // HBM-bound pieces of the VQGAN tokenizer (lwm/vqgan.py), NHWC fp32 activations:
 //   lwm_vq_gn_stats   per-(sample, group) sum and sum of squares for flax nn.GroupNorm() (32 groups,
-//                     statistics over H,W,C/32 — vqgan.py:161,181,251,254)
+//                     statistics over H,W,C/32 — vqgan.py:161,181,251,254); lwm_vq_gn_stats_ordered sums them in an
+//                     order fixed by (H, W, C) alone (torch.use_deterministic_algorithms)
 //   lwm_vq_prep       GroupNorm-apply + SiLU (vqgan.py:251-256) and/or nearest 2x upsampling
 //                     (vqgan.py:312-316) fused with the conversion of the activation into the
 //                     tensor-core operand planes (bf16 hi, bf16 lo = x - hi) the conv kernel reads by TMA
@@ -50,6 +51,74 @@ __global__ void gn_stats_kernel(const float* __restrict__ x, double* __restrict_
     atomicAdd(&stats[((size_t)n * groups) * 2 + i], (double)s_part[i]);
 }
 
+// Ordered variant: block = kGnOrderedPix pixels of one image (a partition fixed by H, W and the block size, which depends
+// on C only); the per-thread sums are added in a fixed order per group and written to part[n][block][group][2].
+constexpr int kGnOrderedPix = 128;
+
+__global__ void gn_stats_partial_kernel(const float* __restrict__ x, float* __restrict__ part, int HW, int C,
+                                        int groups) {
+  extern __shared__ float2 s_red[];   // [blockDim.x] (sum, sumsq) of each thread
+  const int n = blockIdx.y;
+  const int quads = C / 4;
+  const int q = threadIdx.x % quads;
+  const int prow = threadIdx.x / quads;
+  const int prows = blockDim.x / quads;
+  const int p0 = blockIdx.x * kGnOrderedPix;
+  const int p1 = min(HW, p0 + kGnOrderedPix);
+  float s = 0.f, ss = 0.f;
+  const float4* base = reinterpret_cast<const float4*>(x + (size_t)n * HW * C) + q;
+  for (int p = p0 + prow; p < p1; p += prows) {
+    const float4 v = base[(size_t)p * quads];
+    s += (v.x + v.y) + (v.z + v.w);
+    ss += (v.x * v.x + v.y * v.y) + (v.z * v.z + v.w * v.w);
+  }
+  s_red[threadIdx.x] = make_float2(s, ss);
+  __syncthreads();
+  const int qpg = C / groups / 4;   // channel quads per group
+  for (int g = threadIdx.x; g < groups; g += blockDim.x) {
+    float a = 0.f, b = 0.f;
+    for (int r = 0; r < prows; ++r)
+      for (int qq = g * qpg; qq < (g + 1) * qpg; ++qq) {
+        const float2 t = s_red[r * quads + qq];
+        a += t.x;
+        b += t.y;
+      }
+    reinterpret_cast<float2*>(part)[((size_t)n * gridDim.x + blockIdx.x) * groups + g] = make_float2(a, b);
+  }
+}
+
+// stats[n][j] = sum over p of part[n][p][j] in double (j = 2 * group + {0: sum, 1: sumsq}), in a fixed order: thread
+// (r, j) adds rows r, r + 16, ... in ascending order, then thread (0, j) adds the 16 row sums in ascending r.
+__global__ void __launch_bounds__(512) gn_finalize_kernel(const float* __restrict__ part, double* __restrict__ stats,
+                                                          int P, int cols) {
+  __shared__ double s_row[16][32];
+  const int n = blockIdx.y, lane = threadIdx.x & 31, r = threadIdx.x >> 5;
+  const int j = blockIdx.x * 32 + lane;
+  double t = 0.0;
+  if (j < cols)
+    for (int i = r; i < P; i += 16) t += (double)part[((size_t)n * P + i) * cols + j];
+  s_row[r][lane] = t;
+  __syncthreads();
+  if (r == 0 && j < cols) {
+    double sum = 0.0;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) sum += s_row[i][lane];
+    stats[(size_t)n * cols + j] = sum;
+  }
+}
+
+// |x| max of each image's finite elements (n4 float4s per image) as raw bits: atomicMax into out_bits[n]
+__global__ void absmax_per_image_kernel(const uint4* __restrict__ x, long long n4, unsigned* __restrict__ out_bits) {
+  const uint4* xi = x + (size_t)blockIdx.y * n4;
+  unsigned m = 0;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
+    const uint4 v = xi[i];
+    m = max(max(m, finite_abs_bits(v.x)), max(finite_abs_bits(v.y), max(finite_abs_bits(v.z), finite_abs_bits(v.w))));
+  }
+  m = __reduce_max_sync(0xffffffffu, m);
+  if ((threadIdx.x & 31) == 0 && m) atomicMax(out_bits + blockIdx.y, m);
+}
+
 // ------------------------------------------------------------------------------------------------
 // prep: y = [silu(gn(x))] at (h>>up, w>>up); hi = bf16(y); lo = bf16(y - hi). Output planes have
 // C_pad >= C channels (multiple of 64 for the conv's 128-byte TMA rows); padding channels are zero.
@@ -64,7 +133,18 @@ __global__ void gn_stats_kernel(const float* __restrict__ x, double* __restrict_
 //                 (sample, group), n_g the group's element count (|x - mean| <= |x| + |mean| and x^2 <= n_g E[x^2]).
 //                 Every block derives the same bound B from the statistics; s = 1 while B lies in [1, 2^13), which
 //                 is every ordinary layer, and otherwise the power of two that brings B into that range.
-template <bool kF16>
+// kPerImage (with kF16): one scale per sample, scale_out[n], from sample n's own |x|max (absmax_bits[n]) or its own
+// groups' bound, so that no sample's plane depends on the others in the batch.
+__device__ __forceinline__ int gn_plane_shift(float bound) {   // s = 2^shift brings bound into [1, 2^13)
+  const unsigned bits = __float_as_uint(bound);
+  const int e = max(int((bits >> 23) & 0xffu) - 127, -114);
+  return bits ? min(e, 0) + max(e - 12, 0) : 0;
+}
+__device__ __forceinline__ int absmax_plane_shift(unsigned bits) {   // the largest |x| lands in [2^12, 2^13)
+  return bits ? max(int((bits >> 23) & 0xffu) - 127, -114) - 12 : 0;
+}
+
+template <bool kF16, bool kPerImage>
 __global__ void prep_kernel(const float* __restrict__ x, const double* __restrict__ stats,
                             const float* __restrict__ gamma, const float* __restrict__ beta,
                             __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo, int N, int H, int W,
@@ -73,7 +153,9 @@ __global__ void prep_kernel(const float* __restrict__ x, const double* __restric
   // one thread = 8 channels of one output pixel: 2 x 16 B loads, 16 B stores per plane.
   // (mean, rstd) of every (sample, group) are derived once per block from the float64 sums into shared memory: the
   // element loop is then pure fp32 (FFMA + 2 MUFU per element), no float64 arithmetic per quad.
-  extern __shared__ float s_mr[];    // [N*groups][2]
+  extern __shared__ float s_mr[];    // [N*groups][2] (with GroupNorm), then kPerImage: s_inv [N], s_bnd [N]
+  float* s_inv = s_mr + (stats ? 2 * N * groups : 0);   // kPerImage: 1 / scale of each sample
+  unsigned* s_bnd = reinterpret_cast<unsigned*>(s_inv + N);   // kPerImage: bit pattern of each sample's group bound
   const int Ho = H << up, Wo = W << up;
   const int octs = C_pad / 8;
   const size_t total = (size_t)N * Ho * Wo * octs;
@@ -82,6 +164,8 @@ __global__ void prep_kernel(const float* __restrict__ x, const double* __restric
                                      // (sqrt(n_g E[x^2]) + |mean|) * rstd, of max|gamma| and of max|beta|
   if (stats) {
     if (kF16 && threadIdx.x < 3) s_bound[threadIdx.x] = 0u;
+    if constexpr (kPerImage)
+      for (int i = threadIdx.x; i < N; i += blockDim.x) s_bnd[i] = 0u;
     if (kF16) __syncthreads();
     const double inv_cnt = 1.0 / ((double)H * W * cpg);
     const float n_g = float((double)H * W * cpg);
@@ -95,7 +179,10 @@ __global__ void prep_kernel(const float* __restrict__ x, const double* __restric
       s_mr[2 * i + 1] = rsqrtf(var + eps);
       // finite terms only: a (sample, group) with non-finite statistics has a non-finite plane at any scale, and must
       // not flush the planes of the other samples to zero
-      if (kF16) dev_max = fmaxf(dev_max, finite_absf((sqrtf(n_g * msq) + fabsf(mean)) * s_mr[2 * i + 1]));
+      if constexpr (kPerImage)
+        atomicMax(s_bnd + i / groups, __float_as_uint(finite_absf((sqrtf(n_g * msq) + fabsf(mean)) * s_mr[2 * i + 1])));
+      else if (kF16)
+        dev_max = fmaxf(dev_max, finite_absf((sqrtf(n_g * msq) + fabsf(mean)) * s_mr[2 * i + 1]));
     }
     if (kF16) {
       float g_max = 0.f, b_max = 0.f;
@@ -116,17 +203,19 @@ __global__ void prep_kernel(const float* __restrict__ x, const double* __restric
     __syncthreads();
   }
   float inv_scale = 1.f;   // kF16: 1 / s
-  if constexpr (kF16) {
-    int shift;             // s = 2^shift
-    if (stats) {
-      const float bound = __uint_as_float(s_bound[1]) * __uint_as_float(s_bound[0]) + __uint_as_float(s_bound[2]);
-      const unsigned bits = __float_as_uint(bound);
-      const int e = max(int((bits >> 23) & 0xffu) - 127, -114);
-      shift = bits ? min(e, 0) + max(e - 12, 0) : 0;
-    } else {
-      const unsigned bits = *absmax_bits;
-      shift = bits ? max(int((bits >> 23) & 0xffu) - 127, -114) - 12 : 0;
+  if constexpr (kPerImage) {
+    for (int i = threadIdx.x; i < N; i += blockDim.x) {
+      const int shift = stats ? gn_plane_shift(__uint_as_float(s_bound[1]) * __uint_as_float(s_bnd[i]) +
+                                               __uint_as_float(s_bound[2]))
+                              : absmax_plane_shift(absmax_bits[i]);
+      s_inv[i] = __uint_as_float(unsigned(127 - shift) << 23);
+      if (blockIdx.x == 0) scale_out[i] = __uint_as_float(unsigned(127 + shift) << 23);
     }
+    __syncthreads();
+  } else if constexpr (kF16) {
+    const int shift =      // s = 2^shift
+        stats ? gn_plane_shift(__uint_as_float(s_bound[1]) * __uint_as_float(s_bound[0]) + __uint_as_float(s_bound[2]))
+              : absmax_plane_shift(*absmax_bits);
     inv_scale = __uint_as_float(unsigned(127 - shift) << 23);
     if (blockIdx.x == 0 && threadIdx.x == 0) *scale_out = __uint_as_float(unsigned(127 + shift) << 23);
   }
@@ -165,8 +254,9 @@ __global__ void prep_kernel(const float* __restrict__ x, const double* __restric
     uint32_t h4[4], l4[4];
     const size_t o = (((size_t)n * Ho + ho) * Wo + wo) * C_pad + c0;
     if constexpr (kF16) {
+      const float inv = kPerImage ? s_inv[n] : inv_scale;
 #pragma unroll
-      for (int e = 0; e < 4; ++e) h4[e] = pack_f16x2(y[2 * e] * inv_scale, y[2 * e + 1] * inv_scale);
+      for (int e = 0; e < 4; ++e) h4[e] = pack_f16x2(y[2 * e] * inv, y[2 * e + 1] * inv);
       *reinterpret_cast<uint4*>(hi + o) = make_uint4(h4[0], h4[1], h4[2], h4[3]);
     } else {
 #pragma unroll
@@ -386,6 +476,34 @@ extern "C" int lwm_vq_gn_stats(const float* x, double* stats, int N, int H, int 
   return lwm_check_launch("gn_stats_kernel");
 }
 
+// the statistics [N, cols / 2, 2] of per-image partials part [N][P][cols] (lwm_vq_gn_stats_ordered, and
+// lwm_vq_conv2d_f16_ordered's epilogue)
+int lwm_vq_gn_finalize(const float* part, double* stats, int N, int P, int cols, cudaStream_t st) {
+  gn_finalize_kernel<<<dim3((cols + 31) / 32, N), 512, 0, st>>>(part, stats, P, cols);
+  return lwm_check_launch("gn_finalize_kernel");
+}
+
+extern "C" int lwm_vq_gn_stats_ordered(const float* x, double* stats, float* workspace, long long workspace_bytes,
+                                       int N, int H, int W, int C, int groups, void* stream) {
+  if (!x || !stats || !workspace) return lwm_fail(LWM_ERR_ARG, "vq_gn_stats_ordered: null pointer");
+  if (N <= 0 || H <= 0 || W <= 0 || groups <= 0 || C % groups || (C / groups) % 4 || C > 4096)
+    return lwm_fail(LWM_ERR_SHAPE, "vq_gn_stats_ordered: C/groups must be a multiple of 4, C <= 4096, non-empty");
+  const long long HW = (long long)H * W;
+  const long long P = (HW + kGnOrderedPix - 1) / kGnOrderedPix;
+  if (HW > (1ll << 31) - 1) return lwm_fail(LWM_ERR_SHAPE, "vq_gn_stats_ordered: H * W exceeds int32");
+  if (workspace_bytes < (long long)N * P * groups * 2 * (long long)sizeof(float))
+    return lwm_fail(LWM_ERR_SHAPE, "vq_gn_stats_ordered: workspace too small (N * ceil(H*W/128) * groups * 2 floats)");
+  if (!lwm_check_device()) return LWM_ERR_DEVICE;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int quads = C / 4;
+  int threads = ((512 / quads) > 0 ? (512 / quads) : 1) * quads;   // whole pixel rows per block: a function of C
+  if (threads > 1024) threads = quads;
+  gn_stats_partial_kernel<<<dim3(unsigned(P), N), threads, threads * sizeof(float2), st>>>(x, workspace, int(HW), C,
+                                                                                            groups);
+  const int status = lwm_check_launch("gn_stats_partial_kernel");
+  return status != LWM_OK ? status : lwm_vq_gn_finalize(workspace, stats, N, int(P), groups * 2, st);
+}
+
 extern "C" int lwm_vq_prep(const float* x, const double* gn_stats, const float* gamma, const float* beta, void* hi,
                            void* lo, int N, int H, int W, int C, int C_pad, int groups, int upsample2x, float eps,
                            void* stream) {
@@ -399,7 +517,7 @@ extern "C" int lwm_vq_prep(const float* x, const double* gn_stats, const float* 
   const int threads = 256;
   const size_t want = (total + threads - 1) / threads;
   const unsigned blocks = unsigned(want < kNumSMs * 32 ? want : kNumSMs * 32);
-  prep_kernel<false><<<blocks, threads, gn_stats ? size_t(N) * groups * 8 : 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+  prep_kernel<false, false><<<blocks, threads, gn_stats ? size_t(N) * groups * 8 : 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       x, gn_stats, gamma, beta, reinterpret_cast<__nv_bfloat16*>(hi), reinterpret_cast<__nv_bfloat16*>(lo), N, H, W,
       C, C_pad, groups, upsample2x ? 1 : 0, eps, lo != nullptr, nullptr, nullptr);
   return lwm_check_launch("prep_kernel");
@@ -430,10 +548,44 @@ extern "C" int lwm_vq_prep_f16(const float* x, const double* gn_stats, const flo
   const int threads = 256;
   const size_t want = (total + threads - 1) / threads;
   const unsigned blocks = unsigned(want < kNumSMs * 32 ? want : kNumSMs * 32);
-  prep_kernel<true><<<blocks, threads, gn_stats ? size_t(N) * groups * 8 : 0, st>>>(
+  prep_kernel<true, false><<<blocks, threads, gn_stats ? size_t(N) * groups * 8 : 0, st>>>(
       x, gn_stats, gamma, beta, reinterpret_cast<__nv_bfloat16*>(out), nullptr, N, H, W, C, C_pad, groups,
       upsample2x ? 1 : 0, eps, 0, x_absmax, scale_out);
   return lwm_check_launch("prep_kernel<f16>");
+}
+
+// lwm_vq_prep_f16 with one scale per sample: scale_out [N], x_absmax [N] (each sample's |x|max bits; computed here into
+// it unless x_absmax_given, e.g. lwm_vq_conv2d_f16_ordered's absmax_out).
+extern "C" int lwm_vq_prep_f16_ordered(const float* x, const double* gn_stats, const float* gamma, const float* beta,
+                                       void* out, float* scale_out, unsigned* x_absmax, int x_absmax_given, int N, int H,
+                                       int W, int C, int C_pad, int groups, int upsample2x, float eps, void* stream) {
+  if (!x || !out || !scale_out) return lwm_fail(LWM_ERR_ARG, "vq_prep_f16_ordered: null pointer");
+  if (!gn_stats && !x_absmax) return lwm_fail(LWM_ERR_ARG, "vq_prep_f16_ordered: the plane without GroupNorm needs x_absmax");
+  if (N <= 0 || H <= 0 || W <= 0) return lwm_fail(LWM_ERR_SHAPE, "vq_prep_f16_ordered: empty tensor");
+  if (C % 4 || C_pad % 8 || C_pad < C) return lwm_fail(LWM_ERR_SHAPE, "vq_prep_f16_ordered: C % 4 and C_pad % 8 required");
+  if (gn_stats && (!gamma || !beta || groups <= 0 || C % groups || (C / groups) % 4))
+    return lwm_fail(LWM_ERR_SHAPE, "vq_prep_f16_ordered: GroupNorm needs gamma/beta and C/groups % 4 == 0");
+  const size_t smem = (gn_stats ? size_t(N) * groups * 8 : 0) + size_t(N) * 8;
+  if (smem > 40 * 1024) return lwm_fail(LWM_ERR_SHAPE, "vq_prep_f16_ordered: N (* groups) too large for the block's tables");
+  if (!lwm_check_device()) return LWM_ERR_DEVICE;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (!gn_stats && !x_absmax_given) {
+    if (cudaMemsetAsync(x_absmax, 0, sizeof(unsigned) * N, st) != cudaSuccess)
+      return lwm_fail(LWM_ERR_CUDA, "vq_prep_f16_ordered: memset failed");
+    const long long n4 = (long long)H * W * C / 4;
+    const long long want4 = (n4 + 255) / 256, cap = kNumSMs * 8 / N;   // atomicMax: any grid gives the same bits
+    const long long per_image = want4 < cap ? want4 : cap;
+    absmax_per_image_kernel<<<dim3(unsigned(per_image > 0 ? per_image : 1), N), 256, 0, st>>>(
+        reinterpret_cast<const uint4*>(x), n4, x_absmax);
+  }
+  const size_t total = (size_t)N * (H << upsample2x) * (W << upsample2x) * (C_pad / 8);
+  const int threads = 256;
+  const size_t want = (total + threads - 1) / threads;
+  const unsigned blocks = unsigned(want < kNumSMs * 32 ? want : kNumSMs * 32);
+  prep_kernel<true, true><<<blocks, threads, smem, st>>>(
+      x, gn_stats, gamma, beta, reinterpret_cast<__nv_bfloat16*>(out), nullptr, N, H, W, C, C_pad, groups,
+      upsample2x ? 1 : 0, eps, 0, x_absmax, scale_out);
+  return lwm_check_launch("prep_kernel<f16, per image>");
 }
 
 extern "C" int lwm_vq_conv_cin3(const float* x, const float* w_hwio, const float* bias, float* y, int N, int H, int W,

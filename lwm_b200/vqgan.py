@@ -16,7 +16,12 @@ precision (the reference computes these convs in fp32):
                       1e-3 end-to-end relative error on the encoder latents, 2x the algorithmic tensor work.
   'bf16x3'            both operands split into two bf16, three MMAs: fp32-class accuracy (1e-5), 3x the tensor work.
   'bf16'              single pass (≈1e-2 end-to-end relative error, 99.6 % code agreement on synthetic weights).
+
+Under torch.use_deterministic_algorithms(True), every mode runs the ordered entry points (lwm_vq_*_ordered): GroupNorm
+statistics summed in a fixed order and one fp16 plane scale per image, so that a frame's latents, codes and pixels are
+the same bits on every run and whatever batch or video it is encoded in.
 """
+import contextlib
 import pickle
 
 import numpy as np
@@ -162,10 +167,21 @@ class Ops:
         if precision not in ("fp16x2", "bf16x3", "bf16"):
             raise ValueError("precision must be 'fp16x2', 'bf16x3' or 'bf16'")
         self.n_pass = {"fp16x2": 2, "bf16x3": 3, "bf16": 1}[precision]
+        # None: follow torch.are_deterministic_algorithms_enabled() at each call; VQGANModel pins it for one
+        # encode / decode, so that a producer conv and its consumer prep agree on the statistics and scale formats
+        self.ordered = None
+
+    def _ordered(self):
+        return torch.are_deterministic_algorithms_enabled() if self.ordered is None else self.ordered
 
     def gn_stats(self, x):
         N, H, W, C = x.shape
         st = torch.empty(N, GN_GROUPS, 2, dtype=torch.float64, device=x.device)
+        if self._ordered():
+            ws = torch.empty(N * -(-H * W // 128) * GN_GROUPS * 2, dtype=torch.float32, device=x.device)
+            _lib.call("lwm_vq_gn_stats_ordered", _lib.ptr(x), _lib.ptr(st), _lib.ptr(ws), ws.numel() * 4, N, H, W, C,
+                      GN_GROUPS, _lib.stream_ptr())
+            return st
         _lib.call("lwm_vq_gn_stats", _lib.ptr(x), _lib.ptr(st), N, H, W, C, GN_GROUPS, _lib.stream_ptr())
         return st
 
@@ -201,8 +217,19 @@ class Ops:
             # the plane holds y / s for a power of two s (device float, hi._plane_scale) that keeps it finite and normal
             # without GroupNorm, |x|max comes from the producing conv's epilogue when it computed one
             hi = torch.empty(N, H * s, W * s, cpad, dtype=torch.float16, device=x.device)
-            sc = torch.empty(2, dtype=torch.float32, device=x.device)        # [s, |x|max workspace]
             amax = getattr(x, "_absmax_bits", None) if gn is None else None
+            if self._ordered():       # one scale per image: hi._plane_scale [N]
+                sc = torch.empty(2, N, dtype=torch.float32, device=x.device)   # [s, |x|max workspace] per image
+                if amax is not None and amax.numel() != N:
+                    amax = None
+                _lib.call("lwm_vq_prep_f16_ordered", _lib.ptr(x), _lib.ptr(st), _lib.ptr(g), _lib.ptr(b), _lib.ptr(hi),
+                          _lib.ptr(sc[0]), _lib.ptr(sc[1] if amax is None else amax), int(amax is not None), N, H, W, C,
+                          cpad, GN_GROUPS, int(upsample), GN_EPS, _lib.stream_ptr())
+                hi._plane_scale = sc[0]
+                return hi, None
+            if amax is not None and amax.numel() != 1:
+                amax = None
+            sc = torch.empty(2, dtype=torch.float32, device=x.device)        # [s, |x|max workspace]
             _lib.call("lwm_vq_prep_f16", _lib.ptr(x), _lib.ptr(st), _lib.ptr(g), _lib.ptr(b), _lib.ptr(hi), _lib.ptr(sc),
                       _lib.ptr(sc[1:] if amax is None else amax), int(amax is not None), N, H, W, C, cpad, GN_GROUPS,
                       int(upsample), GN_EPS, _lib.stream_ptr())
@@ -224,7 +251,13 @@ class Ops:
         pad = (pc.k // 2) if stride == 1 else 0
         out = torch.empty(N, Ho, Wo, pc.cout, dtype=torch.float32, device=hi.device)
         n_pass = 2 if hi.dtype == torch.float16 else (3 if lo is not None else 1)
+        if n_pass == 2 and self._ordered():
+            return self._conv_f16_ordered(hi, pc, stride, pad, residual, out, clip, want_stats)
         if n_pass == 2:
+            a_scale = getattr(hi, "_plane_scale", None)
+            if a_scale is not None and a_scale.numel() != 1:
+                raise ValueError("this fp16 plane has one scale per image (prepared under "
+                                 "torch.use_deterministic_algorithms): it needs the ordered conv")
             st = amax = None
             if want_stats:         # |out|max too: the scale of a raw fp16 plane of this tensor (Downsample, shortcut)
                 # one zero-filled buffer: [N, groups, 2] float64 statistics, then the |max| bit pattern
@@ -232,7 +265,7 @@ class Ops:
                 amax = buf[-1:].view(torch.int32)[:1]
                 if pc.cout % 16 == 0 and pc.cout % GN_GROUPS == 0 and (pc.cout // GN_GROUPS) % 4 == 0:
                     st = buf[:-1].view(N, GN_GROUPS, 2)
-            _lib.call("lwm_vq_conv2d_f16", _lib.ptr(hi), _lib.ptr(getattr(hi, "_plane_scale", None)),
+            _lib.call("lwm_vq_conv2d_f16", _lib.ptr(hi), _lib.ptr(a_scale),
                       _lib.ptr(pc.w_stack), _lib.ptr(pc.bias), _lib.ptr(residual), _lib.ptr(out), _lib.ptr(st),
                       _lib.ptr(amax), N, Hin, Win, cpad, Ho, Wo, pc.cout, pc.cout_pad, pc.k, stride, pad,
                       pc.w_scale_inv, GN_GROUPS, int(clip), _lib.stream_ptr())
@@ -245,6 +278,30 @@ class Ops:
                   _lib.ptr(pc.w_lo if n_pass == 3 else None), _lib.ptr(pc.bias), _lib.ptr(residual),
                   _lib.ptr(out), N, Hin, Win, cpad, Ho, Wo, pc.cout, pc.cout_pad, pc.k, stride, pad, n_pass,
                   int(clip), _lib.stream_ptr())
+        return out
+
+    def _conv_f16_ordered(self, hi, pc, stride, pad, residual, out, clip, want_stats):
+        """the fp16x2 conv with a scale per image and GroupNorm statistics summed in a fixed order"""
+        N, Hin, Win, cpad = hi.shape
+        _, Ho, Wo, _ = out.shape
+        a_scale = getattr(hi, "_plane_scale", None)
+        if a_scale is not None and a_scale.numel() != N:      # one scale for the whole batch is one per image too
+            a_scale = a_scale.expand(N).contiguous()
+        st = ws = amax = None
+        if want_stats:
+            amax = torch.empty(N, dtype=torch.int32, device=hi.device)      # zeroed by the call
+            cpg = pc.cout // GN_GROUPS
+            if pc.cout % 16 == 0 and pc.cout % GN_GROUPS == 0 and (cpg == 4 or (cpg % 8 == 0 and pc.bn % cpg == 0)):
+                st = torch.empty(N, GN_GROUPS, 2, dtype=torch.float64, device=hi.device)
+                ws = torch.empty(N * (Ho // 8) * (Wo // 16) * 8 * GN_GROUPS * 2, dtype=torch.float32, device=hi.device)
+        _lib.call("lwm_vq_conv2d_f16_ordered", _lib.ptr(hi), _lib.ptr(a_scale), _lib.ptr(pc.w_stack), _lib.ptr(pc.bias),
+                  _lib.ptr(residual), _lib.ptr(out), _lib.ptr(st), _lib.ptr(ws), 0 if ws is None else ws.numel() * 4,
+                  _lib.ptr(amax), N, Hin, Win, cpad, Ho, Wo, pc.cout, pc.cout_pad, pc.k, stride, pad, pc.w_scale_inv,
+                  GN_GROUPS, int(clip), _lib.stream_ptr())
+        if st is not None:
+            out._gn_stats = st
+        if amax is not None:
+            out._absmax_bits = amax
         return out
 
     def conv_cin3(self, x, pc):
@@ -347,7 +404,25 @@ class VQGANModel:
                 h = Upsample(ops, h, blk["Upsample_0"])
         return ops.conv_gn(h, p["Conv_1"], gn=p["GroupNorm_0"], clip=True)   # clip(-1,1): vqgan.py:141
 
+    @contextlib.contextmanager
+    def _order_pinned(self):
+        """reads torch.are_deterministic_algorithms_enabled() once for the whole call (the ordered path: DESIGN.md §4)"""
+        prev = getattr(self.ops, "ordered", None)
+        self.ops.ordered = torch.are_deterministic_algorithms_enabled()
+        try:
+            yield
+        finally:
+            self.ops.ordered = prev
+
     def encode(self, pixel_values):
+        with self._order_pinned():
+            return self._encode(pixel_values)
+
+    def decode(self, encoding, is_codebook_indices=True):
+        with self._order_pinned():
+            return self._decode(encoding, is_codebook_indices)
+
+    def _encode(self, pixel_values):
         x = self._to_dev(pixel_values)
         T = None
         if x.dim() == 5:   # video [B,T,H,W,C] (vqgan.py:118-121)
@@ -361,7 +436,7 @@ class VQGANModel:
             idx = idx.reshape((-1, T) + tuple(idx.shape[1:]))
         return zq, idx
 
-    def decode(self, encoding, is_codebook_indices=True):
+    def _decode(self, encoding, is_codebook_indices):
         enc = torch.as_tensor(encoding).to(self.device)
         z = VectorQuantizer(self.ops, None, self.p["quantize"], enc) if is_codebook_indices else enc.float()
         T = None

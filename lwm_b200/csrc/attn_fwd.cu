@@ -50,6 +50,11 @@ constexpr int kFwdTileBytes = kTile * kHeadDim * 2;  // 32 KB
 constexpr int kFwdThreads = 384;  // 2 consumer warpgroups + 1 producer warpgroup (one TMA warp, 3 idle warps)
 constexpr int kFwdConsumerWarps = 8;
 constexpr int kFwdSmemBytes = (1 + kFwdStages) * kFwdTileBytes + 1024;
+// fp16 P is packed as p * 2^15 (p <= 1, so at most 32768 < 65504): normal down to p = 2^-29 instead of 2^-14. A row
+// whose max sits on a sink key ~10+ nats above the rest otherwise packs the bulk of its mass as fp16 subnormals or
+// zeros while l_run keeps it (DESIGN.md §5). The boost enters the exponent; l_run adds s * 2^-15 (= p), and the
+// epilogues fold 2^-15 into their power-of-two V factor, so m_run, l_run, the carries and lse stay in units of p.
+constexpr float kPBoostLog2 = 15.f, kPBoostInv = 1.f / 32768.f;
 
 struct FwdBarriers {
   uint64_t q_full;
@@ -288,14 +293,20 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         // rounded on its own, never fused with the first += below: l_run keeps its multiply-then-add rounding
         l_run[hh] = __fmul_rn(l_run[hh], alpha[hh]);
       }
-      const float neg_m[2] = {-m_run[0], -m_run[1]};
+      // kF16: s <- p * 2^15 through the exponent (15 - m), and l_run adds the product s * 2^-15 (exact) in the FFMA
+      // that would otherwise be an FADD. Where -m absorbs the 15 (m = kMaskedLogit), s stays p, so l_run gathers
+      // p * 2^-15 and o the unboosted P; the 2^-15 that the epilogues fold into wb / wv then scales o the same way,
+      // so o / l, every carry and every inference partial stay consistent (only such a row's lse, about -1e30 * ln 2,
+      // loses 15 * ln 2, which it cannot show).
+      const float neg_m[2] = {kF16 ? kPBoostLog2 - m_run[0] : -m_run[0], kF16 ? kPBoostLog2 - m_run[1] : -m_run[1]};
       // masked tiles hold s * scale already: fmaf(s, 1, -m) rounds exactly as s - m does
       const float mul = need_mask ? 1.0f : scale;
 #pragma unroll
       for (int i = 0; i < 64; ++i) {
         const int hh = (i >> 1) & 1;
         s[i] = ex2f(fmaf(s[i], mul, neg_m[hh]));
-        l_run[hh] += s[i];
+        if constexpr (kF16) l_run[hh] = fmaf(s[i], kPBoostInv, l_run[hh]);
+        else l_run[hh] += s[i];
       }
     };
     auto pack_p = [&]() {
@@ -373,7 +384,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       const float l_run_row = l_rows[hh];
       if (q_row >= p.Sq) continue;
       const long long pidx = (((long long)b * p.Sq + q_row) * p.H + h) * p.splits + split;
-      const float wv = *p.scale_v;   // V was stored as v16 * scale_v
+      const float wv = *p.scale_v * kPBoostInv;   // V was stored as v16 * scale_v, P as p * 2^15
 #pragma unroll
       for (int g = 0; g < kHeadDim / 8; ++g) {
         const int c = g * 8 + quad * 2;
@@ -402,7 +413,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     float wa = (m_c == -INFINITY) ? 0.f : ex2f(m_c - m_new);          // weight of the carry
     float wb = (m_run[hh] == -INFINITY) ? 0.f : ex2f(m_run[hh] - m_new);  // weight of this step
     const float l_new = wa * l_c + wb * l_run_row;
-    if (p.scale_v) wb *= *p.scale_v;   // V was stored as v16 * scale_v
+    if (p.scale_v) wb *= *p.scale_v * (kF16 ? kPBoostInv : 1.f);   // V was stored as v16 * scale_v, P as p * 2^15
     if (p.last) {
       const float inv = l_new > 0.f ? 1.0f / l_new : 0.f;
       wa *= inv;

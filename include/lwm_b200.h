@@ -121,6 +121,40 @@ int lwm_attn_bwd_step_ordered(const void* q, const void* k, const void* v, const
                               long long bias_stride, const int* segment_ids, long long seg_stride, float softmax_scale,
                               int dkv_init, const int* tiles, const int* tile_count, int* order_ws, void* stream);
 
+/* Attention dropout (the reference's blockwise_kwargs deterministic=False, attn_pdrop=p, dropout_rng): a dropped (q, k)
+ * entry is removed from the numerator and the denominator of the softmax (it takes the masked logit; no 1/(1-p)
+ * rescale), so P = 0 and dS = 0 there in the backward. A row left without a surviving key (every visible key dropped,
+ * or fully masked) writes out = 0 and an lse at the masked level (lwm_attn_bwd_lse turns it into -inf: zero gradients).
+ * The mask is regenerated from (seed, drop_threshold, b, h, GLOBAL q, GLOBAL k) in the tile kernels, never stored
+ * (lwm_b200/csrc/attn_dropout.cuh): Philox4x32-10, key (seed & 0xffffffff, seed >> 32), counter
+ * (((k >> 4) << 2) | ((k >> 1) & 3), q & ~8, h, b), the 16-bit half k & 1 of word 2 ((q >> 3) & 1) + ((k >> 3) & 1);
+ * dropped iff it is below drop_threshold = min(65535, round(p * 65536)). b is the GLOBAL batch row. The same for any
+ * ring layout, chunking, block map or executor.
+ * lwm_attn_fwd_step_dropout / lwm_attn_bwd_step_dropout: the arguments of lwm_attn_fwd_step / lwm_attn_bwd_step, then
+ *   (backward) order_ws: NULL for lwm_attn_bwd_step's unordered dQ reduction, else lwm_attn_bwd_step_ordered's,
+ *   seed (the 64-bit seed, as a signed integer), drop_threshold in [1, 65535] (0 is the plain symbol: LWM_ERR_ARG) and
+ *   batch0 >= 0, the global batch row of the call's batch row 0 (a caller that launches a slice of the batch passes
+ *   its offset, so that every batch row draws its own mask). q_pos0 and k_pos0 must be multiples of 128
+ *   (LWM_ERR_SHAPE).
+ * lwm_attn_dropout_mask: out [n_q, n_k] uint8 = the decisions (1 = dropped) of batch row b, head h, global queries
+ *   q_pos0 .. q_pos0 + n_q - 1 and keys k_pos0 .. k_pos0 + n_k - 1, from the tile kernels' device function. */
+int lwm_attn_fwd_step_dropout(const void* q, const void* k, const void* v, const float* scale_q, const float* scale_k,
+                              const float* scale_v, float* out_f32, void* out, float* lse, float* acc_o, float* acc_m,
+                              float* acc_l, int B, int H, int Sq, int Sk, int D, long long q_pos0, long long k_pos0,
+                              int causal, const float* bias, long long bias_stride, const int* segment_ids,
+                              long long seg_stride, float softmax_scale, int first, int last, const int* tiles,
+                              const int* tile_count, long long seed, unsigned drop_threshold, int batch0,
+                              void* stream);
+int lwm_attn_bwd_step_dropout(const void* q, const void* k, const void* v, const void* dout, const float* scale_q,
+                              const float* scale_k, const float* scale_v, const float* scale_do, const float* lse,
+                              const float* delta, float* dq_acc, float* dk_acc, float* dv_acc, int B, int H, int Sq,
+                              int Sk, int D, long long q_pos0, long long k_pos0, int causal, const float* bias,
+                              long long bias_stride, const int* segment_ids, long long seg_stride, float softmax_scale,
+                              int dkv_init, const int* tiles, const int* tile_count, int* order_ws, long long seed,
+                              unsigned drop_threshold, int batch0, void* stream);
+int lwm_attn_dropout_mask(long long seed, unsigned drop_threshold, int b, int h, long long q_pos0, long long k_pos0,
+                          int n_q, int n_k, unsigned char* out, void* stream);
+
 /* fp16-internal precision mode (optional): the tensor cores take bf16 x bf16 or fp16 x fp16 only, so the
  * higher-precision mode converts every operand once to an exact, power-of-two-scaled fp16 copy
  * (lwm_attn_to_f16: x16 = x / scale, scale = 2^(e-12) with e the exponent of the tensor's largest FINITE |x|,

@@ -22,6 +22,13 @@ _SIGNATURES = {
                                                          c_int, c_void_p, c_void_p, c_void_p],
     "lwm_attn_bwd_step_ordered": [c_void_p] * 13 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll,
                                                                  c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p],
+    "lwm_attn_fwd_step_dropout": [c_void_p] * 12 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll,
+                                                                 c_float, c_int, c_int, c_void_p, c_void_p, c_ll,
+                                                                 ctypes.c_uint, c_int, c_void_p],
+    "lwm_attn_bwd_step_dropout": [c_void_p] * 13 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll,
+                                                                 c_float, c_int, c_void_p, c_void_p, c_void_p, c_ll,
+                                                                 ctypes.c_uint, c_int, c_void_p],
+    "lwm_attn_dropout_mask": [c_ll, ctypes.c_uint, c_int, c_int, c_ll, c_ll, c_int, c_int, c_void_p, c_void_p],
     "lwm_attn_to_f16": [c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_void_p],
     "lwm_attn_step_tilemap": [c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_ll, c_ll, c_int]
                              + [c_void_p] * 6,

@@ -18,6 +18,7 @@
 //   * causal masking by global token position; KV tiles entirely above the diagonal are never
 //     loaded; only diagonal tiles pay for the mask.
 #include "attn_common.cuh"
+#include "attn_dropout.cuh"
 #include "tmap.h"
 #include "capi_internal.h"
 
@@ -43,6 +44,7 @@ struct FwdParams {
   int n_kt, splits;       // KV tiles of the shard; inference: CTAs per Q tile, each takes a contiguous slice of the list
   float* o_part;          // [B*Sq*H, splits, 128] un-normalised numerators (in V's units)
   float* ml_part;         // [B*Sq*H, splits, 2] (max in the log2 domain, denominator)
+  DropParams drop;        // kDrop: the attention-dropout mask (attn_dropout.cuh)
 };
 
 constexpr int kFwdStages = 4;
@@ -85,10 +87,12 @@ LWM_DEVICE float quad_sum(float x) {
 // kMap: the training step with a bias or segment ids, over the block map of lwm_attn_step_tilemap: the CTA walks its
 // Q tile's list of KV tiles (masked ones are not in it); mixed tiles run the per-element mask, clean tiles the same
 // branch with no bias or segment read (the causal compare stays). The epilogue is the training one.
-template <bool kF16, bool kInfer = false, bool kMap = false>
-__global__ void __launch_bounds__(kFwdThreads, 1)
-attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                const __grid_constant__ CUtensorMap tmV, const FwdParams p) {
+// kDrop (training instances): attention dropout. Every visited tile runs the per-element branch, which gives a dropped
+// entry the masked logit; a row left without a surviving key writes out = 0 and an lse at the masked level.
+// The kernel body; attn_fwd_kernel (no dropout) and attn_fwd_dropout_kernel are its entry points.
+template <bool kF16, bool kInfer, bool kMap, bool kDrop>
+__device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
+                                              const FwdParams& p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;                   // 32 KB: d [0,64) | d [64,128), 128 rows each
@@ -225,7 +229,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         mixed = e & 1;
       } else {
         k_tile_pos = p.mask.k_pos0 + j * kTile;
-        need_mask = has_bias || has_seg || (p.mask.causal && (k_tile_pos + kTile - 1 > warp_q_pos0));
+        need_mask = kDrop || has_bias || has_seg || (p.mask.causal && (k_tile_pos + kTile - 1 > warp_q_pos0));
       }
       float mx[2] = {-INFINITY, -INFINITY};
       if (!need_mask) {
@@ -268,6 +272,21 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
           q_pos[hh] = p.mask.q_pos0 + r0 + 8 * hh;
           my_seg[hh] = use_seg ? seg_row[q_pos[hh]] : 0;
         }
+        // kDrop: bit i of dropped is the decision of fragment entry i (row hh = (i >> 1) & 1, key 8 g + 2 quad + e,
+        // g = i >> 2, e = i & 1). Call t covers rows r0, r0 + 8 (q_pos[0] has bit 3 clear) and keys 16 t + 2 quad +
+        // {0, 1, 8, 9} (k_tile_pos is a multiple of 128; both checked on the host): its 8 entries are i = 8 t .. 8 t + 7,
+        // with the row picking the word pair, g & 1 the word and e the half.
+        uint64_t dropped = 0u;
+        if constexpr (kDrop) {
+#pragma unroll 1   // one call at a time: unrolled (fully, or by 2), ptxas interleaves the calls and spills
+          for (int t = 0; t < 8; ++t) {
+            const uint4 r = drop_block(p.drop, q_pos[0], k_tile_pos + 16 * t + 2 * quad, h, b);
+            uint32_t bits = 0u;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) bits |= uint32_t(drop_pick(r, (j >> 1) & 1, (j >> 2) & 1, j & 1, p.drop.thr)) << j;
+            dropped |= uint64_t(bits) << (8 * t);
+          }
+        }
 #pragma unroll
         for (int i = 0; i < 64; ++i) {
           const int hh = (i >> 1) & 1;
@@ -279,6 +298,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
           }
           if (use_seg && seg_row[k_tile_pos + col] != my_seg[hh]) tv = kMaskedLogit;
           if (p.mask.causal && k_tile_pos + col > q_pos[hh]) tv = kMaskedLogit;
+          if (kDrop && ((dropped >> i) & 1u)) tv = kMaskedLogit;
           s[i] = tv;
           mx[hh] = fmaxf(mx[hh], tv);
         }
@@ -413,6 +433,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     float wa = (m_c == -INFINITY) ? 0.f : ex2f(m_c - m_new);          // weight of the carry
     float wb = (m_run[hh] == -INFINITY) ? 0.f : ex2f(m_run[hh] - m_new);  // weight of this step
     const float l_new = wa * l_c + wb * l_run_row;
+    // kDrop: no surviving key in the whole row (its max never left the masked level): out = 0, lse at the masked level
+    const bool dead = kDrop && p.last && m_new <= kMaskedLogit;
     if (p.scale_v) wb *= *p.scale_v * (kF16 ? kPBoostInv : 1.f);   // V was stored as v16 * scale_v, P as p * 2^15
     if (p.last) {
       const float inv = l_new > 0.f ? 1.0f / l_new : 0.f;
@@ -428,6 +450,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         f.x = fmaf(a2.x, wa, f.x);
         f.y = fmaf(a2.y, wa, f.y);
       }
+      if (dead) f = make_float2(0.f, 0.f);
       if (p.last) {
         *reinterpret_cast<uint32_t*>(p.out + o_idx + c) = pack_bf16x2(f.x, f.y);
         if (p.out_f32) *reinterpret_cast<float2*>(p.out_f32 + o_idx + c) = f;
@@ -437,7 +460,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     }
     if (quad == 0) {
       if (p.last) {
-        p.lse[ml_idx] = l_new > 0.f ? (m_new + log2f(l_new)) * kLn2 : -INFINITY;
+        p.lse[ml_idx] = dead ? kMaskedLogit * kLn2 : l_new > 0.f ? (m_new + log2f(l_new)) * kLn2 : -INFINITY;
       } else {
         p.acc_m[ml_idx] = m_new;
         p.acc_l[ml_idx] = l_new;
@@ -445,6 +468,20 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     }
   }
   }
+}
+
+template <bool kF16, bool kInfer = false, bool kMap = false>
+__global__ void __launch_bounds__(kFwdThreads, 1)
+attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                const __grid_constant__ CUtensorMap tmV, const __grid_constant__ FwdParams p) {
+  attn_fwd_body<kF16, kInfer, kMap, false>(tmQ, tmK, tmV, p);
+}
+
+template <bool kF16, bool kMap>
+__global__ void __launch_bounds__(kFwdThreads, 1)
+attn_fwd_dropout_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                        const __grid_constant__ CUtensorMap tmV, const __grid_constant__ FwdParams p) {
+  attn_fwd_body<kF16, false, kMap, true>(tmQ, tmK, tmV, p);
 }
 
 static bool make_qkv_tmap(CUtensorMap* tm, const void* ptr, int B, int S, int H) {
@@ -459,14 +496,31 @@ static bool make_qkv_tmap(CUtensorMap* tm, const void* ptr, int B, int S, int H)
 
 using namespace lwm;
 
-// One ring step (include/lwm_b200.h): the scales select the fp16-operand kernel, tiles / tile_count the block map.
-extern "C" int lwm_attn_fwd_step(const void* q, const void* k, const void* v, const float* scale_q,
-                                 const float* scale_k, const float* scale_v, float* out_f32, void* out, float* lse,
-                                 float* acc_o, float* acc_m, float* acc_l, int B, int H, int Sq, int Sk, int D,
-                                 long long q_pos0, long long k_pos0, int causal, const float* bias,
-                                 long long bias_stride, const int* segment_ids, long long seg_stride,
-                                 float softmax_scale, int first, int last, const int* tiles, const int* tile_count,
-                                 void* stream) {
+template <bool kF16, bool kMap>
+static int launch_fwd_dropout(dim3 grid, cudaStream_t st, const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
+                      const FwdParams& p, const char* what) {
+  static bool attr_set_dev[64] = {};
+  int cur_dev = 0;
+  cudaGetDevice(&cur_dev);
+  bool& attr_set = attr_set_dev[cur_dev & 63];      // function attributes are per device
+  if (!attr_set) {
+    if (cudaFuncSetAttribute(attn_fwd_dropout_kernel<kF16, kMap>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             kFwdSmemBytes) != cudaSuccess)
+      return lwm_fail(LWM_ERR_CUDA, "attn_fwd: cannot raise dynamic shared memory limit");
+    attr_set = true;
+  }
+  attn_fwd_dropout_kernel<kF16, kMap><<<grid, kFwdThreads, kFwdSmemBytes, st>>>(tq, tk, tv, p);
+  return lwm_check_launch(what);
+}
+
+// One ring step (include/lwm_b200.h): the scales select the fp16-operand kernel, tiles / tile_count the block map,
+// drop (null: no dropout) the dropout instances.
+static int fwd_step(const void* q, const void* k, const void* v, const float* scale_q, const float* scale_k,
+                    const float* scale_v, float* out_f32, void* out, float* lse, float* acc_o, float* acc_m,
+                    float* acc_l, int B, int H, int Sq, int Sk, int D, long long q_pos0, long long k_pos0, int causal,
+                    const float* bias, long long bias_stride, const int* segment_ids, long long seg_stride,
+                    float softmax_scale, int first, int last, const int* tiles, const int* tile_count,
+                    const DropParams* drop, void* stream) {
   if (!scale_k != !scale_q || !scale_v != !scale_q)
     return lwm_fail(LWM_ERR_ARG, "attn_fwd: scales are all given (fp16 operands) or all null (bf16)");
   if (out_f32 && !scale_q) return lwm_fail(LWM_ERR_ARG, "attn_fwd: out_f32 needs the fp16 operand scales");
@@ -485,11 +539,15 @@ extern "C" int lwm_attn_fwd_step(const void* q, const void* k, const void* v, co
     return lwm_fail(LWM_ERR_SHAPE, "attn_fwd: bias is indexed by GLOBAL key position: bias_stride < k_pos0 + Sk");
   if (segment_ids && (seg_stride < q_pos0 + Sq || seg_stride < k_pos0 + Sk))
     return lwm_fail(LWM_ERR_SHAPE, "attn_fwd: segment_ids is indexed by GLOBAL position: seg_stride < max(q_pos0 + Sq, k_pos0 + Sk)");
+  if (drop && (q_pos0 % kTile || k_pos0 % kTile))
+    return lwm_fail(LWM_ERR_SHAPE, "attn_fwd_dropout: q_pos0 and k_pos0 must each be a multiple of 128");
+  if (drop && (B > 65535 || H > 65535 || (long long)drop->batch0 + B > 0x7fffffffLL))
+    return lwm_fail(LWM_ERR_SHAPE, "attn_fwd_dropout: B, H <= 65535 and batch0 + B < 2^31");
   if (!lwm_check_device()) return LWM_ERR_DEVICE;
   CUtensorMap tq, tk, tv;
   if (!make_qkv_tmap(&tq, q, B, Sq, H) || !make_qkv_tmap(&tk, k, B, Sk, H) || !make_qkv_tmap(&tv, v, B, Sk, H))
     return lwm_fail(LWM_ERR_CUDA, "attn_fwd: cuTensorMapEncodeTiled failed (pointers must be 16B aligned)");
-  FwdParams p;
+  FwdParams p{};
   p.B = B; p.H = H; p.Sq = Sq; p.Sk = Sk;
   p.scale_log2 = softmax_scale * kLog2e;
   p.mask.q_pos0 = int(q_pos0); p.mask.k_pos0 = int(k_pos0); p.mask.causal = causal;
@@ -502,6 +560,16 @@ extern "C" int lwm_attn_fwd_step(const void* q, const void* k, const void* v, co
   p.out_f32 = out_f32;
   p.bits = nullptr; p.tiles = tiles; p.tile_count = tile_count;
   p.n_kt = Sk / kTile; p.splits = 1;
+  if (drop) {
+    p.drop = *drop;
+    dim3 grid(Sq / kTile, H, B);
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    if (tiles)
+      return scale_q ? launch_fwd_dropout<true, true>(grid, st, tq, tk, tv, p, "attn_fwd_dropout_kernel (block map)")
+                     : launch_fwd_dropout<false, true>(grid, st, tq, tk, tv, p, "attn_fwd_dropout_kernel (block map)");
+    return scale_q ? launch_fwd_dropout<true, false>(grid, st, tq, tk, tv, p, "attn_fwd_dropout_kernel")
+                   : launch_fwd_dropout<false, false>(grid, st, tq, tk, tv, p, "attn_fwd_dropout_kernel");
+  }
   static bool attr_set_dev[64] = {};
   int cur_dev = 0;
   cudaGetDevice(&cur_dev);
@@ -528,6 +596,36 @@ extern "C" int lwm_attn_fwd_step(const void* q, const void* k, const void* v, co
   if (scale_q) attn_fwd_kernel<true><<<grid, kFwdThreads, kFwdSmemBytes, st>>>(tq, tk, tv, p);
   else attn_fwd_kernel<false><<<grid, kFwdThreads, kFwdSmemBytes, st>>>(tq, tk, tv, p);
   return lwm_check_launch("attn_fwd_kernel");
+}
+
+extern "C" int lwm_attn_fwd_step(const void* q, const void* k, const void* v, const float* scale_q,
+                                 const float* scale_k, const float* scale_v, float* out_f32, void* out, float* lse,
+                                 float* acc_o, float* acc_m, float* acc_l, int B, int H, int Sq, int Sk, int D,
+                                 long long q_pos0, long long k_pos0, int causal, const float* bias,
+                                 long long bias_stride, const int* segment_ids, long long seg_stride,
+                                 float softmax_scale, int first, int last, const int* tiles, const int* tile_count,
+                                 void* stream) {
+  return fwd_step(q, k, v, scale_q, scale_k, scale_v, out_f32, out, lse, acc_o, acc_m, acc_l, B, H, Sq, Sk, D, q_pos0,
+                  k_pos0, causal, bias, bias_stride, segment_ids, seg_stride, softmax_scale, first, last, tiles,
+                  tile_count, nullptr, stream);
+}
+
+// lwm_attn_fwd_step with attention dropout (include/lwm_b200.h)
+extern "C" int lwm_attn_fwd_step_dropout(const void* q, const void* k, const void* v, const float* scale_q,
+                                         const float* scale_k, const float* scale_v, float* out_f32, void* out,
+                                         float* lse, float* acc_o, float* acc_m, float* acc_l, int B, int H, int Sq,
+                                         int Sk, int D, long long q_pos0, long long k_pos0, int causal,
+                                         const float* bias, long long bias_stride, const int* segment_ids,
+                                         long long seg_stride, float softmax_scale, int first, int last,
+                                         const int* tiles, const int* tile_count, long long seed,
+                                         unsigned drop_threshold, int batch0, void* stream) {
+  if (drop_threshold == 0 || drop_threshold > 65535)
+    return lwm_fail(LWM_ERR_ARG, "attn_fwd_dropout: drop_threshold must be in [1, 65535] (0 is lwm_attn_fwd_step)");
+  if (batch0 < 0) return lwm_fail(LWM_ERR_ARG, "attn_fwd_dropout: batch0 must be >= 0");
+  const DropParams d = {uint32_t(uint64_t(seed)), uint32_t(uint64_t(seed) >> 32), drop_threshold, uint32_t(batch0)};
+  return fwd_step(q, k, v, scale_q, scale_k, scale_v, out_f32, out, lse, acc_o, acc_m, acc_l, B, H, Sq, Sk, D, q_pos0,
+                  k_pos0, causal, bias, bias_stride, segment_ids, seg_stride, softmax_scale, first, last, tiles,
+                  tile_count, &d, stream);
 }
 
 // Inference mode (ringattention_inference with Q >= kInferMinQ rows): q16 [B,Q,H,128], k16/v16 [B,Sk,H,128] scaled fp16

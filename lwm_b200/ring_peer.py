@@ -449,6 +449,12 @@ def _sc(table, owner, col):
     return None if table is None else table[owner, col:col + 1]
 
 
+def _batch_kw(ops, b):
+    """The steps launch one batch row at a time; with attention dropout (ops carries a `dropout`) they say which global
+    row it is, so that every batch row draws its own mask"""
+    return {"batch0": b} if getattr(ops, "dropout", None) is not None else {}
+
+
 def run_forward(plan, q, k, v, bias, seg, causal, ops, tr, want_f32=False, rope=None, rope_k=True):
     """-> (out [B,Sq,H,D] in bf16 or fp32, residuals). q/k/v: bf16 or fp32 shards (contiguous sharding).
     rope: None, or (positions int32 [B,Sq], inv_freq): q (and k when rope_k, Sq == Sk) are un-rotated and are rotated
@@ -511,7 +517,7 @@ def run_forward(plan, q, k, v, bias, seg, causal, ops, tr, want_f32=False, rope=
                                  None if a[1] is None else a[1][sl], None if a[2] is None else a[2][sl],
                                  plan.q_chunks[qi].pos0, p0, causal, None if bias is None else bias[sl],
                                  None if seg is None else seg[sl], first, last, sc,
-                                 None if out32[qi] is None else out32[qi][sl])
+                                 None if out32[qi] is None else out32[qi][sl], **_batch_kw(ops, b))
     for i in range(n_q):
         if n_launch[i] == 0:     # a chunk that sees no key at all cannot occur with Sq == Sk causal; keep it defined
             out_chunks[i].zero_()
@@ -590,7 +596,8 @@ def run_backward(plan, res, k, v, dout, bias, seg, causal, ops, tr, want_f32=Fal
                     ops.bwd_step(q_chunks[qi][sl], KG[sl, p0:p0 + rows], VG[sl, p0:p0 + rows], do_chunks[qi][sl],
                                  nlse[qi][sl], delta[qi][sl], dq_acc[qi][sl], dKG[sl, p0:p0 + rows],
                                  dVG[sl, p0:p0 + rows], plan.q_chunks[qi].pos0, p0, causal,
-                                 None if bias is None else bias[sl], None if seg is None else seg[sl], sc, init)
+                                 None if bias is None else bias[sl], None if seg is None else seg[sl], sc, init,
+                                 **_batch_kw(ops, b))
         c = g.chunks[0]
         if c.owner != r and g.launches:
             tr.wait_event("push", tr.record("main"))

@@ -16,7 +16,10 @@ Everything numeric happens in liblwm_b200.so; this file only sequences launches 
 There is no fallback: without the library / an sm_90 GPU the op raises.
 """
 import math
+import operator
 import os
+
+import numpy as np
 
 import torch
 import torch.distributed as dist
@@ -88,19 +91,50 @@ def _resolve_group(axis_name):
     return group, dist.get_rank(group), dist.get_world_size(group)
 
 
-def _check_blockwise_kwargs(kw, s_q, s_k):
+def dropout_threshold(p):
+    """attn_pdrop -> the 16-bit drop threshold of the kernels: an entry is dropped iff its Philox u16 < thr, so the
+    realised rate thr / 65536 is within 2^-17 of p. 0 means no dropout."""
+    p = float(p)
+    if not 0.0 <= p < 1.0:
+        raise ValueError("attn_pdrop must be in [0, 1), got %r" % p)
+    return min(65535, int(round(p * 65536)))
+
+
+def _dropout_of(kw, world):
+    """blockwise_kwargs -> None (no dropout) or (seed, thr) for the dropout kernels"""
+    thr = dropout_threshold(kw.get("attn_pdrop", 0.0))
+    if kw.get("deterministic", True) or thr == 0:
+        return None
+    rng = kw.get("dropout_rng")
+    if rng is None:
+        if world > 1:
+            raise ValueError("ringattention: attention dropout on a ring needs dropout_rng, an int seed passed alike on "
+                             "every rank (a seed drawn per rank could differ between them)")
+        rng = int(torch.randint(-2 ** 63, 2 ** 63 - 1, (), dtype=torch.int64))   # torch's default CPU generator
+    else:
+        try:
+            if isinstance(rng, (bool, np.bool_)) or (isinstance(rng, torch.Tensor) and rng.dtype == torch.bool):
+                raise TypeError
+            rng = operator.index(rng)       # any integer: int, numpy integers, 0-d integer tensors
+        except TypeError:
+            raise TypeError("dropout_rng must be an integer seed or None, got %s" % type(rng).__name__) from None
+    seed = int(rng) & (2 ** 64 - 1)
+    return (seed - 2 ** 64 if seed >= 2 ** 63 else seed), thr
+
+
+def _check_blockwise_kwargs(kw, s_q, s_k, world=1):
+    """-> (causal, dropout): dropout is None, or (seed, thr) when deterministic is False and attn_pdrop > 0 (the seed,
+    a signed 64-bit int, is dropout_rng, or drawn from torch's default CPU generator when that is None on one GPU)"""
     kw = dict(kw or {})
     cbs = kw.get("causal_block_size", None)
     if cbs not in (None, 1):
         raise NotImplementedError("causal_block_size must be None or 1 (lwm/llama.py:546 uses 1)")
-    if not kw.get("deterministic", True) and float(kw.get("attn_pdrop", 0.0)) > 0.0:
-        raise NotImplementedError("attention dropout is not supported (attn_pdrop is 0.0 in every LWM config)")
     for name, s in (("query_chunk_size", s_q), ("key_chunk_size", s_k)):
         c = kw.get(name)
         if c is not None and s % int(c) != 0 and s > int(c):
             raise ValueError("%s=%d must divide the per-device sequence length %d" % (name, c, s))
-    # policy / precision / prevent_cse / dropout_rng / dtype are XLA-side knobs: accepted, unused.
-    return cbs is not None
+    # policy / precision / prevent_cse / dtype are XLA-side knobs: accepted, unused.
+    return cbs is not None, _dropout_of(kw, world)
 
 
 def _prep_bias(attn_bias, B):
@@ -119,12 +153,14 @@ def _prep_bias(attn_bias, B):
 class _RingAttnFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, q, k, v, bias, seg, causal, axis_name, layout, precision, rope_pos=None, inv_freq=None,
-                rope_k=True):
+                rope_k=True, dropout=None):
         """rope_pos / inv_freq: None, or q (and k when rope_k) are un-rotated and the rotary embedding at these positions
-        (int32 [B,Sq]) is applied inside the operand staging; k and the positions are saved instead of a rotated k"""
+        (int32 [B,Sq]) is applied inside the operand staging; k and the positions are saved instead of a rotated k.
+        dropout: None or (seed, thr), kept for the backward, which regenerates the same mask"""
         group, rank, world = _resolve_group(axis_name)
         rope = None if rope_pos is None else (rope_pos, inv_freq)
-        out, res = ring_forward(q, k, v, bias, seg, causal, group, rank, world, layout, precision, rope, rope_k)
+        out, res = ring_forward(q, k, v, bias, seg, causal, group, rank, world, layout, precision, rope, rope_k,
+                                dropout=dropout)
         # residuals stay in the schedule's compute layout (zigzag chunks, operand dtype), so the backward only has
         # to permute dout on entry and dq on exit
         ctx.n_chunks = len(res["q_chunks"])
@@ -133,7 +169,7 @@ class _RingAttnFn(torch.autograd.Function):
         ctx.save_for_backward(k, v, bias, seg, rope_pos, *res["q_chunks"], *res["out_chunks"], *res["lse_chunks"],
                               *sc)
         ctx.causal, ctx.axis_name, ctx.layout, ctx.precision = causal, axis_name, layout, precision
-        ctx.inv_freq, ctx.rope_k = inv_freq, rope_k
+        ctx.inv_freq, ctx.rope_k, ctx.dropout = inv_freq, rope_k, dropout
         return out
 
     @staticmethod
@@ -148,8 +184,8 @@ class _RingAttnFn(torch.autograd.Function):
         group, rank, world = _resolve_group(ctx.axis_name)
         rope = None if rope_pos is None else (rope_pos, ctx.inv_freq)
         dq, dk, dv = ring_backward(res, k, v, dout.contiguous(), bias, seg, ctx.causal, group, rank, world,
-                                   ctx.layout, ctx.precision, rope, ctx.rope_k)
-        return dq, dk, dv, None, None, None, None, None, None, None, None, None
+                                   ctx.layout, ctx.precision, rope, ctx.rope_k, dropout=ctx.dropout)
+        return dq, dk, dv, None, None, None, None, None, None, None, None, None, None
 
 
 def _check_mask_extent(bias, seg, rank, world, Sq, Sk):
@@ -210,7 +246,14 @@ def ringattention(q, k, v, attn_bias=None, segment_ids=None, *, axis_name="sp", 
     rotate_k=False: k is already rotated (the KV cache of the generation path, written by ShardedKVCache.concatenate
     with the same keywords) and only q is rotated, at position_ids [B,Sq_loc]; Sq != Sk is allowed (the cached prefill:
     q against the whole cache). Bit-identical to ringattention(apply_rotary_emb(q, ...)[0], k, v, ...) in the same sense;
-    dK is the gradient w.r.t. k as passed, and only dQ gets the conjugate rotation."""
+    dK is the gradient w.r.t. k as passed, and only dQ gets the conjugate rotation.
+
+    Attention dropout: blockwise_kwargs=dict(deterministic=False, attn_pdrop=p, dropout_rng=seed) with 0 < p < 1, as
+    at the reference call site. A dropped (query, key) entry leaves the softmax's numerator and denominator (no 1/(1-p)
+    rescale); a row left without a surviving key outputs 0 and gets zero gradients. The mask is a function of (seed, p,
+    batch row, head, GLOBAL query and key position) only (lwm_b200/csrc/attn_dropout.cuh), regenerated inside the tile
+    kernels, so it is the same for any layout, world size or executor. dropout_rng: an int seed (pass the same one on
+    every rank of the axis group), or None on one GPU for a seed drawn from torch's default CPU generator."""
     precision = precision or _DEFAULT_PRECISION
     if precision not in ("bf16", "fp16"):
         raise ValueError("precision must be 'bf16' or 'fp16'")
@@ -227,7 +270,7 @@ def ringattention(q, k, v, attn_bias=None, segment_ids=None, *, axis_name="sp", 
     group, rank, world = _resolve_group(axis_name)
     native_f32 = in_dtype == torch.float32 and precision == "fp16" and (world == 1 or _transport(group) == "peer")
     B, Sq, H, D = q.shape
-    causal = _check_blockwise_kwargs(blockwise_kwargs, Sq, k.shape[1])
+    causal, dropout = _check_blockwise_kwargs(blockwise_kwargs, Sq, k.shape[1], world)
     if rope is not None:
         to_bf16 = in_dtype == torch.float32 and not native_f32
         if to_bf16 or not (world == 1 or _peer_ready(q, k, causal, group, rank, world, layout, precision)):
@@ -248,7 +291,7 @@ def ringattention(q, k, v, attn_bias=None, segment_ids=None, *, axis_name="sp", 
         seg = segment_ids.to(torch.int32).contiguous()
     _check_mask_extent(bias, seg, rank, world, Sq, k.shape[1])
     out = _RingAttnFn.apply(q.contiguous(), k.contiguous(), v.contiguous(), bias, seg, causal, axis_name, layout,
-                            precision, *(rope or (None, None)), rotate_k)
+                            precision, *(rope or (None, None)), rotate_k, dropout)
     return out if out.dtype == in_dtype else out.to(in_dtype)
 
 
@@ -281,19 +324,24 @@ def step_tilemap(B, Sq, Sk, q_pos0, k_pos0, causal, bias, seg, fwd=True, bwd=Tru
 
 
 def fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last,
-             stream=None, scales=None, out_f32=None, tilemap=None):
+             stream=None, scales=None, out_f32=None, tilemap=None, dropout=None):
     """scales: None (bf16 operands), or the device scales (sq, sk, sv) of fp16 operand copies q/k/v; out_f32 (fp16
     operands only): the un-rounded output, written on the last step. tilemap: None, or the forward map (tiles, counts)
     of step_tilemap for these arguments: the tile kernel then visits only the KV tiles in it (same results, bit for
-    bit)."""
+    bit). dropout: None, or (seed, thr) of attention dropout (lwm_attn_fwd_step_dropout), or (seed, thr, batch0) when
+    q ... are rows batch0 .. batch0 + B - 1 of a larger batch (each batch row draws its own mask)."""
     B, Sq, H, D = q.shape
     sq, sk, sv = scales if scales is not None else (None, None, None)
     tiles, counts = tilemap if tilemap is not None else (None, None)
-    _lib.call("lwm_attn_fwd_step", _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(sq), _lib.ptr(sk), _lib.ptr(sv),
-              _lib.ptr(out_f32), _lib.ptr(out), _lib.ptr(lse), _lib.ptr(acc_o), _lib.ptr(acc_m), _lib.ptr(acc_l), B, H,
-              Sq, k.shape[1], D, int(q_pos0), int(k_pos0), int(bool(causal)), _lib.ptr(bias),
-              0 if bias is None else bias.shape[1], _lib.ptr(seg), 0 if seg is None else seg.shape[1],
-              1.0 / math.sqrt(D), int(first), int(last), _lib.ptr(tiles), _lib.ptr(counts), _lib.stream_ptr(stream))
+    args = (_lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(sq), _lib.ptr(sk), _lib.ptr(sv), _lib.ptr(out_f32),
+            _lib.ptr(out), _lib.ptr(lse), _lib.ptr(acc_o), _lib.ptr(acc_m), _lib.ptr(acc_l), B, H, Sq, k.shape[1], D,
+            int(q_pos0), int(k_pos0), int(bool(causal)), _lib.ptr(bias), 0 if bias is None else bias.shape[1],
+            _lib.ptr(seg), 0 if seg is None else seg.shape[1], 1.0 / math.sqrt(D), int(first), int(last),
+            _lib.ptr(tiles), _lib.ptr(counts))
+    if dropout is None:
+        _lib.call("lwm_attn_fwd_step", *args, _lib.stream_ptr(stream))
+    else:
+        _lib.call("lwm_attn_fwd_step_dropout", *args, *_drop_args(dropout), _lib.stream_ptr(stream))
 
 
 def bwd_prep(out, dout, delta, stream=None, scale_do=None):
@@ -323,13 +371,14 @@ def order_workspace(words, device):
 
 
 def bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg, stream=None,
-             scales=None, init=False, tilemap=None):
+             scales=None, init=False, tilemap=None, dropout=None):
     """`lse` is the PRE-SCALED array returned by lse_for_bwd. scales: None (bf16 operands), or (sq, sk, sv, sdo) of
     fp16 operand copies q/k/v/dout. init=True: dk_acc/dv_acc rows are written, not accumulated.
     tilemap: None, or the backward map (tiles, counts) of step_tilemap for these arguments (dK, dV bit-identical; dQ
     up to the order of its reductions).
     Under torch.use_deterministic_algorithms(True) dQ is reduced in ascending key-tile order
-    (lwm_attn_bwd_step_ordered): the same bits on every run."""
+    (lwm_attn_bwd_step_ordered): the same bits on every run. dropout: None, or the forward's (seed, thr)
+    (lwm_attn_bwd_step_dropout)."""
     B, Sq, H, D = q.shape
     sq, sk, sv, sdo = scales if scales is not None else (None, None, None, None)
     tiles, counts = tilemap if tilemap is not None else (None, None)
@@ -338,8 +387,12 @@ def bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, 
             Sq, k.shape[1], D, int(q_pos0), int(k_pos0), int(bool(causal)), _lib.ptr(bias),
             0 if bias is None else bias.shape[1], _lib.ptr(seg), 0 if seg is None else seg.shape[1], 1.0 / math.sqrt(D),
             int(bool(init)), _lib.ptr(tiles), _lib.ptr(counts))
+    ws = None
     if torch.are_deterministic_algorithms_enabled():
         ws = order_workspace(2 + B * H * (Sq // 64) + (0 if tiles is None else tiles.numel()), q.device)
+    if dropout is not None:
+        _lib.call("lwm_attn_bwd_step_dropout", *args, _lib.ptr(ws), *_drop_args(dropout), _lib.stream_ptr(stream))
+    elif ws is not None:
         _lib.call("lwm_attn_bwd_step_ordered", *args, _lib.ptr(ws), _lib.stream_ptr(stream))
     else:
         _lib.call("lwm_attn_bwd_step", *args, _lib.stream_ptr(stream))
@@ -363,6 +416,17 @@ def mapped_bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k
     """bwd_step over the step's block map whenever a bias or segment ids are given"""
     bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg, **kw,
              **_map_kw(q, k, q_pos0, k_pos0, causal, bias, seg, False))
+
+
+def _drop_args(dropout):
+    """(seed, thr) or (seed, thr, batch0) -> the seed, drop_threshold and batch0 arguments of the _dropout symbols"""
+    seed, thr, batch0 = tuple(dropout) + (0,) * (3 - len(dropout))
+    return int(seed), int(thr), int(batch0)
+
+
+def _drop_kw(dropout):
+    """the `dropout` keyword of a step call: absent without dropout, so the plain call is unchanged"""
+    return {} if dropout is None else {"dropout": dropout}
 
 
 def cast_f32_to_bf16(src, dst, stream=None):
@@ -404,27 +468,55 @@ class CudaOpsF16(CudaOps):
             self._cache[key] = hit
         return hit[0], hit[1]
 
-    def fwd_step(self, q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last):
+    def fwd_step(self, q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last,
+                 dropout=None):
         (q16, sq), (k16, sk), (v16, sv) = self._f16(q), self._f16(k), self._f16(v)
         o32 = None
         if last:
             o32 = torch.empty(out.shape, dtype=torch.float32, device=out.device)
             self.out_f32[out.data_ptr()] = o32
         mapped_fwd_step(q16, k16, v16, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last,
-                        scales=(sq, sk, sv), out_f32=o32)
+                        scales=(sq, sk, sv), out_f32=o32, **_drop_kw(dropout))
 
     @staticmethod
     def lse_for_bwd(lse):
         return lse_for_bwd(lse, f16=True)
 
-    def bwd_step(self, q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg):
+    def bwd_step(self, q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg,
+                 dropout=None):
         (q16, sq), (k16, sk), (v16, sv), (d16, sd) = self._f16(q), self._f16(k), self._f16(v), self._f16(dout)
         mapped_bwd_step(q16, k16, v16, d16, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg,
-                        scales=(sq, sk, sv, sd))
+                        scales=(sq, sk, sv, sd), **_drop_kw(dropout))
+
+
+class DropoutOps:
+    """The step functions of `ops` (any of the Ops classes here, or a CPU stand-in with the same `dropout` keyword)
+    with attention dropout (seed, thr) applied in every fwd_step / bwd_step; everything else is ops' own. The ring
+    executors pass each step its global q_pos0 / k_pos0, which is all the mask depends on."""
+
+    def __init__(self, ops, dropout):
+        self.ops, self.dropout = ops, dropout
+
+    def __getattr__(self, name):
+        return getattr(self.ops, name)
+
+    def fwd_step(self, *args, batch0=0, **kw):
+        """batch0: the global batch row of the step's batch row 0, for executors that launch a slice of the batch"""
+        self.ops.fwd_step(*args, dropout=tuple(self.dropout[:2]) + (batch0,), **kw)
+
+    def bwd_step(self, *args, batch0=0, **kw):
+        self.ops.bwd_step(*args, dropout=tuple(self.dropout[:2]) + (batch0,), **kw)
+
+
+def with_dropout(ops, dropout):
+    """ops itself when dropout is None, else DropoutOps(ops, dropout)"""
+    return ops if dropout is None else DropoutOps(ops, dropout)
 
 
 def _f32_residuals(ops, res):
     """fp16 precision mode: the backward's delta = rowsum(dO o O) is taken from the un-rounded fp32 output."""
+    if isinstance(ops, DropoutOps):
+        ops = ops.ops
     if isinstance(ops, CudaOpsF16):
         res["out_chunks"] = [ops.out_f32.get(o.data_ptr(), o) for o in res["out_chunks"]]
     return res
@@ -469,9 +561,10 @@ class PeerOpsF16:
                   _lib.stream_ptr())
 
     @staticmethod
-    def fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last, scales, out_f32):
+    def fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last, scales, out_f32,
+                 dropout=None):
         mapped_fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last,
-                        scales=scales, out_f32=out_f32)
+                        scales=scales, out_f32=out_f32, **_drop_kw(dropout))
 
     @staticmethod
     def bwd_prep(out, dout, sdo, delta):
@@ -482,9 +575,10 @@ class PeerOpsF16:
         return lse_for_bwd(lse, f16=True)
 
     @staticmethod
-    def bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg, scales, init):
+    def bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg, scales, init,
+                 dropout=None):
         mapped_bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg,
-                        scales=scales, init=init)
+                        scales=scales, init=init, **_drop_kw(dropout))
 
     @staticmethod
     def reduce_cast(srcs, dst):
@@ -541,8 +635,10 @@ class PeerOpsBf16(PeerOpsF16):
         dst.copy_(x)
 
     @staticmethod
-    def fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last, scales, out_f32):
-        mapped_fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last)
+    def fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last, scales, out_f32,
+                 dropout=None):
+        mapped_fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last,
+                        **_drop_kw(dropout))
         if last and out_f32 is not None:
             out_f32.copy_(out)
 
@@ -551,8 +647,10 @@ class PeerOpsBf16(PeerOpsF16):
         return lse_for_bwd(lse, f16=False)
 
     @staticmethod
-    def bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg, scales, init):
-        mapped_bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg, init=init)
+    def bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg, scales, init,
+                 dropout=None):
+        mapped_bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg, init=init,
+                        **_drop_kw(dropout))
 
 
 _PEER_BROKEN = {}      # process group id -> reason: the peer-memory heaps could not be set up for this group
@@ -623,14 +721,15 @@ def _stage_local(ops, x, scale, rope=None):
 
 
 def ring_forward(q, k, v, bias, seg, causal, group, rank, world, layout="auto", precision="bf16", rope=None,
-                 rope_k=True):
+                 rope_k=True, dropout=None):
     """-> (out, residuals). out is fp32 (un-rounded) for fp32 inputs, bf16 otherwise. world == 1 is the
     single-launch path (no carry buffers). rope: None, or (positions int32 [B,Sq], inv_freq): q (and k when rope_k) are
-    un-rotated and are rotated while they are staged (one GPU and the peer-memory executor only)."""
+    un-rotated and are rotated while they are staged (one GPU and the peer-memory executor only). dropout: None, or
+    (seed, thr) of attention dropout."""
     B, Sq, H, D = q.shape
     want_f32 = q.dtype == torch.float32
     if world == 1:
-        ops = _peer_ops(precision)
+        ops = with_dropout(_peer_ops(precision), dropout)
         sq, sk, sv = _local_scales(ops, (q, k, v), rope, 2 if rope_k else 1)
         q16, k16, v16 = (_stage_local(ops, q, sq, rope), _stage_local(ops, k, sk, rope if rope_k else None),
                          _stage_local(ops, v, sv))
@@ -646,27 +745,29 @@ def ring_forward(q, k, v, bias, seg, causal, group, rank, world, layout="auto", 
         pops = _peer_ops(precision)
         tr = _peer_transport(group, q.device, rp._layout_for(plan, q.shape, k.shape[1], pops).total)
         if tr is not None:
-            return rp.run_forward(plan, q, k, v, bias, seg, causal, pops, tr, want_f32, rope, rope_k)
+            return rp.run_forward(plan, q, k, v, bias, seg, causal, with_dropout(pops, dropout), tr, want_f32, rope,
+                                  rope_k)
         if want_f32:        # the NCCL executor takes bf16 operands (documented in ringattention())
             out, res = ring_forward(q.to(torch.bfloat16), k.to(torch.bfloat16), v.to(torch.bfloat16), bias, seg, causal,
-                                    group, rank, world, layout, precision, rope)
+                                    group, rank, world, layout, precision, rope, dropout=dropout)
             return out.float(), res
     if rope is not None:
         raise _lib.LwmError("ring_forward: the rotary embedding is folded into the one-GPU and peer-memory paths only")
-    ops = _ops_for(precision)
+    ops = with_dropout(_ops_for(precision), dropout)
     plan = rs.make_plan(world, rank, Sq, k.shape[1], causal, lay, n_sub_first=rs.auto_sub(world, k.shape[1], lay))
     out, res = rx.run_forward(plan, q, k, v, bias, seg, causal, group, ops)
     return out, _f32_residuals(ops, res)
 
 
 def ring_backward(res, k, v, dout, bias, seg, causal, group, rank, world, layout="auto", precision="bf16", rope=None,
-                  rope_k=True):
-    """rope, rope_k: as ring_forward's; dq (and dk when rope_k) are then the gradients w.r.t. the un-rotated q (and k)"""
+                  rope_k=True, dropout=None):
+    """rope, rope_k: as ring_forward's; dq (and dk when rope_k) are then the gradients w.r.t. the un-rotated q (and k).
+    dropout: the forward's"""
     B, Sk, H, D = k.shape
     dev = k.device
     want_f32 = k.dtype == torch.float32
     if world == 1:
-        ops = _peer_ops(precision)
+        ops = with_dropout(_peer_ops(precision), dropout)
         q16, out, lse = res["q_chunks"][0], res["out_chunks"][0], res["lse_chunks"][0]
         sq, sk, sv = res["scales"]
         Sq = q16.shape[1]
@@ -705,15 +806,15 @@ def ring_backward(res, k, v, dout, bias, seg, causal, group, rank, world, layout
     lay = rs.choose_layout(world, dout.shape[1], Sk, causal, layout)
     if _transport(group) == "peer":
         plan = rs.make_peer_plan(world, rank, dout.shape[1], Sk, causal, lay)
-        return rp.run_backward(plan, res, k, v, dout, bias, seg, causal, _peer_ops(precision),
+        return rp.run_backward(plan, res, k, v, dout, bias, seg, causal, with_dropout(_peer_ops(precision), dropout),
                                rp.CudaPeerTransport.get(group, dev), want_f32, rope, rope_k)
     if rope is not None:
         raise _lib.LwmError("ring_backward: the rotary embedding is folded into the one-GPU and peer-memory paths only")
     if want_f32:            # forward fell back to the NCCL executor: bf16 operands in, fp32 gradients out
         dq, dk, dv = ring_backward(res, k.to(torch.bfloat16), v.to(torch.bfloat16), dout.to(torch.bfloat16), bias, seg,
-                                   causal, group, rank, world, layout, precision)
+                                   causal, group, rank, world, layout, precision, dropout=dropout)
         return dq.float(), dk.float(), dv.float()
-    ops = _ops_for(precision)
+    ops = with_dropout(_ops_for(precision), dropout)
     n_sub = rs.auto_sub(world, Sk, lay)
     plan = rs.make_plan(world, rank, dout.shape[1], Sk, causal, lay, n_sub_first=n_sub, n_sub_last=n_sub)
     return rx.run_backward(plan, res, k, v, dout, bias, seg, causal, group, ops)

@@ -280,6 +280,29 @@ int lwm_kv_cache_write_rope(const void* k_new, const void* v_new, int dtype, voi
                             const int* position_ids, const float* inv_freq, int B, int n_src, long long src0, int n,
                             int L, long long dst0, int H, int D, void* stream);
 
+/* The 8-bit KV cache of the generation path (`ShardedKVCache(..., dtype=torch.int8)`; format in
+ * lwm_b200/csrc/kv_q8.cuh and DESIGN.md §5). A cache tensor is data int8 [B,L,H,128] (codes) plus exp int8 [B,H,L,4]
+ * (one power-of-two exponent per 32-element group, head-major), both 4-byte aligned. A row's value is code * 2^e, exact
+ * in fp32 and bf16; code -128 is NaN.
+ * lwm_kv_cache_write_q8     rows [src0, src0+n) of k_src / v_src [B,n_src,H,128] (src_dtype 0 = fp32, 1 = bf16)
+ *                           quantized into rows [dst0, dst0+n) of the k and v caches [B,L,H,128]. position_ids [B,n_src]
+ *                           int32 and inv_freq [64], or both NULL: k is first rotated and rounded to the source dtype,
+ *                           bit for bit as lwm_kv_cache_write_rope stores it. One launch for k and v.
+ * lwm_attn_decode_partial_q8 lwm_attn_decode_partial with k / v read from the 8-bit cache [B,Sk,H,128]; q in q_dtype
+ *                           (0 = fp32, 1 = bf16). Bit for bit lwm_attn_decode_partial on the cache dequantized to q's
+ *                           dtype.
+ * lwm_kv_dequant_q8         data / exp of [B,L,H,128] rows -> out [B,L,H,128] in out_dtype (0 = fp32, 1 = bf16), exact. */
+int lwm_kv_cache_write_q8(const void* k_src, const void* v_src, int src_dtype, signed char* k_data, signed char* k_exp,
+                          signed char* v_data, signed char* v_exp, const int* position_ids, const float* inv_freq,
+                          int B, int n_src, long long src0, int n, int L, long long dst0, int H, int D, void* stream);
+int lwm_attn_decode_partial_q8(const void* q, int q_dtype, const signed char* k, const signed char* k_exp,
+                               const signed char* v, const signed char* v_exp, const unsigned char* mask,
+                               float* o_part, float* ml_part, void* workspace, int B, int H, int Q, int Sk, int D,
+                               long long k_pos0, long long mask_stride_b, long long mask_stride_q, int splits,
+                               float softmax_scale, const int* position_ids, const float* inv_freq, void* stream);
+int lwm_kv_dequant_q8(const signed char* data, const signed char* exp, void* out, int out_dtype, int B, int L, int H,
+                      int D, void* stream);
+
 /* The operand passes of the attention op with the rotary embedding folded in (`ringattention(..., freqs_cis,
  * position_ids)`): x [B,S,H,128] fp32 (0) or bf16 (1) holds UN-rotated q or k, position_ids int32 [B,S], inv_freq [64]
  * as for lwm_attn_rope. Every pass works on rope(x) rounded to x's dtype — bit for bit what lwm_attn_rope writes — so

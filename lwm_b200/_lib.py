@@ -51,6 +51,11 @@ _SIGNATURES = {
     "lwm_attn_decode_merge": [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_ll, c_void_p],
     "lwm_kv_cache_write_rope": [c_void_p, c_void_p, c_int] + [c_void_p] * 4 + [c_int, c_int, c_ll, c_int, c_int, c_ll,
                                                                                c_int, c_int, c_void_p],
+    "lwm_kv_cache_write_q8": [c_void_p, c_void_p, c_int] + [c_void_p] * 6 + [c_int, c_int, c_ll, c_int, c_int, c_ll,
+                                                                              c_int, c_int, c_void_p],
+    "lwm_attn_decode_partial_q8": [c_void_p, c_int] + [c_void_p] * 8 + [c_int] * 5 + [c_ll, c_ll, c_ll, c_int, c_float]
+                                  + [c_void_p] * 3,
+    "lwm_kv_dequant_q8": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "lwm_attn_mask_pack": [c_void_p, c_ll, c_ll, c_ll, c_int, c_int, c_ll, c_int, c_int, c_void_p, c_void_p, c_void_p],
     "lwm_attn_infer_tilemap": [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p],
     "lwm_attn_infer_partial": [c_void_p] * 12 + [c_int] * 6 + [c_float, c_void_p],

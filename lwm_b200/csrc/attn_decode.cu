@@ -12,10 +12,15 @@
 //                          rows only; longer queries go to the tensor-core inference mode of attn_fwd_kernel.
 //                          kRope: q is un-rotated and is rotated at its position as it is loaded (lane l's dims are
 //                          the whole pairs 2l, 2l+1), rounded to q's dtype first: the value lwm_attn_rope would write.
+//                          KV = signed char: the 8-bit cache of kv_q8.cuh (the q8 instances): lane l loads one
+//                          32-bit code word per key row (128 B per warp) and the row's exponent word, dequantizes
+//                          exactly into fp32 and runs the same arithmetic in the same key order, so its partials are
+//                          bit for bit those of the T instance on the dequantized (to T) cache.
 //   decode_merge_kernel    merges `n_part` partials per (b, q, h): used for the key splits (of both kernels) and,
 //                          after the exchange, for the ranks; writes bf16 or fp32.
 #include "attn_common.cuh"
 #include "capi_internal.h"
+#include "kv_q8.cuh"
 #include "rope_common.cuh"
 
 #include <type_traits>
@@ -24,16 +29,18 @@ namespace lwm {
 
 constexpr int kDecWarps = 4;
 
-template <typename T, bool kRope = false>
+template <typename T, bool kRope = false, typename KV = T>
 __global__ void __launch_bounds__(kDecWarps * 32)
-decode_partial_kernel(const T* __restrict__ q, const T* __restrict__ k,
-                      const T* __restrict__ v, const unsigned char* __restrict__ mask,
+decode_partial_kernel(const T* __restrict__ q, const KV* __restrict__ k,
+                      const KV* __restrict__ v, const unsigned char* __restrict__ mask,
                       float* __restrict__ o_part, float* __restrict__ ml_part, int B, int H, int Q, int Sk,
                       long long k_pos0, long long mask_stride_b, long long mask_stride_q, int splits,
                       float scale_log2, const int* __restrict__ position_ids = nullptr,
-                      const float* __restrict__ inv_freq = nullptr) {
+                      const float* __restrict__ inv_freq = nullptr, const unsigned* __restrict__ k_exp = nullptr,
+                      const unsigned* __restrict__ v_exp = nullptr) {
   constexpr bool kF32 = std::is_same<T, float>::value;   // fp32 rows: one float4 per lane, bf16 rows: one uint2
-  using Raw = typename std::conditional<kF32, float4, uint2>::type;
+  constexpr bool kQ8 = std::is_same<KV, signed char>::value;   // 8-bit rows: one code word per lane
+  using Raw = typename std::conditional<kQ8, unsigned, typename std::conditional<kF32, float4, uint2>::type>::type;
   const int split = blockIdx.x, h = blockIdx.y;
   const int b = blockIdx.z / Q, qi = blockIdx.z % Q;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -71,12 +78,14 @@ decode_partial_kernel(const T* __restrict__ q, const T* __restrict__ k,
 
   float m = -INFINITY, l = 0.f, a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
   const size_t row_stride = (size_t)H * kHeadDim;   // elements between consecutive keys of one head
-  const T* kb = k + ((size_t)b * Sk) * row_stride + (size_t)h * kHeadDim;
-  const T* vb = v + ((size_t)b * Sk) * row_stride + (size_t)h * kHeadDim;
+  const KV* kb = k + ((size_t)b * Sk) * row_stride + (size_t)h * kHeadDim;
+  const KV* vb = v + ((size_t)b * Sk) * row_stride + (size_t)h * kHeadDim;
+  const size_t exp0 = ((size_t)b * H + h) * Sk;     // the exponent words of this (b, h), one per key
   // each warp strides over the CTA's key range, 4 keys in flight per iteration
   for (int j0 = k_begin + warp * 4; j0 < k_end; j0 += kDecWarps * 4) {
     float s[4];
     Raw vr[4];
+    unsigned ve[4];   // kQ8: the exponent words of the value rows
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
       const int j = j0 + u;
@@ -85,7 +94,11 @@ decode_partial_kernel(const T* __restrict__ q, const T* __restrict__ k,
       if (j < k_end) {
         const Raw kr = reinterpret_cast<const Raw*>(kb + (size_t)j * row_stride)[lane];
         vr[u] = reinterpret_cast<const Raw*>(vb + (size_t)j * row_stride)[lane];
-        if constexpr (kF32) {
+        if constexpr (kQ8) {
+          ve[u] = v_exp[exp0 + j];
+          const float4 kf = q8_dequant4(kr, k_exp[exp0 + j], lane);
+          part = q0 * kf.x + q1 * kf.y + q2 * kf.z + q3 * kf.w;
+        } else if constexpr (kF32) {
           part = q0 * kr.x + q1 * kr.y + q2 * kr.z + q3 * kr.w;
         } else {
           const __nv_bfloat162 k01 = *reinterpret_cast<const __nv_bfloat162*>(&kr.x);
@@ -109,7 +122,9 @@ decode_partial_kernel(const T* __restrict__ q, const T* __restrict__ k,
         const float m_new = fmaxf(m, t);
         const float c = ex2f(m - m_new), p = ex2f(t - m_new);
         float4 vf;
-        if constexpr (kF32) {
+        if constexpr (kQ8) {
+          vf = q8_dequant4(vr[u], ve[u], lane);
+        } else if constexpr (kF32) {
           vf = vr[u];
         } else {
           const __nv_bfloat162 v01 = *reinterpret_cast<const __nv_bfloat162*>(&vr[u].x);
@@ -204,11 +219,12 @@ void lwm_decode_merge_partials(const float* o_parts, const float* ml_parts, int 
                                                                        o_merged, ml_merged, rows);
 }
 
-template <typename T, bool kRope>
+template <typename T, bool kRope, typename KV = T>
 static int decode_partial_launch(const void* q, const void* k, const void* v, const unsigned char* mask,
                                  float* o_part, float* ml_part, void* workspace, int B, int H, int Q, int Sk, int D,
                                  long long k_pos0, long long mask_stride_b, long long mask_stride_q, int splits,
-                                 float softmax_scale, const int* position_ids, const float* inv_freq, void* stream) {
+                                 float softmax_scale, const int* position_ids, const float* inv_freq, void* stream,
+                                 const void* k_exp = nullptr, const void* v_exp = nullptr) {
   if (D != kHeadDim) return lwm_fail(LWM_ERR_SHAPE, "attn_decode: head_dim must be 128");
   if (!q || !k || !v || !o_part || !ml_part || !workspace) return lwm_fail(LWM_ERR_ARG, "attn_decode: null pointer");
   if (B <= 0 || H <= 0 || Q <= 0 || Sk <= 0 || splits <= 0 || (long long)B * Q > 65535)
@@ -219,9 +235,10 @@ static int decode_partial_launch(const void* q, const void* k, const void* v, co
   float* ws_o = reinterpret_cast<float*>(workspace);
   float* ws_ml = ws_o + rows * splits * kHeadDim;
   dim3 grid(splits, H, B * Q);
-  decode_partial_kernel<T, kRope><<<grid, kDecWarps * 32, 0, st>>>(
-      reinterpret_cast<const T*>(q), reinterpret_cast<const T*>(k), reinterpret_cast<const T*>(v), mask, ws_o, ws_ml,
-      B, H, Q, Sk, k_pos0, mask_stride_b, mask_stride_q, splits, softmax_scale * kLog2e, position_ids, inv_freq);
+  decode_partial_kernel<T, kRope, KV><<<grid, kDecWarps * 32, 0, st>>>(
+      reinterpret_cast<const T*>(q), reinterpret_cast<const KV*>(k), reinterpret_cast<const KV*>(v), mask, ws_o, ws_ml,
+      B, H, Q, Sk, k_pos0, mask_stride_b, mask_stride_q, splits, softmax_scale * kLog2e, position_ids, inv_freq,
+      reinterpret_cast<const unsigned*>(k_exp), reinterpret_cast<const unsigned*>(v_exp));
   lwm_decode_merge_partials(ws_o, ws_ml, splits, o_part, ml_part, rows, st);
   return lwm_check_launch("attn_decode kernels");
 }
@@ -244,7 +261,31 @@ extern "C" int lwm_attn_decode_partial(const void* q, const void* k, const void*
                                    : decode_partial_launch<__nv_bfloat16, false>)
                             : (rope ? decode_partial_launch<float, true> : decode_partial_launch<float, false>);
   return launch(q, k, v, mask, o_part, ml_part, workspace, B, H, Q, Sk, D, k_pos0, mask_stride_b, mask_stride_q, splits,
-                softmax_scale, position_ids, inv_freq, stream);
+                softmax_scale, position_ids, inv_freq, stream, nullptr, nullptr);
+}
+
+// lwm_attn_decode_partial on the 8-bit cache (kv_q8.cuh): k / v data int8 [B,Sk,H,128] and exp int8 [B,H,Sk,4] of
+// this rank's shard, q fp32 (q_dtype 0) or bf16 (1); everything else as lwm_attn_decode_partial. The partials equal,
+// bit for bit, lwm_attn_decode_partial's on the cache dequantized to q's dtype (lwm_kv_dequant_q8).
+extern "C" int lwm_attn_decode_partial_q8(const void* q, int q_dtype, const signed char* k, const signed char* k_exp,
+                                          const signed char* v, const signed char* v_exp, const unsigned char* mask,
+                                          float* o_part, float* ml_part, void* workspace, int B, int H, int Q, int Sk,
+                                          int D, long long k_pos0, long long mask_stride_b, long long mask_stride_q,
+                                          int splits, float softmax_scale, const int* position_ids,
+                                          const float* inv_freq, void* stream) {
+  if (q_dtype != 0 && q_dtype != 1) return lwm_fail(LWM_ERR_ARG, "attn_decode_q8: q dtype codes are 0 (fp32) or 1 (bf16)");
+  if (!position_ids != !inv_freq) return lwm_fail(LWM_ERR_ARG, "attn_decode_q8: null position_ids / inv_freq");
+  if (!k_exp || !v_exp) return lwm_fail(LWM_ERR_ARG, "attn_decode_q8: null pointer");
+  if (((reinterpret_cast<size_t>(k) | reinterpret_cast<size_t>(v) | reinterpret_cast<size_t>(k_exp) |
+        reinterpret_cast<size_t>(v_exp)) & 3) != 0)
+    return lwm_fail(LWM_ERR_ARG, "attn_decode_q8: data and exp must be 4-byte aligned");
+  const bool rope = position_ids != nullptr;
+  using S8 = signed char;
+  auto* launch = q_dtype == 1 ? (rope ? decode_partial_launch<__nv_bfloat16, true, S8>
+                                      : decode_partial_launch<__nv_bfloat16, false, S8>)
+                              : (rope ? decode_partial_launch<float, true, S8> : decode_partial_launch<float, false, S8>);
+  return launch(q, k, v, mask, o_part, ml_part, workspace, B, H, Q, Sk, D, k_pos0, mask_stride_b, mask_stride_q, splits,
+                softmax_scale, position_ids, inv_freq, stream, k_exp, v_exp);
 }
 
 // merge n_part partials per row (e.g. the all-gathered per-rank partials) into out, bf16 (out_dtype 1) or the

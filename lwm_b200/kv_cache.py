@@ -11,7 +11,11 @@ Without the rotary keywords this is pure data movement (copies and one all-gathe
 the new keys arrive un-rotated and are rotated as they are written (lwm_kv_cache_write_rope: one launch for k and v), so
 the cache holds what apply_rotary_emb followed by the plain update would leave in it, bit for bit. The cache shards are
 exactly the k / v arguments `ringattention` (prefill: "K/V = whole cache") and `ringattention_inference` (decode) take
-(with rotate_k=False when q is rotated inside the op)."""
+(with rotate_k=False when q is rotated inside the op).
+
+dtype=torch.int8 is the 8-bit cache (QuantizedKV below; DESIGN.md §5): every new row is quantized as it is written
+(lwm_kv_cache_write_q8, the keys rotated first when the rotary keywords are given), and both attention ops read it.
+It is lossy and meant for generation only."""
 import torch
 import torch.distributed as dist
 
@@ -29,10 +33,79 @@ def kv_cache_write_rope(k_src, v_src, src0, n, cache_k, cache_v, dst0, pos, inv_
               int(dst0), H, D, _lib.stream_ptr())
 
 
+def kv_cache_write_q8(k_src, v_src, src0, n, cache_k, cache_v, dst0, pos=None, inv_freq=None):
+    """rows [src0, src0+n) of k_src / v_src [B,n_src,H,128] (bf16 or fp32, one dtype) quantized into rows
+    [dst0, dst0+n) of the QuantizedKV caches cache_k / cache_v; pos int32 [B,n_src] and inv_freq given: k is rotated at
+    pos and rounded to its dtype first, as kv_cache_write_rope stores it (lwm_kv_cache_write_q8)"""
+    B, n_src, H, D = k_src.shape
+    _lib.call("lwm_kv_cache_write_q8", _lib.ptr(k_src), _lib.ptr(v_src), _dt(k_src), _lib.ptr(cache_k.data),
+              _lib.ptr(cache_k.exp), _lib.ptr(cache_v.data), _lib.ptr(cache_v.exp), _lib.ptr(pos), _lib.ptr(inv_freq),
+              B, n_src, int(src0), int(n), cache_k.shape[1], int(dst0), H, D, _lib.stream_ptr())
+
+
+class QuantizedKV:
+    """One tensor (keys or values) of the 8-bit KV cache, [B,L,H,128] rows: data int8 [B,L,H,128] holds the codes and
+    exp int8 [B,H,L,4] one power-of-two exponent per 32-element group, head-major (lwm_b200/csrc/kv_q8.cuh). A value is
+    code * 2^e, exact in fp32 and bf16; code -128 is NaN. It stands where a cache shard goes: ringattention_inference
+    and ringattention(..., rotate_k=False) accept it for k and v (generation only, no gradient)."""
+    dtype = torch.int8
+    requires_grad = False
+
+    def __init__(self, data, exp):
+        if data.dtype != torch.int8 or exp.dtype != torch.int8:
+            raise TypeError("QuantizedKV: data and exp must be int8, got %s and %s" % (data.dtype, exp.dtype))
+        if data.dim() != 4 or data.shape[-1] != 128:
+            raise ValueError("QuantizedKV: data must be [B,L,H,128], got %s" % (tuple(data.shape),))
+        B, L, H, _ = data.shape
+        if tuple(exp.shape) != (B, H, L, 4):
+            raise ValueError("QuantizedKV: exp must be [B,H,L,4] = %s, got %s" % ((B, H, L, 4), tuple(exp.shape)))
+        if not (data.is_contiguous() and exp.is_contiguous()) or data.device != exp.device:
+            raise ValueError("QuantizedKV: data and exp must be contiguous and on one device")
+        self.data, self.exp = data, exp
+
+    @classmethod
+    def zeros(cls, batch, length, num_heads, device="cuda"):
+        """an all-zero cache (the value of a bf16 / fp32 cache of zeros)"""
+        return cls(torch.zeros((batch, length, num_heads, 128), dtype=torch.int8, device=device),
+                   torch.zeros((batch, num_heads, length, 4), dtype=torch.int8, device=device))
+
+    @property
+    def shape(self):
+        return self.data.shape
+
+    @property
+    def device(self):
+        return self.data.device
+
+    @property
+    def is_cuda(self):
+        return self.data.is_cuda
+
+    @property
+    def nbytes(self):
+        return self.data.numel() + self.exp.numel()
+
+    def contiguous(self):
+        return self
+
+    def dequantize(self, dtype):
+        """-> the rows' values [B,L,H,128] in bf16 or fp32 (exact; lwm_kv_dequant_q8)"""
+        if dtype not in (torch.bfloat16, torch.float32):
+            raise ValueError("QuantizedKV.dequantize: dtype must be bfloat16 or float32, got %s" % dtype)
+        if not self.is_cuda:
+            raise _lib.LwmError("QuantizedKV.dequantize: the cache must live on an sm_90 GPU (no CPU fallback)")
+        B, L, H, D = self.shape
+        out = torch.empty(self.shape, dtype=dtype, device=self.device)
+        _lib.call("lwm_kv_dequant_q8", _lib.ptr(self.data), _lib.ptr(self.exp), _lib.ptr(out), _dt(out), B, L, H, D,
+                  _lib.stream_ptr())
+        return out
+
+
 class ShardedKVCache:
     """comm: None (torch.distributed over `group`, or a ring of one), or an object with TorchComm's all_gather and
     `world` / `rank` attributes (e.g. an in-process stand-in that runs the real kernels on emulated ranks)."""
     write_rope = staticmethod(kv_cache_write_rope)
+    write_q8 = staticmethod(kv_cache_write_q8)
 
     def __init__(self, batch, max_length, num_heads, head_dim, dtype=torch.bfloat16, device="cuda", group=None,
                  comm=None):
@@ -49,8 +122,15 @@ class ShardedKVCache:
         self.max_length = max_length
         self.shard_len = max_length // self.world
         shape = (batch, self.shard_len, num_heads, head_dim)
-        self.cached_key = torch.zeros(shape, dtype=dtype, device=device)       # jnp.zeros (llama.py:444-445)
-        self.cached_value = torch.zeros(shape, dtype=dtype, device=device)
+        self.quantized = dtype == torch.int8
+        if self.quantized:
+            if head_dim != 128:
+                raise ValueError("ShardedKVCache: the 8-bit cache needs head_dim 128, got %d" % head_dim)
+            self.cached_key = QuantizedKV.zeros(batch, self.shard_len, num_heads, device)
+            self.cached_value = QuantizedKV.zeros(batch, self.shard_len, num_heads, device)
+        else:
+            self.cached_key = torch.zeros(shape, dtype=dtype, device=device)       # jnp.zeros (llama.py:444-445)
+            self.cached_value = torch.zeros(shape, dtype=dtype, device=device)
         self.cache_index = 0
 
     def concatenate(self, key, value, *, freqs_cis=None, position_ids=None):
@@ -61,9 +141,14 @@ class ShardedKVCache:
         position_ids [B,1] (decode, replicated) or [B,q_loc] (prefill, this rank's rows) are the positions of the new
         rows (checked as ringattention checks them); key and value must then have the cache's dtype. Decode: the owner
         of the slot makes one write launch. Prefill: the positions travel with the rows through the all-gather and
-        every rank rotates only the slice it keeps, straight into its shard."""
+        every rank rotates only the slice it keeps, straight into its shard.
+        The 8-bit cache (dtype=torch.int8): key and value are bf16 or fp32, of one dtype, and every write goes through
+        write_q8 (one launch for k and v, rotating the keys first when the rotary keywords are given); each rank
+        quantizes only the rows it keeps. The returned pair is QuantizedKV."""
         rope = _rope.check_position_ids("ShardedKVCache.concatenate", freqs_cis, position_ids,
                                         (key.shape[0], key.shape[1]), key.device)
+        if self.quantized:
+            return self._concatenate_q8(key, value, rope)
         if rope is not None and not (key.dtype == value.dtype == self.cached_key.dtype):
             raise ValueError("ShardedKVCache.concatenate: with the rotary keywords key and value must have the cache "
                              "dtype %s, got %s and %s" % (self.cached_key.dtype, key.dtype, value.dtype))
@@ -95,6 +180,31 @@ class ShardedKVCache:
                 full = self._gather_rows(new.contiguous())
                 if b > a:
                     cache[:, a - lo:b - lo].copy_(full[:, a - self.cache_index:b - self.cache_index])
+        self.cache_index += n_new
+        return self.cached_key, self.cached_value
+
+    def _concatenate_q8(self, key, value, rope):
+        if not (key.dtype == value.dtype and key.dtype in (torch.bfloat16, torch.float32)):
+            raise ValueError("ShardedKVCache.concatenate: the 8-bit cache takes bfloat16 or float32 key and value of one "
+                             "dtype, got %s and %s" % (key.dtype, value.dtype))
+        pos, inv_freq = rope if rope is not None else (None, None)
+        lo = self.rank * self.shard_len
+        if key.shape[1] == 1 and value.shape[1] == 1 and self._is_decode(key):
+            cur = self.cache_index - lo
+            if 0 <= cur < self.shard_len:
+                self.write_q8(key.contiguous(), value.contiguous(), 0, 1, self.cached_key, self.cached_value, cur,
+                              None if pos is None else pos.contiguous(), inv_freq)
+            self.cache_index += 1
+            return self.cached_key, self.cached_value
+        n_new = key.shape[1] * self.world
+        if self.cache_index + n_new > self.max_length:
+            raise ValueError("cache overflow: %d + %d > %d" % (self.cache_index, n_new, self.max_length))
+        a, b = max(self.cache_index, lo), min(self.cache_index + n_new, lo + self.shard_len)
+        k_all, v_all = self._gather_rows(key.contiguous()), self._gather_rows(value.contiguous())
+        p_all = None if pos is None else self._gather_rows(pos.contiguous()).contiguous()
+        if b > a:
+            self.write_q8(k_all.contiguous(), v_all.contiguous(), a - self.cache_index, b - a, self.cached_key,
+                          self.cached_value, a - lo, p_all, inv_freq)
         self.cache_index += n_new
         return self.cached_key, self.cached_value
 

@@ -209,6 +209,23 @@ def _check_rope(freqs_cis, position_ids, q, k, rotate_k=True):
     return _rope.check_position_ids("ringattention", freqs_cis, position_ids, (q.shape[0], q.shape[1]), q.device)
 
 
+def _quantized_kv(op, q, k, v, rotates_k):
+    """whether k and v are the 8-bit cache (kv_cache.QuantizedKV); raises ValueError where it does not apply"""
+    from .kv_cache import QuantizedKV
+    qk, qv = isinstance(k, QuantizedKV), isinstance(v, QuantizedKV)
+    if not (qk or qv):
+        return False
+    if qk != qv:
+        raise ValueError("%s: k and v must both be QuantizedKV or neither" % op)
+    if q.dtype not in (torch.bfloat16, torch.float32):
+        raise ValueError("%s: with an 8-bit cache q must be bfloat16 or float32, got %s" % (op, q.dtype))
+    if rotates_k:
+        raise ValueError("%s: the 8-bit cache holds rotated keys; pass rotate_k=False with the rotary keywords" % op)
+    if torch.is_grad_enabled() and q.requires_grad:
+        raise ValueError("%s: the 8-bit cache is for generation only (no gradient); run under torch.no_grad()" % op)
+    return True
+
+
 def _peer_ready(q, k, causal, group, rank, world, layout, precision):
     """world > 1: whether this call runs on the peer-memory executor (sets up its heap, as ring_forward would)"""
     if _transport(group) != "peer":
@@ -248,6 +265,10 @@ def ringattention(q, k, v, attn_bias=None, segment_ids=None, *, axis_name="sp", 
     q against the whole cache). Bit-identical to ringattention(apply_rotary_emb(q, ...)[0], k, v, ...) in the same sense;
     dK is the gradient w.r.t. k as passed, and only dQ gets the conjugate rotation.
 
+    k, v may be the 8-bit cache (kv_cache.QuantizedKV, both or neither) in the cached prefill: q bf16 or fp32 without
+    gradient, and rotate_k=False when the rotary keywords are given. The shards are dequantized to q's dtype (exact; one
+    transient copy of each) and the op runs on them as above.
+
     Attention dropout: blockwise_kwargs=dict(deterministic=False, attn_pdrop=p, dropout_rng=seed) with 0 < p < 1, as
     at the reference call site. A dropped (query, key) entry leaves the softmax's numerator and denominator (no 1/(1-p)
     rescale); a row left without a surviving key outputs 0 and gets zero gradients. The mask is a function of (seed, p,
@@ -259,6 +280,8 @@ def ringattention(q, k, v, attn_bias=None, segment_ids=None, *, axis_name="sp", 
         raise ValueError("precision must be 'bf16' or 'fp16'")
     if cache_idx is not None:
         raise NotImplementedError("cache_idx is always None at the reference call site (lwm/llama.py:544)")
+    if _quantized_kv("ringattention", q, k, v, bool(rotate_k) and freqs_cis is not None):
+        k, v = k.dequantize(q.dtype), v.dequantize(q.dtype)
     rope = _check_rope(freqs_cis, position_ids, q, k, rotate_k)
     rotate_k = bool(rotate_k)
     if not q.is_cuda:
@@ -836,8 +859,9 @@ def _check_infer_dtypes(q, k, v):
 
 
 def decode_partial(q, k, v, mask_u8, k_pos0, stream=None, rope=None):
-    """This rank's partial over its KV shard with the GEMV kernel (bf16 or fp32 q/k/v, read as they are)
-    -> (o_part [B*Q*H,128] fp32, ml_part [B*Q*H,2] fp32). rope: None, or (positions int32 [B,Q], inv_freq): q is
+    """This rank's partial over its KV shard with the GEMV kernel (bf16 or fp32 q/k/v, read as they are; or k / v
+    the 8-bit cache, kv_cache.QuantizedKV, with bf16 or fp32 q: bit for bit the partial on the cache dequantized to q's
+    dtype) -> (o_part [B*Q*H,128] fp32, ml_part [B*Q*H,2] fp32). rope: None, or (positions int32 [B,Q], inv_freq): q is
     un-rotated and the kernel rotates it as it loads it."""
     B, Q, H, D = q.shape
     Sk = k.shape[1]
@@ -850,9 +874,13 @@ def decode_partial(q, k, v, mask_u8, k_pos0, stream=None, rope=None):
     if mask_u8 is not None:
         sb, sq = mask_u8.stride(0), mask_u8.stride(-2)
     pos, inv_freq = rope if rope is not None else (None, None)
-    _lib.call("lwm_attn_decode_partial", _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _dt(q), _lib.ptr(mask_u8),
-              _lib.ptr(o_part), _lib.ptr(ml_part), _lib.ptr(ws), B, H, Q, Sk, D, int(k_pos0), int(sb), int(sq), splits,
-              1.0 / math.sqrt(D), _lib.ptr(pos), _lib.ptr(inv_freq), _lib.stream_ptr(stream))
+    tail = (_lib.ptr(mask_u8), _lib.ptr(o_part), _lib.ptr(ml_part), _lib.ptr(ws), B, H, Q, Sk, D, int(k_pos0), int(sb),
+            int(sq), splits, 1.0 / math.sqrt(D), _lib.ptr(pos), _lib.ptr(inv_freq), _lib.stream_ptr(stream))
+    if k.dtype == torch.int8:       # the 8-bit cache
+        _lib.call("lwm_attn_decode_partial_q8", _lib.ptr(q), _dt(q), _lib.ptr(k.data), _lib.ptr(k.exp),
+                  _lib.ptr(v.data), _lib.ptr(v.exp), *tail)
+    else:
+        _lib.call("lwm_attn_decode_partial", _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _dt(q), *tail)
     return o_part, ml_part
 
 
@@ -1248,17 +1276,26 @@ def ringattention_inference(q, k, v, attn_mask, axis_name="sp", *, freqs_cis=Non
       * rotate_k=True (no KV cache: q and k are the same rows, Q_loc == S_loc): k is rotated at the same positions, by a
         pass of its own before the GEMV kernel, or inside its staging for the tensor cores.
     Bit-identical to the call on apply_rotary_emb's rotated q (and k) under autograd (dQ up to the order of its fp32
-    sums); dQ (and dK with rotate_k) are the gradients w.r.t. the un-rotated rows, and position_ids gets none."""
+    sums); dQ (and dK with rotate_k) are the gradients w.r.t. the un-rotated rows, and position_ids gets none.
+
+    k, v may be the 8-bit cache (kv_cache.QuantizedKV, both or neither) with q bf16 or fp32, without gradient and with
+    rotate_k=False when the rotary keywords are given. Below INFER_MIN_Q query rows (world * Q_loc on a q-sharded
+    ring) the GEMV kernel reads it directly, bit for bit the call on the cache dequantized to q's dtype; from there on
+    the shard is dequantized to q's dtype (exact; one transient copy) for the tensor-core path."""
     group, rank, world = _resolve_group(axis_name)
     B, Q, H, D = q.shape
     Sk = k.shape[1]
     rope = _rope.check_position_ids("ringattention_inference", freqs_cis, position_ids, (B, Q), q.device)
+    quantized = _quantized_kv("ringattention_inference", q, k, v, rope is not None and bool(rotate_k))
     if rope is not None and rotate_k and Q != Sk:
         raise ValueError("ringattention_inference: rotate_k=True rotates q and k at the same positions, which needs "
                          "Q_loc == S_loc (got %d and %d); with a rotated KV cache pass rotate_k=False" % (Q, Sk))
     if not q.is_cuda:
         raise _lib.LwmError("ringattention_inference: tensors must live on an sm_90 GPU (no CPU fallback)")
-    _check_infer_dtypes(q, k, v)
+    if not quantized:
+        _check_infer_dtypes(q, k, v)
+    elif (Q if world == 1 or Q == 1 else world * Q) >= INFER_MIN_Q:
+        k, v = k.dequantize(q.dtype), v.dequantize(q.dtype)      # the tensor-core path (see the docstring)
     if attn_mask is not None:
         if attn_mask.dim() != 4 or attn_mask.shape[1] != 1 or attn_mask.shape[2] != Q or attn_mask.shape[0] not in (1, B):
             raise ValueError("attn_mask must be [B,1,Q,K_global] (lwm/llama.py:585-590)")

@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define LWM_B200_ABI_VERSION 4
+#define LWM_B200_ABI_VERSION 5
 
 #define LWM_OK 0
 #define LWM_ERR_DEVICE 1
@@ -63,14 +63,34 @@ const char* lwm_last_error(void);
  *   softmax_scale 1/sqrt(D)
  *   tiles, tile_count  both NULL, or the forward block map of lwm_attn_step_tilemap built from the same arguments (bias
  *                or segment_ids required then): the kernel visits only the KV tiles in it. Results are bit-identical.
+ *   seed, drop_threshold, batch0  attention dropout (below); drop_threshold 0: none, seed is ignored.
  * Constraints: D == 128; Sq, Sk multiples of 128. A partial set of scales, out_f32 without scales, or only one of
  * tiles / tile_count is LWM_ERR_ARG.
+ *
+ * Attention dropout (the reference's blockwise_kwargs deterministic=False, attn_pdrop=p, dropout_rng): a dropped (q, k)
+ * entry is removed from the numerator and the denominator of the softmax (it takes the masked logit; no 1/(1-p)
+ * rescale), so P = 0 and dS = 0 there in the backward. A row left without a surviving key (every visible key dropped,
+ * or fully masked) writes out = 0 and an lse at the masked level (lwm_attn_bwd_lse turns it into -inf: zero gradients).
+ * The mask is regenerated from (seed, drop_threshold, b, h, GLOBAL q, GLOBAL k) in the tile kernels, never stored
+ * (lwm_b200/csrc/attn_dropout.cuh): Philox4x32-10, key (seed & 0xffffffff, seed >> 32), counter
+ * (((k >> 4) << 2) | ((k >> 1) & 3), q & ~8, h, b), the 16-bit half k & 1 of word 2 ((q >> 3) & 1) + ((k >> 3) & 1);
+ * dropped iff it is below drop_threshold = min(65535, round(p * 65536)). b is the GLOBAL batch row: batch0 >= 0 is the
+ * global batch row of the call's batch row 0 (a caller that launches a slice of the batch passes its offset, so that
+ * every batch row draws its own mask). The same for any ring layout, chunking, block map or executor.
+ * drop_threshold > 65535 or batch0 < 0 is LWM_ERR_ARG. With dropout, q_pos0 and k_pos0 must be multiples of 128, B and
+ * H <= 65535 and batch0 + B < 2^31 (LWM_ERR_SHAPE).
+ * lwm_attn_dropout_mask: out [n_q, n_k] uint8 = the decisions (1 = dropped) of batch row b, head h, global queries
+ *   q_pos0 .. q_pos0 + n_q - 1 and keys k_pos0 .. k_pos0 + n_k - 1 (drop_threshold in [1, 65535]), from the tile
+ *   kernels' device function.
  */
 int lwm_attn_fwd_step(const void* q, const void* k, const void* v, const float* scale_q, const float* scale_k,
                       const float* scale_v, float* out_f32, void* out, float* lse, float* acc_o, float* acc_m,
                       float* acc_l, int B, int H, int Sq, int Sk, int D, long long q_pos0, long long k_pos0, int causal,
                       const float* bias, long long bias_stride, const int* segment_ids, long long seg_stride,
-                      float softmax_scale, int first, int last, const int* tiles, const int* tile_count, void* stream);
+                      float softmax_scale, int first, int last, const int* tiles, const int* tile_count, long long seed,
+                      unsigned drop_threshold, int batch0, void* stream);
+int lwm_attn_dropout_mask(long long seed, unsigned drop_threshold, int b, int h, long long q_pos0, long long k_pos0,
+                          int n_q, int n_k, unsigned char* out, void* stream);
 
 /* Ring attention, backward.
  * lwm_attn_bwd_prep: delta[b,h,s] = sum_d dout[b,s,h,d] * out[b,s,h,d]  (fp32), once per backward. out fp32
@@ -92,7 +112,18 @@ int lwm_attn_fwd_step(const void* q, const void* k, const void* v, const float* 
  *   scale_q/k/v/do: all NULL (bf16 operands) or all given (fp16 operand mode, dout its scaled fp16 copy too);
  *   tiles, tile_count: both NULL, or the backward block map of lwm_attn_step_tilemap (bias or segment_ids required):
  *   dK and dV are bit-identical to the call without it, dQ differs only by the order of its fp32 reductions, which
- *   already varies from run to run. Other arguments as for lwm_attn_fwd_step.
+ *   already varies from run to run;
+ *   order_ws: NULL, or the workspace of the ordered dQ reduction (below);
+ *   seed, drop_threshold, batch0: the forward's attention dropout. Other arguments as for lwm_attn_fwd_step.
+ * Reproducible dQ (what torch.use_deterministic_algorithms(True) asks for): with an order_ws, every dQ element receives
+ * its key tiles' fp32 contributions in ascending key-tile order, so dQ is the same bits on every run (dK and dV already
+ * are); lwm_attn_infer_bwd (below) takes it the same way. order_ws is a caller-owned int32 workspace of
+ *     2 + B * H * ceil(Sq/64)                    words without a block map,
+ *     2 + B * H * ceil(Sq/64) + B * n_kt * ceil(Sq/64)   with one (n_kt = ceil(Sk/128); Sq = Q for the inference op),
+ * used on the call's stream and zeroed there by the call; it must not be shared by calls that may run concurrently.
+ * B, H <= 65535, and the workspace words and B * H * n_kt must fit in int32 (LWM_ERR_SHAPE).
+ * Word 1 is an error flag: nonzero after the call if a dQ tile waited more than 4 s for its turn (a bug, never expected;
+ * the reduction then went on unordered).
  */
 #define LWM_ATTN_F16_P_BOOST_LOG2 14.0f
 int lwm_attn_bwd_prep(const void* out, int out_dtype, const void* dout, const float* scale_do, float* delta, int B,
@@ -103,57 +134,8 @@ int lwm_attn_bwd_step(const void* q, const void* k, const void* v, const void* d
                       const float* delta, float* dq_acc, float* dk_acc, float* dv_acc, int B, int H, int Sq, int Sk,
                       int D, long long q_pos0, long long k_pos0, int causal, const float* bias, long long bias_stride,
                       const int* segment_ids, long long seg_stride, float softmax_scale, int dkv_init,
-                      const int* tiles, const int* tile_count, void* stream);
-
-/* Reproducible dQ (what torch.use_deterministic_algorithms(True) asks for): lwm_attn_bwd_step_ordered and
- * lwm_attn_infer_bwd_ordered (below) compute the same as lwm_attn_bwd_step / lwm_attn_infer_bwd, but every dQ element
- * receives its key tiles' fp32 contributions in ascending key-tile order, so dQ is the same bits on every run (dK and dV
- * already are). order_ws is a caller-owned int32 workspace of
- *     2 + B * H * ceil(Sq/64)                    words without a block map,
- *     2 + B * H * ceil(Sq/64) + B * n_kt * ceil(Sq/64)   with one (n_kt = ceil(Sk/128); Sq = Q for the inference op),
- * used on the call's stream and zeroed there by the call; it must not be shared by calls that may run concurrently.
- * Word 1 is an error flag: nonzero after the call if a dQ tile waited more than 4 s for its turn (a bug, never expected;
- * the reduction then went on unordered). A null order_ws is LWM_ERR_ARG. */
-int lwm_attn_bwd_step_ordered(const void* q, const void* k, const void* v, const void* dout, const float* scale_q,
-                              const float* scale_k, const float* scale_v, const float* scale_do, const float* lse,
-                              const float* delta, float* dq_acc, float* dk_acc, float* dv_acc, int B, int H, int Sq,
-                              int Sk, int D, long long q_pos0, long long k_pos0, int causal, const float* bias,
-                              long long bias_stride, const int* segment_ids, long long seg_stride, float softmax_scale,
-                              int dkv_init, const int* tiles, const int* tile_count, int* order_ws, void* stream);
-
-/* Attention dropout (the reference's blockwise_kwargs deterministic=False, attn_pdrop=p, dropout_rng): a dropped (q, k)
- * entry is removed from the numerator and the denominator of the softmax (it takes the masked logit; no 1/(1-p)
- * rescale), so P = 0 and dS = 0 there in the backward. A row left without a surviving key (every visible key dropped,
- * or fully masked) writes out = 0 and an lse at the masked level (lwm_attn_bwd_lse turns it into -inf: zero gradients).
- * The mask is regenerated from (seed, drop_threshold, b, h, GLOBAL q, GLOBAL k) in the tile kernels, never stored
- * (lwm_b200/csrc/attn_dropout.cuh): Philox4x32-10, key (seed & 0xffffffff, seed >> 32), counter
- * (((k >> 4) << 2) | ((k >> 1) & 3), q & ~8, h, b), the 16-bit half k & 1 of word 2 ((q >> 3) & 1) + ((k >> 3) & 1);
- * dropped iff it is below drop_threshold = min(65535, round(p * 65536)). b is the GLOBAL batch row. The same for any
- * ring layout, chunking, block map or executor.
- * lwm_attn_fwd_step_dropout / lwm_attn_bwd_step_dropout: the arguments of lwm_attn_fwd_step / lwm_attn_bwd_step, then
- *   (backward) order_ws: NULL for lwm_attn_bwd_step's unordered dQ reduction, else lwm_attn_bwd_step_ordered's,
- *   seed (the 64-bit seed, as a signed integer), drop_threshold in [1, 65535] (0 is the plain symbol: LWM_ERR_ARG) and
- *   batch0 >= 0, the global batch row of the call's batch row 0 (a caller that launches a slice of the batch passes
- *   its offset, so that every batch row draws its own mask). q_pos0 and k_pos0 must be multiples of 128
- *   (LWM_ERR_SHAPE).
- * lwm_attn_dropout_mask: out [n_q, n_k] uint8 = the decisions (1 = dropped) of batch row b, head h, global queries
- *   q_pos0 .. q_pos0 + n_q - 1 and keys k_pos0 .. k_pos0 + n_k - 1, from the tile kernels' device function. */
-int lwm_attn_fwd_step_dropout(const void* q, const void* k, const void* v, const float* scale_q, const float* scale_k,
-                              const float* scale_v, float* out_f32, void* out, float* lse, float* acc_o, float* acc_m,
-                              float* acc_l, int B, int H, int Sq, int Sk, int D, long long q_pos0, long long k_pos0,
-                              int causal, const float* bias, long long bias_stride, const int* segment_ids,
-                              long long seg_stride, float softmax_scale, int first, int last, const int* tiles,
-                              const int* tile_count, long long seed, unsigned drop_threshold, int batch0,
-                              void* stream);
-int lwm_attn_bwd_step_dropout(const void* q, const void* k, const void* v, const void* dout, const float* scale_q,
-                              const float* scale_k, const float* scale_v, const float* scale_do, const float* lse,
-                              const float* delta, float* dq_acc, float* dk_acc, float* dv_acc, int B, int H, int Sq,
-                              int Sk, int D, long long q_pos0, long long k_pos0, int causal, const float* bias,
-                              long long bias_stride, const int* segment_ids, long long seg_stride, float softmax_scale,
-                              int dkv_init, const int* tiles, const int* tile_count, int* order_ws, long long seed,
-                              unsigned drop_threshold, int batch0, void* stream);
-int lwm_attn_dropout_mask(long long seed, unsigned drop_threshold, int b, int h, long long q_pos0, long long k_pos0,
-                          int n_q, int n_k, unsigned char* out, void* stream);
+                      const int* tiles, const int* tile_count, int* order_ws, long long seed, unsigned drop_threshold,
+                      int batch0, void* stream);
 
 /* fp16-internal precision mode (optional): the tensor cores take bf16 x bf16 or fp16 x fp16 only, so the
  * higher-precision mode converts every operand once to an exact, power-of-two-scaled fp16 copy
@@ -199,14 +181,15 @@ int lwm_reduce_cast_f32(const float* const* host_srcs, int n_src, void* dst, int
  * explicit boolean mask [B,1,Q,K_global] (nonzero = attend; masked logits take finfo.min semantics).
  * lwm_attn_decode_partial reduces the local shard to one partial per (b, q, h): numerator o_part [B*Q*H,128] fp32 and
  * ml_part [B*Q*H,2] = (max in the log2 domain, denominator). q, k, v are all fp32 (dtype 0, read directly) or all bf16
- * (1). position_ids int32 [B,Q] and inv_freq [64] as for lwm_attn_rope, or both NULL: q is UN-rotated and is rotated as
+ * (1), k_exp and v_exp NULL; or k_exp and v_exp are both given: k / v are then the 8-bit KV cache (below) with these
+ * exponents, dtype is q's, and the partials are bit for bit those on the cache dequantized to q's dtype. position_ids int32 [B,Q] and inv_freq [64] as for lwm_attn_rope, or both NULL: q is UN-rotated and is rotated as
  * it is loaded, rounded to its dtype — bit for bit lwm_attn_rope (out_dtype = dtype) followed by the call without
  * them, without the rotated q in memory. workspace >= splits * B*Q*H * 130 floats. HBM-bound: K and V are streamed
  * exactly once.
  * lwm_attn_decode_merge folds n_part partials (the all-gathered per-rank partials, laid out [row][n_part]) into out
  * [B,Q,H,128], bf16 (out_dtype 1) or the un-rounded fp32 (0), and lse [B*Q*H]. */
-int lwm_attn_decode_partial(const void* q, const void* k, const void* v, int dtype, const unsigned char* mask,
-                            float* o_part, float* ml_part, void* workspace, int B, int H, int Q, int Sk, int D,
+int lwm_attn_decode_partial(const void* q, const void* k, const void* v, int dtype, const signed char* k_exp,
+                            const signed char* v_exp, const unsigned char* mask, float* o_part, float* ml_part, void* workspace, int B, int H, int Q, int Sk, int D,
                             long long k_pos0, long long mask_stride_b, long long mask_stride_q, int splits,
                             float softmax_scale, const int* position_ids, const float* inv_freq, void* stream);
 int lwm_attn_decode_merge(const float* o_parts, const float* ml_parts, int n_part, void* out, int out_dtype, float* lse,
@@ -244,20 +227,15 @@ int lwm_attn_infer_partial(const void* q16, const void* k16, const void* v16, co
  *                         -inf for rows with no visible key, and delta = rowsum(dout o out), both [B,H,Qp] with
  *                         Qp = Q rounded up to 64 (rows >= Q: lse -inf). dq_acc [B,Q,H,128] fp32 is accumulated into;
  *                         dk_acc / dv_acc [B,Sk,H,128] fp32 are written. Masked entries and keys >= Sk contribute
- *                         nothing; nothing outside the tensors' rows is read or written. */
+ *                         nothing; nothing outside the tensors' rows is read or written. order_ws: NULL, or the
+ *                         workspace of the ordered dQ reduction, as for lwm_attn_bwd_step with its block map. */
 int lwm_attn_infer_bwd_tilemap(const unsigned* bits, const int* row_any, int B, int Q, int Sk, int* tiles,
                                int* tile_count, void* stream);
 int lwm_attn_infer_bwd(const void* q16, const void* k16, const void* v16, const void* dout16, const float* scale_q,
                        const float* scale_k, const float* scale_v, const float* scale_do, const float* lse,
                        const float* delta, const unsigned* bits, const int* tiles, const int* tile_count,
                        float* dq_acc, float* dk_acc, float* dv_acc, int B, int H, int Q, int Sk, int D,
-                       float softmax_scale, void* stream);
-/* lwm_attn_infer_bwd with dQ reduced in a fixed order: order_ws as for lwm_attn_bwd_step_ordered, with its block map */
-int lwm_attn_infer_bwd_ordered(const void* q16, const void* k16, const void* v16, const void* dout16,
-                               const float* scale_q, const float* scale_k, const float* scale_v, const float* scale_do,
-                               const float* lse, const float* delta, const unsigned* bits, const int* tiles,
-                               const int* tile_count, float* dq_acc, float* dk_acc, float* dv_acc, int B, int H, int Q,
-                               int Sk, int D, float softmax_scale, int* order_ws, void* stream);
+                       float softmax_scale, int* order_ws, void* stream);
 
 /* Attention prologue: rotary position embedding (lwm/llama.py:344-375 precompute_freqs_cis / apply_rotary_emb, applied
  * at llama.py:517-519 on the head-split projections right before the ring-attention call; SURVEY.md §8f next-row 2).
@@ -288,18 +266,10 @@ int lwm_kv_cache_write_rope(const void* k_new, const void* v_new, int dtype, voi
  *                           quantized into rows [dst0, dst0+n) of the k and v caches [B,L,H,128]. position_ids [B,n_src]
  *                           int32 and inv_freq [64], or both NULL: k is first rotated and rounded to the source dtype,
  *                           bit for bit as lwm_kv_cache_write_rope stores it. One launch for k and v.
- * lwm_attn_decode_partial_q8 lwm_attn_decode_partial with k / v read from the 8-bit cache [B,Sk,H,128]; q in q_dtype
- *                           (0 = fp32, 1 = bf16). Bit for bit lwm_attn_decode_partial on the cache dequantized to q's
- *                           dtype.
  * lwm_kv_dequant_q8         data / exp of [B,L,H,128] rows -> out [B,L,H,128] in out_dtype (0 = fp32, 1 = bf16), exact. */
 int lwm_kv_cache_write_q8(const void* k_src, const void* v_src, int src_dtype, signed char* k_data, signed char* k_exp,
                           signed char* v_data, signed char* v_exp, const int* position_ids, const float* inv_freq,
                           int B, int n_src, long long src0, int n, int L, long long dst0, int H, int D, void* stream);
-int lwm_attn_decode_partial_q8(const void* q, int q_dtype, const signed char* k, const signed char* k_exp,
-                               const signed char* v, const signed char* v_exp, const unsigned char* mask,
-                               float* o_part, float* ml_part, void* workspace, int B, int H, int Q, int Sk, int D,
-                               long long k_pos0, long long mask_stride_b, long long mask_stride_q, int splits,
-                               float softmax_scale, const int* position_ids, const float* inv_freq, void* stream);
 int lwm_kv_dequant_q8(const signed char* data, const signed char* exp, void* out, int out_dtype, int B, int L, int H,
                       int D, void* stream);
 

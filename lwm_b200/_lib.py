@@ -15,19 +15,13 @@ c_void_p, c_int, c_ll, c_float = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlon
 _SIGNATURES = {
     "lwm_abi_version": [],
     "lwm_attn_fwd_step": [c_void_p] * 12 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll, c_float,
-                                                         c_int, c_int, c_void_p, c_void_p, c_void_p],
+                                                         c_int, c_int, c_void_p, c_void_p, c_ll, ctypes.c_uint, c_int,
+                                                         c_void_p],
     "lwm_attn_bwd_prep": [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
     "lwm_attn_bwd_lse": [c_void_p, c_void_p, c_ll, c_float, c_void_p],
     "lwm_attn_bwd_step": [c_void_p] * 13 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll, c_float,
-                                                         c_int, c_void_p, c_void_p, c_void_p],
-    "lwm_attn_bwd_step_ordered": [c_void_p] * 13 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll,
-                                                                 c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p],
-    "lwm_attn_fwd_step_dropout": [c_void_p] * 12 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll,
-                                                                 c_float, c_int, c_int, c_void_p, c_void_p, c_ll,
-                                                                 ctypes.c_uint, c_int, c_void_p],
-    "lwm_attn_bwd_step_dropout": [c_void_p] * 13 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll,
-                                                                 c_float, c_int, c_void_p, c_void_p, c_void_p, c_ll,
-                                                                 ctypes.c_uint, c_int, c_void_p],
+                                                         c_int, c_void_p, c_void_p, c_void_p, c_ll, ctypes.c_uint, c_int,
+                                                         c_void_p],
     "lwm_attn_dropout_mask": [c_ll, ctypes.c_uint, c_int, c_int, c_ll, c_ll, c_int, c_int, c_void_p, c_void_p],
     "lwm_attn_to_f16": [c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_void_p],
     "lwm_attn_step_tilemap": [c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_ll, c_ll, c_int]
@@ -46,22 +40,19 @@ _SIGNATURES = {
     "lwm_ring_ctx_destroy": [c_void_p],
     "lwm_ring_plan": [c_int, c_int, c_ll, c_ll, c_int, c_int, c_int, c_void_p],
     "lwm_ring_layout": [c_int, c_ll, c_ll, c_int, c_int, c_int, c_int, c_int, c_void_p],
-    "lwm_attn_decode_partial": [c_void_p] * 3 + [c_int] + [c_void_p] * 4 + [c_int] * 5 + [c_ll, c_ll, c_ll, c_int, c_float]
+    "lwm_attn_decode_partial": [c_void_p] * 3 + [c_int] + [c_void_p] * 6 + [c_int] * 5 + [c_ll, c_ll, c_ll, c_int, c_float]
                                + [c_void_p] * 3,
     "lwm_attn_decode_merge": [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_ll, c_void_p],
     "lwm_kv_cache_write_rope": [c_void_p, c_void_p, c_int] + [c_void_p] * 4 + [c_int, c_int, c_ll, c_int, c_int, c_ll,
                                                                                c_int, c_int, c_void_p],
     "lwm_kv_cache_write_q8": [c_void_p, c_void_p, c_int] + [c_void_p] * 6 + [c_int, c_int, c_ll, c_int, c_int, c_ll,
                                                                               c_int, c_int, c_void_p],
-    "lwm_attn_decode_partial_q8": [c_void_p, c_int] + [c_void_p] * 8 + [c_int] * 5 + [c_ll, c_ll, c_ll, c_int, c_float]
-                                  + [c_void_p] * 3,
     "lwm_kv_dequant_q8": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "lwm_attn_mask_pack": [c_void_p, c_ll, c_ll, c_ll, c_int, c_int, c_ll, c_int, c_int, c_void_p, c_void_p, c_void_p],
     "lwm_attn_infer_tilemap": [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p],
     "lwm_attn_infer_partial": [c_void_p] * 12 + [c_int] * 6 + [c_float, c_void_p],
     "lwm_attn_infer_bwd_tilemap": [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p],
-    "lwm_attn_infer_bwd": [c_void_p] * 16 + [c_int] * 5 + [c_float, c_void_p],
-    "lwm_attn_infer_bwd_ordered": [c_void_p] * 16 + [c_int] * 5 + [c_float, c_void_p, c_void_p],
+    "lwm_attn_infer_bwd": [c_void_p] * 16 + [c_int] * 5 + [c_float, c_void_p, c_void_p],
     "lwm_cast_f32_to_bf16": [c_void_p, c_void_p, c_ll, c_void_p],
     "lwm_add_f32": [c_void_p, c_void_p, c_ll, c_void_p],
     "lwm_vq_gn_stats": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],

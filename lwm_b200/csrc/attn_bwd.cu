@@ -88,7 +88,7 @@ constexpr int kOffEntry = kOffBars + 96;
 constexpr int kOffTicket = kOffEntry + 2 * 4;
 static_assert(sizeof(BwdBarriers) <= 96 && 96 + 5 * 4 <= 128, "attn_bwd: barrier block layout");
 
-// ---- kOrdered: dQ reduced in a fixed key-tile order (lwm_attn_bwd_step_ordered, lwm_attn_infer_bwd_ordered)
+// ---- kOrdered: dQ reduced in a fixed key-tile order (lwm_attn_bwd_step and lwm_attn_infer_bwd given an order_ws)
 // Every element of dQ tile (b, h, 64-row Q tile i) receives the contributions of its key tiles in ascending key-tile
 // order, so dQ is the same bits on every run. Each (b, h, i) has a semaphore, the number of key tiles that have added
 // into the tile. Warp 9 of key tile n waits until it equals n's turn, the number of key tiles below n that reduce into
@@ -236,8 +236,10 @@ dq_turns_kernel(const int* __restrict__ tiles, const int* __restrict__ counts, i
   }
 }
 
-template <bool kF16, bool kMap, bool kBits, bool kOrdered, bool kDrop = false>
-static int launch_bwd(dim3 grid, cudaStream_t st, const CUtensorMap (&tm)[5], const BwdParams& p, const char* what) {
+// One attn_bwd_kernel or attn_bwd_dropout_kernel instance; its dynamic shared-memory limit is raised once per device.
+template <bool kF16, bool kMap, bool kBits, bool kOrdered, bool kDrop>
+static int launch_bwd(dim3 grid, cudaStream_t st, const CUtensorMap (&tm)[5], const BwdParams& p) {
+  static_assert(!(kBits && kDrop), "the inference backward has no dropout instance");
   void (*kernel)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, BwdParams);
   if constexpr (kDrop) kernel = attn_bwd_dropout_kernel<kF16, kMap, kOrdered>;
   else kernel = attn_bwd_kernel<kF16, kMap, kBits, kOrdered>;
@@ -251,7 +253,7 @@ static int launch_bwd(dim3 grid, cudaStream_t st, const CUtensorMap (&tm)[5], co
     attr_set = true;
   }
   kernel<<<grid, kBwdThreads, kBwdSmemBytes, st>>>(tm[0], tm[1], tm[2], tm[3], tm[4], p);
-  return lwm_check_launch(what);
+  return lwm_check_launch(kDrop ? "attn_bwd_dropout_kernel" : kBits ? "attn_bwd_kernel (inference)" : "attn_bwd_kernel");
 }
 
 // The ordered launches' set-up on the call's stream: the ticket, the error flag and n_sem dQ semaphores are zeroed, and
@@ -282,13 +284,16 @@ static bool order_fits(int B, int H, int n_kt, int n_q64, bool map) {
 
 using namespace lwm;
 
-// One ring step; order_ws null: the unordered reduction of lwm_attn_bwd_step, else lwm_attn_bwd_step_ordered's.
-static int bwd_step(const void* q, const void* k, const void* v, const void* dout, const float* scale_q,
-                    const float* scale_k, const float* scale_v, const float* scale_do, const float* lse,
-                    const float* delta, float* dq_acc, float* dk_acc, float* dv_acc, int B, int H, int Sq, int Sk,
-                    int D, long long q_pos0, long long k_pos0, int causal, const float* bias, long long bias_stride,
-                    const int* segment_ids, long long seg_stride, float softmax_scale, int dkv_init, const int* tiles,
-                    const int* tile_count, int* order_ws, const DropParams* drop, void* stream) {
+// One ring step (include/lwm_b200.h): the scales select the fp16-operand kernel, tiles / tile_count the block map,
+// order_ws the ordered dQ reduction, drop_threshold > 0 the dropout instances.
+extern "C" int lwm_attn_bwd_step(const void* q, const void* k, const void* v, const void* dout, const float* scale_q,
+                                 const float* scale_k, const float* scale_v, const float* scale_do, const float* lse,
+                                 const float* delta, float* dq_acc, float* dk_acc, float* dv_acc, int B, int H,
+                                 int Sq, int Sk, int D, long long q_pos0, long long k_pos0, int causal,
+                                 const float* bias, long long bias_stride, const int* segment_ids,
+                                 long long seg_stride, float softmax_scale, int dkv_init, const int* tiles,
+                                 const int* tile_count, int* order_ws, long long seed, unsigned drop_threshold,
+                                 int batch0, void* stream) {
   if (!scale_k != !scale_q || !scale_v != !scale_q || !scale_do != !scale_q)
     return lwm_fail(LWM_ERR_ARG, "attn_bwd: scales are all given (fp16 operands) or all null (bf16)");
   if (!tiles != !tile_count) return lwm_fail(LWM_ERR_ARG, "attn_bwd: tiles and tile_count are both given or both null");
@@ -307,11 +312,9 @@ static int bwd_step(const void* q, const void* k, const void* v, const void* dou
   if (tiles && (long long)B * (Sk / kTile) * (Sq / kBQ) > 0x7fffffffLL)
     return lwm_fail(LWM_ERR_SHAPE, "attn_bwd: B * Sk/128 * Sq/64 must fit in int32 with a block map");
   if (order_ws && !order_fits(B, H, Sk / kTile, Sq / kBQ, tiles != nullptr))
-    return lwm_fail(LWM_ERR_SHAPE, "attn_bwd_ordered: B, H <= 65535 and the order_ws words, B * H * Sk/128 must fit in int32");
-  if (drop && (q_pos0 % kTile || k_pos0 % kTile))
-    return lwm_fail(LWM_ERR_SHAPE, "attn_bwd_dropout: q_pos0 and k_pos0 must each be a multiple of 128");
-  if (drop && (B > 65535 || H > 65535 || (long long)drop->batch0 + B > 0x7fffffffLL))
-    return lwm_fail(LWM_ERR_SHAPE, "attn_bwd_dropout: B, H <= 65535 and batch0 + B < 2^31");
+    return lwm_fail(LWM_ERR_SHAPE, "attn_bwd (ordered): B, H <= 65535 and the order_ws words, B * H * Sk/128 must fit in int32");
+  DropParams drop;
+  if (const int s = decode_drop_params(seed, drop_threshold, batch0, B, H, q_pos0, k_pos0, "attn_bwd", &drop)) return s;
   if (!lwm_check_device()) return LWM_ERR_DEVICE;
   CUtensorMap tm[5];   // q, k, v, dout, dq_acc
   if (!make_bf16_tmap(&tm[0], q, B, Sq, H, kBQ) || !make_bf16_tmap(&tm[1], k, B, Sk, H, kTile) ||
@@ -330,99 +333,31 @@ static int bwd_step(const void* q, const void* k, const void* v, const void* dou
   p.dkv_init = dkv_init ? 1 : 0;
   p.tiles = tiles; p.tile_count = tile_count;
   p.order_ws = nullptr; p.turns = nullptr;
-  dim3 grid(Sk / kTile, H, B);
+  p.drop = drop;
+  const dim3 grid(Sk / kTile, H, B);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (order_ws) {
     const int s = order_prologue(order_ws, (long long)B * H * (Sq / kBQ), tiles, tile_count, B, Sk / kTile, Sq / kBQ,
                                  st, p);
     if (s) return s;
-    if (drop) {
-      p.drop = *drop;
-      if (tiles)
-        return scale_q ? launch_bwd<true, true, false, true, true>(grid, st, tm, p, "attn_bwd_dropout_kernel (ordered, block map)")
-                       : launch_bwd<false, true, false, true, true>(grid, st, tm, p, "attn_bwd_dropout_kernel (ordered, block map)");
-      return scale_q ? launch_bwd<true, false, false, true, true>(grid, st, tm, p, "attn_bwd_dropout_kernel (ordered)")
-                     : launch_bwd<false, false, false, true, true>(grid, st, tm, p, "attn_bwd_dropout_kernel (ordered)");
-    }
-    if (tiles)
-      return scale_q ? launch_bwd<true, true, false, true>(grid, st, tm, p, "attn_bwd_kernel (ordered, block map)")
-                     : launch_bwd<false, true, false, true>(grid, st, tm, p, "attn_bwd_kernel (ordered, block map)");
-    return scale_q ? launch_bwd<true, false, false, true>(grid, st, tm, p, "attn_bwd_kernel (ordered)")
-                   : launch_bwd<false, false, false, true>(grid, st, tm, p, "attn_bwd_kernel (ordered)");
   }
-  if (drop) {
-    p.drop = *drop;
-    if (tiles)
-      return scale_q ? launch_bwd<true, true, false, false, true>(grid, st, tm, p, "attn_bwd_dropout_kernel (block map)")
-                     : launch_bwd<false, true, false, false, true>(grid, st, tm, p, "attn_bwd_dropout_kernel (block map)");
-    return scale_q ? launch_bwd<true, false, false, false, true>(grid, st, tm, p, "attn_bwd_dropout_kernel")
-                   : launch_bwd<false, false, false, false, true>(grid, st, tm, p, "attn_bwd_dropout_kernel");
-  }
-  if (tiles)
-    return scale_q ? launch_bwd<true, true, false, false>(grid, st, tm, p, "attn_bwd_kernel (block map)")
-                   : launch_bwd<false, true, false, false>(grid, st, tm, p, "attn_bwd_kernel (block map)");
-  return scale_q ? launch_bwd<true, false, false, false>(grid, st, tm, p, "attn_bwd_kernel")
-                 : launch_bwd<false, false, false, false>(grid, st, tm, p, "attn_bwd_kernel");
+  return with_flags([&](auto f16, auto map, auto ordered, auto dropout) {
+    return launch_bwd<f16, map, false, ordered, dropout>(grid, st, tm, p);
+  }, scale_q != nullptr, tiles != nullptr, order_ws != nullptr, drop.thr != 0);
 }
 
-// One ring step (include/lwm_b200.h): the scales select the fp16-operand kernel, tiles / tile_count the block map.
-extern "C" int lwm_attn_bwd_step(const void* q, const void* k, const void* v, const void* dout, const float* scale_q,
-                                 const float* scale_k, const float* scale_v, const float* scale_do, const float* lse,
-                                 const float* delta, float* dq_acc, float* dk_acc, float* dv_acc, int B, int H,
-                                 int Sq, int Sk, int D, long long q_pos0, long long k_pos0, int causal,
-                                 const float* bias, long long bias_stride, const int* segment_ids,
-                                 long long seg_stride, float softmax_scale, int dkv_init, const int* tiles,
-                                 const int* tile_count, void* stream) {
-  return bwd_step(q, k, v, dout, scale_q, scale_k, scale_v, scale_do, lse, delta, dq_acc, dk_acc, dv_acc, B, H, Sq, Sk,
-                  D, q_pos0, k_pos0, causal, bias, bias_stride, segment_ids, seg_stride, softmax_scale, dkv_init, tiles,
-                  tile_count, nullptr, nullptr, stream);
-}
-
-// lwm_attn_bwd_step with dQ reduced in ascending key-tile order (include/lwm_b200.h)
-extern "C" int lwm_attn_bwd_step_ordered(const void* q, const void* k, const void* v, const void* dout,
-                                         const float* scale_q, const float* scale_k, const float* scale_v,
-                                         const float* scale_do, const float* lse, const float* delta, float* dq_acc,
-                                         float* dk_acc, float* dv_acc, int B, int H, int Sq, int Sk, int D,
-                                         long long q_pos0, long long k_pos0, int causal, const float* bias,
-                                         long long bias_stride, const int* segment_ids, long long seg_stride,
-                                         float softmax_scale, int dkv_init, const int* tiles, const int* tile_count,
-                                         int* order_ws, void* stream) {
-  if (!order_ws) return lwm_fail(LWM_ERR_ARG, "attn_bwd_ordered: null order_ws");
-  return bwd_step(q, k, v, dout, scale_q, scale_k, scale_v, scale_do, lse, delta, dq_acc, dk_acc, dv_acc, B, H, Sq, Sk,
-                  D, q_pos0, k_pos0, causal, bias, bias_stride, segment_ids, seg_stride, softmax_scale, dkv_init, tiles,
-                  tile_count, order_ws, nullptr, stream);
-}
-
-// lwm_attn_bwd_step (order_ws null) or lwm_attn_bwd_step_ordered (order_ws given) with attention dropout
-// (include/lwm_b200.h)
-extern "C" int lwm_attn_bwd_step_dropout(const void* q, const void* k, const void* v, const void* dout,
-                                         const float* scale_q, const float* scale_k, const float* scale_v,
-                                         const float* scale_do, const float* lse, const float* delta, float* dq_acc,
-                                         float* dk_acc, float* dv_acc, int B, int H, int Sq, int Sk, int D,
-                                         long long q_pos0, long long k_pos0, int causal, const float* bias,
-                                         long long bias_stride, const int* segment_ids, long long seg_stride,
-                                         float softmax_scale, int dkv_init, const int* tiles, const int* tile_count,
-                                         int* order_ws, long long seed, unsigned drop_threshold, int batch0,
-                                         void* stream) {
-  if (drop_threshold == 0 || drop_threshold > 65535)
-    return lwm_fail(LWM_ERR_ARG, "attn_bwd_dropout: drop_threshold must be in [1, 65535] (0 is lwm_attn_bwd_step)");
-  if (batch0 < 0) return lwm_fail(LWM_ERR_ARG, "attn_bwd_dropout: batch0 must be >= 0");
-  const DropParams d = {uint32_t(uint64_t(seed)), uint32_t(uint64_t(seed) >> 32), drop_threshold, uint32_t(batch0)};
-  return bwd_step(q, k, v, dout, scale_q, scale_k, scale_v, scale_do, lse, delta, dq_acc, dk_acc, dv_acc, B, H, Sq, Sk,
-                  D, q_pos0, k_pos0, causal, bias, bias_stride, segment_ids, seg_stride, softmax_scale, dkv_init, tiles,
-                  tile_count, order_ws, &d, stream);
-}
-
-// Backward of ringattention_inference (attn_bwd_kernel<true, true, true>): any Q and Sk. q16 / dout16 [B,Q,H,128],
-// k16 / v16 [B,Sk,H,128] scaled fp16 copies with their device scales; lse (pre-scaled by lwm_attn_bwd_lse with the fp16
-// offset, -inf for rows without a visible key) and delta [B,H,Qp], Qp = Q rounded up to 64, rows >= Q: lse = -inf;
-// bits [B,Q,ceil(Sk/128)*4] or null; tiles / tile_count from lwm_attn_infer_bwd_tilemap. dq_acc [B,Q,H,128] fp32 is
-// accumulated into (zero it first); dk_acc / dv_acc [B,Sk,H,128] fp32 are written. order_ws: as in bwd_step.
-static int infer_bwd(const void* q16, const void* k16, const void* v16, const void* dout16, const float* scale_q,
-                     const float* scale_k, const float* scale_v, const float* scale_do, const float* lse,
-                     const float* delta, const unsigned* bits, const int* tiles, const int* tile_count, float* dq_acc,
-                     float* dk_acc, float* dv_acc, int B, int H, int Q, int Sk, int D, float softmax_scale,
-                     int* order_ws, void* stream) {
+// Backward of ringattention_inference (attn_bwd_kernel<true, true, true, kOrdered>): any Q and Sk. q16 / dout16
+// [B,Q,H,128], k16 / v16 [B,Sk,H,128] scaled fp16 copies with their device scales; lse (pre-scaled by lwm_attn_bwd_lse
+// with the fp16 offset, -inf for rows without a visible key) and delta [B,H,Qp], Qp = Q rounded up to 64, rows >= Q:
+// lse = -inf; bits [B,Q,ceil(Sk/128)*4] or null; tiles / tile_count from lwm_attn_infer_bwd_tilemap. dq_acc
+// [B,Q,H,128] fp32 is accumulated into (zero it first); dk_acc / dv_acc [B,Sk,H,128] fp32 are written. order_ws: as
+// for lwm_attn_bwd_step.
+extern "C" int lwm_attn_infer_bwd(const void* q16, const void* k16, const void* v16, const void* dout16,
+                                  const float* scale_q, const float* scale_k, const float* scale_v,
+                                  const float* scale_do, const float* lse, const float* delta, const unsigned* bits,
+                                  const int* tiles, const int* tile_count, float* dq_acc, float* dk_acc, float* dv_acc,
+                                  int B, int H, int Q, int Sk, int D, float softmax_scale, int* order_ws,
+                                  void* stream) {
   if (D != kHeadDim) return lwm_fail(LWM_ERR_SHAPE, "attn_infer_bwd: head_dim must be 128");
   if (!q16 || !k16 || !v16 || !dout16 || !scale_q || !scale_k || !scale_v || !scale_do || !lse || !delta || !tiles ||
       !tile_count || !dq_acc || !dk_acc || !dv_acc)
@@ -433,7 +368,7 @@ static int infer_bwd(const void* q16, const void* k16, const void* v16, const vo
   if ((long long)B * n_kt * (qp / kBQ) > 0x7fffffffLL || (long long)Q + kBQ > 0x7fffffffLL)
     return lwm_fail(LWM_ERR_SHAPE, "attn_infer_bwd: B * ceil(Sk/128) * ceil(Q/64) must fit in int32");
   if (order_ws && !order_fits(B, H, n_kt, qp / kBQ, true))
-    return lwm_fail(LWM_ERR_SHAPE, "attn_infer_bwd_ordered: the order_ws words and B * H * ceil(Sk/128) must fit in int32");
+    return lwm_fail(LWM_ERR_SHAPE, "attn_infer_bwd (ordered): the order_ws words and B * H * ceil(Sk/128) must fit in int32");
   if (!lwm_check_device()) return LWM_ERR_DEVICE;
   CUtensorMap tm[5];
   if (!make_bf16_tmap(&tm[0], q16, B, Q, H, kBQ) || !make_bf16_tmap(&tm[1], k16, B, Sk, H, kTile) ||
@@ -451,31 +386,7 @@ static int infer_bwd(const void* q16, const void* k16, const void* v16, const vo
   p.bits = bits; p.q_rows = Q;
   const dim3 grid(n_kt, H, B);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (order_ws) {
-    const int s = order_prologue(order_ws, (long long)B * H * (qp / kBQ), tiles, tile_count, B, n_kt, qp / kBQ, st, p);
-    if (s) return s;
-    return launch_bwd<true, true, true, true>(grid, st, tm, p, "attn_bwd_kernel (inference, ordered)");
-  }
-  return launch_bwd<true, true, true, false>(grid, st, tm, p, "attn_bwd_kernel (inference)");
-}
-
-extern "C" int lwm_attn_infer_bwd(const void* q16, const void* k16, const void* v16, const void* dout16,
-                                  const float* scale_q, const float* scale_k, const float* scale_v,
-                                  const float* scale_do, const float* lse, const float* delta, const unsigned* bits,
-                                  const int* tiles, const int* tile_count, float* dq_acc, float* dk_acc, float* dv_acc,
-                                  int B, int H, int Q, int Sk, int D, float softmax_scale, void* stream) {
-  return infer_bwd(q16, k16, v16, dout16, scale_q, scale_k, scale_v, scale_do, lse, delta, bits, tiles, tile_count,
-                   dq_acc, dk_acc, dv_acc, B, H, Q, Sk, D, softmax_scale, nullptr, stream);
-}
-
-// lwm_attn_infer_bwd with dQ reduced in ascending key-tile order (include/lwm_b200.h)
-extern "C" int lwm_attn_infer_bwd_ordered(const void* q16, const void* k16, const void* v16, const void* dout16,
-                                          const float* scale_q, const float* scale_k, const float* scale_v,
-                                          const float* scale_do, const float* lse, const float* delta,
-                                          const unsigned* bits, const int* tiles, const int* tile_count,
-                                          float* dq_acc, float* dk_acc, float* dv_acc, int B, int H, int Q, int Sk,
-                                          int D, float softmax_scale, int* order_ws, void* stream) {
-  if (!order_ws) return lwm_fail(LWM_ERR_ARG, "attn_infer_bwd_ordered: null order_ws");
-  return infer_bwd(q16, k16, v16, dout16, scale_q, scale_k, scale_v, scale_do, lse, delta, bits, tiles, tile_count,
-                   dq_acc, dk_acc, dv_acc, B, H, Q, Sk, D, softmax_scale, order_ws, stream);
+  if (!order_ws) return launch_bwd<true, true, true, false, false>(grid, st, tm, p);
+  const int s = order_prologue(order_ws, (long long)B * H * (qp / kBQ), tiles, tile_count, B, n_kt, qp / kBQ, st, p);
+  return s ? s : launch_bwd<true, true, true, true, false>(grid, st, tm, p);
 }

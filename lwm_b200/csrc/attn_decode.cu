@@ -224,7 +224,7 @@ static int decode_partial_launch(const void* q, const void* k, const void* v, co
                                  float* o_part, float* ml_part, void* workspace, int B, int H, int Q, int Sk, int D,
                                  long long k_pos0, long long mask_stride_b, long long mask_stride_q, int splits,
                                  float softmax_scale, const int* position_ids, const float* inv_freq, void* stream,
-                                 const void* k_exp = nullptr, const void* v_exp = nullptr) {
+                                 const void* k_exp, const void* v_exp) {
   if (D != kHeadDim) return lwm_fail(LWM_ERR_SHAPE, "attn_decode: head_dim must be 128");
   if (!q || !k || !v || !o_part || !ml_part || !workspace) return lwm_fail(LWM_ERR_ARG, "attn_decode: null pointer");
   if (B <= 0 || H <= 0 || Q <= 0 || Sk <= 0 || splits <= 0 || (long long)B * Q > 65535)
@@ -244,48 +244,34 @@ static int decode_partial_launch(const void* q, const void* k, const void* v, co
 }
 
 // q [B,Q,H,128], k,v [B,Sk,H,128] (this rank's KV shard), all fp32 (dtype 0: read directly, one float4 per lane and
-// row) or all bf16 (1); mask uint8 [B, ., Q, .] addressed as mask[b*mask_stride_b + q*mask_stride_q + k_pos0 + j]
+// row) or all bf16 (1); or, with k_exp / v_exp, k / v the 8-bit cache (kv_q8.cuh: data int8 [B,Sk,H,128], exp int8
+// [B,H,Sk,4]) and dtype q's: the partials then equal, bit for bit, those on the cache dequantized to q's dtype
+// (lwm_kv_dequant_q8). mask uint8 [B, ., Q, .] addressed as mask[b*mask_stride_b + q*mask_stride_q + k_pos0 + j]
 // (nonzero = attend) or NULL; o_part [B*Q*H, 128] fp32 + ml_part [B*Q*H, 2] fp32 : this rank's partial (numerator,
 // (max_log2, denominator)); workspace: splits * B*Q*H * (128 + 2) floats. position_ids int32 [B,Q] and inv_freq [64]
 // (as for lwm_attn_rope), or both null: q is un-rotated and is rotated as it is loaded, so the result equals
 // lwm_attn_rope (out_dtype = q's) followed by the call without them, bit for bit.
-extern "C" int lwm_attn_decode_partial(const void* q, const void* k, const void* v, int dtype, const unsigned char* mask,
-                                       float* o_part, float* ml_part, void* workspace, int B, int H, int Q, int Sk,
-                                       int D, long long k_pos0, long long mask_stride_b, long long mask_stride_q,
-                                       int splits, float softmax_scale, const int* position_ids, const float* inv_freq,
+extern "C" int lwm_attn_decode_partial(const void* q, const void* k, const void* v, int dtype, const signed char* k_exp,
+                                       const signed char* v_exp, const unsigned char* mask, float* o_part,
+                                       float* ml_part, void* workspace, int B, int H, int Q, int Sk, int D,
+                                       long long k_pos0, long long mask_stride_b, long long mask_stride_q, int splits,
+                                       float softmax_scale, const int* position_ids, const float* inv_freq,
                                        void* stream) {
   if (dtype != 0 && dtype != 1) return lwm_fail(LWM_ERR_ARG, "attn_decode: dtype codes are 0 (fp32) or 1 (bf16)");
   if (!position_ids != !inv_freq) return lwm_fail(LWM_ERR_ARG, "attn_decode: null position_ids / inv_freq");
-  const bool rope = position_ids != nullptr;
-  auto* launch = dtype == 1 ? (rope ? decode_partial_launch<__nv_bfloat16, true>
-                                   : decode_partial_launch<__nv_bfloat16, false>)
-                            : (rope ? decode_partial_launch<float, true> : decode_partial_launch<float, false>);
-  return launch(q, k, v, mask, o_part, ml_part, workspace, B, H, Q, Sk, D, k_pos0, mask_stride_b, mask_stride_q, splits,
-                softmax_scale, position_ids, inv_freq, stream, nullptr, nullptr);
-}
-
-// lwm_attn_decode_partial on the 8-bit cache (kv_q8.cuh): k / v data int8 [B,Sk,H,128] and exp int8 [B,H,Sk,4] of
-// this rank's shard, q fp32 (q_dtype 0) or bf16 (1); everything else as lwm_attn_decode_partial. The partials equal,
-// bit for bit, lwm_attn_decode_partial's on the cache dequantized to q's dtype (lwm_kv_dequant_q8).
-extern "C" int lwm_attn_decode_partial_q8(const void* q, int q_dtype, const signed char* k, const signed char* k_exp,
-                                          const signed char* v, const signed char* v_exp, const unsigned char* mask,
-                                          float* o_part, float* ml_part, void* workspace, int B, int H, int Q, int Sk,
-                                          int D, long long k_pos0, long long mask_stride_b, long long mask_stride_q,
-                                          int splits, float softmax_scale, const int* position_ids,
-                                          const float* inv_freq, void* stream) {
-  if (q_dtype != 0 && q_dtype != 1) return lwm_fail(LWM_ERR_ARG, "attn_decode_q8: q dtype codes are 0 (fp32) or 1 (bf16)");
-  if (!position_ids != !inv_freq) return lwm_fail(LWM_ERR_ARG, "attn_decode_q8: null position_ids / inv_freq");
-  if (!k_exp || !v_exp) return lwm_fail(LWM_ERR_ARG, "attn_decode_q8: null pointer");
-  if (((reinterpret_cast<size_t>(k) | reinterpret_cast<size_t>(v) | reinterpret_cast<size_t>(k_exp) |
-        reinterpret_cast<size_t>(v_exp)) & 3) != 0)
-    return lwm_fail(LWM_ERR_ARG, "attn_decode_q8: data and exp must be 4-byte aligned");
-  const bool rope = position_ids != nullptr;
-  using S8 = signed char;
-  auto* launch = q_dtype == 1 ? (rope ? decode_partial_launch<__nv_bfloat16, true, S8>
-                                      : decode_partial_launch<__nv_bfloat16, false, S8>)
-                              : (rope ? decode_partial_launch<float, true, S8> : decode_partial_launch<float, false, S8>);
-  return launch(q, k, v, mask, o_part, ml_part, workspace, B, H, Q, Sk, D, k_pos0, mask_stride_b, mask_stride_q, splits,
-                softmax_scale, position_ids, inv_freq, stream, k_exp, v_exp);
+  if (!k_exp != !v_exp)
+    return lwm_fail(LWM_ERR_ARG, "attn_decode: null pointer: k_exp and v_exp are both given (8-bit cache) or both null");
+  const bool q8 = k_exp != nullptr;
+  if (q8 && ((reinterpret_cast<size_t>(k) | reinterpret_cast<size_t>(v) | reinterpret_cast<size_t>(k_exp) |
+              reinterpret_cast<size_t>(v_exp)) & 3) != 0)
+    return lwm_fail(LWM_ERR_ARG, "attn_decode: the 8-bit cache's data and exp must be 4-byte aligned");
+  return with_flags([&](auto bf16, auto rope, auto cache8) {
+    using T = std::conditional_t<bf16, __nv_bfloat16, float>;
+    using KV = std::conditional_t<cache8, signed char, T>;
+    return decode_partial_launch<T, rope, KV>(q, k, v, mask, o_part, ml_part, workspace, B, H, Q, Sk, D, k_pos0,
+                                              mask_stride_b, mask_stride_q, splits, softmax_scale, position_ids,
+                                              inv_freq, stream, k_exp, v_exp);
+  }, dtype == 1, position_ids != nullptr, q8);
 }
 
 // merge n_part partials per row (e.g. the all-gathered per-rank partials) into out, bf16 (out_dtype 1) or the

@@ -39,6 +39,12 @@ struct DropParams {
   uint32_t batch0;             // global batch row of the launch's batch row 0 (blockIdx.z / the CTA's b is added)
 };
 
+// attn_dropout.cu: the dropout arguments (seed, drop_threshold, batch0) of a tile-kernel launch over B batch rows and
+// H heads from global positions q_pos0 / k_pos0, checked and decoded into *drop. drop_threshold 0 is no dropout
+// (drop->thr = 0, seed unused). Returns LWM_OK, or the status of the first failed check with `what` leading the message.
+int decode_drop_params(long long seed, unsigned drop_threshold, int batch0, int B, int H, long long q_pos0,
+                       long long k_pos0, const char* what, DropParams* drop);
+
 LWM_DEVICE uint32_t drop_ctr0(uint32_t k) { return ((k >> 4) << 2) | ((k >> 1) & 3u); }
 
 // The Philox block of queries {q, q + 8} and keys {k, k + 1, k + 8, k + 9} (bit 3 of q and bits 0, 3 of k ignored);

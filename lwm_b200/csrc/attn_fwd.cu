@@ -496,31 +496,36 @@ static bool make_qkv_tmap(CUtensorMap* tm, const void* ptr, int B, int S, int H)
 
 using namespace lwm;
 
-template <bool kF16, bool kMap>
-static int launch_fwd_dropout(dim3 grid, cudaStream_t st, const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
-                      const FwdParams& p, const char* what) {
+// One attn_fwd_kernel or attn_fwd_dropout_kernel instance; its dynamic shared-memory limit is raised once per device.
+template <bool kF16, bool kInfer, bool kMap, bool kDrop>
+static int launch_fwd(dim3 grid, cudaStream_t st, const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
+                      const FwdParams& p) {
+  static_assert(!(kInfer && (kMap || kDrop)), "the inference mode has no block-map or dropout instance");
+  void (*kernel)(CUtensorMap, CUtensorMap, CUtensorMap, FwdParams);
+  if constexpr (kDrop) kernel = attn_fwd_dropout_kernel<kF16, kMap>;
+  else kernel = attn_fwd_kernel<kF16, kInfer, kMap>;
   static bool attr_set_dev[64] = {};
   int cur_dev = 0;
   cudaGetDevice(&cur_dev);
   bool& attr_set = attr_set_dev[cur_dev & 63];      // function attributes are per device
   if (!attr_set) {
-    if (cudaFuncSetAttribute(attn_fwd_dropout_kernel<kF16, kMap>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             kFwdSmemBytes) != cudaSuccess)
+    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kFwdSmemBytes) != cudaSuccess)
       return lwm_fail(LWM_ERR_CUDA, "attn_fwd: cannot raise dynamic shared memory limit");
     attr_set = true;
   }
-  attn_fwd_dropout_kernel<kF16, kMap><<<grid, kFwdThreads, kFwdSmemBytes, st>>>(tq, tk, tv, p);
-  return lwm_check_launch(what);
+  kernel<<<grid, kFwdThreads, kFwdSmemBytes, st>>>(tq, tk, tv, p);
+  return lwm_check_launch(kDrop ? "attn_fwd_dropout_kernel" : kInfer ? "attn_fwd_kernel (inference)" : "attn_fwd_kernel");
 }
 
 // One ring step (include/lwm_b200.h): the scales select the fp16-operand kernel, tiles / tile_count the block map,
-// drop (null: no dropout) the dropout instances.
-static int fwd_step(const void* q, const void* k, const void* v, const float* scale_q, const float* scale_k,
-                    const float* scale_v, float* out_f32, void* out, float* lse, float* acc_o, float* acc_m,
-                    float* acc_l, int B, int H, int Sq, int Sk, int D, long long q_pos0, long long k_pos0, int causal,
-                    const float* bias, long long bias_stride, const int* segment_ids, long long seg_stride,
-                    float softmax_scale, int first, int last, const int* tiles, const int* tile_count,
-                    const DropParams* drop, void* stream) {
+// drop_threshold > 0 the dropout instances.
+extern "C" int lwm_attn_fwd_step(const void* q, const void* k, const void* v, const float* scale_q,
+                                 const float* scale_k, const float* scale_v, float* out_f32, void* out, float* lse,
+                                 float* acc_o, float* acc_m, float* acc_l, int B, int H, int Sq, int Sk, int D,
+                                 long long q_pos0, long long k_pos0, int causal, const float* bias,
+                                 long long bias_stride, const int* segment_ids, long long seg_stride,
+                                 float softmax_scale, int first, int last, const int* tiles, const int* tile_count,
+                                 long long seed, unsigned drop_threshold, int batch0, void* stream) {
   if (!scale_k != !scale_q || !scale_v != !scale_q)
     return lwm_fail(LWM_ERR_ARG, "attn_fwd: scales are all given (fp16 operands) or all null (bf16)");
   if (out_f32 && !scale_q) return lwm_fail(LWM_ERR_ARG, "attn_fwd: out_f32 needs the fp16 operand scales");
@@ -539,10 +544,8 @@ static int fwd_step(const void* q, const void* k, const void* v, const float* sc
     return lwm_fail(LWM_ERR_SHAPE, "attn_fwd: bias is indexed by GLOBAL key position: bias_stride < k_pos0 + Sk");
   if (segment_ids && (seg_stride < q_pos0 + Sq || seg_stride < k_pos0 + Sk))
     return lwm_fail(LWM_ERR_SHAPE, "attn_fwd: segment_ids is indexed by GLOBAL position: seg_stride < max(q_pos0 + Sq, k_pos0 + Sk)");
-  if (drop && (q_pos0 % kTile || k_pos0 % kTile))
-    return lwm_fail(LWM_ERR_SHAPE, "attn_fwd_dropout: q_pos0 and k_pos0 must each be a multiple of 128");
-  if (drop && (B > 65535 || H > 65535 || (long long)drop->batch0 + B > 0x7fffffffLL))
-    return lwm_fail(LWM_ERR_SHAPE, "attn_fwd_dropout: B, H <= 65535 and batch0 + B < 2^31");
+  DropParams drop;
+  if (const int s = decode_drop_params(seed, drop_threshold, batch0, B, H, q_pos0, k_pos0, "attn_fwd", &drop)) return s;
   if (!lwm_check_device()) return LWM_ERR_DEVICE;
   CUtensorMap tq, tk, tv;
   if (!make_qkv_tmap(&tq, q, B, Sq, H) || !make_qkv_tmap(&tk, k, B, Sk, H) || !make_qkv_tmap(&tv, v, B, Sk, H))
@@ -560,72 +563,12 @@ static int fwd_step(const void* q, const void* k, const void* v, const float* sc
   p.out_f32 = out_f32;
   p.bits = nullptr; p.tiles = tiles; p.tile_count = tile_count;
   p.n_kt = Sk / kTile; p.splits = 1;
-  if (drop) {
-    p.drop = *drop;
-    dim3 grid(Sq / kTile, H, B);
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    if (tiles)
-      return scale_q ? launch_fwd_dropout<true, true>(grid, st, tq, tk, tv, p, "attn_fwd_dropout_kernel (block map)")
-                     : launch_fwd_dropout<false, true>(grid, st, tq, tk, tv, p, "attn_fwd_dropout_kernel (block map)");
-    return scale_q ? launch_fwd_dropout<true, false>(grid, st, tq, tk, tv, p, "attn_fwd_dropout_kernel")
-                   : launch_fwd_dropout<false, false>(grid, st, tq, tk, tv, p, "attn_fwd_dropout_kernel");
-  }
-  static bool attr_set_dev[64] = {};
-  int cur_dev = 0;
-  cudaGetDevice(&cur_dev);
-  bool& attr_set = attr_set_dev[cur_dev & 63];      // function attributes are per device
-  if (!attr_set) {
-    if (cudaFuncSetAttribute(attn_fwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFwdSmemBytes) !=
-            cudaSuccess ||
-        cudaFuncSetAttribute(attn_fwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFwdSmemBytes) !=
-            cudaSuccess ||
-        cudaFuncSetAttribute(attn_fwd_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             kFwdSmemBytes) != cudaSuccess ||
-        cudaFuncSetAttribute(attn_fwd_kernel<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             kFwdSmemBytes) != cudaSuccess)
-      return lwm_fail(LWM_ERR_CUDA, "attn_fwd: cannot raise dynamic shared memory limit");
-    attr_set = true;
-  }
-  dim3 grid(Sq / kTile, H, B);
+  p.drop = drop;
+  const dim3 grid(Sq / kTile, H, B);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (tiles) {
-    if (scale_q) attn_fwd_kernel<true, false, true><<<grid, kFwdThreads, kFwdSmemBytes, st>>>(tq, tk, tv, p);
-    else attn_fwd_kernel<false, false, true><<<grid, kFwdThreads, kFwdSmemBytes, st>>>(tq, tk, tv, p);
-    return lwm_check_launch("attn_fwd_kernel (block map)");
-  }
-  if (scale_q) attn_fwd_kernel<true><<<grid, kFwdThreads, kFwdSmemBytes, st>>>(tq, tk, tv, p);
-  else attn_fwd_kernel<false><<<grid, kFwdThreads, kFwdSmemBytes, st>>>(tq, tk, tv, p);
-  return lwm_check_launch("attn_fwd_kernel");
-}
-
-extern "C" int lwm_attn_fwd_step(const void* q, const void* k, const void* v, const float* scale_q,
-                                 const float* scale_k, const float* scale_v, float* out_f32, void* out, float* lse,
-                                 float* acc_o, float* acc_m, float* acc_l, int B, int H, int Sq, int Sk, int D,
-                                 long long q_pos0, long long k_pos0, int causal, const float* bias,
-                                 long long bias_stride, const int* segment_ids, long long seg_stride,
-                                 float softmax_scale, int first, int last, const int* tiles, const int* tile_count,
-                                 void* stream) {
-  return fwd_step(q, k, v, scale_q, scale_k, scale_v, out_f32, out, lse, acc_o, acc_m, acc_l, B, H, Sq, Sk, D, q_pos0,
-                  k_pos0, causal, bias, bias_stride, segment_ids, seg_stride, softmax_scale, first, last, tiles,
-                  tile_count, nullptr, stream);
-}
-
-// lwm_attn_fwd_step with attention dropout (include/lwm_b200.h)
-extern "C" int lwm_attn_fwd_step_dropout(const void* q, const void* k, const void* v, const float* scale_q,
-                                         const float* scale_k, const float* scale_v, float* out_f32, void* out,
-                                         float* lse, float* acc_o, float* acc_m, float* acc_l, int B, int H, int Sq,
-                                         int Sk, int D, long long q_pos0, long long k_pos0, int causal,
-                                         const float* bias, long long bias_stride, const int* segment_ids,
-                                         long long seg_stride, float softmax_scale, int first, int last,
-                                         const int* tiles, const int* tile_count, long long seed,
-                                         unsigned drop_threshold, int batch0, void* stream) {
-  if (drop_threshold == 0 || drop_threshold > 65535)
-    return lwm_fail(LWM_ERR_ARG, "attn_fwd_dropout: drop_threshold must be in [1, 65535] (0 is lwm_attn_fwd_step)");
-  if (batch0 < 0) return lwm_fail(LWM_ERR_ARG, "attn_fwd_dropout: batch0 must be >= 0");
-  const DropParams d = {uint32_t(uint64_t(seed)), uint32_t(uint64_t(seed) >> 32), drop_threshold, uint32_t(batch0)};
-  return fwd_step(q, k, v, scale_q, scale_k, scale_v, out_f32, out, lse, acc_o, acc_m, acc_l, B, H, Sq, Sk, D, q_pos0,
-                  k_pos0, causal, bias, bias_stride, segment_ids, seg_stride, softmax_scale, first, last, tiles,
-                  tile_count, &d, stream);
+  return with_flags([&](auto f16, auto map, auto dropout) {
+    return launch_fwd<f16, false, map, dropout>(grid, st, tq, tk, tv, p);
+  }, scale_q != nullptr, tiles != nullptr, drop.thr != 0);
 }
 
 // Inference mode (ringattention_inference with Q >= kInferMinQ rows): q16 [B,Q,H,128], k16/v16 [B,Sk,H,128] scaled fp16
@@ -660,18 +603,9 @@ extern "C" int lwm_attn_infer_partial(const void* q16, const void* k16, const vo
   p.splits = splits;
   p.o_part = splits > 1 ? reinterpret_cast<float*>(workspace) : o_part;
   p.ml_part = splits > 1 ? reinterpret_cast<float*>(workspace) + rows * splits * kHeadDim : ml_part;
-  static bool attr_set_dev[64] = {};
-  int cur_dev = 0;
-  cudaGetDevice(&cur_dev);
-  bool& attr_set = attr_set_dev[cur_dev & 63];
-  if (!attr_set) {
-    if (cudaFuncSetAttribute(attn_fwd_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             kFwdSmemBytes) != cudaSuccess)
-      return lwm_fail(LWM_ERR_CUDA, "attn_infer_partial: cannot raise dynamic shared memory limit");
-    attr_set = true;
-  }
-  dim3 grid(unsigned((Q + kTile - 1) / kTile * splits), H, B);
-  attn_fwd_kernel<true, true><<<grid, kFwdThreads, kFwdSmemBytes, st>>>(tq, tk, tv, p);
-  if (splits > 1) lwm_decode_merge_partials(p.o_part, p.ml_part, splits, o_part, ml_part, rows, st);
-  return lwm_check_launch("attn_fwd_kernel (inference)");
+  const dim3 grid(unsigned((Q + kTile - 1) / kTile * splits), H, B);
+  const int s = launch_fwd<true, true, false, false>(grid, st, tq, tk, tv, p);
+  if (s || splits == 1) return s;
+  lwm_decode_merge_partials(p.o_part, p.ml_part, splits, o_part, ml_part, rows, st);
+  return lwm_check_launch("decode_merge_kernel");
 }

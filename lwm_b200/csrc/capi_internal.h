@@ -1,6 +1,7 @@
 // Internal helpers shared by the C-ABI entry points (status codes, last-error string, device check).
 #pragma once
 #include <cuda_runtime.h>
+#include <type_traits>
 
 enum {
   LWM_OK = 0,
@@ -13,6 +14,18 @@ enum {
 int lwm_fail(int code, const char* msg);          // records msg, returns code
 bool lwm_check_device();                          // true iff current device is compute capability 9.x
 int lwm_check_launch(const char* what);           // cudaGetLastError -> status
+
+// with_flags(f, b0, b1, ...) = f(std::bool_constant<b0>{}, std::bool_constant<b1>{}, ...): turns an entry point's
+// run-time options into the template arguments of the kernel instance that serves them, in one place.
+template <typename F>
+static int with_flags(F&& f) {
+  return f();
+}
+template <typename F, typename... Bs>
+static int with_flags(F&& f, bool b, Bs... rest) {
+  if (b) return with_flags([&](auto... t) { return f(std::true_type{}, t...); }, rest...);
+  return with_flags([&](auto... t) { return f(std::false_type{}, t...); }, rest...);
+}
 
 // SM count of the H100 SXM: cap of the grid-stride launches (one or a few waves of resident blocks)
 constexpr long long kNumSMs = 132;

@@ -351,20 +351,17 @@ def fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bia
     """scales: None (bf16 operands), or the device scales (sq, sk, sv) of fp16 operand copies q/k/v; out_f32 (fp16
     operands only): the un-rounded output, written on the last step. tilemap: None, or the forward map (tiles, counts)
     of step_tilemap for these arguments: the tile kernel then visits only the KV tiles in it (same results, bit for
-    bit). dropout: None, or (seed, thr) of attention dropout (lwm_attn_fwd_step_dropout), or (seed, thr, batch0) when
-    q ... are rows batch0 .. batch0 + B - 1 of a larger batch (each batch row draws its own mask)."""
+    bit). dropout: None, or (seed, thr) of attention dropout, or (seed, thr, batch0) when q ... are rows
+    batch0 .. batch0 + B - 1 of a larger batch (each batch row draws its own mask)."""
     B, Sq, H, D = q.shape
     sq, sk, sv = scales if scales is not None else (None, None, None)
     tiles, counts = tilemap if tilemap is not None else (None, None)
-    args = (_lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(sq), _lib.ptr(sk), _lib.ptr(sv), _lib.ptr(out_f32),
-            _lib.ptr(out), _lib.ptr(lse), _lib.ptr(acc_o), _lib.ptr(acc_m), _lib.ptr(acc_l), B, H, Sq, k.shape[1], D,
-            int(q_pos0), int(k_pos0), int(bool(causal)), _lib.ptr(bias), 0 if bias is None else bias.shape[1],
-            _lib.ptr(seg), 0 if seg is None else seg.shape[1], 1.0 / math.sqrt(D), int(first), int(last),
-            _lib.ptr(tiles), _lib.ptr(counts))
-    if dropout is None:
-        _lib.call("lwm_attn_fwd_step", *args, _lib.stream_ptr(stream))
-    else:
-        _lib.call("lwm_attn_fwd_step_dropout", *args, *_drop_args(dropout), _lib.stream_ptr(stream))
+    _lib.call("lwm_attn_fwd_step", _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(sq), _lib.ptr(sk), _lib.ptr(sv),
+              _lib.ptr(out_f32), _lib.ptr(out), _lib.ptr(lse), _lib.ptr(acc_o), _lib.ptr(acc_m), _lib.ptr(acc_l), B, H,
+              Sq, k.shape[1], D, int(q_pos0), int(k_pos0), int(bool(causal)), _lib.ptr(bias),
+              0 if bias is None else bias.shape[1], _lib.ptr(seg), 0 if seg is None else seg.shape[1],
+              1.0 / math.sqrt(D), int(first), int(last), _lib.ptr(tiles), _lib.ptr(counts), *_drop_args(dropout),
+              _lib.stream_ptr(stream))
 
 
 def bwd_prep(out, dout, delta, stream=None, scale_do=None):
@@ -388,8 +385,8 @@ def lse_for_bwd(lse, stream=None, f16=False):
 
 
 def order_workspace(words, device):
-    """the int32 workspace of an ordered dQ reduction (include/lwm_b200.h: lwm_attn_bwd_step_ordered); the call zeroes
-    it on its stream. Word 1 is the call's error flag."""
+    """the int32 workspace of an ordered dQ reduction (include/lwm_b200.h: lwm_attn_bwd_step's order_ws); the call
+    zeroes it on its stream. Word 1 is the call's error flag."""
     return torch.empty(words, dtype=torch.int32, device=device)
 
 
@@ -399,26 +396,20 @@ def bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, 
     fp16 operand copies q/k/v/dout. init=True: dk_acc/dv_acc rows are written, not accumulated.
     tilemap: None, or the backward map (tiles, counts) of step_tilemap for these arguments (dK, dV bit-identical; dQ
     up to the order of its reductions).
-    Under torch.use_deterministic_algorithms(True) dQ is reduced in ascending key-tile order
-    (lwm_attn_bwd_step_ordered): the same bits on every run. dropout: None, or the forward's (seed, thr)
-    (lwm_attn_bwd_step_dropout)."""
+    Under torch.use_deterministic_algorithms(True) dQ is reduced in ascending key-tile order (an order_ws
+    workspace): the same bits on every run. dropout: None, or the forward's (seed, thr)."""
     B, Sq, H, D = q.shape
     sq, sk, sv, sdo = scales if scales is not None else (None, None, None, None)
     tiles, counts = tilemap if tilemap is not None else (None, None)
-    args = (_lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(dout), _lib.ptr(sq), _lib.ptr(sk), _lib.ptr(sv),
-            _lib.ptr(sdo), _lib.ptr(lse), _lib.ptr(delta), _lib.ptr(dq_acc), _lib.ptr(dk_acc), _lib.ptr(dv_acc), B, H,
-            Sq, k.shape[1], D, int(q_pos0), int(k_pos0), int(bool(causal)), _lib.ptr(bias),
-            0 if bias is None else bias.shape[1], _lib.ptr(seg), 0 if seg is None else seg.shape[1], 1.0 / math.sqrt(D),
-            int(bool(init)), _lib.ptr(tiles), _lib.ptr(counts))
     ws = None
     if torch.are_deterministic_algorithms_enabled():
         ws = order_workspace(2 + B * H * (Sq // 64) + (0 if tiles is None else tiles.numel()), q.device)
-    if dropout is not None:
-        _lib.call("lwm_attn_bwd_step_dropout", *args, _lib.ptr(ws), *_drop_args(dropout), _lib.stream_ptr(stream))
-    elif ws is not None:
-        _lib.call("lwm_attn_bwd_step_ordered", *args, _lib.ptr(ws), _lib.stream_ptr(stream))
-    else:
-        _lib.call("lwm_attn_bwd_step", *args, _lib.stream_ptr(stream))
+    _lib.call("lwm_attn_bwd_step", _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _lib.ptr(dout), _lib.ptr(sq), _lib.ptr(sk),
+              _lib.ptr(sv), _lib.ptr(sdo), _lib.ptr(lse), _lib.ptr(delta), _lib.ptr(dq_acc), _lib.ptr(dk_acc),
+              _lib.ptr(dv_acc), B, H, Sq, k.shape[1], D, int(q_pos0), int(k_pos0), int(bool(causal)), _lib.ptr(bias),
+              0 if bias is None else bias.shape[1], _lib.ptr(seg), 0 if seg is None else seg.shape[1], 1.0 / math.sqrt(D),
+              int(bool(init)), _lib.ptr(tiles), _lib.ptr(counts), _lib.ptr(ws), *_drop_args(dropout),
+              _lib.stream_ptr(stream))
 
 
 def _map_kw(q, k, q_pos0, k_pos0, causal, bias, seg, fwd):
@@ -442,14 +433,12 @@ def mapped_bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k
 
 
 def _drop_args(dropout):
-    """(seed, thr) or (seed, thr, batch0) -> the seed, drop_threshold and batch0 arguments of the _dropout symbols"""
+    """None, (seed, thr) or (seed, thr, batch0) -> the seed, drop_threshold and batch0 arguments of the step calls
+    (drop_threshold 0: no dropout)"""
+    if dropout is None:
+        return 0, 0, 0
     seed, thr, batch0 = tuple(dropout) + (0,) * (3 - len(dropout))
     return int(seed), int(thr), int(batch0)
-
-
-def _drop_kw(dropout):
-    """the `dropout` keyword of a step call: absent without dropout, so the plain call is unchanged"""
-    return {} if dropout is None else {"dropout": dropout}
 
 
 def cast_f32_to_bf16(src, dst, stream=None):
@@ -491,25 +480,23 @@ class CudaOpsF16(CudaOps):
             self._cache[key] = hit
         return hit[0], hit[1]
 
-    def fwd_step(self, q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last,
-                 dropout=None):
+    def fwd_step(self, q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last, **kw):
         (q16, sq), (k16, sk), (v16, sv) = self._f16(q), self._f16(k), self._f16(v)
         o32 = None
         if last:
             o32 = torch.empty(out.shape, dtype=torch.float32, device=out.device)
             self.out_f32[out.data_ptr()] = o32
         mapped_fwd_step(q16, k16, v16, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last,
-                        scales=(sq, sk, sv), out_f32=o32, **_drop_kw(dropout))
+                        scales=(sq, sk, sv), out_f32=o32, **kw)
 
     @staticmethod
     def lse_for_bwd(lse):
         return lse_for_bwd(lse, f16=True)
 
-    def bwd_step(self, q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg,
-                 dropout=None):
+    def bwd_step(self, q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg, **kw):
         (q16, sq), (k16, sk), (v16, sv), (d16, sd) = self._f16(q), self._f16(k), self._f16(v), self._f16(dout)
         mapped_bwd_step(q16, k16, v16, d16, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg,
-                        scales=(sq, sk, sv, sd), **_drop_kw(dropout))
+                        scales=(sq, sk, sv, sd), **kw)
 
 
 class DropoutOps:
@@ -585,9 +572,9 @@ class PeerOpsF16:
 
     @staticmethod
     def fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last, scales, out_f32,
-                 dropout=None):
+                 **kw):
         mapped_fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last,
-                        scales=scales, out_f32=out_f32, **_drop_kw(dropout))
+                        scales=scales, out_f32=out_f32, **kw)
 
     @staticmethod
     def bwd_prep(out, dout, sdo, delta):
@@ -599,9 +586,9 @@ class PeerOpsF16:
 
     @staticmethod
     def bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg, scales, init,
-                 dropout=None):
+                 **kw):
         mapped_bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg,
-                        scales=scales, init=init, **_drop_kw(dropout))
+                        scales=scales, init=init, **kw)
 
     @staticmethod
     def reduce_cast(srcs, dst):
@@ -659,9 +646,8 @@ class PeerOpsBf16(PeerOpsF16):
 
     @staticmethod
     def fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last, scales, out_f32,
-                 dropout=None):
-        mapped_fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last,
-                        **_drop_kw(dropout))
+                 **kw):
+        mapped_fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last, **kw)
         if last and out_f32 is not None:
             out_f32.copy_(out)
 
@@ -671,9 +657,9 @@ class PeerOpsBf16(PeerOpsF16):
 
     @staticmethod
     def bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg, scales, init,
-                 dropout=None):
+                 **kw):
         mapped_bwd_step(q, k, v, dout, lse, delta, dq_acc, dk_acc, dv_acc, q_pos0, k_pos0, causal, bias, seg, init=init,
-                        **_drop_kw(dropout))
+                        **kw)
 
 
 _PEER_BROKEN = {}      # process group id -> reason: the peer-memory heaps could not be set up for this group
@@ -874,13 +860,11 @@ def decode_partial(q, k, v, mask_u8, k_pos0, stream=None, rope=None):
     if mask_u8 is not None:
         sb, sq = mask_u8.stride(0), mask_u8.stride(-2)
     pos, inv_freq = rope if rope is not None else (None, None)
-    tail = (_lib.ptr(mask_u8), _lib.ptr(o_part), _lib.ptr(ml_part), _lib.ptr(ws), B, H, Q, Sk, D, int(k_pos0), int(sb),
-            int(sq), splits, 1.0 / math.sqrt(D), _lib.ptr(pos), _lib.ptr(inv_freq), _lib.stream_ptr(stream))
-    if k.dtype == torch.int8:       # the 8-bit cache
-        _lib.call("lwm_attn_decode_partial_q8", _lib.ptr(q), _dt(q), _lib.ptr(k.data), _lib.ptr(k.exp),
-                  _lib.ptr(v.data), _lib.ptr(v.exp), *tail)
-    else:
-        _lib.call("lwm_attn_decode_partial", _lib.ptr(q), _lib.ptr(k), _lib.ptr(v), _dt(q), *tail)
+    q8 = k.dtype == torch.int8      # the 8-bit cache
+    _lib.call("lwm_attn_decode_partial", _lib.ptr(q), _lib.ptr(k.data if q8 else k), _lib.ptr(v.data if q8 else v),
+              _dt(q), _lib.ptr(k.exp if q8 else None), _lib.ptr(v.exp if q8 else None), _lib.ptr(mask_u8),
+              _lib.ptr(o_part), _lib.ptr(ml_part), _lib.ptr(ws), B, H, Q, Sk, D, int(k_pos0), int(sb), int(sq), splits,
+              1.0 / math.sqrt(D), _lib.ptr(pos), _lib.ptr(inv_freq), _lib.stream_ptr(stream))
     return o_part, ml_part
 
 
@@ -966,7 +950,7 @@ def infer_backward(q16, k16, v16, do16, scales, lse, delta, bits, row_any):
     scaled fp16 copies, scales = (sq, sk, sv, sdo); lse [B,H,Q] (natural log, -inf for rows with no visible key),
     delta [B,H,Q] = rowsum(dO o O); bits [B,Q,kw] / row_any [B,Q] (over the whole ring) or None
     -> fp32 (dq [B,Q,H,128], dk, dv [B,Sk,H,128]). Under torch.use_deterministic_algorithms(True) dQ is reduced in
-    ascending key-tile order (lwm_attn_infer_bwd_ordered), as in bwd_step."""
+    ascending key-tile order, as in bwd_step."""
     B, Q, H, D = q16.shape
     Sk = k16.shape[1]
     dev = q16.device
@@ -985,14 +969,13 @@ def infer_backward(q16, k16, v16, do16, scales, lse, delta, bits, row_any):
     dk = torch.empty((B, Sk, H, D), dtype=torch.float32, device=dev)
     dv = torch.empty((B, Sk, H, D), dtype=torch.float32, device=dev)
     sq, sk, sv, sdo = scales
-    args = (_lib.ptr(q16), _lib.ptr(k16), _lib.ptr(v16), _lib.ptr(do16), _lib.ptr(sq), _lib.ptr(sk), _lib.ptr(sv),
-            _lib.ptr(sdo), _lib.ptr(nlse), _lib.ptr(delta_p), _lib.ptr(bits), _lib.ptr(tiles), _lib.ptr(counts),
-            _lib.ptr(dq), _lib.ptr(dk), _lib.ptr(dv), B, H, Q, Sk, D, 1.0 / math.sqrt(D))
+    ws = None
     if torch.are_deterministic_algorithms_enabled():
         ws = order_workspace(2 + B * H * (Qp // 64) + tiles.numel(), dev)
-        _lib.call("lwm_attn_infer_bwd_ordered", *args, _lib.ptr(ws), _lib.stream_ptr())
-    else:
-        _lib.call("lwm_attn_infer_bwd", *args, _lib.stream_ptr())
+    _lib.call("lwm_attn_infer_bwd", _lib.ptr(q16), _lib.ptr(k16), _lib.ptr(v16), _lib.ptr(do16), _lib.ptr(sq),
+              _lib.ptr(sk), _lib.ptr(sv), _lib.ptr(sdo), _lib.ptr(nlse), _lib.ptr(delta_p), _lib.ptr(bits),
+              _lib.ptr(tiles), _lib.ptr(counts), _lib.ptr(dq), _lib.ptr(dk), _lib.ptr(dv), B, H, Q, Sk, D,
+              1.0 / math.sqrt(D), _lib.ptr(ws), _lib.stream_ptr())
     return dq, dk, dv
 
 

@@ -16,18 +16,23 @@ def _declared():
     return sorted(set(re.findall(r"\b(lwm_[a-z0-9_]+)\s*\(", src)))
 
 
-def test_library_exports_every_declared_symbol_and_its_abi_version(lib):
+def test_library_exports_every_declared_symbol_and_no_folded_variant(lib):
     names = _declared()
     assert len(names) >= 13
     for n in names:
         assert hasattr(lib, n), "liblwm_b200.so does not export %s" % n
-    # version 4: the attention passes take their options as nullable arguments of one entry point each
-    # (lwm_attn_fwd_step / lwm_attn_bwd_step: scales, block map; lwm_attn_bwd_prep: out dtype, scale_do;
-    # lwm_attn_decode_partial: dtype, position_ids / inv_freq; lwm_attn_decode_merge: out dtype), and the per-option
-    # variants of them are no longer exported
+    # version 5: the attention passes take their options as nullable arguments of one entry point each
+    # (lwm_attn_fwd_step: scales, block map, dropout; lwm_attn_bwd_step: the same and order_ws; lwm_attn_bwd_prep: out
+    # dtype, scale_do; lwm_attn_decode_partial: dtype, the 8-bit cache's k_exp / v_exp, position_ids / inv_freq;
+    # lwm_attn_infer_bwd: order_ws; lwm_attn_decode_merge: out dtype), and the per-option variants of them are neither
+    # declared nor exported
     src = open(os.path.join(ROOT, "include", "lwm_b200.h")).read()
-    assert re.search(r"#define LWM_B200_ABI_VERSION 4\b", src)
-    assert lib.lwm_abi_version() == 4
+    assert re.search(r"#define LWM_B200_ABI_VERSION 5\b", src)
+    assert lib.lwm_abi_version() == 5
+    for gone in ("lwm_attn_fwd_step_dropout", "lwm_attn_bwd_step_dropout", "lwm_attn_bwd_step_ordered",
+                 "lwm_attn_infer_bwd_ordered", "lwm_attn_decode_partial_q8"):
+        assert gone not in names and not re.search(r"\b%s\b" % gone, src), gone
+        assert not hasattr(lib, gone), "liblwm_b200.so still exports %s" % gone
 
 
 def test_python_binding_covers_header():

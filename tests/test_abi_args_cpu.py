@@ -7,7 +7,7 @@ import ctypes
 import pytest
 import torch
 
-from helpers import abi_row_id
+from helpers import FOLDED_ENTRY_POINTS, abi_row_id, with_options
 
 P = ctypes.c_void_p(0x1000)      # fake non-null pointer
 N = None
@@ -24,20 +24,20 @@ BAD_CALLS = [
     # (entry, args, expected status, message fragment)
     # lwm_attn_fwd_step(q, k, v, scale_q, scale_k, scale_v, out_f32, out, lse, acc_o, acc_m, acc_l, B, H, Sq, Sk, D,
     #                   q_pos0, k_pos0, causal, bias, bias_stride, segment_ids, seg_stride, softmax_scale, first, last,
-    #                   tiles, tile_count, stream)
-    ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 128, 128, 64, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, N), SHAPE, "head_dim"),
-    ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 100, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, N), SHAPE, "multiples of 128"),
-    ("lwm_attn_fwd_step", (N, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, N), ARG, "null"),
-    ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, N, N, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, N), ARG, "last step"),
-    ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 0, N, N, N), ARG, "carry"),
-    ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 128, 128, 128, 1 << 31, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, N), SHAPE, "int32"),
-    ("lwm_attn_fwd_step", (P, P, P, P, N, P, P, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, N), ARG, "scales"),
-    ("lwm_attn_fwd_step", (P, P, P, N, N, N, P, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, N), ARG, "out_f32"),
+    #                   tiles, tile_count, seed, drop_threshold, batch0, stream)
+    ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 128, 128, 64, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, 0, 0, 0, N), SHAPE, "head_dim"),
+    ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 100, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, 0, 0, 0, N), SHAPE, "multiples of 128"),
+    ("lwm_attn_fwd_step", (N, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, 0, 0, 0, N), ARG, "null"),
+    ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, N, N, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, 0, 0, 0, N), ARG, "last step"),
+    ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 0, N, N, 0, 0, 0, N), ARG, "carry"),
+    ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 128, 128, 128, 1 << 31, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, 0, 0, 0, N), SHAPE, "int32"),
+    ("lwm_attn_fwd_step", (P, P, P, P, N, P, P, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, 0, 0, 0, N), ARG, "scales"),
+    ("lwm_attn_fwd_step", (P, P, P, N, N, N, P, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, 0, 0, 0, N), ARG, "out_f32"),
     # lwm_attn_bwd_step(q, k, v, dout, scale_q, scale_k, scale_v, scale_do, lse, delta, dq_acc, dk_acc, dv_acc, B, H, Sq,
     #                   Sk, D, q_pos0, k_pos0, causal, bias, bias_stride, segment_ids, seg_stride, softmax_scale,
-    #                   dkv_init, tiles, tile_count, stream)
-    ("lwm_attn_bwd_step", (P, P, P, P, N, N, N, N, P, P, P, P, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 0, N, N, N), ARG, "null"),
-    ("lwm_attn_bwd_step", (P, P, P, P, N, N, N, N, P, P, P, P, P, 1, 2, 128, 192, 128, 0, 0, 1, N, 0, N, 0, 0.1, 0, N, N, N), SHAPE, "multiples of 128"),
+    #                   dkv_init, tiles, tile_count, order_ws, seed, drop_threshold, batch0, stream)
+    ("lwm_attn_bwd_step", (P, P, P, P, N, N, N, N, P, P, P, P, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 0, N, N, N, 0, 0, 0, N), ARG, "null"),
+    ("lwm_attn_bwd_step", (P, P, P, P, N, N, N, N, P, P, P, P, P, 1, 2, 128, 192, 128, 0, 0, 1, N, 0, N, 0, 0.1, 0, N, N, N, 0, 0, 0, N), SHAPE, "multiples of 128"),
     ("lwm_attn_absmax", (P, 2, 64, P, N), ARG, "bad arguments"),
     ("lwm_attn_to_f16_scaled", (P, 1, P, P, 12, N), ARG, "n % 8"),
     ("lwm_attn_bwd_prep", (P, 0, P, P, P, 1, 2, 128, 64, N), SHAPE, "head_dim"),
@@ -49,8 +49,8 @@ BAD_CALLS = [
     ("lwm_attn_bwd_prep", (P, 2, P, N, P, 1, 2, 128, 128, N), ARG, "out dtype"),
     ("lwm_attn_bwd_lse", (P, P, 0, 0.0, N), ARG, "bad args"),
     ("lwm_attn_to_f16", (P, P, P, P, 12, N), SHAPE, "multiple of 8"),
-    ("lwm_attn_decode_partial", (P, P, P, 1, N, P, P, N, 1, 2, 1, 128, 128, 0, 0, 0, 4, 0.1, N, N, N), ARG, "null"),
-    ("lwm_attn_decode_partial", (P, P, P, 2, N, P, P, P, 1, 2, 1, 128, 128, 0, 0, 0, 4, 0.1, N, N, N), ARG, "dtype"),
+    ("lwm_attn_decode_partial", (P, P, P, 1, N, N, N, P, P, N, 1, 2, 1, 128, 128, 0, 0, 0, 4, 0.1, N, N, N), ARG, "null"),
+    ("lwm_attn_decode_partial", (P, P, P, 2, N, N, N, P, P, P, 1, 2, 1, 128, 128, 0, 0, 0, 4, 0.1, N, N, N), ARG, "dtype"),
     ("lwm_attn_decode_merge", (P, P, 0, P, 1, P, 8, N), ARG, "bad args"),
     ("lwm_attn_decode_merge", (P, P, 2, P, 2, P, 8, N), ARG, "dtype"),
     ("lwm_attn_rope", (P, P, 0, P, P, 2, P, P, 1, 8, 2, 2, 128, 0, N), ARG, "dtype"),
@@ -77,6 +77,9 @@ BAD_CALLS = [
     ("lwm_vq_unframe_tokens", (N, P, 4, 256, N), ARG, "null"),
 ]
 
+# the same rows with the options of the folded entry points turned on: no option slot bypasses these checks
+BAD_CALLS += [(n, with_options(n, a, P), c, f) for n, a, c, f in BAD_CALLS if n in FOLDED_ENTRY_POINTS]
+
 
 @pytest.mark.parametrize("name,args,code,frag", BAD_CALLS,
                          ids=["%s-%s" % (abi_row_id(*c[:2]), c[3].replace(" ", "_")) for c in BAD_CALLS])
@@ -87,10 +90,10 @@ def test_bad_arguments_are_rejected_with_a_message(lib, name, args, code, frag):
 
 
 GOOD_CALLS = [
-    ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, N)),
-    ("lwm_attn_fwd_step", (P, P, P, P, P, P, P, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, N)),
-    ("lwm_attn_bwd_step", (P, P, P, P, N, N, N, N, P, P, P, P, P, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, N, N, N)),
-    ("lwm_attn_bwd_step", (P, P, P, P, P, P, P, P, P, P, P, P, P, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, N, N, N)),
+    ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, 0, 0, 0, N)),
+    ("lwm_attn_fwd_step", (P, P, P, P, P, P, P, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1, N, N, 0, 0, 0, N)),
+    ("lwm_attn_bwd_step", (P, P, P, P, N, N, N, N, P, P, P, P, P, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, N, N, N, 0, 0, 0, N)),
+    ("lwm_attn_bwd_step", (P, P, P, P, P, P, P, P, P, P, P, P, P, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, N, N, N, 0, 0, 0, N)),
     ("lwm_attn_absmax", (P, 1, 64, P, N)),
     ("lwm_attn_bwd_prep", (P, 0, P, P, P, 1, 2, 128, 128, N)),
     ("lwm_attn_bwd_prep", (P, 0, P, N, P, 1, 2, 128, 128, N)),
@@ -106,6 +109,8 @@ GOOD_CALLS = [
     ("lwm_vq_frame_tokens", (P, N, P, 1, 4, 4, 256, 8192, 8193, N)),
     ("lwm_cast_f32_to_bf16", (P, P, 0, N)),           # even an empty call does not succeed without a device
 ]
+
+GOOD_CALLS += [(n, with_options(n, a, P)) for n, a in GOOD_CALLS if n in FOLDED_ENTRY_POINTS]
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="fake pointers: only meaningful where the device check fails")

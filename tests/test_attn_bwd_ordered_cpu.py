@@ -1,6 +1,6 @@
-"""The ordered dQ reduction without a GPU: argument validation of lwm_attn_bwd_step_ordered and
-lwm_attn_infer_bwd_ordered (bad calls are rejected with a message before the device check, well-formed ones fail with
-LWM_ERR_DEVICE), and the machine code of the five ordered attn_bwd_kernel instances: no local memory (warp 9's wait,
+"""The ordered dQ reduction without a GPU: argument validation of lwm_attn_bwd_step and lwm_attn_infer_bwd given an
+order_ws (bad calls are rejected with a message before the device check, well-formed ones fail with LWM_ERR_DEVICE;
+a null order_ws is the unordered call, to which the ordered limits do not apply), and the machine code of the five ordered attn_bwd_kernel instances: no local memory (warp 9's wait,
 turn load and ticket fit the 24 registers it keeps after setmaxnreg.dec, and the consumers still fit theirs), a
 backed-off wait in every ordered instance and in none of the others.
 Pointers are fake non-null addresses: nothing dereferences them before the device check."""
@@ -27,37 +27,49 @@ def _status(lib, name, *args):
     return getattr(lib, name)(*args), lib.lwm_last_error().decode()
 
 
-def _step(scales=False, B=1, H=2, Sq=256, Sk=512, D=128, bias=None, tiles=None, counts=None, ws=P):
-    """lwm_attn_bwd_step_ordered's arguments: (q, k, v, dout, scale_q, scale_k, scale_v, scale_do, lse, delta, dq_acc,
-    dk_acc, dv_acc, B, H, Sq, Sk, D, q_pos0, k_pos0, causal, bias, bias_stride, segment_ids, seg_stride,
-    softmax_scale, dkv_init, tiles, tile_count, order_ws, stream)"""
+def _step(scales=False, B=1, H=2, Sq=256, Sk=512, D=128, q_pos0=0, bias=None, tiles=None, counts=None, ws=P, thr=0):
+    """lwm_attn_bwd_step's arguments: (q, k, v, dout, scale_q, scale_k, scale_v, scale_do, lse, delta, dq_acc, dk_acc,
+    dv_acc, B, H, Sq, Sk, D, q_pos0, k_pos0, causal, bias, bias_stride, segment_ids, seg_stride, softmax_scale,
+    dkv_init, tiles, tile_count, order_ws, seed, drop_threshold, batch0, stream)"""
     s = P if scales else N
-    return (P, P, P, P, s, s, s, s, P, P, P, P, P, B, H, Sq, Sk, D, 0, 0, 1, bias, 0 if bias is None else Sk, N, 0,
-            0.1, 1, tiles, counts, ws, N)
+    return (P, P, P, P, s, s, s, s, P, P, P, P, P, B, H, Sq, Sk, D, q_pos0, 0, 1, bias, 0 if bias is None else Sk, N,
+            0, 0.1, 1, tiles, counts, ws, 7, thr, 0, N)
 
 
 def _infer(B=1, H=2, Q=72, Sk=300, D=128, ws=P, counts=P):
-    """lwm_attn_infer_bwd_ordered's arguments: (q16, k16, v16, dout16, scale_q, scale_k, scale_v, scale_do, lse, delta,
-    bits, tiles, tile_count, dq_acc, dk_acc, dv_acc, B, H, Q, Sk, D, softmax_scale, order_ws, stream)"""
+    """lwm_attn_infer_bwd's arguments: (q16, k16, v16, dout16, scale_q, scale_k, scale_v, scale_do, lse, delta, bits,
+    tiles, tile_count, dq_acc, dk_acc, dv_acc, B, H, Q, Sk, D, softmax_scale, order_ws, stream)"""
     return (P, P, P, P, P, P, P, P, P, P, N, P, counts, P, P, P, B, H, Q, Sk, D, 0.1, ws, N)
 
 
+# shapes whose ordered call is over the int32 limits of the workspace; the unordered call takes them (GOOD_CALLS)
+_SEM_OVER = dict(B=64, H=65535, Sq=65536)
+_TURNS_OVER = dict(H=100, Sq=2 ** 30, Sk=64 * 128, bias=P, tiles=P, counts=P)    # the block map's turns tip it over
+_INFER_SEM_OVER = dict(H=65535, Q=64 * 40000, Sk=128)
+
 BAD_CALLS = [
-    ("null_workspace", "lwm_attn_bwd_step_ordered", _step(ws=N), ARG, "order_ws"),
-    ("null_workspace_map", "lwm_attn_bwd_step_ordered", _step(bias=P, tiles=P, counts=P, ws=N), ARG, "order_ws"),
-    ("map_without_counts", "lwm_attn_bwd_step_ordered", _step(bias=P, tiles=P), ARG, "tile_count"),
-    ("map_without_mask", "lwm_attn_bwd_step_ordered", _step(tiles=P, counts=P), ARG, "bias or segment_ids"),
-    ("partial_scales", "lwm_attn_bwd_step_ordered", _step()[:4] + (P, N, N, N) + _step()[8:], ARG, "scales"),
-    ("seq_not_128", "lwm_attn_bwd_step_ordered", _step(Sq=192), SHAPE, "multiples of 128"),
-    ("head_dim", "lwm_attn_bwd_step_ordered", _step(D=64), SHAPE, "head_dim"),
-    ("semaphores_over_int32", "lwm_attn_bwd_step_ordered", _step(B=64, H=65535, Sq=65536), SHAPE, "int32"),
-    ("infer_null_workspace", "lwm_attn_infer_bwd_ordered", _infer(ws=N), ARG, "order_ws"),
-    ("infer_map_without_counts", "lwm_attn_infer_bwd_ordered", _infer(counts=N), ARG, "null"),
-    ("infer_head_dim", "lwm_attn_infer_bwd_ordered", _infer(D=96), SHAPE, "head_dim"),
-    ("infer_bad_shape", "lwm_attn_infer_bwd_ordered", _infer(Q=0), SHAPE, "bad shape"),
-    ("infer_tickets_over_int32", "lwm_attn_infer_bwd_ordered", _infer(B=4096, H=4096, Q=64, Sk=128 * 200), SHAPE,
+    ("map_without_counts", "lwm_attn_bwd_step", _step(bias=P, tiles=P), ARG, "tile_count"),
+    ("map_without_mask", "lwm_attn_bwd_step", _step(tiles=P, counts=P), ARG, "bias or segment_ids"),
+    ("partial_scales", "lwm_attn_bwd_step", _step()[:4] + (P, N, N, N) + _step()[8:], ARG, "scales"),
+    ("seq_not_128", "lwm_attn_bwd_step", _step(Sq=192), SHAPE, "multiples of 128"),
+    ("head_dim", "lwm_attn_bwd_step", _step(D=64), SHAPE, "head_dim"),
+    ("semaphores_over_int32", "lwm_attn_bwd_step", _step(**_SEM_OVER), SHAPE, "int32"),
+    ("turns_over_int32", "lwm_attn_bwd_step", _step(**_TURNS_OVER), SHAPE, "int32"),
+    ("dropout_q_pos0", "lwm_attn_bwd_step", _step(q_pos0=64, thr=6554), SHAPE, "multiple of 128"),
+    ("infer_map_without_counts", "lwm_attn_infer_bwd", _infer(counts=N), ARG, "null"),
+    ("infer_head_dim", "lwm_attn_infer_bwd", _infer(D=96), SHAPE, "head_dim"),
+    ("infer_bad_shape", "lwm_attn_infer_bwd", _infer(Q=0), SHAPE, "bad shape"),
+    ("infer_tickets_over_int32", "lwm_attn_infer_bwd", _infer(B=4096, H=4096, Q=64, Sk=128 * 200), SHAPE,
      "int32"),
+    ("infer_semaphores_over_int32", "lwm_attn_infer_bwd", _infer(**_INFER_SEM_OVER), SHAPE, "int32"),
 ]
+# the general checks give the same verdict without the workspace and, on the training step, with dropout on
+_GENERAL = ("map_without_counts", "map_without_mask", "partial_scales", "seq_not_128", "head_dim",
+            "infer_map_without_counts", "infer_head_dim", "infer_bad_shape")
+BAD_CALLS += [(c + "_unordered", n, a[:-2] + (N, N) if n == "lwm_attn_infer_bwd" else a[:29] + (N,) + a[30:], code, f)
+              for c, n, a, code, f in BAD_CALLS if c in _GENERAL]
+BAD_CALLS += [(c + "_dropout", n, a[:31] + (6554,) + a[32:], code, f)
+              for c, n, a, code, f in BAD_CALLS if c in _GENERAL and n == "lwm_attn_bwd_step"]
 
 
 @pytest.mark.parametrize("case,name,args,code,frag", BAD_CALLS, ids=[c[0] for c in BAD_CALLS])
@@ -68,11 +80,16 @@ def test_bad_arguments_are_rejected_with_a_message(lib, case, name, args, code, 
 
 
 GOOD_CALLS = [
-    ("bf16", "lwm_attn_bwd_step_ordered", _step()),
-    ("f16", "lwm_attn_bwd_step_ordered", _step(scales=True)),
-    ("bf16_map", "lwm_attn_bwd_step_ordered", _step(bias=P, tiles=P, counts=P)),
-    ("f16_map", "lwm_attn_bwd_step_ordered", _step(scales=True, bias=P, tiles=P, counts=P)),
-    ("infer", "lwm_attn_infer_bwd_ordered", _infer()),
+    ("bf16", "lwm_attn_bwd_step", _step()),
+    ("f16", "lwm_attn_bwd_step", _step(scales=True)),
+    ("bf16_map", "lwm_attn_bwd_step", _step(bias=P, tiles=P, counts=P)),
+    ("f16_map", "lwm_attn_bwd_step", _step(scales=True, bias=P, tiles=P, counts=P)),
+    ("infer", "lwm_attn_infer_bwd", _infer()),
+    ("bf16_dropout", "lwm_attn_bwd_step", _step(thr=6554)),
+    ("semaphores_over_int32_unordered", "lwm_attn_bwd_step", _step(ws=N, **_SEM_OVER)),
+    ("turns_over_int32_unordered", "lwm_attn_bwd_step", _step(ws=N, **_TURNS_OVER)),
+    ("turns_over_int32_without_map", "lwm_attn_bwd_step", _step(**dict(_TURNS_OVER, tiles=N, counts=N))),
+    ("infer_semaphores_over_int32_unordered", "lwm_attn_infer_bwd", _infer(ws=N, **_INFER_SEM_OVER)),
 ]
 
 

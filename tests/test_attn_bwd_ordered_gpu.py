@@ -1,5 +1,5 @@
 """The attention backward under torch.use_deterministic_algorithms(True): dQ reduced in ascending key-tile order
-(lwm_attn_bwd_step_ordered / lwm_attn_infer_bwd_ordered, DESIGN §3.3).
+(lwm_attn_bwd_step / lwm_attn_infer_bwd given an order_ws, DESIGN §3.3).
 
   * the turns pass against a numpy count over the backward lists: packed segments, left padding, the call-site zero bias
     with packed segments, and random inference masks (Q = 72, not a multiple of 64); the semaphores end at the number
@@ -385,13 +385,14 @@ def test_nccl_ring_two_runs_bit_identical(deterministic, monkeypatch, world, lay
 
 
 # ------------------------------------------------------------------------------------------------ plumbing
-def test_entry_points_follow_the_flag(monkeypatch):
+def test_order_workspace_follows_the_flag(monkeypatch):
     from lwm_b200 import _lib
-    names = []
+    calls = []     # (name, whether its order_ws slot holds a workspace; None for calls without one)
     call = _lib.call
+    ws_slot = {"lwm_attn_bwd_step": 29, "lwm_attn_infer_bwd": 22}
 
     def spy(name, *args):
-        names.append(name)
+        calls.append((name, args[ws_slot[name]] is not None if name in ws_slot else None))
         return call(name, *args)
 
     monkeypatch.setattr(_lib, "call", spy)
@@ -402,11 +403,11 @@ def test_entry_points_follow_the_flag(monkeypatch):
     qi, ki, vi, doi = _qkv(B, 200, 300, H, torch.bfloat16, 62)
 
     def run():
-        del names[:]
+        del calls[:]
         _op_grads(q, k, v, do, None, None, True, "fp16")
         _op_grads(q, k, v, do, bias, seg, True, "bf16")
         _infer_grads(qi, ki, vi, doi, mask)
-        return list(names)
+        return list(calls)
 
     prev = torch.are_deterministic_algorithms_enabled()
     try:
@@ -416,10 +417,9 @@ def test_entry_points_follow_the_flag(monkeypatch):
         on = run()
     finally:
         torch.use_deterministic_algorithms(prev)
-    assert not [n for n in off if n.endswith("_ordered")]
-    assert off.count("lwm_attn_bwd_step") == 2 and off.count("lwm_attn_infer_bwd") == 1
-    assert on.count("lwm_attn_bwd_step_ordered") == 2 and on.count("lwm_attn_infer_bwd_ordered") == 1
-    assert "lwm_attn_bwd_step" not in on and "lwm_attn_infer_bwd" not in on
-    # apart from the backward launches, the flag changes no call
-    strip = {"lwm_attn_bwd_step_ordered": "lwm_attn_bwd_step", "lwm_attn_infer_bwd_ordered": "lwm_attn_infer_bwd"}
-    assert [strip.get(n, n) for n in on] == off
+    assert off.count(("lwm_attn_bwd_step", False)) == 2 and off.count(("lwm_attn_infer_bwd", False)) == 1
+    assert not [c for c in off if c[1]]
+    assert on.count(("lwm_attn_bwd_step", True)) == 2 and on.count(("lwm_attn_infer_bwd", True)) == 1
+    assert not [c for c in on if c[1] is False]
+    # apart from the backward launches' workspace, the flag changes no call
+    assert [n for n, _ in on] == [n for n, _ in off]

@@ -117,7 +117,7 @@ def test_blockwise_kwargs():
 
 
 def _fwd_args(**kw):
-    """lwm_attn_fwd_step_dropout's arguments (fake non-null pointers), overridable by name"""
+    """lwm_attn_fwd_step's arguments with dropout on (fake non-null pointers), overridable by name"""
     a = dict(q=1, k=1, v=1, sq=None, sk=None, sv=None, o32=None, out=1, lse=1, ao=None, am=None, al=None, B=1, H=1,
              Sq=256, Sk=256, D=128, q_pos0=0, k_pos0=0, causal=1, bias=None, bias_stride=0, seg=None, seg_stride=0,
              scale=0.088, first=1, last=1, tiles=None, counts=None, seed=7, thr=6554, batch0=0, stream=None)
@@ -149,22 +149,22 @@ def _status(lib, name, args):
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="fake pointers: only meaningful where the device check fails")
-def test_symbols_check_arguments_before_the_device(lib):
+def test_step_entry_points_check_dropout_arguments_before_the_device(lib):
     cases = [
-        ("lwm_attn_fwd_step_dropout", _fwd_args(thr=0), 3, "drop_threshold"),
-        ("lwm_attn_fwd_step_dropout", _fwd_args(thr=65536), 3, "drop_threshold"),
-        ("lwm_attn_fwd_step_dropout", _fwd_args(k_pos0=64), 2, "multiple of 128"),
-        ("lwm_attn_fwd_step_dropout", _fwd_args(q_pos0=128 + 8), 2, "multiple of 128"),
-        ("lwm_attn_fwd_step_dropout", _fwd_args(batch0=-1), 3, "batch0"),
-        ("lwm_attn_fwd_step_dropout", _fwd_args(batch0=2 ** 31 - 1), 2, "batch0 + B"),
-        ("lwm_attn_fwd_step_dropout", _fwd_args(Sq=100), 2, "multiples of 128"),
-        ("lwm_attn_fwd_step_dropout", _fwd_args(tiles=1), 3, "tiles and tile_count"),
-        ("lwm_attn_bwd_step_dropout", _bwd_args(thr=0), 3, "drop_threshold"),
-        ("lwm_attn_bwd_step_dropout", _bwd_args(thr=70000), 3, "drop_threshold"),
-        ("lwm_attn_bwd_step_dropout", _bwd_args(k_pos0=128 + 16), 2, "multiple of 128"),
-        ("lwm_attn_bwd_step_dropout", _bwd_args(q_pos0=64), 2, "multiple of 128"),
-        ("lwm_attn_bwd_step_dropout", _bwd_args(batch0=-5), 3, "batch0"),
-        ("lwm_attn_bwd_step_dropout", _bwd_args(dq=None), 3, "null pointer"),
+        ("lwm_attn_fwd_step", _fwd_args(q_pos0=64), 2, "multiple of 128"),       # accepted without dropout (below)
+        ("lwm_attn_fwd_step", _fwd_args(thr=65536), 3, "drop_threshold"),
+        ("lwm_attn_fwd_step", _fwd_args(k_pos0=64), 2, "multiple of 128"),
+        ("lwm_attn_fwd_step", _fwd_args(q_pos0=128 + 8), 2, "multiple of 128"),
+        ("lwm_attn_fwd_step", _fwd_args(batch0=-1), 3, "batch0"),
+        ("lwm_attn_fwd_step", _fwd_args(batch0=2 ** 31 - 1), 2, "batch0 + B"),
+        ("lwm_attn_fwd_step", _fwd_args(Sq=100), 2, "multiples of 128"),
+        ("lwm_attn_fwd_step", _fwd_args(tiles=1), 3, "tiles and tile_count"),
+        ("lwm_attn_bwd_step", _bwd_args(batch0=2 ** 31 - 1), 2, "batch0 + B"),  # accepted without dropout (below)
+        ("lwm_attn_bwd_step", _bwd_args(thr=70000), 3, "drop_threshold"),
+        ("lwm_attn_bwd_step", _bwd_args(k_pos0=128 + 16), 2, "multiple of 128"),
+        ("lwm_attn_bwd_step", _bwd_args(q_pos0=64), 2, "multiple of 128"),
+        ("lwm_attn_bwd_step", _bwd_args(batch0=-5), 3, "batch0"),
+        ("lwm_attn_bwd_step", _bwd_args(dq=None), 3, "null pointer"),
         ("lwm_attn_dropout_mask", _mask_args(thr=0), 3, "drop_threshold"),
         ("lwm_attn_dropout_mask", _mask_args(out=None), 3, "null out"),
         ("lwm_attn_dropout_mask", _mask_args(n_q=0), 2, "n_q"),
@@ -173,8 +173,11 @@ def test_symbols_check_arguments_before_the_device(lib):
     for name, args, code, msg in cases:
         st, err = _status(lib, name, args)
         assert st == code and msg in err, (name, st, err)
-    for name, args in (("lwm_attn_fwd_step_dropout", _fwd_args(k_pos0=256, q_pos0=384, batch0=3)),
-                       ("lwm_attn_bwd_step_dropout", _bwd_args(ws=1, thr=65535, batch0=1)),
+    for name, args in (("lwm_attn_fwd_step", _fwd_args(k_pos0=256, q_pos0=384, batch0=3)),
+                       ("lwm_attn_bwd_step", _bwd_args(ws=1, thr=65535, batch0=1)),
+                       # drop_threshold 0 is the call without dropout: the dropout-only shape rules do not apply
+                       ("lwm_attn_fwd_step", _fwd_args(q_pos0=64, thr=0)),
+                       ("lwm_attn_bwd_step", _bwd_args(batch0=2 ** 31 - 1, thr=0)),
                        ("lwm_attn_dropout_mask", _mask_args(b=3, h=31, q_pos0=2 ** 20))):
         st, err = _status(lib, name, args)
         assert st == 1, (name, st, err)     # LWM_ERR_DEVICE: the arguments were accepted

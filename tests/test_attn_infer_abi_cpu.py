@@ -6,7 +6,7 @@ import ctypes
 import pytest
 import torch
 
-from helpers import abi_row_id
+from helpers import FOLDED_ENTRY_POINTS, abi_row_id, with_options
 
 P = ctypes.c_void_p(0x1000)
 N = None
@@ -20,8 +20,8 @@ def _status(lib, name, *args):
 
 
 BAD_CALLS = [
-    ("lwm_attn_decode_partial", (P, P, P, 0, N, P, P, N, 1, 2, 1, 128, 128, 0, 0, 0, 4, 0.1, N, N, N), ARG, "null"),
-    ("lwm_attn_decode_partial", (P, P, P, 0, N, P, P, P, 1, 2, 1, 128, 64, 0, 0, 0, 4, 0.1, N, N, N), SHAPE, "head_dim"),
+    ("lwm_attn_decode_partial", (P, P, P, 0, N, N, N, P, P, N, 1, 2, 1, 128, 128, 0, 0, 0, 4, 0.1, N, N, N), ARG, "null"),
+    ("lwm_attn_decode_partial", (P, P, P, 0, N, N, N, P, P, P, 1, 2, 1, 128, 64, 0, 0, 0, 4, 0.1, N, N, N), SHAPE, "head_dim"),
     ("lwm_attn_decode_merge", (P, P, 0, P, 0, P, 8, N), ARG, "bad args"),
     ("lwm_attn_decode_merge", (P, P, 2, N, 0, P, 8, N), ARG, "bad args"),
     ("lwm_attn_mask_pack", (N, 0, 64, 1, 1, 4, 0, 64, 1, P, P, N), ARG, "null"),
@@ -37,6 +37,9 @@ BAD_CALLS = [
     ("lwm_attn_infer_partial", (P, P, P, P, P, P, N, P, P, P, P, P, 1, 2, 200, 300, 128, 0, 0.1, N), SHAPE, "splits"),
 ]
 
+# the same rows with the options of the folded entry points turned on: no option slot bypasses these checks
+BAD_CALLS += [(n, with_options(n, a, P), c, f) for n, a, c, f in BAD_CALLS if n in FOLDED_ENTRY_POINTS]
+
 
 @pytest.mark.parametrize("name,args,code,frag", BAD_CALLS,
                          ids=["%s-%d" % (abi_row_id(*c[:2]), i) for i, c in enumerate(BAD_CALLS)])
@@ -47,13 +50,15 @@ def test_bad_arguments_are_rejected_with_a_message(lib, name, args, code, frag):
 
 
 GOOD_CALLS = [
-    ("lwm_attn_decode_partial", (P, P, P, 0, N, P, P, P, 1, 2, 1, 128, 128, 0, 0, 0, 4, 0.1, N, N, N)),
+    ("lwm_attn_decode_partial", (P, P, P, 0, N, N, N, P, P, P, 1, 2, 1, 128, 128, 0, 0, 0, 4, 0.1, N, N, N)),
     ("lwm_attn_decode_merge", (P, P, 2, P, 0, P, 8, N)),
     ("lwm_attn_mask_pack", (P, 0, 300, 1, 2, 200, 0, 150, 2, P, P, N)),
     ("lwm_attn_infer_tilemap", (N, N, 2, 200, 300, P, P, N)),
     ("lwm_attn_infer_partial", (P, P, P, P, P, P, N, P, P, P, P, N, 1, 2, 200, 300, 128, 1, 0.1, N)),
     ("lwm_attn_infer_partial", (P, P, P, P, P, P, P, P, P, P, P, P, 1, 2, 200, 300, 128, 3, 0.1, N)),
 ]
+
+GOOD_CALLS += [(n, with_options(n, a, P)) for n, a in GOOD_CALLS if n in FOLDED_ENTRY_POINTS]
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="fake pointers: only meaningful where the device check fails")

@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 import torch
 
+from helpers import FOLDED_ENTRY_POINTS, with_options
 from infer_grad_model import attention_inference_vjp, bwd_tilemap_brute, bwd_tilemap_model, pack_bits
 
 
@@ -129,7 +130,7 @@ def _bwd_args(**kw):
     ptrs.update({k: v for k, v in kw.items() if k in ptrs})
     dims = dict(B=1, H=2, Q=200, Sk=300, D=128)
     dims.update({k: v for k, v in kw.items() if k in dims})
-    return tuple(ptrs.values()) + tuple(dims.values()) + (0.1, N)
+    return tuple(ptrs.values()) + tuple(dims.values()) + (0.1, N, N)     # softmax_scale, order_ws, stream
 
 
 BAD_CALLS = [
@@ -149,6 +150,9 @@ BAD_CALLS = [
     ("lwm_attn_infer_bwd", _bwd_args(B=60000, Q=2 ** 30, Sk=2 ** 20), SHAPE, "int32"),
 ]
 
+# the same rows with the options of the folded entry points turned on: no option slot bypasses these checks
+BAD_CALLS += [(n, with_options(n, a, P), c, f) for n, a, c, f in BAD_CALLS if n in FOLDED_ENTRY_POINTS]
+
 
 @pytest.mark.parametrize("name,args,code,frag", BAD_CALLS, ids=["%s-%d" % (c[0][4:], i) for i, c in enumerate(BAD_CALLS)])
 def test_bad_arguments_are_rejected_with_a_message(lib, name, args, code, frag):
@@ -163,6 +167,8 @@ GOOD_CALLS = [
     ("lwm_attn_infer_bwd", _bwd_args()),
     ("lwm_attn_infer_bwd", _bwd_args(bits=P, Q=1, Sk=1)),
 ]
+
+GOOD_CALLS += [(n, with_options(n, a, P)) for n, a in GOOD_CALLS if n in FOLDED_ENTRY_POINTS]
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="fake pointers: only meaningful where the device check fails")

@@ -9,7 +9,7 @@ import pytest
 import torch
 
 import tilemap_model as tm
-from helpers import abi_row_id
+from helpers import FOLDED_ENTRY_POINTS, abi_row_id, with_options
 
 CASES = tm.sweep_cases()
 
@@ -97,33 +97,36 @@ BAD_CALLS = [
     ("lwm_attn_step_tilemap", (N, 0, P, 256, 1, 256, 256, 128, 0, 1, P, P, P, P, P, N), SHAPE, "seg_stride"),
     # lwm_attn_fwd_step(q, k, v, scale_q, scale_k, scale_v, out_f32, out, lse, acc_o, acc_m, acc_l, B, H, Sq, Sk, D,
     #                   q_pos0, k_pos0, causal, bias, bias_stride, segment_ids, seg_stride, softmax_scale, first, last,
-    #                   tiles, tile_count, stream)
+    #                   tiles, tile_count, seed, drop_threshold, batch0, stream)
     ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1, 1,
-                           P, P, N), ARG, "bias or segment_ids"),
+                           P, P, 0, 0, 0, N), ARG, "bias or segment_ids"),
     ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, P, 128, N, 0, 0.1, 1, 1,
-                           N, P, N), ARG, "tiles"),
+                           N, P, 0, 0, 0, N), ARG, "tiles"),
     ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, P, 64, N, 0, 0.1, 1, 1,
-                           P, P, N), SHAPE, "bias_stride"),
+                           P, P, 0, 0, 0, N), SHAPE, "bias_stride"),
     ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 100, 128, 128, 0, 0, 1, P, 128, N, 0, 0.1, 1, 1,
-                           P, P, N), SHAPE, "multiples of 128"),
+                           P, P, 0, 0, 0, N), SHAPE, "multiples of 128"),
     ("lwm_attn_fwd_step", (P, P, P, N, P, P, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, P, 128, N, 0, 0.1, 1, 1,
-                           P, P, N), ARG, "scales"),
+                           P, P, 0, 0, 0, N), ARG, "scales"),
     ("lwm_attn_fwd_step", (P, P, P, P, P, P, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, P, 128, 0.1, 1, 1,
-                           P, N, N), ARG, "tiles"),
+                           P, N, 0, 0, 0, N), ARG, "tiles"),
     # lwm_attn_bwd_step(q, k, v, dout, scale_q, scale_k, scale_v, scale_do, lse, delta, dq_acc, dk_acc, dv_acc, B, H, Sq,
     #                   Sk, D, q_pos0, k_pos0, causal, bias, bias_stride, segment_ids, seg_stride, softmax_scale,
-    #                   dkv_init, tiles, tile_count, stream)
+    #                   dkv_init, tiles, tile_count, order_ws, seed, drop_threshold, batch0, stream)
     ("lwm_attn_bwd_step", (P, P, P, P, N, N, N, N, P, P, P, P, P, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, N, 0, 0.1, 1,
-                           P, P, N), ARG, "bias or segment_ids"),
+                           P, P, N, 0, 0, 0, N), ARG, "bias or segment_ids"),
     ("lwm_attn_bwd_step", (P, P, P, P, N, N, N, N, P, P, P, P, P, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, P, 128, 0.1, 1,
-                           P, N, N), ARG, "tiles"),
+                           P, N, N, 0, 0, 0, N), ARG, "tiles"),
     ("lwm_attn_bwd_step", (P, P, P, P, N, N, N, N, P, P, P, P, P, 1, 2, 128, 128, 128, 128, 0, 1, N, 0, P, 128, 0.1, 1,
-                           P, P, N), SHAPE, "seg_stride"),
+                           P, P, N, 0, 0, 0, N), SHAPE, "seg_stride"),
     ("lwm_attn_bwd_step", (P, P, P, P, P, P, P, N, P, P, P, P, P, 1, 2, 128, 128, 128, 0, 0, 1, P, 128, N, 0, 0.1, 1,
-                           P, P, N), ARG, "scales"),
+                           P, P, N, 0, 0, 0, N), ARG, "scales"),
     ("lwm_attn_bwd_step", (P, P, P, P, P, P, P, P, P, P, P, P, P, 1, 2, 128, 128, 128, 0, 0, 1, P, 128, N, 0, 0.1, 1,
-                           N, P, N), ARG, "tiles"),
+                           N, P, N, 0, 0, 0, N), ARG, "tiles"),
 ]
+
+# the same rows with the options of the folded entry points turned on: no option slot bypasses these checks
+BAD_CALLS += [(n, with_options(n, a, P), c, f) for n, a, c, f in BAD_CALLS if n in FOLDED_ENTRY_POINTS]
 
 
 def _status(lib, name, *args):
@@ -144,14 +147,16 @@ GOOD_CALLS = [
     ("lwm_attn_step_tilemap", (P, 256, N, 0, 1, 256, 256, 0, 0, 1, P, P, P, P, P, N)),
     ("lwm_attn_step_tilemap", (N, 0, P, 512, 2, 256, 256, 256, 0, 1, N, N, P, P, P, N)),
     ("lwm_attn_fwd_step", (P, P, P, N, N, N, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, P, 128, N, 0, 0.1, 1, 1,
-                           P, P, N)),
+                           P, P, 0, 0, 0, N)),
     ("lwm_attn_fwd_step", (P, P, P, P, P, P, N, P, P, N, N, N, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, P, 128, 0.1, 1, 1,
-                           P, P, N)),
+                           P, P, 0, 0, 0, N)),
     ("lwm_attn_bwd_step", (P, P, P, P, N, N, N, N, P, P, P, P, P, 1, 2, 128, 128, 128, 0, 0, 1, P, 128, N, 0, 0.1, 1,
-                           P, P, N)),
+                           P, P, N, 0, 0, 0, N)),
     ("lwm_attn_bwd_step", (P, P, P, P, P, P, P, P, P, P, P, P, P, 1, 2, 128, 128, 128, 0, 0, 1, N, 0, P, 128, 0.1, 0,
-                           P, P, N)),
+                           P, P, N, 0, 0, 0, N)),
 ]
+
+GOOD_CALLS += [(n, with_options(n, a, P)) for n, a in GOOD_CALLS if n in FOLDED_ENTRY_POINTS]
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="fake pointers: only meaningful where the device check fails")

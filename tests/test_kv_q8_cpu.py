@@ -2,8 +2,8 @@
   * the format (tests/kv_q8_model.py) against its definition on sweeps: the exponent rule, half-to-even rounding, the
     +-127 clamp, the NaN code, all-zero groups and groups at the exponent clamp;
   * the exactness claim, exhaustively: every code at every exponent dequantizes exactly to fp32 and to bf16;
-  * the C ABI of the three new entry points: declared, exported and bound, and bad arguments rejected before the
-    device check;
+  * the C ABI of the two new entry points and of lwm_attn_decode_partial's 8-bit cache arguments: declared, exported
+    and bound, and bad arguments rejected before the device check;
   * ShardedKVCache(dtype=torch.int8) bookkeeping under gloo at world 1, 2 and 4, with a CPU stand-in for the
     quantizing write: a prefill whose slice crosses rank boundaries, decode writes on rank edges, and overflow."""
 import ctypes
@@ -16,6 +16,7 @@ import pytest
 import torch
 
 import kv_q8_model as m8
+from helpers import abi_row_id
 
 P = ctypes.c_void_p(0x1000)
 P_ODD = ctypes.c_void_p(0x1001)
@@ -114,10 +115,10 @@ def test_every_code_at_every_exponent_is_exact_in_fp32_and_bf16():
 # ------------------------------------------------------------------------------------------------
 # C ABI
 # ------------------------------------------------------------------------------------------------
-NEW_SYMBOLS = ("lwm_kv_cache_write_q8", "lwm_attn_decode_partial_q8", "lwm_kv_dequant_q8")
+NEW_SYMBOLS = ("lwm_kv_cache_write_q8", "lwm_kv_dequant_q8")
 
 
-def test_new_symbols_are_declared_exported_and_bound(lib):
+def test_q8_symbols_are_declared_exported_and_bound(lib):
     from lwm_b200 import _lib
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     header = open(os.path.join(root, "include", "lwm_b200.h")).read()
@@ -125,15 +126,15 @@ def test_new_symbols_are_declared_exported_and_bound(lib):
         assert "int %s(" % name in header
         assert hasattr(lib, name)
         assert name in _lib._SIGNATURES
-    assert lib.lwm_abi_version() == 4
+    assert lib.lwm_abi_version() == 5
 
 
 # lwm_kv_cache_write_q8(k_src, v_src, src_dtype, k_data, k_exp, v_data, v_exp, pos, inv_freq, B, n_src, src0, n, L,
 #                       dst0, H, D, stream)
 KW = (P, P, 1, P, P, P, P, N, N, 2, 8, 0, 8, 64, 0, 4, 128, N)
-# lwm_attn_decode_partial_q8(q, q_dtype, k, k_exp, v, v_exp, mask, o_part, ml_part, workspace, B, H, Q, Sk, D, k_pos0,
-#                            mask_stride_b, mask_stride_q, splits, scale, pos, inv_freq, stream)
-DEC = (P, 1, P, P, P, P, N, P, P, P, 1, 2, 1, 128, 128, 0, 0, 0, 4, 0.1, N, N, N)
+# lwm_attn_decode_partial(q, k, v, dtype, k_exp, v_exp, mask, o_part, ml_part, workspace, B, H, Q, Sk, D, k_pos0,
+#                         mask_stride_b, mask_stride_q, splits, scale, pos, inv_freq, stream) on the 8-bit cache
+DEC = (P, P, P, 1, P, P, N, P, P, P, 1, 2, 1, 128, 128, 0, 0, 0, 4, 0.1, N, N, N)
 # lwm_kv_dequant_q8(data, exp, out, out_dtype, B, L, H, D, stream)
 DQ = (P, P, P, 0, 2, 64, 4, 128, N)
 
@@ -154,18 +155,19 @@ BAD_CALLS = [
     ("lwm_kv_cache_write_q8", _with(KW, a7=P), ARG, "position_ids"),
     ("lwm_kv_cache_write_q8", _with(KW, a2=2), ARG, "dtype codes"),
     ("lwm_kv_cache_write_q8", _with(KW, a4=P_ODD), ARG, "aligned"),
-    ("lwm_attn_decode_partial_q8", _with(DEC, a14=64), SHAPE, "head_dim"),
-    ("lwm_attn_decode_partial_q8", _with(DEC, a1=3), ARG, "dtype codes"),
-    ("lwm_attn_decode_partial_q8", _with(DEC, a3=N), ARG, "null pointer"),
-    ("lwm_attn_decode_partial_q8", _with(DEC, a9=N), ARG, "null pointer"),
-    ("lwm_attn_decode_partial_q8", _with(DEC, a21=P), ARG, "position_ids"),
-    ("lwm_attn_decode_partial_q8", _with(DEC, a5=P_ODD), ARG, "aligned"),
-    ("lwm_attn_decode_partial_q8", _with(DEC, a13=0), SHAPE, "bad shape"),
+    ("lwm_attn_decode_partial", _with(DEC, a14=64), SHAPE, "head_dim"),
+    ("lwm_attn_decode_partial", _with(DEC, a3=3), ARG, "dtype codes"),
+    ("lwm_attn_decode_partial", _with(DEC, a4=N), ARG, "null pointer"),       # v_exp without k_exp
+    ("lwm_attn_decode_partial", _with(DEC, a9=N), ARG, "null pointer"),
+    ("lwm_attn_decode_partial", _with(DEC, a21=P), ARG, "position_ids"),
+    ("lwm_attn_decode_partial", _with(DEC, a5=P_ODD), ARG, "aligned"),
+    ("lwm_attn_decode_partial", _with(DEC, a13=0), SHAPE, "bad shape"),
     ("lwm_kv_dequant_q8", _with(DQ, a7=64), SHAPE, "head_dim"),
     ("lwm_kv_dequant_q8", _with(DQ, a5=0), SHAPE, "bad sizes"),
     ("lwm_kv_dequant_q8", _with(DQ, a2=N), ARG, "null pointer"),
     ("lwm_kv_dequant_q8", _with(DQ, a3=2), ARG, "dtype codes"),
     ("lwm_kv_dequant_q8", _with(DQ, a0=P_ODD), ARG, "aligned"),
+    ("lwm_attn_decode_partial", _with(DEC, a5=N), ARG, "null pointer"),       # k_exp without v_exp
 ]
 
 
@@ -175,7 +177,8 @@ def _status(lib, name, *args):
     return getattr(lib, name)(*args), lib.lwm_last_error().decode()
 
 
-@pytest.mark.parametrize("name,args,code,frag", BAD_CALLS, ids=["%s-%d" % (c[0][4:], i) for i, c in enumerate(BAD_CALLS)])
+@pytest.mark.parametrize("name,args,code,frag", BAD_CALLS,
+                         ids=["%s-%d" % (abi_row_id(*c[:2]), i) for i, c in enumerate(BAD_CALLS)])
 def test_bad_arguments_are_rejected_with_a_message(lib, name, args, code, frag):
     status, msg = _status(lib, name, *args)
     assert status == code, (status, msg)
@@ -183,12 +186,12 @@ def test_bad_arguments_are_rejected_with_a_message(lib, name, args, code, frag):
 
 
 GOOD_CALLS = [("lwm_kv_cache_write_q8", KW), ("lwm_kv_cache_write_q8", _with(KW, a7=P, a8=P, a2=0)),
-              ("lwm_attn_decode_partial_q8", DEC), ("lwm_attn_decode_partial_q8", _with(DEC, a20=P, a21=P)),
-              ("lwm_kv_dequant_q8", DQ)]
+              ("lwm_attn_decode_partial", DEC), ("lwm_attn_decode_partial", _with(DEC, a20=P, a21=P)),
+              ("lwm_kv_dequant_q8", DQ), ("lwm_attn_decode_partial", _with(DEC, a3=0))]
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="fake pointers: only meaningful where the device check fails")
-@pytest.mark.parametrize("name,args", GOOD_CALLS, ids=["%s-%d" % (c[0][4:], i) for i, c in enumerate(GOOD_CALLS)])
+@pytest.mark.parametrize("name,args", GOOD_CALLS, ids=["%s-%d" % (abi_row_id(*c), i) for i, c in enumerate(GOOD_CALLS)])
 def test_well_formed_calls_fail_with_device_error_without_gpu(lib, name, args):
     status, msg = _status(lib, name, *args)
     assert status == DEVICE, (status, msg)

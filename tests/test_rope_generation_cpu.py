@@ -12,15 +12,15 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import abi_row_id
+from helpers import FOLDED_ENTRY_POINTS, abi_row_id, with_options
 
 P = ctypes.c_void_p(0x1000)      # fake non-null pointer
 N = None
 SHAPE, ARG, DEVICE = 2, 3, 1
 
-# lwm_attn_decode_partial(q, k, v, dtype, mask, o_part, ml_part, ws, B, H, Q, Sk, D, k_pos0, sb, sq, splits, scale,
-#                         position_ids, inv_freq, stream), bf16 (dtype 1) and fp32 (0)
-DEC = (P, P, P, 1, N, P, P, P, 1, 2, 1, 128, 128, 0, 0, 0, 4, 0.1, P, P, N)
+# lwm_attn_decode_partial(q, k, v, dtype, k_exp, v_exp, mask, o_part, ml_part, ws, B, H, Q, Sk, D, k_pos0, sb, sq,
+#                         splits, scale, position_ids, inv_freq, stream), bf16 (dtype 1) and fp32 (0)
+DEC = (P, P, P, 1, N, N, N, P, P, P, 1, 2, 1, 128, 128, 0, 0, 0, 4, 0.1, P, P, N)
 # lwm_kv_cache_write_rope(k_new, v_new, dtype, cache_k, cache_v, position_ids, inv_freq, B, n_src, src0, n, L, dst0,
 #                         H, D, stream)
 KVW = (P, P, 1, P, P, P, P, 2, 8, 0, 8, 64, 8, 2, 128, N)
@@ -36,12 +36,12 @@ def _with(args, **at):
 DEC32 = _with(DEC, a3=0)
 
 BAD_CALLS = [
-    ("lwm_attn_decode_partial", _with(DEC, a18=N), ARG, "null position_ids"),
-    ("lwm_attn_decode_partial", _with(DEC, a19=N), ARG, "null position_ids"),
+    ("lwm_attn_decode_partial", _with(DEC, a20=N), ARG, "null position_ids"),
+    ("lwm_attn_decode_partial", _with(DEC, a21=N), ARG, "null position_ids"),
     ("lwm_attn_decode_partial", _with(DEC, a0=N), ARG, "null pointer"),
-    ("lwm_attn_decode_partial", _with(DEC, a12=64), SHAPE, "head_dim"),
-    ("lwm_attn_decode_partial", _with(DEC32, a18=N), ARG, "null position_ids"),
-    ("lwm_attn_decode_partial", _with(DEC32, a10=0), SHAPE, "bad shape"),
+    ("lwm_attn_decode_partial", _with(DEC, a14=64), SHAPE, "head_dim"),
+    ("lwm_attn_decode_partial", _with(DEC32, a20=N), ARG, "null position_ids"),
+    ("lwm_attn_decode_partial", _with(DEC32, a12=0), SHAPE, "bad shape"),
     ("lwm_kv_cache_write_rope", _with(KVW, a14=64), SHAPE, "head_dim"),
     ("lwm_kv_cache_write_rope", _with(KVW, a10=0), SHAPE, "bad sizes"),
     ("lwm_kv_cache_write_rope", _with(KVW, a9=1), SHAPE, "out of range"),       # src0 + n > n_src
@@ -52,6 +52,9 @@ BAD_CALLS = [
     ("lwm_kv_cache_write_rope", _with(KVW, a3=N), ARG, "null pointer"),
     ("lwm_kv_cache_write_rope", _with(KVW, a2=2), ARG, "dtype codes"),
 ]
+
+# the same rows with the options of the folded entry points turned on: no option slot bypasses these checks
+BAD_CALLS += [(n, with_options(n, a, P), c, f) for n, a, c, f in BAD_CALLS if n in FOLDED_ENTRY_POINTS]
 
 
 def _status(lib, name, *args):
@@ -70,6 +73,8 @@ def test_new_entries_reject_bad_arguments(lib, name, args, code, frag):
 
 GOOD_CALLS = [("lwm_attn_decode_partial", DEC), ("lwm_attn_decode_partial", DEC32),
               ("lwm_kv_cache_write_rope", KVW), ("lwm_kv_cache_write_rope", _with(KVW, a2=0, a9=3, a10=5, a12=59))]
+
+GOOD_CALLS += [(n, with_options(n, a, P)) for n, a in GOOD_CALLS if n in FOLDED_ENTRY_POINTS]
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="fake pointers: only meaningful where the device check fails")

@@ -2,8 +2,8 @@
 
 One GPU, B = 1, H = 32, causal, single step (q_pos0 = k_pos0 = 0), S = 32768 and 131072, both precision modes, with the
 call site's zero bias (the block-map kernels) and without a mask (the plain kernels). Per configuration it alternates
-p = 0 (lwm_attn_fwd_step / lwm_attn_bwd_step) and p = 0.1 (the _dropout symbols) in one process, times each step with
-CUDA events and prints one JSON line: ms per kernel (median of the alternating rounds) and the ratio. The card, its
+p = 0 and p = 0.1 (lwm_attn_fwd_step / lwm_attn_bwd_step with drop_threshold 0 and 6554) in one process, times each
+step with CUDA events and prints one JSON line: ms per kernel (median of the alternating rounds) and the ratio. The card, its
 power limit and SM clock are read in the same run.
 
 usage: python tools/perf_attn_dropout.py [--sizes 32768,131072] [--modes fp16,bf16] [--rounds 3] [--json OUT]"""

@@ -3,7 +3,8 @@
 1. The backward tile step, unordered against ordered, alternating in one process: B = 1, H = 32, causal, S = 32768 and
    131072, both precision modes, without a mask and with the call-site bias (zero bias and segment ids: the block-map
    path). Each timed call is the step as the op makes it (ringattention's one-GPU backward: block map, then
-   lwm_attn_bwd_step or lwm_attn_bwd_step_ordered with its workspace zeroing and turns pass), timed with CUDA events;
+   lwm_attn_bwd_step without or with an order_ws, the latter with its workspace zeroing and turns pass), timed with
+   CUDA events;
    median over the rounds. The two dQ are compared within 1e-5 of max|dQ| and dK / dV bit for bit.
 2. One full forward + backward of ringattention at S = 32768 (fp16 mode, no mask) with the flag off and on, and with
    torch.utils.deterministic.fill_uninitialized_memory at its default (True) and False.

@@ -273,6 +273,31 @@ int lwm_kv_cache_write_q8(const void* k_src, const void* v_src, int src_dtype, s
 int lwm_kv_dequant_q8(const signed char* data, const signed char* exp, void* out, int out_dtype, int B, int L, int H,
                       int D, void* stream);
 
+/* The decode step without host values that change from token to token, so that it can be captured once in a CUDA graph
+ * and replayed (`ShardedKVCache` with torch.cuda.graph; INTEGRATION.md "Decode in a CUDA graph").
+ * lwm_kv_cache_write_at     the decode write of k_new / v_new [B,1,H,128] (src_dtype 0 = fp32, 1 = bf16) into this
+ *                           rank's shard [B,L,H,128] of a max_length-row cache, whose rows are [lo, lo + L), at the
+ *                           global slot cursor[0]. cursor is int32 [2]: the slot, then an arrival counter that must be
+ *                           zero and is zero again after the call; the call advances the slot by one, on every rank.
+ *                           Only the owner of the slot writes. The cache is, like the existing writes store it:
+ *                             k_exp, v_exp NULL, no positions: bf16 / fp32 of src_dtype, rows copied bit for bit;
+ *                             k_exp, v_exp NULL, positions: as lwm_kv_cache_write_rope;
+ *                             k_exp, v_exp given: the 8-bit cache (cache_k / cache_v its codes), as lwm_kv_cache_write_q8.
+ *                           position_ids int32 [B] and inv_freq [64], or both NULL; max_position bounds the positions.
+ *                           A slot >= max_length, or any position outside [0, max_position), writes nothing and ORs
+ *                           LWM_DEVICE_ERR_SLOT / LWM_DEVICE_ERR_POSITION into *err, a sticky int32 the caller reads
+ *                           and clears.
+ * lwm_rope_check_positions  ORs LWM_DEVICE_ERR_POSITION into *err if any of position_ids [n] is outside
+ *                           [0, max_position): the range check of a rotating op's positions without a device->host
+ *                           copy. */
+#define LWM_DEVICE_ERR_SLOT 1
+#define LWM_DEVICE_ERR_POSITION 2
+int lwm_kv_cache_write_at(const void* k_new, const void* v_new, int src_dtype, void* cache_k, void* cache_v,
+                          signed char* k_exp, signed char* v_exp, const int* position_ids, const float* inv_freq,
+                          int max_position, int* cursor, long long lo, int L, int max_length, int B, int H, int D,
+                          int* err, void* stream);
+int lwm_rope_check_positions(const int* position_ids, long long n, int max_position, int* err, void* stream);
+
 /* The operand passes of the attention op with the rotary embedding folded in (`ringattention(..., freqs_cis,
  * position_ids)`): x [B,S,H,128] fp32 (0) or bf16 (1) holds UN-rotated q or k, position_ids int32 [B,S], inv_freq [64]
  * as for lwm_attn_rope. Every pass works on rope(x) rounded to x's dtype — bit for bit what lwm_attn_rope writes — so

@@ -48,6 +48,9 @@ _SIGNATURES = {
     "lwm_kv_cache_write_q8": [c_void_p, c_void_p, c_int] + [c_void_p] * 6 + [c_int, c_int, c_ll, c_int, c_int, c_ll,
                                                                               c_int, c_int, c_void_p],
     "lwm_kv_dequant_q8": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
+    "lwm_kv_cache_write_at": [c_void_p, c_void_p, c_int] + [c_void_p] * 6 + [c_int, c_void_p, c_ll] + [c_int] * 5
+                             + [c_void_p, c_void_p],
+    "lwm_rope_check_positions": [c_void_p, c_ll, c_int, c_void_p, c_void_p],
     "lwm_attn_mask_pack": [c_void_p, c_ll, c_ll, c_ll, c_int, c_int, c_ll, c_int, c_int, c_void_p, c_void_p, c_void_p],
     "lwm_attn_infer_tilemap": [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p],
     "lwm_attn_infer_partial": [c_void_p] * 12 + [c_int] * 6 + [c_float, c_void_p],

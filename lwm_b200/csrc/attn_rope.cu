@@ -11,6 +11,7 @@
 // amortised over H heads and the kernel is a pure HBM stream: each element is read once and written once.
 // The [B,S,H*D] projection output and the op's [B,S,H,D] input are the same memory: the head split is free.
 #include "capi_internal.h"
+#include "kv_write.cuh"
 #include "rope_common.cuh"
 
 namespace lwm {
@@ -67,10 +68,8 @@ static int launch_rope(const void* xq, const void* xk, void* oq, void* ok, const
   return lwm_check_launch("rope_kernel");
 }
 
-// KV-cache write of new rows with the rotary embedding on the keys: token t of the B*n new rows per tensor is (b, i),
-// source row b*n_src + src0 + i of k_new / v_new [B,n_src,H,128], destination row b*L + dst0 + i of the cache shards
-// [B,L,H,128]; k is rotated at position_ids[b*n_src + src0 + i] and rounded to T (rope_kernel<T, T>'s bits), v is
-// copied bit for bit. One CTA serves kRopePos tokens, like rope_kernel.
+// KV-cache write of new rows with the rotary embedding on the keys (kv_write.cuh: kv_write_rows), one CTA per kRopePos
+// tokens like rope_kernel.
 template <typename T>
 __global__ void __launch_bounds__(256) kv_write_rope_kernel(const T* __restrict__ k_new, const T* __restrict__ v_new,
                                                             T* __restrict__ cache_k, T* __restrict__ cache_v,
@@ -78,52 +77,8 @@ __global__ void __launch_bounds__(256) kv_write_rope_kernel(const T* __restrict_
                                                             const float* __restrict__ inv_freq, int n_src,
                                                             long long src0, int n, int L, long long dst0, int H,
                                                             long long n_tok) {
-  __shared__ float2 cs[kRopePos][kRopePairs];
-  const long long tok0 = (long long)blockIdx.x * kRopePos;
-  {
-    const int p = threadIdx.x >> 6, j = threadIdx.x & 63;
-    const long long tok = tok0 + p;
-    if (tok < n_tok) {
-      const long long b = tok / n, i = tok - b * n;
-      cs[p][j] = rope_cos_sin(position_ids, inv_freq, b * n_src + src0 + i, j, 1.0f);
-    }
-  }
-  __syncthreads();
-  const int vh = H * (kRopeDim / 8), vt = 2 * vh;      // 8-element vectors of one row of k (then of v)
-  constexpr int kBatch = Raw8<T>::kBatch;
-  const int total = kRopePos * vt;
-  for (int base = threadIdx.x; base < total; base += kBatch * blockDim.x) {
-    Raw8<T> raw[kBatch];
-    long long src[kBatch], dst[kBatch];
-    int cs_idx[kBatch];
-    bool live[kBatch], is_k[kBatch];
-#pragma unroll
-    for (int u = 0; u < kBatch; ++u) {
-      const int v = base + u * blockDim.x;
-      const int p = v / vt, r = v - p * vt;
-      const long long tok = tok0 + p;
-      live[u] = v < total && tok < n_tok;
-      is_k[u] = r < vh;
-      const int rr = is_k[u] ? r : r - vh;
-      const long long b = tok / n, i = tok - b * n;
-      src[u] = (b * n_src + src0 + i) * H * kRopeDim + rr * 8;
-      dst[u] = (b * L + dst0 + i) * H * kRopeDim + rr * 8;
-      cs_idx[u] = p * kRopePairs + (rr & 15) * 4;
-      if (live[u]) raw[u].load((is_k[u] ? k_new : v_new) + src[u]);
-    }
-#pragma unroll
-    for (int u = 0; u < kBatch; ++u) {
-      if (!live[u]) continue;
-      if (is_k[u]) {
-        float x[8], y[8];
-        raw[u].unpack(x);
-        rope_rotate8(x, y, &cs[0][0], cs_idx[u]);
-        store8<T>(cache_k + dst[u], y);
-      } else {
-        raw[u].store(cache_v + dst[u]);
-      }
-    }
-  }
+  kv_write_rows<T, true>(k_new, v_new, cache_k, cache_v, position_ids, inv_freq, n_src, src0, n, L, dst0, H, n_tok,
+                         (long long)blockIdx.x * kRopePos);
 }
 
 }  // namespace lwm

@@ -101,11 +101,34 @@ class QuantizedKV:
         return out
 
 
+def kv_cache_write_at(key, value, cache_k, cache_v, cursor, lo, max_length, pos=None, inv_freq=None, max_position=0):
+    """the decode write of key / value [B,1,H,128] (bf16 or fp32, contiguous) into this rank's shards cache_k / cache_v
+    [B,L,H,128] of a max_length-row cache (tensors of key's dtype, or QuantizedKV) at the global slot cursor[0]
+    (cursor: int32 [2] on the GPU, the slot and a zero word), which it advances by one on the device. Only the owner of
+    the slot (lo <= slot < lo + L) writes, as kv_cache_write_rope / kv_cache_write_q8 / a row copy at that row would.
+    pos int32 [B,1] and inv_freq: k is rotated first. A slot >= max_length or a position outside [0, max_position)
+    writes nothing and sets a bit of the device error word (rope.error_word). No host synchronisation: the call can be
+    captured in a CUDA graph (lwm_kv_cache_write_at)."""
+    B, _, H, D = key.shape
+    q8 = isinstance(cache_k, QuantizedKV)
+    _lib.call("lwm_kv_cache_write_at", _lib.ptr(key), _lib.ptr(value), _dt(key),
+              _lib.ptr(cache_k.data if q8 else cache_k), _lib.ptr(cache_v.data if q8 else cache_v),
+              _lib.ptr(cache_k.exp if q8 else None), _lib.ptr(cache_v.exp if q8 else None), _lib.ptr(pos),
+              _lib.ptr(inv_freq), int(max_position), _lib.ptr(cursor), int(lo), cache_k.shape[1], int(max_length), B,
+              H, D, _lib.ptr(_rope.error_word(key.device)), _lib.stream_ptr())
+
+
 class ShardedKVCache:
     """comm: None (torch.distributed over `group`, or a ring of one), or an object with TorchComm's all_gather and
-    `world` / `rank` attributes (e.g. an in-process stand-in that runs the real kernels on emulated ranks)."""
+    `world` / `rank` attributes (e.g. an in-process stand-in that runs the real kernels on emulated ranks).
+
+    On a GPU the write slot is kept twice: cache_index on the host and `cursor`, an int32 on the device. Every decode
+    write goes through kv_cache_write_at, which reads the slot from the cursor and advances it on the device, eager or
+    captured, so the decode step can be recorded once in a CUDA graph and replayed token after token (INTEGRATION.md
+    "Decode in a CUDA graph"). The prefill stays eager. A CPU cache (host bookkeeping) writes at the host index."""
     write_rope = staticmethod(kv_cache_write_rope)
     write_q8 = staticmethod(kv_cache_write_q8)
+    write_at = staticmethod(kv_cache_write_at)
 
     def __init__(self, batch, max_length, num_heads, head_dim, dtype=torch.bfloat16, device="cuda", group=None,
                  comm=None):
@@ -131,7 +154,61 @@ class ShardedKVCache:
         else:
             self.cached_key = torch.zeros(shape, dtype=dtype, device=device)       # jnp.zeros (llama.py:444-445)
             self.cached_value = torch.zeros(shape, dtype=dtype, device=device)
-        self.cache_index = 0
+        self._on_gpu = self.cached_key.device.type == "cuda"
+        self._index = 0
+        self._cursor = None             # made on first use (_device_cursor): the cache allocates only its rows here
+        self._captured = False          # a decode write was captured: replays move the cursor without the host
+
+    def _device_cursor(self):
+        """[the slot, the write kernel's arrival counter (zero between writes)], int32 on the cache's device; made by the
+        first eager decode write or `cursor` read, with the GPU's error word. Not inside a capture: the fill would be
+        recorded and every replay would rewind the slot."""
+        if self._cursor is None:
+            if _rope.capturing():
+                raise RuntimeError("ShardedKVCache: the device cursor does not exist yet; run the decode step once "
+                                   "eagerly (the warm-up) before capturing it")
+            cursor = torch.zeros(2, dtype=torch.int32, device=self.cached_key.device)
+            cursor[0].fill_(self._index)
+            if self._on_gpu:
+                _rope.error_word(cursor.device)
+            self._cursor = cursor
+        return self._cursor
+
+    @property
+    def cursor(self):
+        """the slot of the next write as a 0-d int32 device tensor (a view of the cursor). A decode write advances it,
+        so whatever a step derives from it (decode_attention_mask, position_ids) is computed before concatenate."""
+        return self._device_cursor()[0]
+
+    @property
+    def cache_index(self):
+        """the global slot of the next write (the reference's cache_index). Once a decode write has been captured in a
+        CUDA graph, replays advance the device cursor behind the host's back, and each read synchronises once to fetch
+        it."""
+        if self._captured:
+            if _rope.capturing():
+                raise RuntimeError("ShardedKVCache.cache_index cannot be read while capturing a CUDA graph (it would "
+                                   "need a synchronisation); use the device tensor `cursor`")
+            self._index = int(self._cursor[0].item())
+        return self._index
+
+    @cache_index.setter
+    def cache_index(self, value):
+        value = int(value)
+        if value < 0:
+            raise ValueError("ShardedKVCache.cache_index must be >= 0, got %d" % value)
+        self._index = value
+        if self._cursor is not None:
+            self._cursor[0].fill_(value)
+
+    def take_errors(self):
+        """-> the bits the device checks have set since the last call, and clears them: rope.ERR_SLOT (a decode write at
+        a slot >= max_length: nothing was written) and rope.ERR_POSITION (a position outside [0, max_position) of the
+        rotary table: nothing was written, or a captured ringattention_inference rotated q at it). The word belongs to
+        the GPU: every cache and capturing op on it shares it. One synchronisation."""
+        if not self._on_gpu:
+            return 0
+        return _rope.take_errors(self.cached_key.device)
 
     def concatenate(self, key, value, *, freqs_cis=None, position_ids=None):
         """key/value: the new rows. Decode: [B,1,H,D], replicated along the ring. Prefill: this rank's shard
@@ -144,17 +221,35 @@ class ShardedKVCache:
         every rank rotates only the slice it keeps, straight into its shard.
         The 8-bit cache (dtype=torch.int8): key and value are bf16 or fp32, of one dtype, and every write goes through
         write_q8 (one launch for k and v, rotating the keys first when the rotary keywords are given); each rank
-        quantizes only the rows it keeps. The returned pair is QuantizedKV."""
+        quantizes only the rows it keeps. The returned pair is QuantizedKV.
+        On a GPU the decode write is one kv_cache_write_at launch on every rank (only the owner writes) at the device
+        cursor, and it can be captured in a CUDA graph: key, value and position_ids are then device tensors, and a slot
+        past max_length or a position outside the table writes nothing and sets a bit that take_errors reports (the
+        eager decode past max_length writes nothing either). The prefill cannot be captured."""
+        decode = key.shape[1] == 1 and value.shape[1] == 1 and self._is_decode(key)
+        capturing = _rope.capturing()
+        if capturing and not decode:
+            raise RuntimeError("ShardedKVCache.concatenate: only the decode step (one new row) can be captured in a CUDA "
+                               "graph; run the prefill eagerly before capturing")
+        # (the decode write on a GPU checks its positions on the device itself)
         rope = _rope.check_position_ids("ShardedKVCache.concatenate", freqs_cis, position_ids,
-                                        (key.shape[0], key.shape[1]), key.device)
+                                        (key.shape[0], key.shape[1]), key.device, device_check=False)
         if self.quantized:
-            return self._concatenate_q8(key, value, rope)
-        if rope is not None and not (key.dtype == value.dtype == self.cached_key.dtype):
+            if not (key.dtype == value.dtype and key.dtype in (torch.bfloat16, torch.float32)):
+                raise ValueError("ShardedKVCache.concatenate: the 8-bit cache takes bfloat16 or float32 key and value "
+                                 "of one dtype, got %s and %s" % (key.dtype, value.dtype))
+        elif rope is not None and not (key.dtype == value.dtype == self.cached_key.dtype):
             raise ValueError("ShardedKVCache.concatenate: with the rotary keywords key and value must have the cache "
                              "dtype %s, got %s and %s" % (self.cached_key.dtype, key.dtype, value.dtype))
+        if decode and self._on_gpu:
+            self._write_decode(key, value, rope, freqs_cis, capturing)
+            return self.cached_key, self.cached_value
+        if self.quantized:
+            return self._concatenate_q8(key, value, rope)
         lo = self.rank * self.shard_len
-        if key.shape[1] == 1 and value.shape[1] == 1 and self._is_decode(key):
-            cur = self.cache_index - lo
+        ci = self.cache_index
+        if decode:
+            cur = ci - lo
             if 0 <= cur < self.shard_len:
                 if rope is None:
                     self.cached_key[:, cur].copy_(key[:, -1])
@@ -165,47 +260,70 @@ class ShardedKVCache:
             n_new = 1
         else:
             n_new = key.shape[1] * self.world
-            if self.cache_index + n_new > self.max_length:
-                raise ValueError("cache overflow: %d + %d > %d" % (self.cache_index, n_new, self.max_length))
-            # global slots [cache_index, cache_index + n_new) intersected with my rows [lo, lo + shard_len)
-            a, b = max(self.cache_index, lo), min(self.cache_index + n_new, lo + self.shard_len)
+            if ci + n_new > self.max_length:
+                raise ValueError("cache overflow: %d + %d > %d" % (ci, n_new, self.max_length))
+            # global slots [ci, ci + n_new) intersected with my rows [lo, lo + shard_len)
+            a, b = max(ci, lo), min(ci + n_new, lo + self.shard_len)
             if rope is not None:
                 k_all, v_all, p_all = (self._gather_rows(t.contiguous()) for t in (key, value, rope[0]))
                 if b > a:
-                    self.write_rope(k_all.contiguous(), v_all.contiguous(), a - self.cache_index, b - a,
+                    self.write_rope(k_all.contiguous(), v_all.contiguous(), a - ci, b - a,
                                     self.cached_key, self.cached_value, a - lo, p_all.contiguous(), rope[1])
-                self.cache_index += n_new
+                self.cache_index = ci + n_new
                 return self.cached_key, self.cached_value
             for new, cache in ((key, self.cached_key), (value, self.cached_value)):
                 full = self._gather_rows(new.contiguous())
                 if b > a:
-                    cache[:, a - lo:b - lo].copy_(full[:, a - self.cache_index:b - self.cache_index])
-        self.cache_index += n_new
+                    cache[:, a - lo:b - lo].copy_(full[:, a - ci:b - ci])
+        self.cache_index = ci + n_new
         return self.cached_key, self.cached_value
 
+    def _write_decode(self, key, value, rope, freqs_cis, capturing):
+        """the decode write of a GPU cache at the device cursor (eager and captured alike)"""
+        B, _, H, D = self.cached_key.shape
+        if tuple(key.shape) != (B, 1, H, D) or tuple(value.shape) != (B, 1, H, D):
+            raise ValueError("ShardedKVCache.concatenate: the decode rows must be [B,1,H,D] = %s, got %s and %s"
+                             % ((B, 1, H, D), tuple(key.shape), tuple(value.shape)))
+        if capturing and not (key.is_cuda and value.is_cuda):
+            raise ValueError("ShardedKVCache.concatenate: while capturing a CUDA graph key and value must be device "
+                             "tensors")
+        cursor = self._device_cursor()
+        dev = cursor.device
+        if self.quantized:
+            key, value = key.to(device=dev).contiguous(), value.to(device=dev).contiguous()
+        else:       # (a row copy casts to the cache dtype)
+            dt = self.cached_key.dtype
+            key = key.to(device=dev, dtype=dt).contiguous()
+            value = value.to(device=dev, dtype=dt).contiguous()
+        pos, inv_freq = rope if rope is not None else (None, None)
+        self.write_at(key, value, self.cached_key, self.cached_value, cursor, self.rank * self.shard_len,
+                      self.max_length, pos, inv_freq, 0 if rope is None else freqs_cis.max_position)
+        if capturing:
+            self._captured = True
+        else:
+            self._index += 1
+
     def _concatenate_q8(self, key, value, rope):
-        if not (key.dtype == value.dtype and key.dtype in (torch.bfloat16, torch.float32)):
-            raise ValueError("ShardedKVCache.concatenate: the 8-bit cache takes bfloat16 or float32 key and value of one "
-                             "dtype, got %s and %s" % (key.dtype, value.dtype))
         pos, inv_freq = rope if rope is not None else (None, None)
         lo = self.rank * self.shard_len
+        ci = self.cache_index
         if key.shape[1] == 1 and value.shape[1] == 1 and self._is_decode(key):
-            cur = self.cache_index - lo
+            cur = ci - lo
             if 0 <= cur < self.shard_len:
                 self.write_q8(key.contiguous(), value.contiguous(), 0, 1, self.cached_key, self.cached_value, cur,
                               None if pos is None else pos.contiguous(), inv_freq)
-            self.cache_index += 1
+            self.cache_index = ci + 1
             return self.cached_key, self.cached_value
         n_new = key.shape[1] * self.world
-        if self.cache_index + n_new > self.max_length:
-            raise ValueError("cache overflow: %d + %d > %d" % (self.cache_index, n_new, self.max_length))
-        a, b = max(self.cache_index, lo), min(self.cache_index + n_new, lo + self.shard_len)
+        if ci + n_new > self.max_length:
+            raise ValueError("cache overflow: %d + %d > %d" % (ci, n_new, self.max_length))
+        a, b = max(ci, lo), min(ci + n_new, lo + self.shard_len)
         k_all, v_all = self._gather_rows(key.contiguous()), self._gather_rows(value.contiguous())
         p_all = None if pos is None else self._gather_rows(pos.contiguous()).contiguous()
         if b > a:
-            self.write_q8(k_all.contiguous(), v_all.contiguous(), a - self.cache_index, b - a, self.cached_key,
+            self.write_q8(k_all.contiguous(), v_all.contiguous(), a - ci, b - a, self.cached_key,
                           self.cached_value, a - lo, p_all, inv_freq)
-        self.cache_index += n_new
+        self.cache_index = ci + n_new
         return self.cached_key, self.cached_value
 
     def _is_decode(self, key):

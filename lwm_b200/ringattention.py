@@ -63,10 +63,18 @@ def attention_bias_from_mask(attention_mask, dtype=torch.bfloat16):
 def decode_attention_mask(attention_mask, query_length, cache_index, max_decoder_length=None):
     """Boolean mask [B,1,Q,K] for `ringattention_inference` while decoding from a KV cache (lwm/llama.py:574-591):
     causal_mask[i, j] = j <= i + cache_index over the cache length, combined (AND) with the padding mask
-    attention_mask [B,K] (combine_masks)."""
+    attention_mask [B,K] (combine_masks). cache_index: an int, or a 0-d integer device tensor such as
+    ShardedKVCache.cursor (read on the device, so the mask can be part of a captured decode step)."""
     K = attention_mask.shape[-1] if max_decoder_length is None else int(max_decoder_length)
     dev = attention_mask.device
-    causal = torch.arange(K, device=dev)[None, :] <= (torch.arange(query_length, device=dev) + int(cache_index))[:, None]
+    if isinstance(cache_index, torch.Tensor):
+        if cache_index.dim() != 0 or cache_index.is_floating_point():
+            raise ValueError("decode_attention_mask: cache_index must be an int or a 0-d integer tensor, got %s %s"
+                             % (cache_index.dtype, tuple(cache_index.shape)))
+        start = cache_index.to(device=dev)
+    else:
+        start = int(cache_index)
+    causal = torch.arange(K, device=dev)[None, :] <= (torch.arange(query_length, device=dev) + start)[:, None]
     return (attention_mask[:, None, None, :K] > 0) & causal[None, None]
 
 
@@ -1264,10 +1272,22 @@ def ringattention_inference(q, k, v, attn_mask, axis_name="sp", *, freqs_cis=Non
     k, v may be the 8-bit cache (kv_cache.QuantizedKV, both or neither) with q bf16 or fp32, without gradient and with
     rotate_k=False when the rotary keywords are given. Below INFER_MIN_Q query rows (world * Q_loc on a q-sharded
     ring) the GEMV kernel reads it directly, bit for bit the call on the cache dequantized to q's dtype; from there on
-    the shard is dequantized to q's dtype (exact; one transient copy) for the tensor-core path."""
+    the shard is dequantized to q's dtype (exact; one transient copy) for the tensor-core path.
+
+    CUDA graphs: on one GPU the GEMV call (Q < INFER_MIN_Q) can be captured with torch.cuda.graph, together with the
+    ShardedKVCache decode write, and replayed (INTEGRATION.md "Decode in a CUDA graph"). While capturing, position_ids
+    must be a device tensor and is range-checked on the device (rope.ERR_POSITION in rope.error_word) instead of on the
+    host; a ring of more than one rank or Q >= INFER_MIN_Q raises NotImplementedError."""
     group, rank, world = _resolve_group(axis_name)
     B, Q, H, D = q.shape
     Sk = k.shape[1]
+    if _rope.capturing():
+        if world > 1:
+            raise NotImplementedError("ringattention_inference: capturing in a CUDA graph is supported on one GPU only, "
+                                      "not across a ring of %d ranks" % world)
+        if Q >= INFER_MIN_Q:
+            raise NotImplementedError("ringattention_inference: only the GEMV decode path (Q < INFER_MIN_Q = %d query "
+                                      "rows) can be captured in a CUDA graph, got Q = %d" % (INFER_MIN_Q, Q))
     rope = _rope.check_position_ids("ringattention_inference", freqs_cis, position_ids, (B, Q), q.device)
     quantized = _quantized_kv("ringattention_inference", q, k, v, rope is not None and bool(rotate_k))
     if rope is not None and rotate_k and Q != Sk:

@@ -84,11 +84,59 @@ def rotate(x, freqs_cis, dtype, *, position_ids):
     return _Rope.apply(x, x[:, :, :0], position_ids, freqs_cis, dtype)[0]
 
 
-def check_position_ids(who, freqs_cis, position_ids, shape, device):
+ERR_SLOT, ERR_POSITION = 1, 2        # bits of the device error word (LWM_DEVICE_ERR_* in include/lwm_b200.h)
+_ERROR_WORDS = {}
+
+
+def error_word(device):
+    """The sticky int32 [1] error word of a GPU, shared by every check of the capturable decode step on it: the KV-cache
+    write at the device cursor (ERR_SLOT: a slot past the cache, ERR_POSITION) and the position check of
+    ringattention_inference while capturing (ERR_POSITION). take_errors reads and clears it. The word is created with the
+    first cache cursor on the device (ShardedKVCache.cursor, or its first eager decode write), never inside a capture,
+    where its zero-fill would be recorded and replayed."""
+    device = torch.device(device)
+    if device.index is None:
+        device = torch.device(device.type, torch.cuda.current_device())
+    word = _ERROR_WORDS.get(device)
+    if word is None:
+        if capturing():
+            raise RuntimeError("the decode error word of %s does not exist yet: run the step once eagerly (the warm-up) "
+                               "before capturing it" % device)
+        word = _ERROR_WORDS[device] = torch.zeros(1, dtype=torch.int32, device=device)
+    return word
+
+
+def take_errors(device):
+    """-> the error bits (ERR_SLOT | ERR_POSITION) the device checks have set on `device` since the last call, and clears
+    them. One device->host synchronisation; 0 means every write and position since then was in range."""
+    word = error_word(device)
+    bits = int(word.item())
+    if bits:
+        word.zero_()
+    return bits
+
+
+def capturing():
+    """whether the current CUDA stream is capturing a CUDA graph (False without a GPU)"""
+    return torch.cuda.is_available() and torch.cuda.is_current_stream_capturing()
+
+
+def check_positions_on_device(position_ids, max_position):
+    """ERR_POSITION into the device's error word if any of position_ids (int32, contiguous, on a GPU) is outside
+    [0, max_position): the range check without a device->host copy (lwm_rope_check_positions)"""
+    _lib.call("lwm_rope_check_positions", _lib.ptr(position_ids), position_ids.numel(), int(max_position),
+              _lib.ptr(error_word(position_ids.device)), _lib.stream_ptr())
+
+
+def check_position_ids(who, freqs_cis, position_ids, shape, device, device_check=True):
     """The rotary-embedding keywords of the ops that rotate inside their own passes -> None (both None) or
     (position_ids int32 [shape] contiguous on `device`, inv_freq). Raises ValueError unless they come together, freqs_cis
     is a RotaryTable, position_ids has `shape` and every position is in [0, max_position). Device positions cost one
-    device->host synchronisation (the range check); host positions none (the copy to the device is asynchronous)."""
+    device->host synchronisation (the range check); host positions none (the copy to the device is asynchronous).
+    While the current stream is capturing a CUDA graph, position_ids must be a device tensor (a host tensor's copy would
+    be recorded with the values it has now) and the range check runs on the device instead, without a synchronisation:
+    an out-of-range position sets ERR_POSITION in error_word (device_check=False leaves the check to the caller's
+    kernel)."""
     if freqs_cis is None and position_ids is None:
         return None
     if freqs_cis is None or position_ids is None:
@@ -97,6 +145,14 @@ def check_position_ids(who, freqs_cis, position_ids, shape, device):
         raise ValueError("%s: freqs_cis must come from lwm_b200.rope.precompute_freqs_cis" % who)
     if tuple(position_ids.shape) != tuple(shape):
         raise ValueError("%s: position_ids must be [B, S_loc] = %s, got %s" % (who, tuple(shape), tuple(position_ids.shape)))
+    if capturing():
+        if not position_ids.is_cuda:
+            raise ValueError("%s: while capturing a CUDA graph position_ids must be a device tensor (the copy of a host "
+                             "tensor would replay the values it has at capture)" % who)
+        pos = position_ids.to(device=device, dtype=torch.int32).contiguous()
+        if device_check and pos.numel():
+            check_positions_on_device(pos, freqs_cis.max_position)
+        return pos, freqs_cis.inv_freq
     if position_ids.numel():
         lo, hi = torch.stack(torch.aminmax(position_ids)).tolist()
         if lo < 0 or hi >= freqs_cis.max_position:

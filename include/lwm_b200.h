@@ -92,6 +92,21 @@ int lwm_attn_fwd_step(const void* q, const void* k, const void* v, const float* 
 int lwm_attn_dropout_mask(long long seed, unsigned drop_threshold, int b, int h, long long q_pos0, long long k_pos0,
                           int n_q, int n_k, unsigned char* out, void* stream);
 
+/* Ring attention, forward step of the fp8 mode (no gradient: the prefill under torch.no_grad()). S = Q K^T runs on the
+ * FP8 tensor cores; P V, the softmax, the carries and the epilogue are those of the fp16 operand mode.
+ *   q8, k8       [B, Sq, H, 128] / [B, Sk, H, 128] e4m3 copies x8 = e4m3(x / scale), scale = 2^(e-7) with e the
+ *                exponent of the tensor's largest finite |x| (lwm_attn_e4m3_scale_from_absmax, lwm_attn_to_e4m3_scaled)
+ *   v16          [B, Sk, H, 128] fp16 copy of v as in the fp16 operand mode (scale 2^(e-12), lwm_attn_to_f16_scaled)
+ *   scale_q/k/v  their device scales, all required
+ * The logits are (q8 . k8) * scale_q * scale_k in fp32. Every other argument, constraint and output is that of
+ * lwm_attn_fwd_step in the fp16 operand mode (out_f32 optional); there is no dropout. */
+int lwm_attn_fwd_e4m3_step(const void* q8, const void* k8, const void* v16, const float* scale_q, const float* scale_k,
+                           const float* scale_v, float* out_f32, void* out, float* lse, float* acc_o, float* acc_m,
+                           float* acc_l, int B, int H, int Sq, int Sk, int D, long long q_pos0, long long k_pos0,
+                           int causal, const float* bias, long long bias_stride, const int* segment_ids,
+                           long long seg_stride, float softmax_scale, int first, int last, const int* tiles,
+                           const int* tile_count, void* stream);
+
 /* Ring attention, backward.
  * lwm_attn_bwd_prep: delta[b,h,s] = sum_d dout[b,s,h,d] * out[b,s,h,d]  (fp32), once per backward. out fp32
  *                    (out_dtype 0) or bf16 (1); dout bf16 when scale_do is NULL, else its scaled fp16 copy with its
@@ -174,6 +189,15 @@ int lwm_attn_absmax(const void* x, int dtype, long long n, unsigned* out_bits, v
 int lwm_attn_absmax_scale(const void* x, int dtype, long long n, unsigned* workspace, float* scale_out, void* stream);
 int lwm_attn_scale_from_absmax(const unsigned* bits, int n, int stride, float* scale_out, void* stream);
 int lwm_attn_to_f16_scaled(const void* x, int dtype, void* dst_f16, const float* scale, long long n, void* stream);
+/* e4m3 operand copies of the fp8 mode (lwm_attn_fwd_e4m3_step), same protocol with a smaller top exponent:
+ * lwm_attn_e4m3_scale_from_absmax: *scale_out = 2^(e-7) from the gathered patterns (e clamped at -114; 1 when every
+ *   pattern is 0), so the largest finite |x| / scale lies in [128, 256), below e4m3's 448: nothing saturates.
+ * lwm_attn_to_e4m3_scaled: dst [n] bytes = e4m3(x / *scale), round to nearest even, bit for bit torch's
+ *   x.div(scale).to(torch.float8_e4m3fn) for finite x. e4m3fn has no infinity: +-inf become the NaN bytes 0x7f / 0xff
+ *   (as torch's cast) and a NaN a NaN byte of either sign, where the fp16 copies keep +-inf. dtype 0 = fp32, 1 = bf16;
+ *   n % 8 == 0. */
+int lwm_attn_e4m3_scale_from_absmax(const unsigned* bits, int n, int stride, float* scale_out, void* stream);
+int lwm_attn_to_e4m3_scaled(const void* x, int dtype, void* dst_e4m3, const float* scale, long long n, void* stream);
 int lwm_reduce_cast_f32(const float* const* host_srcs, int n_src, void* dst, int dst_dtype, long long n, void* stream);
 
 /* Decode-time attention — the reference's `ringattention_inference(q, k, v, attn_mask, axis_name)` (call site
@@ -304,7 +328,8 @@ int lwm_rope_check_positions(const int* position_ids, long long n, int max_posit
  * each equals lwm_attn_rope followed by the plain pass, without the rotated tensor in memory.
  * lwm_attn_absmax_rope      atomicMax of the finite |rope(x)| bit patterns into *out_bits (caller zeroes it), as lwm_attn_absmax.
  * lwm_attn_stage_rope       dst_dtype 2: dst = fp16(rope(x) / *scale), as lwm_attn_to_f16_scaled; dst_dtype 1: dst =
- *                           bf16(rope(x)), the bf16 operand mode's copy (scale unused, may be null).
+ *                           bf16(rope(x)), the bf16 operand mode's copy (scale unused, may be null); dst_dtype 3:
+ *                           dst = e4m3(rope(x) / *scale), as lwm_attn_to_e4m3_scaled (one byte per element).
  * lwm_reduce_cast_rope_f32  dst [B,S,H,128] = T(rope*(T(sum of n_src <= 16 fp32 arrays, fixed order))), T = fp32 (0) or
  *                           bf16 (1), rope* the conjugate rotation: lwm_reduce_cast_f32 followed by lwm_attn_rope(conj=1)
  *                           in one pass (the gradient w.r.t. the un-rotated q / k). host_srcs: HOST array of device

@@ -17,6 +17,8 @@ _SIGNATURES = {
     "lwm_attn_fwd_step": [c_void_p] * 12 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll, c_float,
                                                          c_int, c_int, c_void_p, c_void_p, c_ll, ctypes.c_uint, c_int,
                                                          c_void_p],
+    "lwm_attn_fwd_e4m3_step": [c_void_p] * 12 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll,
+                                                              c_float, c_int, c_int, c_void_p, c_void_p, c_void_p],
     "lwm_attn_bwd_prep": [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
     "lwm_attn_bwd_lse": [c_void_p, c_void_p, c_ll, c_float, c_void_p],
     "lwm_attn_bwd_step": [c_void_p] * 13 + [c_int] * 5 + [c_ll, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll, c_float,
@@ -30,6 +32,8 @@ _SIGNATURES = {
     "lwm_attn_absmax_scale": [c_void_p, c_int, c_ll, c_void_p, c_void_p, c_void_p],
     "lwm_attn_scale_from_absmax": [c_void_p, c_int, c_int, c_void_p, c_void_p],
     "lwm_attn_to_f16_scaled": [c_void_p, c_int, c_void_p, c_void_p, c_ll, c_void_p],
+    "lwm_attn_e4m3_scale_from_absmax": [c_void_p, c_int, c_int, c_void_p, c_void_p],
+    "lwm_attn_to_e4m3_scaled": [c_void_p, c_int, c_void_p, c_void_p, c_ll, c_void_p],
     "lwm_reduce_cast_f32": [c_void_p, c_int, c_void_p, c_int, c_ll, c_void_p],
     "lwm_ring_ctx_create": [c_int, c_int, c_ll, c_int, c_void_p],
     "lwm_ring_ctx_get_handle": [c_void_p, c_void_p],

@@ -17,6 +17,7 @@
 //     two warpgroups take turns issuing (named barriers 1 and 2), so one's softmax also runs under the other's GEMMs.
 //   * causal masking by global token position; KV tiles entirely above the diagonal are never
 //     loaded; only diagonal tiles pay for the mask.
+#include <cstdio>
 #include "attn_common.cuh"
 #include "attn_dropout.cuh"
 #include "tmap.h"
@@ -69,6 +70,11 @@ LWM_DEVICE void load_tile(uint8_t* dst, const CUtensorMap* tm, uint64_t* bar, in
   tma_load_4d(dst, tm, bar, 0, h, row0, b);
   tma_load_4d(dst + kFwdTileBytes / 2, tm, bar, 64, h, row0, b);
 }
+// an e4m3 Q or K tile: 128 rows of 128 bytes, one box (the first half of a 32 KB slot)
+LWM_DEVICE void load_tile_e4m3(uint8_t* dst, const CUtensorMap* tm, uint64_t* bar, int h, int row0, int b) {
+  mbar_arrive_expect_tx(bar, kFwdTileBytes / 2);
+  tma_load_4d(dst, tm, bar, 0, h, row0, b);
+}
 
 LWM_DEVICE float quad_max(float x) {
   x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 1));
@@ -89,8 +95,11 @@ LWM_DEVICE float quad_sum(float x) {
 // branch with no bias or segment read (the causal compare stays). The epilogue is the training one.
 // kDrop (training instances): attention dropout. Every visited tile runs the per-element branch, which gives a dropped
 // entry the masked logit; a row left without a surviving key writes out = 0 and an lse at the masked level.
-// The kernel body; attn_fwd_kernel (no dropout) and attn_fwd_dropout_kernel are its entry points.
-template <bool kF16, bool kInfer, bool kMap, bool kDrop>
+// kQK8 (with kF16): the no-gradient fp8 mode. Q and K are power-of-two-scaled e4m3 copies, one 16 KB TMA box per tile
+// (a 128-byte row holds all 128 dimensions, so the 128B swizzle covers the whole row), and S = Q K^T runs as four
+// m64n128k32 e4m3 steps along that row. V, P and everything after the S GEMM are the fp16 instance's.
+// The kernel body; attn_fwd_kernel (no dropout), attn_fwd_dropout_kernel and attn_fwd_e4m3_kernel are its entry points.
+template <bool kF16, bool kInfer, bool kMap, bool kDrop, bool kQK8>
 __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
                                               const FwdParams& p) {
   extern __shared__ uint8_t smem_raw[];
@@ -145,13 +154,15 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmQ, const CUte
       tma_prefetch_desc(&tmQ);
       tma_prefetch_desc(&tmK);
       tma_prefetch_desc(&tmV);
-      load_tile(sQ, &tmQ, &bars.q_full, h, m0, b);
+      if constexpr (kQK8) load_tile_e4m3(sQ, &tmQ, &bars.q_full, h, m0, b);
+      else load_tile(sQ, &tmQ, &bars.q_full, h, m0, b);
       for (int i = 0; i < 2 * n_kv; ++i) {
         const int slot = i % kFwdStages;
         const uint32_t ph = (i / kFwdStages) & 1;
         mbar_wait(&bars.kv_empty[slot], ph ^ 1);
         const int kt = (kInfer || kMap) ? (list[i >> 1] >> 1) : (i >> 1);
-        load_tile(sKV + slot * kFwdTileBytes, (i & 1) ? &tmV : &tmK, &bars.kv_full[slot], h, kt * kTile, b);
+        if (kQK8 && !(i & 1)) load_tile_e4m3(sKV + slot * kFwdTileBytes, &tmK, &bars.kv_full[slot], h, kt * kTile, b);
+        else load_tile(sKV + slot * kFwdTileBytes, (i & 1) ? &tmV : &tmK, &bars.kv_full[slot], h, kt * kTile, b);
       }
     }
     return;
@@ -198,10 +209,16 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmQ, const CUte
     // S = Q K_j^T, one commit group
     auto issue_s = [&](int j) {
       const uint64_t kd = desc_kmajor_sw128(kv_base + ((2 * j) % kFwdStages) * kFwdTileBytes);
+      if constexpr (kQK8) {
 #pragma unroll
-      for (int ks = 0; ks < kHeadDim / 16; ++ks) {
-        const uint32_t off = (ks >> 2) * (kFwdTileBytes / 2) + (ks & 3) * 32;
-        wgmma_ss<128, kF16, 0, 0>(s, desc_advance(q_desc, off), desc_advance(kd, off), ks > 0);
+        for (int ks = 0; ks < kHeadDim / 32; ++ks)
+          wgmma_ss_n128_e4m3(s, desc_advance(q_desc, ks * 32), desc_advance(kd, ks * 32), ks > 0);
+      } else {
+#pragma unroll
+        for (int ks = 0; ks < kHeadDim / 16; ++ks) {
+          const uint32_t off = (ks >> 2) * (kFwdTileBytes / 2) + (ks & 3) * 32;
+          wgmma_ss<128, kF16, 0, 0>(s, desc_advance(q_desc, off), desc_advance(kd, off), ks > 0);
+        }
       }
       wgmma_commit();
     };
@@ -474,14 +491,22 @@ template <bool kF16, bool kInfer = false, bool kMap = false>
 __global__ void __launch_bounds__(kFwdThreads, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const __grid_constant__ FwdParams p) {
-  attn_fwd_body<kF16, kInfer, kMap, false>(tmQ, tmK, tmV, p);
+  attn_fwd_body<kF16, kInfer, kMap, false, false>(tmQ, tmK, tmV, p);
 }
 
 template <bool kF16, bool kMap>
 __global__ void __launch_bounds__(kFwdThreads, 1)
 attn_fwd_dropout_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                         const __grid_constant__ CUtensorMap tmV, const __grid_constant__ FwdParams p) {
-  attn_fwd_body<kF16, false, kMap, true>(tmQ, tmK, tmV, p);
+  attn_fwd_body<kF16, false, kMap, true, false>(tmQ, tmK, tmV, p);
+}
+
+// the fp8 mode (kQK8): e4m3 Q and K, fp16 V; training-step epilogue, no dropout
+template <bool kMap>
+__global__ void __launch_bounds__(kFwdThreads, 1)
+attn_fwd_e4m3_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                     const __grid_constant__ CUtensorMap tmV, const __grid_constant__ FwdParams p) {
+  attn_fwd_body<true, false, kMap, false, true>(tmQ, tmK, tmV, p);
 }
 
 static bool make_qkv_tmap(CUtensorMap* tm, const void* ptr, int B, int S, int H) {
@@ -492,17 +517,28 @@ static bool make_qkv_tmap(CUtensorMap* tm, const void* ptr, int B, int S, int H)
   return encode_tmap(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, ptr, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
+static bool make_e4m3_tmap(CUtensorMap* tm, const void* ptr, int B, int S, int H) {
+  // [B, S, H, 128] e4m3 -> dims (d, h, s, b) in bytes; one box = the whole 128-byte row x 128 rows of one head
+  uint64_t dims[4] = {uint64_t(kHeadDim), uint64_t(H), uint64_t(S), uint64_t(B)};
+  uint64_t strides[3] = {uint64_t(kHeadDim), uint64_t(H) * kHeadDim, uint64_t(S) * H * kHeadDim};
+  uint32_t box[4] = {uint32_t(kHeadDim), 1, uint32_t(kTile), 1};
+  return encode_tmap(tm, CU_TENSOR_MAP_DATA_TYPE_UINT8, 4, ptr, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
+}
+
 }  // namespace lwm
 
 using namespace lwm;
 
-// One attn_fwd_kernel or attn_fwd_dropout_kernel instance; its dynamic shared-memory limit is raised once per device.
-template <bool kF16, bool kInfer, bool kMap, bool kDrop>
+// One attn_fwd_kernel, attn_fwd_dropout_kernel or attn_fwd_e4m3_kernel (kQK8) instance; its dynamic shared-memory limit
+// is raised once per device.
+template <bool kF16, bool kInfer, bool kMap, bool kDrop, bool kQK8 = false>
 static int launch_fwd(dim3 grid, cudaStream_t st, const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
                       const FwdParams& p) {
   static_assert(!(kInfer && (kMap || kDrop)), "the inference mode has no block-map or dropout instance");
+  static_assert(!kQK8 || (kF16 && !kInfer && !kDrop), "the fp8 mode has fp16 V and no inference or dropout instance");
   void (*kernel)(CUtensorMap, CUtensorMap, CUtensorMap, FwdParams);
-  if constexpr (kDrop) kernel = attn_fwd_dropout_kernel<kF16, kMap>;
+  if constexpr (kQK8) kernel = attn_fwd_e4m3_kernel<kMap>;
+  else if constexpr (kDrop) kernel = attn_fwd_dropout_kernel<kF16, kMap>;
   else kernel = attn_fwd_kernel<kF16, kInfer, kMap>;
   static bool attr_set_dev[64] = {};
   int cur_dev = 0;
@@ -514,7 +550,59 @@ static int launch_fwd(dim3 grid, cudaStream_t st, const CUtensorMap& tq, const C
     attr_set = true;
   }
   kernel<<<grid, kFwdThreads, kFwdSmemBytes, st>>>(tq, tk, tv, p);
-  return lwm_check_launch(kDrop ? "attn_fwd_dropout_kernel" : kInfer ? "attn_fwd_kernel (inference)" : "attn_fwd_kernel");
+  return lwm_check_launch(kQK8 ? "attn_fwd_e4m3_kernel" : kDrop ? "attn_fwd_dropout_kernel"
+                          : kInfer ? "attn_fwd_kernel (inference)" : "attn_fwd_kernel");
+}
+
+// LWM_OK, or the status and message ("<fn>: <reason>") of the first bad argument of a ring step that every step entry
+// point shares; checked before any device access.
+static int fwd_step_check(const char* fn, const void* q, const void* k, const void* v, void* out, float* lse,
+                          float* acc_o, float* acc_m, float* acc_l, int B, int H, int Sq, int Sk, int D,
+                          long long q_pos0, long long k_pos0, const float* bias, long long bias_stride,
+                          const int* segment_ids, long long seg_stride, int first, int last, const int* tiles,
+                          const int* tile_count) {
+  auto fail = [&](int code, const char* reason) {
+    char msg[160];
+    snprintf(msg, sizeof(msg), "%s: %s", fn, reason);
+    return lwm_fail(code, msg);
+  };
+  if (!tiles != !tile_count) return fail(LWM_ERR_ARG, "tiles and tile_count are both given or both null");
+  if (tiles && !bias && !segment_ids) return fail(LWM_ERR_ARG, "a block map needs bias or segment_ids");
+  if (D != kHeadDim) return fail(LWM_ERR_SHAPE, "head_dim must be 128");
+  if (B <= 0 || H <= 0 || Sq <= 0 || Sk <= 0 || Sq % kTile || Sk % kTile)
+    return fail(LWM_ERR_SHAPE, "Sq and Sk must be positive multiples of 128");
+  if (!q || !k || !v) return fail(LWM_ERR_ARG, "null q/k/v");
+  if (last && (!out || !lse)) return fail(LWM_ERR_ARG, "out/lse required on the last step");
+  if (!(first && last) && (!acc_o || !acc_m || !acc_l)) return fail(LWM_ERR_ARG, "carry buffers required unless first && last");
+  if (q_pos0 + Sq > 0x7fffffffLL || k_pos0 + Sk > 0x7fffffffLL)
+    return fail(LWM_ERR_SHAPE, "global positions must fit in int32");
+  if (bias && bias_stride < k_pos0 + Sk)
+    return fail(LWM_ERR_SHAPE, "bias is indexed by GLOBAL key position: bias_stride < k_pos0 + Sk");
+  if (segment_ids && (seg_stride < q_pos0 + Sq || seg_stride < k_pos0 + Sk))
+    return fail(LWM_ERR_SHAPE, "segment_ids is indexed by GLOBAL position: seg_stride < max(q_pos0 + Sq, k_pos0 + Sk)");
+  return LWM_OK;
+}
+
+// The FwdParams of a training-form ring step (no dropout: p.drop stays zero)
+static FwdParams fwd_step_params(const float* scale_q, const float* scale_k, const float* scale_v, float* out_f32,
+                                 void* out, float* lse, float* acc_o, float* acc_m, float* acc_l, int B, int H, int Sq,
+                                 int Sk, long long q_pos0, long long k_pos0, int causal, const float* bias,
+                                 long long bias_stride, const int* segment_ids, long long seg_stride,
+                                 float softmax_scale, int first, int last, const int* tiles, const int* tile_count) {
+  FwdParams p{};
+  p.B = B; p.H = H; p.Sq = Sq; p.Sk = Sk;
+  p.scale_log2 = softmax_scale * kLog2e;
+  p.mask.q_pos0 = int(q_pos0); p.mask.k_pos0 = int(k_pos0); p.mask.causal = causal;
+  p.mask.bias = bias; p.mask.bias_stride = bias_stride;
+  p.mask.seg = segment_ids; p.mask.seg_stride = seg_stride;
+  p.out = reinterpret_cast<__nv_bfloat16*>(out);
+  p.lse = lse; p.acc_o = acc_o; p.acc_m = acc_m; p.acc_l = acc_l;
+  p.first = first; p.last = last;
+  p.scale_q = scale_q; p.scale_k = scale_k; p.scale_v = scale_v;
+  p.out_f32 = out_f32;
+  p.bits = nullptr; p.tiles = tiles; p.tile_count = tile_count;
+  p.n_kt = Sk / kTile; p.splits = 1;
+  return p;
 }
 
 // One ring step (include/lwm_b200.h): the scales select the fp16-operand kernel, tiles / tile_count the block map,
@@ -529,46 +617,50 @@ extern "C" int lwm_attn_fwd_step(const void* q, const void* k, const void* v, co
   if (!scale_k != !scale_q || !scale_v != !scale_q)
     return lwm_fail(LWM_ERR_ARG, "attn_fwd: scales are all given (fp16 operands) or all null (bf16)");
   if (out_f32 && !scale_q) return lwm_fail(LWM_ERR_ARG, "attn_fwd: out_f32 needs the fp16 operand scales");
-  if (!tiles != !tile_count) return lwm_fail(LWM_ERR_ARG, "attn_fwd: tiles and tile_count are both given or both null");
-  if (tiles && !bias && !segment_ids) return lwm_fail(LWM_ERR_ARG, "attn_fwd: a block map needs bias or segment_ids");
-  if (D != kHeadDim) return lwm_fail(LWM_ERR_SHAPE, "attn_fwd: head_dim must be 128");
-  if (B <= 0 || H <= 0 || Sq <= 0 || Sk <= 0 || Sq % kTile || Sk % kTile)
-    return lwm_fail(LWM_ERR_SHAPE, "attn_fwd: Sq and Sk must be positive multiples of 128");
-  if (!q || !k || !v) return lwm_fail(LWM_ERR_ARG, "attn_fwd: null q/k/v");
-  if (last && (!out || !lse)) return lwm_fail(LWM_ERR_ARG, "attn_fwd: out/lse required on the last step");
-  if (!(first && last) && (!acc_o || !acc_m || !acc_l))
-    return lwm_fail(LWM_ERR_ARG, "attn_fwd: carry buffers required unless first && last");
-  if (q_pos0 + Sq > 0x7fffffffLL || k_pos0 + Sk > 0x7fffffffLL)
-    return lwm_fail(LWM_ERR_SHAPE, "attn_fwd: global positions must fit in int32");
-  if (bias && bias_stride < k_pos0 + Sk)
-    return lwm_fail(LWM_ERR_SHAPE, "attn_fwd: bias is indexed by GLOBAL key position: bias_stride < k_pos0 + Sk");
-  if (segment_ids && (seg_stride < q_pos0 + Sq || seg_stride < k_pos0 + Sk))
-    return lwm_fail(LWM_ERR_SHAPE, "attn_fwd: segment_ids is indexed by GLOBAL position: seg_stride < max(q_pos0 + Sq, k_pos0 + Sk)");
+  if (const int s = fwd_step_check("attn_fwd", q, k, v, out, lse, acc_o, acc_m, acc_l, B, H, Sq, Sk, D, q_pos0, k_pos0,
+                                   bias, bias_stride, segment_ids, seg_stride, first, last, tiles, tile_count))
+    return s;
   DropParams drop;
   if (const int s = decode_drop_params(seed, drop_threshold, batch0, B, H, q_pos0, k_pos0, "attn_fwd", &drop)) return s;
   if (!lwm_check_device()) return LWM_ERR_DEVICE;
   CUtensorMap tq, tk, tv;
   if (!make_qkv_tmap(&tq, q, B, Sq, H) || !make_qkv_tmap(&tk, k, B, Sk, H) || !make_qkv_tmap(&tv, v, B, Sk, H))
     return lwm_fail(LWM_ERR_CUDA, "attn_fwd: cuTensorMapEncodeTiled failed (pointers must be 16B aligned)");
-  FwdParams p{};
-  p.B = B; p.H = H; p.Sq = Sq; p.Sk = Sk;
-  p.scale_log2 = softmax_scale * kLog2e;
-  p.mask.q_pos0 = int(q_pos0); p.mask.k_pos0 = int(k_pos0); p.mask.causal = causal;
-  p.mask.bias = bias; p.mask.bias_stride = bias_stride;
-  p.mask.seg = segment_ids; p.mask.seg_stride = seg_stride;
-  p.out = reinterpret_cast<__nv_bfloat16*>(out);
-  p.lse = lse; p.acc_o = acc_o; p.acc_m = acc_m; p.acc_l = acc_l;
-  p.first = first; p.last = last;
-  p.scale_q = scale_q; p.scale_k = scale_k; p.scale_v = scale_v;
-  p.out_f32 = out_f32;
-  p.bits = nullptr; p.tiles = tiles; p.tile_count = tile_count;
-  p.n_kt = Sk / kTile; p.splits = 1;
+  FwdParams p = fwd_step_params(scale_q, scale_k, scale_v, out_f32, out, lse, acc_o, acc_m, acc_l, B, H, Sq, Sk, q_pos0,
+                                k_pos0, causal, bias, bias_stride, segment_ids, seg_stride, softmax_scale, first, last,
+                                tiles, tile_count);
   p.drop = drop;
   const dim3 grid(Sq / kTile, H, B);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   return with_flags([&](auto f16, auto map, auto dropout) {
     return launch_fwd<f16, false, map, dropout>(grid, st, tq, tk, tv, p);
   }, scale_q != nullptr, tiles != nullptr, drop.thr != 0);
+}
+
+// One ring step of the fp8 mode (include/lwm_b200.h): q8 / k8 e4m3, v16 fp16, all three scales required.
+extern "C" int lwm_attn_fwd_e4m3_step(const void* q8, const void* k8, const void* v16, const float* scale_q,
+                                      const float* scale_k, const float* scale_v, float* out_f32, void* out, float* lse,
+                                      float* acc_o, float* acc_m, float* acc_l, int B, int H, int Sq, int Sk, int D,
+                                      long long q_pos0, long long k_pos0, int causal, const float* bias,
+                                      long long bias_stride, const int* segment_ids, long long seg_stride,
+                                      float softmax_scale, int first, int last, const int* tiles,
+                                      const int* tile_count, void* stream) {
+  if (!scale_q || !scale_k || !scale_v) return lwm_fail(LWM_ERR_ARG, "attn_fwd_e4m3: the three operand scales are required");
+  if (const int s = fwd_step_check("attn_fwd_e4m3", q8, k8, v16, out, lse, acc_o, acc_m, acc_l, B, H, Sq, Sk, D, q_pos0,
+                                   k_pos0, bias, bias_stride, segment_ids, seg_stride, first, last, tiles, tile_count))
+    return s;
+  if (!lwm_check_device()) return LWM_ERR_DEVICE;
+  CUtensorMap tq, tk, tv;
+  if (!make_e4m3_tmap(&tq, q8, B, Sq, H) || !make_e4m3_tmap(&tk, k8, B, Sk, H) || !make_qkv_tmap(&tv, v16, B, Sk, H))
+    return lwm_fail(LWM_ERR_CUDA, "attn_fwd_e4m3: cuTensorMapEncodeTiled failed (pointers must be 16B aligned)");
+  const FwdParams p = fwd_step_params(scale_q, scale_k, scale_v, out_f32, out, lse, acc_o, acc_m, acc_l, B, H, Sq, Sk,
+                                      q_pos0, k_pos0, causal, bias, bias_stride, segment_ids, seg_stride, softmax_scale,
+                                      first, last, tiles, tile_count);
+  const dim3 grid(Sq / kTile, H, B);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  return with_flags([&](auto map) {
+    return launch_fwd<true, false, map, false, true>(grid, st, tq, tk, tv, p);
+  }, tiles != nullptr);
 }
 
 // Inference mode (ringattention_inference with Q >= kInferMinQ rows): q16 [B,Q,H,128], k16/v16 [B,Sk,H,128] scaled fp16

@@ -5,7 +5,9 @@
 //   lwm_attn_*_rope       the operand passes with the rotary embedding of q / k applied on the fly
 #include "attn_common.cuh"
 #include <cuda_fp16.h>
+#include <cuda_fp8.h>
 #include <cstdio>
+#include <type_traits>
 #include "capi_internal.h"
 #include "rope_common.cuh"
 #include "../../include/lwm_b200.h"
@@ -144,13 +146,15 @@ __global__ void absmax_f32_kernel(const uint4* __restrict__ x, long long n4, uns
   if ((threadIdx.x & 31) == 0 && m) atomicMax(out_bits, m);
 }
 
-// scale = 2^(e-12), e = exponent of max_i bits[i*stride] (1.0 for all-zero): one thread. The ring executor feeds it
+// scale = 2^(e-kTop), e = exponent of max_i bits[i*stride] (1.0 for all-zero): one thread. The ring executor feeds it
 // the |max| bit patterns of every rank's shard, so that all ranks derive the SAME scale for a sharded tensor.
+// kTop = 12: the fp16 operand copies (the maximum lands in [2^12, 2^13)); 7: the e4m3 ones ([2^7, 2^8), below 448).
+template <int kTop>
 __global__ void scale_from_absmax_kernel(const unsigned* __restrict__ bits, int n, int stride, float* __restrict__ scale_out) {
   unsigned m = 0;
   for (int i = 0; i < n; ++i) m = max(m, bits[(long long)i * stride]);
-  const int e = max(int(m >> 23) - 127, -114);   // keeps 2^(e-12) a normal float
-  *scale_out = m ? __uint_as_float(unsigned(127 + (e - 12)) << 23) : 1.0f;
+  const int e = max(int(m >> 23) - 127, -114);   // keeps 2^(e-kTop) and 2^(kTop-e) normal floats
+  *scale_out = m ? __uint_as_float(unsigned(127 + (e - kTop)) << 23) : 1.0f;
 }
 
 // x16 = fp16(x / *scale) for a power-of-two scale held on the device; source bf16 (exact for every value above
@@ -176,6 +180,45 @@ __global__ void f32_to_f16_by_scale_kernel(const float4* __restrict__ x, uint2* 
        i += (long long)gridDim.x * blockDim.x) {
     const float4 v = x[i];
     y[i] = make_uint2(pack_f16x2(v.x * inv, v.y * inv), pack_f16x2(v.z * inv, v.w * inv));
+  }
+}
+
+// e4m3 (RN) of two fp32 values, x in the low byte. The callers' power-of-two scales keep every finite value below 256,
+// so nothing saturates; NaN and +-inf become the NaN byte (sign | 0x7f, what torch's cast to float8_e4m3fn gives; a
+// NaN's sign is whatever the scaling multiply left): e4m3fn has no infinity, and the hardware conversion alone
+// (satfinite) would turn +-inf into +-448.
+__device__ __forceinline__ uint32_t pack_e4m3x2(float lo, float hi) {
+  uint32_t r = __nv_cvt_float2_to_fp8x2(make_float2(lo, hi), __NV_SATFINITE, __NV_E4M3);
+  const uint32_t a = __float_as_uint(lo), b = __float_as_uint(hi);
+  if ((a & 0x7fffffffu) >= 0x7f800000u) r = (r & 0xff00u) | ((a >> 24) & 0x80u) | 0x7fu;
+  if ((b & 0x7fffffffu) >= 0x7f800000u) r = (r & 0x00ffu) | ((((b >> 24) & 0x80u) | 0x7fu) << 8);
+  return r;
+}
+__device__ __forceinline__ uint32_t pack_e4m3x4(float a, float b, float c, float d) {
+  return pack_e4m3x2(a, b) | (pack_e4m3x2(c, d) << 16);
+}
+
+// x8 = e4m3(x / *scale) for a power-of-two scale held on the device (lwm_attn_to_e4m3_scaled), 8 elements per item
+__global__ void bf16_to_e4m3_by_scale_kernel(const uint4* __restrict__ x, uint2* __restrict__ y, long long n8,
+                                             const float* __restrict__ scale) {
+  const float inv = 1.0f / *scale;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n8;
+       i += (long long)gridDim.x * blockDim.x) {
+    const uint4 v = x[i];
+    y[i] = make_uint2(pack_e4m3x4(__uint_as_float(v.x << 16) * inv, __uint_as_float(v.x & 0xffff0000u) * inv,
+                                  __uint_as_float(v.y << 16) * inv, __uint_as_float(v.y & 0xffff0000u) * inv),
+                      pack_e4m3x4(__uint_as_float(v.z << 16) * inv, __uint_as_float(v.z & 0xffff0000u) * inv,
+                                  __uint_as_float(v.w << 16) * inv, __uint_as_float(v.w & 0xffff0000u) * inv));
+  }
+}
+__global__ void f32_to_e4m3_by_scale_kernel(const float4* __restrict__ x, uint2* __restrict__ y, long long n8,
+                                            const float* __restrict__ scale) {
+  const float inv = 1.0f / *scale;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n8;
+       i += (long long)gridDim.x * blockDim.x) {
+    const float4 a = x[2 * i], b = x[2 * i + 1];
+    y[i] = make_uint2(pack_e4m3x4(a.x * inv, a.y * inv, a.z * inv, a.w * inv),
+                      pack_e4m3x4(b.x * inv, b.y * inv, b.z * inv, b.w * inv));
   }
 }
 
@@ -296,20 +339,26 @@ __global__ void __launch_bounds__(256) absmax_rope_kernel(const TIn* __restrict_
   if ((threadIdx.x & 31) == 0 && m) atomicMax(out_bits, m);
 }
 
-// *_to_f16_by_scale_kernel of rope(x) (kF16: fp16(value / *scale)), or the bf16 operand mode's copy (bf16(value))
-template <typename TIn, bool kF16>
-__global__ void __launch_bounds__(256) stage_rope_kernel(const TIn* __restrict__ x, uint4* __restrict__ dst,
+// *_to_f16_by_scale_kernel of rope(x) (kDst 2: fp16(value / *scale)), the bf16 operand mode's copy (kDst 1:
+// bf16(value)), or *_to_e4m3_by_scale_kernel of rope(x) (kDst 3: e4m3(value / *scale))
+template <typename TIn, int kDst>
+__global__ void __launch_bounds__(256) stage_rope_kernel(const TIn* __restrict__ x, void* __restrict__ dst,
                                                          const float* __restrict__ scale, const int* __restrict__ pos,
                                                          const float* __restrict__ inv_freq, long long n_tok, int H) {
   __shared__ float2 cs[kRopePos][kRopePairs];
-  const float inv = kF16 ? 1.0f / *scale : 1.0f;
+  const float inv = kDst != 1 ? 1.0f / *scale : 1.0f;
   for (long long tok0 = (long long)blockIdx.x * kRopePos; tok0 < n_tok; tok0 += (long long)gridDim.x * kRopePos) {
     rope_group_apply<TIn>(x, pos, inv_freq, tok0, n_tok, H, cs, [&](long long e, const float (&y)[8]) {
-      unsigned o[4];
+      if constexpr (kDst == 3) {
+        reinterpret_cast<uint2*>(dst)[e / 8] = make_uint2(pack_e4m3x4(y[0] * inv, y[1] * inv, y[2] * inv, y[3] * inv),
+                                                          pack_e4m3x4(y[4] * inv, y[5] * inv, y[6] * inv, y[7] * inv));
+      } else {
+        unsigned o[4];
 #pragma unroll
-      for (int k = 0; k < 4; ++k)
-        o[k] = kF16 ? pack_f16x2(y[2 * k] * inv, y[2 * k + 1] * inv) : pack_bf16x2(y[2 * k], y[2 * k + 1]);
-      dst[e / 8] = make_uint4(o[0], o[1], o[2], o[3]);
+        for (int k = 0; k < 4; ++k)
+          o[k] = kDst == 2 ? pack_f16x2(y[2 * k] * inv, y[2 * k + 1] * inv) : pack_bf16x2(y[2 * k], y[2 * k + 1]);
+        reinterpret_cast<uint4*>(dst)[e / 8] = make_uint4(o[0], o[1], o[2], o[3]);
+      }
     });
   }
 }
@@ -437,14 +486,14 @@ extern "C" int lwm_attn_absmax_scale(const void* x, int dtype, long long n, unsi
   if (cudaMemsetAsync(workspace, 0, 4, st) != cudaSuccess) return lwm_fail(LWM_ERR_CUDA, "attn_absmax_scale: memset failed");
   if (dtype == 1) absmax_bf16_kernel<<<grid_for(n / 8, 256, 8), 256, 0, st>>>(reinterpret_cast<const uint4*>(x), n / 8, workspace);
   else absmax_f32_kernel<<<grid_for(n / 4, 256, 8), 256, 0, st>>>(reinterpret_cast<const uint4*>(x), n / 4, workspace);
-  scale_from_absmax_kernel<<<1, 1, 0, st>>>(workspace, 1, 1, scale_out);
+  scale_from_absmax_kernel<12><<<1, 1, 0, st>>>(workspace, 1, 1, scale_out);
   return lwm_check_launch("absmax_scale kernels");
 }
 
 extern "C" int lwm_attn_scale_from_absmax(const unsigned* bits, int n, int stride, float* scale_out, void* stream) {
   if (!bits || !scale_out || n <= 0 || stride <= 0) return lwm_fail(LWM_ERR_ARG, "attn_scale_from_absmax: bad arguments");
   if (!lwm_check_device()) return LWM_ERR_DEVICE;
-  scale_from_absmax_kernel<<<1, 1, 0, reinterpret_cast<cudaStream_t>(stream)>>>(bits, n, stride, scale_out);
+  scale_from_absmax_kernel<12><<<1, 1, 0, reinterpret_cast<cudaStream_t>(stream)>>>(bits, n, stride, scale_out);
   return lwm_check_launch("scale_from_absmax_kernel");
 }
 
@@ -457,6 +506,27 @@ extern "C" int lwm_attn_to_f16_scaled(const void* x, int dtype, void* dst_f16, c
   else
     f32_to_f16_by_scale_kernel<<<grid_for(n / 4, 256, 8), 256, 0, st>>>(reinterpret_cast<const float4*>(x), reinterpret_cast<uint2*>(dst_f16), n / 4, scale);
   return lwm_check_launch("to_f16_by_scale kernel");
+}
+
+extern "C" int lwm_attn_e4m3_scale_from_absmax(const unsigned* bits, int n, int stride, float* scale_out, void* stream) {
+  if (!bits || !scale_out || n <= 0 || stride <= 0) return lwm_fail(LWM_ERR_ARG, "attn_e4m3_scale_from_absmax: bad arguments");
+  if (!lwm_check_device()) return LWM_ERR_DEVICE;
+  scale_from_absmax_kernel<7><<<1, 1, 0, reinterpret_cast<cudaStream_t>(stream)>>>(bits, n, stride, scale_out);
+  return lwm_check_launch("scale_from_absmax_kernel");
+}
+
+extern "C" int lwm_attn_to_e4m3_scaled(const void* x, int dtype, void* dst_e4m3, const float* scale, long long n,
+                                       void* stream) {
+  if (!x || !dst_e4m3 || !scale || n <= 0 || n % 8 || (dtype != 0 && dtype != 1))
+    return lwm_fail(LWM_ERR_ARG, "attn_to_e4m3_scaled: bad arguments (n % 8 == 0)");
+  if (!lwm_check_device()) return LWM_ERR_DEVICE;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  uint2* y = reinterpret_cast<uint2*>(dst_e4m3);
+  if (dtype == 1)
+    bf16_to_e4m3_by_scale_kernel<<<grid_for(n / 8, 256, 8), 256, 0, st>>>(reinterpret_cast<const uint4*>(x), y, n / 8, scale);
+  else
+    f32_to_e4m3_by_scale_kernel<<<grid_for(n / 8, 256, 8), 256, 0, st>>>(reinterpret_cast<const float4*>(x), y, n / 8, scale);
+  return lwm_check_launch("to_e4m3_by_scale kernel");
 }
 
 // delta = rowsum(out o dout); out fp32 (out_dtype 0) or bf16 (1); dout bf16, or its scaled fp16 copy when scale_do is
@@ -541,23 +611,24 @@ extern "C" int lwm_attn_stage_rope(const void* x, int dtype, void* dst, int dst_
                                    const int* position_ids, const float* inv_freq, int B, int S, int H, void* stream) {
   if (int e = rope_input_args("attn_stage_rope", x, dtype, position_ids, inv_freq, B, S, H)) return e;
   if (!dst) return lwm_fail(LWM_ERR_ARG, "attn_stage_rope: null pointer");
-  if (dst_dtype != 1 && dst_dtype != 2)
-    return lwm_fail(LWM_ERR_ARG, "attn_stage_rope: dst dtype codes are 1 (bf16) or 2 (scaled fp16)");
-  if (dst_dtype == 2 && !scale) return lwm_fail(LWM_ERR_ARG, "attn_stage_rope: scaled fp16 needs a scale");
+  if (dst_dtype != 1 && dst_dtype != 2 && dst_dtype != 3)
+    return lwm_fail(LWM_ERR_ARG, "attn_stage_rope: dst dtype codes are 1 (bf16), 2 (scaled fp16) or 3 (scaled e4m3)");
+  if (dst_dtype != 1 && !scale) return lwm_fail(LWM_ERR_ARG, "attn_stage_rope: scaled fp16 / e4m3 needs a scale");
   if (!lwm_check_device()) return LWM_ERR_DEVICE;
   const long long n_tok = (long long)B * S;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  uint4* y = reinterpret_cast<uint4*>(dst);
   const unsigned g = rope_grid(n_tok);
-  if (dtype == 1) {
-    const __nv_bfloat16* xb = reinterpret_cast<const __nv_bfloat16*>(x);
-    if (dst_dtype == 2) stage_rope_kernel<__nv_bfloat16, true><<<g, 256, 0, st>>>(xb, y, scale, position_ids, inv_freq, n_tok, H);
-    else stage_rope_kernel<__nv_bfloat16, false><<<g, 256, 0, st>>>(xb, y, scale, position_ids, inv_freq, n_tok, H);
-  } else {
-    const float* xf = reinterpret_cast<const float*>(x);
-    if (dst_dtype == 2) stage_rope_kernel<float, true><<<g, 256, 0, st>>>(xf, y, scale, position_ids, inv_freq, n_tok, H);
-    else stage_rope_kernel<float, false><<<g, 256, 0, st>>>(xf, y, scale, position_ids, inv_freq, n_tok, H);
-  }
+  auto launch = [&](auto src, auto mode) {
+    using TIn = std::remove_const_t<std::remove_pointer_t<decltype(src)>>;
+    stage_rope_kernel<TIn, decltype(mode)::value><<<g, 256, 0, st>>>(src, dst, scale, position_ids, inv_freq, n_tok, H);
+  };
+  auto by_dst = [&](auto src) {
+    if (dst_dtype == 3) launch(src, std::integral_constant<int, 3>{});
+    else if (dst_dtype == 2) launch(src, std::integral_constant<int, 2>{});
+    else launch(src, std::integral_constant<int, 1>{});
+  };
+  if (dtype == 1) by_dst(reinterpret_cast<const __nv_bfloat16*>(x));
+  else by_dst(reinterpret_cast<const float*>(x));
   return lwm_check_launch("stage_rope_kernel");
 }
 

@@ -70,9 +70,11 @@ class Layout:
     def base(self, which):
         return which * self.set_bytes
 
-    def kv_row_off(self, region, which, b, pos):
-        """byte offset of global key row `pos` of batch b in the K (region='kg') or V array"""
-        return self.base(which) + getattr(self, region) + (b * self.world * self.Sk + pos) * self.row * self.isz
+    def kv_row_off(self, region, which, b, pos, itemsize=None):
+        """byte offset of global key row `pos` of batch b in the K (region='kg') or V array; itemsize: of the array's
+        elements when they are narrower than the operand itemsize the region is sized for (the fp8 mode's e4m3 K)"""
+        isz = self.isz if itemsize is None else itemsize
+        return self.base(which) + getattr(self, region) + (b * self.world * self.Sk + pos) * self.row * isz
 
     def q_row_off(self, region, which, b, row, itemsize):
         return self.base(which) + getattr(self, region) + (b * self.Sq + row) * self.row * itemsize
@@ -286,6 +288,11 @@ def _span(tr, label, stream):
 # ------------------------------------------------------------------------------------------------
 # executor
 # ------------------------------------------------------------------------------------------------
+def v_ops(ops):
+    """the ops that stage V: ops itself, except in the fp8 mode, whose V is the fp16 mode's copy (ops.v_ops)"""
+    return getattr(ops, "v_ops", ops)
+
+
 def _layout_for(plan, q_shape, Sk, ops):
     B, Sq, H, D = q_shape
     return Layout(B, Sq, Sk, H, D, plan.world, plan.chunks_per_rank, ops.op_itemsize)
@@ -302,31 +309,32 @@ def _stage_and_announce(tr, lay, which, pid, ops, k, v, x, cols, known=None, rop
     needed (rope_k=False: x's positions [B,Sq])."""
     P, r = tr.world, tr.rank
     B, Sk = k.shape[0], k.shape[1]
+    vops = v_ops(ops)
     table = tr.heap_view(lay.base(which) + lay.abs, (P, 4), torch.float32)
     KG = tr.heap_view(lay.base(which) + lay.kg, (B, P * Sk) + tuple(k.shape[2:]), ops.op_dtype)
-    VG = tr.heap_view(lay.base(which) + lay.vg, (B, P * Sk) + tuple(k.shape[2:]), ops.op_dtype)
+    VG = tr.heap_view(lay.base(which) + lay.vg, (B, P * Sk) + tuple(k.shape[2:]), vops.op_dtype)
     QS = tr.heap_view(lay.base(which) + lay.qs, tuple(x.shape), ops.op_dtype)
     rot = (rope is not None and rope_k, False, rope is not None and rope_x)
     sc = []
-    for t, c, rt in zip((k, v, x), cols, rot):
+    for t, c, rt, o in zip((k, v, x), cols, rot, (ops, vops, ops)):
         dst = table[r, c:c + 1]
-        if not ops.scaled:
+        if not o.scaled:
             sc.append(None)
         elif known is not None and c in known:
             dst.copy_(known[c])
             sc.append(dst)
         elif rt:
-            ops.scale_of_rope(t, dst, *rope)
+            o.scale_of_rope(t, dst, *rope)
             sc.append(dst)
         else:
-            ops.scale_of(t, dst)
+            o.scale_of(t, dst)
             sc.append(dst)
     for b in range(B):
         if rot[0]:
             ops.stage_rope(k[b], KG[b, r * Sk:(r + 1) * Sk], sc[0], rope[0][b], rope[1])
         else:
             ops.stage(k[b], KG[b, r * Sk:(r + 1) * Sk], sc[0])
-        ops.stage(v[b], VG[b, r * Sk:(r + 1) * Sk], sc[1])
+        vops.stage(v[b], VG[b, r * Sk:(r + 1) * Sk], sc[1])
     if rot[2]:
         ops.stage_rope(x, QS, sc[2], *rope)
     else:
@@ -375,7 +383,7 @@ def _gather_q_chunks(tr, lay, which, plan, QS, gate, ops):
             buf = torch.empty((B, qc.length) + tuple(QS.shape[2:]), dtype=QS.dtype, device=QS.device)
             gate(qc.owner, "pull")
             for b in range(B):
-                _pull_striped(tr, buf[b], qc.owner, lay.q_row_off("qs", which, b, qc.start, lay.isz))
+                _pull_striped(tr, buf[b], qc.owner, lay.q_row_off("qs", which, b, qc.start, QS.element_size()))
             chunks.append(buf)
     return chunks
 
@@ -390,7 +398,8 @@ def _pull_group(tr, lay, which, group, KG, VG, gate):
         gate(c.owner, "pull")
         for b in range(B):
             for region, arr in (("kg", KG), ("vg", VG)):
-                _pull_striped(tr, arr[b, c.pos0:c.pos0 + c.length], c.owner, lay.kv_row_off(region, which, b, c.pos0))
+                _pull_striped(tr, arr[b, c.pos0:c.pos0 + c.length], c.owner,
+                              lay.kv_row_off(region, which, b, c.pos0, arr.element_size()))
     return tr.record("pull")
 
 

@@ -234,6 +234,21 @@ def _quantized_kv(op, q, k, v, rotates_k):
     return True
 
 
+def _check_fp8(q, k, v, blockwise_kwargs, axis_name):
+    """precision='fp8' runs only where it is defined: a forward without gradient, without dropout, on one GPU or the
+    peer-memory ring"""
+    if torch.is_grad_enabled() and any(t.requires_grad for t in (q, k, v)):
+        raise ValueError("ringattention: precision='fp8' is a forward without gradient (a prefill): run it under "
+                         "torch.no_grad() or with inputs that do not require grad")
+    group, _, world = _resolve_group(axis_name)
+    kw = dict(blockwise_kwargs or {})
+    if not kw.get("deterministic", True) and dropout_threshold(kw.get("attn_pdrop", 0.0)) > 0:
+        raise ValueError("ringattention: precision='fp8' has no attention dropout")
+    if world > 1 and _transport(group) != "peer":
+        raise NotImplementedError("ringattention: precision='fp8' runs on one GPU and on the peer-memory ring, not on "
+                                  "the two-sided NCCL executor")
+
+
 def _peer_ready(q, k, causal, group, rank, world, layout, precision):
     """world > 1: whether this call runs on the peer-memory executor (sets up its heap, as ring_forward would)"""
     if _transport(group) != "peer":
@@ -258,7 +273,10 @@ def ringattention(q, k, v, attn_bias=None, segment_ids=None, *, axis_name="sp", 
     float32_logits: logits/softmax/carries are always fp32 here (the reference default, True).
     layout: 'contiguous' = the reference's schedule; 'zigzag' = internally rebalance the causal
     work across ranks (same inputs/outputs); 'auto' picks zigzag when it applies.
-    precision: None -> module default (set_default_precision / $LWM_ATTN_PRECISION): 'fp16' | 'bf16'.
+    precision: None -> module default (set_default_precision / $LWM_ATTN_PRECISION): 'fp16' | 'bf16'. As this keyword
+    only, 'fp8': the no-gradient forward of a prefill (grad disabled, or no input requiring it; no dropout; one GPU or
+    the peer-memory ring): q and k are staged as power-of-two-scaled e4m3 copies and S = QK^T runs on the FP8 tensor
+    cores, while v, P, the softmax and the output are the fp16 mode's. Lossy: the error model is DESIGN.md §5.
 
     freqs_cis, position_ids: both None (the reference call), or q and k are the UN-rotated head-split projections and
     the op applies the rotary embedding of lwm/llama.py:517-519 itself: freqs_cis is the RotaryTable of
@@ -283,15 +301,21 @@ def ringattention(q, k, v, attn_bias=None, segment_ids=None, *, axis_name="sp", 
     batch row, head, GLOBAL query and key position) only (lwm_b200/csrc/attn_dropout.cuh), regenerated inside the tile
     kernels, so it is the same for any layout, world size or executor. dropout_rng: an int seed (pass the same one on
     every rank of the axis group), or None on one GPU for a seed drawn from torch's default CPU generator."""
-    precision = precision or _DEFAULT_PRECISION
-    if precision not in ("bf16", "fp16"):
-        raise ValueError("precision must be 'bf16' or 'fp16'")
+    if precision:
+        if precision not in ("bf16", "fp16", "fp8"):
+            raise ValueError("precision must be 'bf16', 'fp16' or 'fp8'")
+    else:
+        precision = _DEFAULT_PRECISION
+        if precision not in ("bf16", "fp16"):
+            raise ValueError("precision must be 'bf16' or 'fp16'")
     if cache_idx is not None:
         raise NotImplementedError("cache_idx is always None at the reference call site (lwm/llama.py:544)")
     if _quantized_kv("ringattention", q, k, v, bool(rotate_k) and freqs_cis is not None):
         k, v = k.dequantize(q.dtype), v.dequantize(q.dtype)
     rope = _check_rope(freqs_cis, position_ids, q, k, rotate_k)
     rotate_k = bool(rotate_k)
+    if precision == "fp8":
+        _check_fp8(q, k, v, blockwise_kwargs, axis_name)
     if not q.is_cuda:
         raise _lib.LwmError("ringattention: tensors must live on an sm_90 GPU (no CPU fallback)")
     in_dtype = q.dtype
@@ -299,7 +323,8 @@ def ringattention(q, k, v, attn_bias=None, segment_ids=None, *, axis_name="sp", 
         raise TypeError("ringattention: q, k, v must all be bfloat16 or all float32 (fp32 logits and accumulation "
                         "are internal)")
     group, rank, world = _resolve_group(axis_name)
-    native_f32 = in_dtype == torch.float32 and precision == "fp16" and (world == 1 or _transport(group) == "peer")
+    native_f32 = (in_dtype == torch.float32 and precision in ("fp16", "fp8")
+                  and (world == 1 or _transport(group) == "peer"))
     B, Sq, H, D = q.shape
     causal, dropout = _check_blockwise_kwargs(blockwise_kwargs, Sq, k.shape[1], world)
     if rope is not None:
@@ -370,6 +395,20 @@ def fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bia
               0 if bias is None else bias.shape[1], _lib.ptr(seg), 0 if seg is None else seg.shape[1],
               1.0 / math.sqrt(D), int(first), int(last), _lib.ptr(tiles), _lib.ptr(counts), *_drop_args(dropout),
               _lib.stream_ptr(stream))
+
+
+def fwd_e4m3_step(q8, k8, v16, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last, scales,
+                  stream=None, out_f32=None, tilemap=None):
+    """fwd_step of the fp8 mode (include/lwm_b200.h: lwm_attn_fwd_e4m3_step): q8 / k8 the e4m3 copies of q and k, v16
+    the fp16 copy of v, scales = (sq, sk, sv) their device scales"""
+    B, Sq, H, D = q8.shape
+    sq, sk, sv = scales
+    tiles, counts = tilemap if tilemap is not None else (None, None)
+    _lib.call("lwm_attn_fwd_e4m3_step", _lib.ptr(q8), _lib.ptr(k8), _lib.ptr(v16), _lib.ptr(sq), _lib.ptr(sk),
+              _lib.ptr(sv), _lib.ptr(out_f32), _lib.ptr(out), _lib.ptr(lse), _lib.ptr(acc_o), _lib.ptr(acc_m),
+              _lib.ptr(acc_l), B, H, Sq, k8.shape[1], D, int(q_pos0), int(k_pos0), int(bool(causal)), _lib.ptr(bias),
+              0 if bias is None else bias.shape[1], _lib.ptr(seg), 0 if seg is None else seg.shape[1],
+              1.0 / math.sqrt(D), int(first), int(last), _lib.ptr(tiles), _lib.ptr(counts), _lib.stream_ptr(stream))
 
 
 def bwd_prep(out, dout, delta, stream=None, scale_do=None):
@@ -670,6 +709,52 @@ class PeerOpsBf16(PeerOpsF16):
                         **kw)
 
 
+class PeerOpsE4m3(PeerOpsF16):
+    """fp8 mode (forward only): q and k are power-of-two-scaled e4m3 copies (scale 2^(e-7)), one scale per sharded
+    tensor as in the fp16 mode; v is the fp16 mode's copy (v_ops). The copies fill half of the regions the peer heap
+    sizes for 2-byte operands (op_itemsize), and K and Q travel at one byte per element."""
+    op_dtype = torch.float8_e4m3fn
+    v_ops = PeerOpsF16
+    _STAGE_DST = 3          # lwm_attn_stage_rope: scaled e4m3
+
+    @staticmethod
+    def make_scale(table, col):
+        s = torch.empty(1, dtype=torch.float32, device=table.device)
+        _lib.call("lwm_attn_e4m3_scale_from_absmax", _lib.ptr(table.view(-1)[col:]), table.shape[0], table.shape[1],
+                  _lib.ptr(s), _lib.stream_ptr())
+        return s
+
+    @staticmethod
+    def scale_of(x, out):
+        """out[0] = 2^(e-7), e the exponent of |x|max (the power-of-two scale of the e4m3 operand copy of x)"""
+        bits = torch.zeros(1, dtype=torch.int32, device=x.device)
+        PeerOpsF16.absmax(x, bits)
+        _lib.call("lwm_attn_e4m3_scale_from_absmax", _lib.ptr(bits), 1, 1, _lib.ptr(out), _lib.stream_ptr())
+
+    @classmethod
+    def scale_of_rope(cls, x, out, pos, inv_freq):
+        bits = torch.zeros(1, dtype=torch.int32, device=x.device)
+        cls.absmax_rope(x, bits, pos, inv_freq)
+        _lib.call("lwm_attn_e4m3_scale_from_absmax", _lib.ptr(bits), 1, 1, _lib.ptr(out), _lib.stream_ptr())
+
+    @staticmethod
+    def stage(x, dst, scale):
+        _lib.call("lwm_attn_to_e4m3_scaled", _lib.ptr(x), _dt(x), _lib.ptr(dst), _lib.ptr(scale), x.numel(),
+                  _lib.stream_ptr())
+
+    @staticmethod
+    def fwd_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last, scales, out_f32,
+                 **kw):
+        fwd_e4m3_step(q, k, v, out, lse, acc_o, acc_m, acc_l, q_pos0, k_pos0, causal, bias, seg, first, last, scales,
+                      out_f32=out_f32, **kw, **_map_kw(q, k, q_pos0, k_pos0, causal, bias, seg, True))
+
+    @staticmethod
+    def _no_backward(*args, **kw):
+        raise NotImplementedError("precision='fp8' is forward-only: it has no backward")
+
+    bwd_prep = lse_for_bwd = bwd_step = reduce_cast = reduce_cast_rope = rope_conj = _no_backward
+
+
 _PEER_BROKEN = {}      # process group id -> reason: the peer-memory heaps could not be set up for this group
 
 
@@ -701,11 +786,14 @@ def _peer_transport(group, device, nbytes_hint=0):
 
 
 def _ops_for(precision):
+    if precision == "fp8":
+        raise NotImplementedError("precision='fp8' runs on one GPU and on the peer-memory ring, not on the two-sided "
+                                  "NCCL executor")
     return CudaOpsF16() if precision == "fp16" else CudaOps
 
 
 def _peer_ops(precision):
-    return PeerOpsF16 if precision == "fp16" else PeerOpsBf16
+    return {"fp16": PeerOpsF16, "fp8": PeerOpsE4m3}.get(precision, PeerOpsBf16)
 
 
 def _local_scales(ops, tensors, rope=None, n_rot=2):
@@ -747,9 +835,11 @@ def ring_forward(q, k, v, bias, seg, causal, group, rank, world, layout="auto", 
     want_f32 = q.dtype == torch.float32
     if world == 1:
         ops = with_dropout(_peer_ops(precision), dropout)
-        sq, sk, sv = _local_scales(ops, (q, k, v), rope, 2 if rope_k else 1)
+        vops = rp.v_ops(ops)
+        sq, sk = _local_scales(ops, (q, k), rope, 2 if rope_k else 1)
+        sv, = _local_scales(vops, (v,))
         q16, k16, v16 = (_stage_local(ops, q, sq, rope), _stage_local(ops, k, sk, rope if rope_k else None),
-                         _stage_local(ops, v, sv))
+                         _stage_local(vops, v, sv))
         out = torch.empty((B, Sq, H, D), dtype=torch.bfloat16, device=q.device)
         out32 = torch.empty((B, Sq, H, D), dtype=torch.float32, device=q.device) if (ops.scaled or want_f32) else None
         lse = torch.empty((B, H, Sq), dtype=torch.float32, device=q.device)
@@ -764,6 +854,8 @@ def ring_forward(q, k, v, bias, seg, causal, group, rank, world, layout="auto", 
         if tr is not None:
             return rp.run_forward(plan, q, k, v, bias, seg, causal, with_dropout(pops, dropout), tr, want_f32, rope,
                                   rope_k)
+        if precision == "fp8":
+            _ops_for(precision)     # raises: no fp8 on the NCCL executor
         if want_f32:        # the NCCL executor takes bf16 operands (documented in ringattention())
             out, res = ring_forward(q.to(torch.bfloat16), k.to(torch.bfloat16), v.to(torch.bfloat16), bias, seg, causal,
                                     group, rank, world, layout, precision, rope, dropout=dropout)

@@ -296,6 +296,19 @@ int lwm_kv_cache_write_q8(const void* k_src, const void* v_src, int src_dtype, s
                           int B, int n_src, long long src0, int n, int L, long long dst0, int H, int D, void* stream);
 int lwm_kv_dequant_q8(const signed char* data, const signed char* exp, void* out, int out_dtype, int B, int L, int H,
                       int D, void* stream);
+/* The operand passes of the tensor-core attention paths (lwm_attn_absmax, lwm_attn_to_f16_scaled,
+ * lwm_attn_to_e4m3_scaled) read straight from the cache rows, with no dequantized copy in memory. Both give the bits the
+ * plain pass gives on lwm_kv_dequant_q8's output (fp32 or bf16: the values are exact in both). B = 1 with data / exp at
+ * batch row b (data + b*L*H*128, exp + b*H*L*4) passes one row of the batch.
+ * lwm_kv_q8_absmax          atomicMax of the largest finite |code * 2^e| bit pattern into *out_bits (caller zeroes it;
+ *                           the NaN code is skipped). Composes with lwm_attn_scale_from_absmax and
+ *                           lwm_attn_e4m3_scale_from_absmax like lwm_attn_absmax.
+ * lwm_kv_q8_stage           dst [B,L,H,128] = fp16(value / *scale) (dst_dtype 2, dst 8-byte aligned) or e4m3(value /
+ *                           *scale) (dst_dtype 3, 4-byte aligned), the codes of lwm_attn_stage_rope. */
+int lwm_kv_q8_absmax(const signed char* data, const signed char* exp, int B, int L, int H, int D, unsigned* out_bits,
+                     void* stream);
+int lwm_kv_q8_stage(const signed char* data, const signed char* exp, void* dst, int dst_dtype, const float* scale,
+                    int B, int L, int H, int D, void* stream);
 
 /* The decode step without host values that change from token to token, so that it can be captured once in a CUDA graph
  * and replayed (`ShardedKVCache` with torch.cuda.graph; INTEGRATION.md "Decode in a CUDA graph").

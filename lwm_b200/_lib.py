@@ -52,6 +52,8 @@ _SIGNATURES = {
     "lwm_kv_cache_write_q8": [c_void_p, c_void_p, c_int] + [c_void_p] * 6 + [c_int, c_int, c_ll, c_int, c_int, c_ll,
                                                                               c_int, c_int, c_void_p],
     "lwm_kv_dequant_q8": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
+    "lwm_kv_q8_absmax": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p],
+    "lwm_kv_q8_stage": [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
     "lwm_kv_cache_write_at": [c_void_p, c_void_p, c_int] + [c_void_p] * 6 + [c_int, c_void_p, c_ll] + [c_int] * 5
                              + [c_void_p, c_void_p],
     "lwm_rope_check_positions": [c_void_p, c_ll, c_int, c_void_p, c_void_p],

@@ -9,6 +9,7 @@
 #include <cstdio>
 #include <type_traits>
 #include "capi_internal.h"
+#include "e4m3.cuh"
 #include "rope_common.cuh"
 #include "../../include/lwm_b200.h"
 
@@ -181,21 +182,6 @@ __global__ void f32_to_f16_by_scale_kernel(const float4* __restrict__ x, uint2* 
     const float4 v = x[i];
     y[i] = make_uint2(pack_f16x2(v.x * inv, v.y * inv), pack_f16x2(v.z * inv, v.w * inv));
   }
-}
-
-// e4m3 (RN) of two fp32 values, x in the low byte. The callers' power-of-two scales keep every finite value below 256,
-// so nothing saturates; NaN and +-inf become the NaN byte (sign | 0x7f, what torch's cast to float8_e4m3fn gives; a
-// NaN's sign is whatever the scaling multiply left): e4m3fn has no infinity, and the hardware conversion alone
-// (satfinite) would turn +-inf into +-448.
-__device__ __forceinline__ uint32_t pack_e4m3x2(float lo, float hi) {
-  uint32_t r = __nv_cvt_float2_to_fp8x2(make_float2(lo, hi), __NV_SATFINITE, __NV_E4M3);
-  const uint32_t a = __float_as_uint(lo), b = __float_as_uint(hi);
-  if ((a & 0x7fffffffu) >= 0x7f800000u) r = (r & 0xff00u) | ((a >> 24) & 0x80u) | 0x7fu;
-  if ((b & 0x7fffffffu) >= 0x7f800000u) r = (r & 0x00ffu) | ((((b >> 24) & 0x80u) | 0x7fu) << 8);
-  return r;
-}
-__device__ __forceinline__ uint32_t pack_e4m3x4(float a, float b, float c, float d) {
-  return pack_e4m3x2(a, b) | (pack_e4m3x2(c, d) << 16);
 }
 
 // x8 = e4m3(x / *scale) for a power-of-two scale held on the device (lwm_attn_to_e4m3_scaled), 8 elements per item

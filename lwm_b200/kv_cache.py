@@ -47,7 +47,8 @@ class QuantizedKV:
     """One tensor (keys or values) of the 8-bit KV cache, [B,L,H,128] rows: data int8 [B,L,H,128] holds the codes and
     exp int8 [B,H,L,4] one power-of-two exponent per 32-element group, head-major (lwm_b200/csrc/kv_q8.cuh). A value is
     code * 2^e, exact in fp32 and bf16; code -128 is NaN. It stands where a cache shard goes: ringattention_inference
-    and ringattention(..., rotate_k=False) accept it for k and v (generation only, no gradient)."""
+    and ringattention(..., rotate_k=False) accept it for k and v (generation only, no gradient) and stage their operand
+    copies straight from the codes."""
     dtype = torch.int8
     requires_grad = False
 
@@ -87,6 +88,12 @@ class QuantizedKV:
 
     def contiguous(self):
         return self
+
+    def __getitem__(self, b):
+        """batch row b as a cache of one row, [1,L,H,128] (views of data[b] and exp[b]): the peer-memory executor
+        stages a shard one batch row at a time"""
+        b = range(self.shape[0])[b]
+        return QuantizedKV(self.data[b:b + 1], self.exp[b:b + 1])
 
     def dequantize(self, dtype):
         """-> the rows' values [B,L,H,128] in bf16 or fp32 (exact; lwm_kv_dequant_q8)"""

@@ -304,6 +304,8 @@ def _stage_and_announce(tr, lay, which, pid, ops, k, v, x, cols, known=None, rop
     cols = (column of k, of v, of x) in the table row [sq, sk, sv, sdo]; known = {column: scale tensor} to reuse (the
     backward re-stages K/V with the forward's scales). Every operand has its OWNER's scale: no cross-rank agreement and
     therefore no exchange is needed — a launch only ever combines one Q-side owner with one K/V owner.
+    k, v may be the 8-bit cache (kv_cache.QuantizedKV, the forward only): ops stage it from its codes, batch row by batch
+    row, into the same heap regions and with the same bytes as its dequantized values would give.
     rope: None, or (positions int32 [B,Sk], inv_freq): k (unless not rope_k) and x (when rope_x) are un-rotated, and their
     scales and staged copies are those of the rotated rows. Every rank stages its own rows, so only local positions are
     needed (rope_k=False: x's positions [B,Sq])."""

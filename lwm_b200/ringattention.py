@@ -292,8 +292,10 @@ def ringattention(q, k, v, attn_bias=None, segment_ids=None, *, axis_name="sp", 
     dK is the gradient w.r.t. k as passed, and only dQ gets the conjugate rotation.
 
     k, v may be the 8-bit cache (kv_cache.QuantizedKV, both or neither) in the cached prefill: q bf16 or fp32 without
-    gradient, and rotate_k=False when the rotary keywords are given. The shards are dequantized to q's dtype (exact; one
-    transient copy of each) and the op runs on them as above.
+    gradient, and rotate_k=False when the rotary keywords are given. Bit for bit the call on k.dequantize(q.dtype),
+    v.dequantize(q.dtype), without those copies: in the fp16 and fp8 modes (one GPU and the peer-memory ring) the passes
+    that stage the scaled operand copies read the cache's codes, and the bf16 mode and the two-sided NCCL executor,
+    which take bf16 operands, dequantize the cache straight into bf16 (exact).
 
     Attention dropout: blockwise_kwargs=dict(deterministic=False, attn_pdrop=p, dropout_rng=seed) with 0 < p < 1, as
     at the reference call site. A dropped (query, key) entry leaves the softmax's numerator and denominator (no 1/(1-p)
@@ -310,8 +312,7 @@ def ringattention(q, k, v, attn_bias=None, segment_ids=None, *, axis_name="sp", 
             raise ValueError("precision must be 'bf16' or 'fp16'")
     if cache_idx is not None:
         raise NotImplementedError("cache_idx is always None at the reference call site (lwm/llama.py:544)")
-    if _quantized_kv("ringattention", q, k, v, bool(rotate_k) and freqs_cis is not None):
-        k, v = k.dequantize(q.dtype), v.dequantize(q.dtype)
+    quantized = _quantized_kv("ringattention", q, k, v, bool(rotate_k) and freqs_cis is not None)
     rope = _check_rope(freqs_cis, position_ids, q, k, rotate_k)
     rotate_k = bool(rotate_k)
     if precision == "fp8":
@@ -319,7 +320,7 @@ def ringattention(q, k, v, attn_bias=None, segment_ids=None, *, axis_name="sp", 
     if not q.is_cuda:
         raise _lib.LwmError("ringattention: tensors must live on an sm_90 GPU (no CPU fallback)")
     in_dtype = q.dtype
-    if not (k.dtype == in_dtype and v.dtype == in_dtype and in_dtype in (torch.bfloat16, torch.float32)):
+    if not ((quantized or k.dtype == v.dtype == in_dtype) and in_dtype in (torch.bfloat16, torch.float32)):
         raise TypeError("ringattention: q, k, v must all be bfloat16 or all float32 (fp32 logits and accumulation "
                         "are internal)")
     group, rank, world = _resolve_group(axis_name)
@@ -340,14 +341,20 @@ def ringattention(q, k, v, attn_bias=None, segment_ids=None, *, axis_name="sp", 
             rope = None
     if in_dtype == torch.float32 and not native_f32:
         # bf16 operand mode / NCCL transport: fp32 callers go through one rounding of q/k/v to bf16 (2^-9 relative)
-        q, k, v = q.to(torch.bfloat16), k.to(torch.bfloat16), v.to(torch.bfloat16)
+        q, k, v = q.to(torch.bfloat16), _bf16(k), _bf16(v)
     bias = _prep_bias(attn_bias, B)
     seg = None
     if segment_ids is not None:
         seg = segment_ids.to(torch.int32).contiguous()
     _check_mask_extent(bias, seg, rank, world, Sq, k.shape[1])
-    out = _RingAttnFn.apply(q.contiguous(), k.contiguous(), v.contiguous(), bias, seg, causal, axis_name, layout,
-                            precision, *(rope or (None, None)), rotate_k, dropout)
+    if _is_q8(k):
+        # the 8-bit cache: a forward without gradient (checked above), run without the autograd Function, whose
+        # save_for_backward takes tensors only; the operand passes read the cache's codes
+        out, _ = ring_forward(q.contiguous(), k, v, bias, seg, causal, group, rank, world, layout, precision, rope,
+                              rotate_k, dropout=dropout)
+    else:
+        out = _RingAttnFn.apply(q.contiguous(), k.contiguous(), v.contiguous(), bias, seg, causal, axis_name, layout,
+                                precision, *(rope or (None, None)), rotate_k, dropout)
     return out if out.dtype == in_dtype else out.to(in_dtype)
 
 
@@ -590,12 +597,40 @@ def _dt(t):
     raise TypeError("expected float32 or bfloat16, got %s" % t.dtype)
 
 
+def _is_q8(x):
+    """whether x is the 8-bit cache (kv_cache.QuantizedKV), the one int8 operand the ops below take"""
+    return x.dtype == torch.int8
+
+
+def _bf16(x):
+    """x in bf16: a tensor rounded, the 8-bit cache dequantized (exact)"""
+    return x.dequantize(torch.bfloat16) if _is_q8(x) else x.to(torch.bfloat16)
+
+
+def kv_q8_absmax(x, bits):
+    """atomicMax of the largest finite |value| of the 8-bit cache x into bits, as absmax on x.dequantize(...) would
+    (include/lwm_b200.h: lwm_kv_q8_absmax)"""
+    _lib.call("lwm_kv_q8_absmax", _lib.ptr(x.data), _lib.ptr(x.exp), *x.shape, _lib.ptr(bits), _lib.stream_ptr())
+
+
+def kv_q8_stage(x, dst, dst_code, scale):
+    """dst = the scaled operand copy of the 8-bit cache x, straight from its codes: dst_code 2 = fp16, 3 = e4m3 (the
+    bytes lwm_attn_to_f16_scaled / lwm_attn_to_e4m3_scaled write from x.dequantize(...); lwm_kv_q8_stage)"""
+    _lib.call("lwm_kv_q8_stage", _lib.ptr(x.data), _lib.ptr(x.exp), _lib.ptr(dst), dst_code, _lib.ptr(scale),
+              *x.shape, _lib.stream_ptr())
+
+
 class PeerOpsF16:
-    """fp16 operand mode: operands are power-of-two-scaled fp16 copies sharing ONE scale per sharded tensor."""
+    """fp16 operand mode: operands are power-of-two-scaled fp16 copies sharing ONE scale per sharded tensor.
+    absmax, scale_of and stage also take the 8-bit cache (kv_cache.QuantizedKV, or a batch row of it) for x and read
+    its codes directly: the same scale and the same copy as on the cache dequantized to fp32 or bf16."""
     op_dtype, op_itemsize, scaled = torch.float16, 2, True
 
     @staticmethod
     def absmax(x, bits):
+        if _is_q8(x):
+            kv_q8_absmax(x, bits)
+            return
         _lib.call("lwm_attn_absmax", _lib.ptr(x), _dt(x), x.numel(), _lib.ptr(bits), _lib.stream_ptr())
 
     @staticmethod
@@ -608,12 +643,20 @@ class PeerOpsF16:
     @staticmethod
     def scale_of(x, out):
         """out[0] = 2^(e-12), e the exponent of |x|max (the power-of-two scale of the fp16 operand copy of x)"""
+        if _is_q8(x):
+            bits = torch.zeros(1, dtype=torch.int32, device=x.device)
+            kv_q8_absmax(x, bits)
+            _lib.call("lwm_attn_scale_from_absmax", _lib.ptr(bits), 1, 1, _lib.ptr(out), _lib.stream_ptr())
+            return
         bits = torch.empty(1, dtype=torch.int32, device=x.device)
         st = _lib.stream_ptr()
         _lib.call("lwm_attn_absmax_scale", _lib.ptr(x), _dt(x), x.numel(), _lib.ptr(bits), _lib.ptr(out), st)
 
     @staticmethod
     def stage(x, dst, scale):
+        if _is_q8(x):
+            kv_q8_stage(x, dst, 2, scale)
+            return
         _lib.call("lwm_attn_to_f16_scaled", _lib.ptr(x), _dt(x), _lib.ptr(dst), _lib.ptr(scale), x.numel(),
                   _lib.stream_ptr())
 
@@ -683,12 +726,17 @@ class PeerOpsF16:
 
 
 class PeerOpsBf16(PeerOpsF16):
-    """bf16 operand mode: staging is a plain copy (fp32 inputs are rounded to bf16 there), no scales."""
+    """bf16 operand mode: staging is a plain copy (fp32 inputs are rounded to bf16 there, the 8-bit cache is
+    dequantized into dst, exactly), no scales."""
     op_dtype, op_itemsize, scaled = torch.bfloat16, 2, False
     _STAGE_DST = 1          # lwm_attn_stage_rope: bf16, the copy's rounding
 
     @staticmethod
     def stage(x, dst, scale):
+        if _is_q8(x):
+            _lib.call("lwm_kv_dequant_q8", _lib.ptr(x.data), _lib.ptr(x.exp), _lib.ptr(dst), _dt(dst), *x.shape,
+                      _lib.stream_ptr())
+            return
         dst.copy_(x)
 
     @staticmethod
@@ -739,6 +787,9 @@ class PeerOpsE4m3(PeerOpsF16):
 
     @staticmethod
     def stage(x, dst, scale):
+        if _is_q8(x):
+            kv_q8_stage(x, dst, 3, scale)
+            return
         _lib.call("lwm_attn_to_e4m3_scaled", _lib.ptr(x), _dt(x), _lib.ptr(dst), _lib.ptr(scale), x.numel(),
                   _lib.stream_ptr())
 
@@ -857,11 +908,13 @@ def ring_forward(q, k, v, bias, seg, causal, group, rank, world, layout="auto", 
         if precision == "fp8":
             _ops_for(precision)     # raises: no fp8 on the NCCL executor
         if want_f32:        # the NCCL executor takes bf16 operands (documented in ringattention())
-            out, res = ring_forward(q.to(torch.bfloat16), k.to(torch.bfloat16), v.to(torch.bfloat16), bias, seg, causal,
-                                    group, rank, world, layout, precision, rope, dropout=dropout)
+            out, res = ring_forward(q.to(torch.bfloat16), _bf16(k), _bf16(v), bias, seg, causal, group, rank, world,
+                                    layout, precision, rope, dropout=dropout)
             return out.float(), res
     if rope is not None:
         raise _lib.LwmError("ring_forward: the rotary embedding is folded into the one-GPU and peer-memory paths only")
+    if _is_q8(k):           # the 8-bit cache on the NCCL executor: its bf16 operands, exact
+        k, v = _bf16(k), _bf16(v)
     ops = with_dropout(_ops_for(precision), dropout)
     plan = rs.make_plan(world, rank, Sq, k.shape[1], causal, lay, n_sub_first=rs.auto_sub(world, k.shape[1], lay))
     out, res = rx.run_forward(plan, q, k, v, bias, seg, causal, group, ops)
@@ -1363,8 +1416,9 @@ def ringattention_inference(q, k, v, attn_mask, axis_name="sp", *, freqs_cis=Non
 
     k, v may be the 8-bit cache (kv_cache.QuantizedKV, both or neither) with q bf16 or fp32, without gradient and with
     rotate_k=False when the rotary keywords are given. Below INFER_MIN_Q query rows (world * Q_loc on a q-sharded
-    ring) the GEMV kernel reads it directly, bit for bit the call on the cache dequantized to q's dtype; from there on
-    the shard is dequantized to q's dtype (exact; one transient copy) for the tensor-core path.
+    ring) the GEMV kernel reads it directly; from there on the passes that stage the scaled fp16 copies of k and v for
+    the tensor cores read the cache's codes. Either way bit for bit the call on the cache dequantized to q's dtype,
+    without a dequantized copy of the shard in memory.
 
     CUDA graphs: on one GPU the GEMV call (Q < INFER_MIN_Q) can be captured with torch.cuda.graph, together with the
     ShardedKVCache decode write, and replayed (INTEGRATION.md "Decode in a CUDA graph"). While capturing, position_ids
@@ -1389,8 +1443,6 @@ def ringattention_inference(q, k, v, attn_mask, axis_name="sp", *, freqs_cis=Non
         raise _lib.LwmError("ringattention_inference: tensors must live on an sm_90 GPU (no CPU fallback)")
     if not quantized:
         _check_infer_dtypes(q, k, v)
-    elif (Q if world == 1 or Q == 1 else world * Q) >= INFER_MIN_Q:
-        k, v = k.dequantize(q.dtype), v.dequantize(q.dtype)      # the tensor-core path (see the docstring)
     if attn_mask is not None:
         if attn_mask.dim() != 4 or attn_mask.shape[1] != 1 or attn_mask.shape[2] != Q or attn_mask.shape[0] not in (1, B):
             raise ValueError("attn_mask must be [B,1,Q,K_global] (lwm/llama.py:585-590)")
